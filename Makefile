@@ -1,6 +1,6 @@
-# Build the C-ABI CUDA library (sm_100a only) and the oracle's C/compiled pieces.
+# Build the C-ABI CUDA library (sm_90a only) and the oracle's C/compiled pieces.
 NVCC ?= /usr/local/cuda/bin/nvcc
-ARCH := -gencode arch=compute_100a,code=sm_100a
+ARCH := -gencode arch=compute_90a,code=sm_90a
 NVFLAGS := $(ARCH) -O3 -std=c++17 -lineinfo -Xcompiler -fPIC -Xcompiler -Wall --expt-relaxed-constexpr
 CSRC := pixray_b200/csrc
 OBJDIR := build/obj

@@ -51,7 +51,7 @@ def config_dict(cfg, world, shard, extra=None):
          "drawer": cfg["drawer"], "weights": "seeded random (no checkpoints offline)",
          "parallelism": (f"one problem, {cfg['cutn']} cutouts sharded over {world} rank(s) ({cfg['cutn'] // max(world, 1)} each), "
                          "drawer replicated" if shard else f"{world} independent replica(s), one problem per GPU"),
-         "l2": "per-step working set (saved activations, GBs) >> 126 MB L2, no explicit flush"}
+         "l2": "per-step working set (saved activations, GBs) >> 50 MB L2, no explicit flush"}
     if extra:
         d.update(extra)
     return d
@@ -64,11 +64,12 @@ def measured_peaks():
         return dict(hbm_gbs=p["hbm_gbs"], tflops_burst=p["bf16_tflops"], tflops_sustained=p["bf16_tflops_sustained"],
                     source="measured (MEASURED_PEAKS.json)")
     except Exception:
-        return dict(hbm_gbs=6650.0, tflops_burst=1590.0, tflops_sustained=1400.0, source="fallback (B200_PROFILING.md)")
+        return dict(hbm_gbs=3350.0, tflops_burst=989.0, tflops_sustained=989.0,
+                    source="fallback: H100 SXM data sheet (700 W), dense FP16")
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -350,6 +351,8 @@ def run_engine(args, cfg, rank, world):
     sampler.stop_flag = True
     ms = e0.elapsed_time(e1)
     launches = eng.num_launches() - n0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"z": z, "losses": eng.read_losses()})
     # ---- per-kernel split for the roofline of the dominant kernel family
     prof = eng.profile_iteration(z, lr, args.warmup + args.steps)
     barrier()
@@ -405,15 +408,7 @@ def run_engine(args, cfg, rank, world):
         return
     peaks = measured_peaks()
     clocks = sampler.summary()
-    # DRAM bytes per tensor-core launch from the committed ncu pass over one iteration (not measurable live without a profiler)
-    traffic, traffic_src = None, None
-    for name in ("r02_gemm_traffic.json", "r01_gemm_traffic.json"):
-        tp = os.path.join(ROOT, "profiles", name)
-        if os.path.exists(tp) and world == 1 and args.config == 2:
-            with open(tp) as f:
-                tj = json.load(f)
-            traffic, traffic_src = tj["gemm_dram_bytes_per_launch"], tj["source"]
-            break
+    traffic, traffic_src = None, None  # DRAM bytes per launch need a profiler pass: not measured live
     S_flops = algorithmic_flops(cfg)
     gemm_tflops = prof["gemm_flops"] / (prof["gemm_ms"] * 1e-3) / 1e12 if prof["gemm_ms"] > 0 else 0.0
     nl = max(1, prof["gemm_launches"])
@@ -430,7 +425,7 @@ def run_engine(args, cfg, rank, world):
                 "d2h_bytes_per_step": d2h, "through": "pixray_b200.api.do_init + api.train (the loop of pixray.run())",
                 "host_sync_per_step": not getattr(st, "managed", False), "last_losses": last_losses},
         "gpu_launches": launches,
-        "roofline": {"kernel": "tcgen05 family: gemm_tc*/gemm_tce* (GEMM / implicit-GEMM conv) + attn_fwd/attn_bwd (fused attention)", "bound": "tensor",
+        "roofline": {"kernel": "tensor-core family: gemm_tc*/gemm_tce* (wgmma GEMM / implicit-GEMM conv) + attn_fwd/attn_bwd_* (fused attention)", "bound": "tensor",
                      "achieved": gemm_tflops, "peak": peaks["tflops_sustained"], "unit": "TFLOP/s",
                      "frac": gemm_tflops / peaks["tflops_sustained"], "traffic": traffic,
                      "traffic_unit": "bytes/launch (dram read+write)", "traffic_source": traffic_src,
@@ -452,6 +447,15 @@ def run_engine(args, cfg, rank, world):
     emit(line)
     if world > 1:
         dist.destroy_process_group()
+
+
+def dump_outputs(out_dir, arrays):
+    """--dump-outputs: what the last timed step handed its caller -- the optimised variable z after the Adam step and
+    clip, and that step's loss vector -- as float32 .npy files, for output-by-output comparison of two builds."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        a = a.detach().float().cpu().numpy() if torch.is_tensor(a) else np.asarray(a, dtype=np.float32)
+        np.save(os.path.join(out_dir, name + ".npy"), np.ascontiguousarray(a, dtype=np.float32))
 
 
 _JSON_FD = None
@@ -480,9 +484,13 @@ def main():
     ap.add_argument("--impl", default="engine", choices=["engine", "reference"])
     ap.add_argument("--config", type=int, default=2, choices=sorted(CONFIGS), help="BASELINE.json configuration (default 2)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's outputs (z, losses) to DIR/<name>.npy (float32)")
     ap.add_argument("--parallel", default="shard", choices=["shard", "replicas"],
                     help="N > 1: shard the cutouts of one problem over the ranks (default) or run N independent replicas")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl != "engine":
+        ap.error("--dump-outputs writes what the engine's timed path computed; it needs --impl engine")
     if args.warmup < 3:
         args.warmup = 3
     cfg = CONFIGS[args.config]

@@ -1,4 +1,4 @@
-/* pixray_b200 -- C ABI of the B200-native engine for pixray's per-iteration hot path.
+/* pixray_b200 -- C ABI of the H100-native (sm_90a) engine for pixray's per-iteration hot path.
  *
  * Plain C: pointers and sizes only, no torch types.  Every entry point below replaces one method the reference's
  * Python loop calls each iteration (file:line are relative to the reference checkout, pixray/pixray @ 37b03cf):
@@ -286,7 +286,7 @@ typedef struct {
   void* stream;
   int repeat;
   int n_store; /* fused-softmax epilogues (act 3 / 4): zero-fill columns [N, n_store) */
-  int cta_group; /* 0 auto, 1 single-CTA tiles, 2 CTA pairs (tcgen05 cta_group::2) */
+  int cta_group; /* ignored: sm_90 has no CTA-pair MMA, every GEMM runs single-CTA tiles (kept for the struct layout) */
   int tma_epi;   /* 0 auto (tensor-map epilogue when the tensors allow it), -1 force the generic epilogue */
 } pxr_test_gemm_desc;
 
@@ -306,7 +306,7 @@ int pxr_test_color_jitter_device(const float* rgb, int n, int code, float satura
 int pxr_test_pool_bounds(int in_size, int out_size, int* starts, int* ends);
 
 /* fused ViT attention (attn_tc.cu): forward, and backward when d_o != NULL.  qkv [B*T, 3W], o / d_o [B*T, W],
- * gqkv [B*T, 3W] fp16 device tensors, lse [B*H*T] fp32; heads are 64 wide (W = 64 H), T <= 256 */
+ * gqkv [B*T, 3W] fp16 device tensors, lse [B*H*T] fp32; heads are 64 wide (W = 64 H), T <= 240 */
 int pxr_test_attention(const void* qkv, void* o, float* lse, const void* d_o, void* gqkv, int B, int T, int H, int W,
                        float scale, int repeat, char* err, int errlen);
 

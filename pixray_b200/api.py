@@ -1,4 +1,4 @@
-"""pixray's module-level entry points on the B200 engine: `run`, `reset_settings`, `add_settings`, `get_settings`,
+"""pixray's module-level entry points on the H100 engine: `run`, `reset_settings`, `add_settings`, `get_settings`,
 `apply_settings`, `do_init`, `do_run`, `add_custom_loss` (pixray.py:2005-2124) -- the five calls the reference's
 front-ends use (run.py, cogrun.py) plus the notebook one-liner.
 

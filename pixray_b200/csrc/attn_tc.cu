@@ -1,881 +1,375 @@
-// See attn_tc.cuh.  sm_100a only (tcgen05 + TMA + TMEM).
-//
-// Shared-memory operand layouts are the ones gemm_tc.cu uses (and verifies on hardware): every operand tile is a stack
-// of 128-byte rows (64 fp16) with the 128-byte swizzle, 8-row groups 1024 B apart.  A tile loaded as rows = tokens,
-// columns = head channels is at the same time
-//   * a K-major operand whose reduction runs over the channels  (S = Q K^T, dP = dO V^T), and
-//   * an MN-major operand whose reduction runs over the tokens   (O = P V, dQ = dS K, dV = P^T dO, dK = dS^T Q),
-// so Q, K, V and dO are each loaded once per (image, head) and serve every product.  P / dS are written by the
-// softmax threads straight into that layout (chunk index XOR row % 8), one 128 x 64 atom per 64 key columns.
+// See attn_tc.cuh.  sm_90a: tensor-core mma.sync m16n8k16 (fp16 x fp16 -> fp32), operands staged in shared memory.
 #include "attn_tc.cuh"
 #include "launch.cuh"
-#include "gemm_tc.cuh"
-#include "ptx.cuh"
+#include <cmath>
 #include <cstdio>
 #include <mutex>
 
 namespace pxr {
-using namespace ptx;
-
 namespace {
 
-constexpr int ATT_THREADS = 576;  // warp 0 TMA producer, warp 1 MMA issuer (+TMEM owner), warps 2..17 softmax / epilogue
-constexpr int ATT_EPI_WARPS = 16;  // four per TMEM lane quarter: they split the score columns of a row
-constexpr uint32_t KiB = 1024;
-constexpr uint32_t ATOM = 16 * KiB;  // 128 rows x 128 bytes
+constexpr int AT_THREADS = 128;  // four warps, 16 rows each: one 64-row block per CTA
+constexpr int LDS = 72;          // row pitch (halves) of [rows][64] tiles: 144 B, conflict-free fragment loads
 constexpr float LOG2E = 1.4426950408889634f;
+constexpr float LN2 = 0.6931471805599453f;
 
-__device__ __forceinline__ uint4 pack8h(const float* x) {
-  uint4 u;
-  __half2* h = reinterpret_cast<__half2*>(&u);
-#pragma unroll
-  for (int j = 0; j < 4; ++j) h[j] = __floats2half2_rn(x[2 * j], x[2 * j + 1]);
-  return u;
+__device__ __forceinline__ void mma16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+      "{%0, %1, %2, %3};"
+      : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
-// 8 accumulator words (fp32 bit patterns) scaled by `mul` -> 8 fp16
-__device__ __forceinline__ uint4 pack8h_acc(const uint32_t* r, float mul) {
-  uint4 u;
-  __half2* h = reinterpret_cast<__half2*>(&u);
-#pragma unroll
-  for (int j = 0; j < 4; ++j) h[j] = __floats2half2_rn(__uint_as_float(r[2 * j]) * mul, __uint_as_float(r[2 * j + 1]) * mul);
-  return u;
+__device__ __forceinline__ uint32_t ld32(const __half* p) { return *reinterpret_cast<const uint32_t*>(p); }
+__device__ __forceinline__ uint32_t pack(float x, float y) {
+  __half2 h = __floats2half2_rn(x, y);
+  return *reinterpret_cast<uint32_t*>(&h);
 }
-__device__ __forceinline__ void unpack8h(const uint4& u, float* x) {
-  const __half2* h = reinterpret_cast<const __half2*>(&u);
+// A fragment (16 x 16) of a row-major tile X[row][k] with pitch ld: rows r0.., k k0..
+__device__ __forceinline__ void load_a(uint32_t (&a)[4], const __half* X, int ld, int r0, int k0, int g, int t) {
+  a[0] = ld32(X + (r0 + g) * ld + k0 + 2 * t);
+  a[1] = ld32(X + (r0 + g + 8) * ld + k0 + 2 * t);
+  a[2] = ld32(X + (r0 + g) * ld + k0 + 2 * t + 8);
+  a[3] = ld32(X + (r0 + g + 8) * ld + k0 + 2 * t + 8);
+}
+// A fragment of a 16-column slice (columns 2c, 2c+1 of the 8-column accumulator tiles) of accumulator rows
+__device__ __forceinline__ void acc_to_a(uint32_t (&a)[4], const float (&x0)[4], const float (&x1)[4]) {
+  a[0] = pack(x0[0], x0[1]);
+  a[1] = pack(x0[2], x0[3]);
+  a[2] = pack(x1[0], x1[1]);
+  a[3] = pack(x1[2], x1[3]);
+}
+// Y[rows][64] <- rows [r0, r0 + n) of the [B*T, ld] tensor at column c0 (one image), zero past T
+__device__ __forceinline__ void load_rows(__half* Y, const __half* src, int ld, int c0, int r0, int n, int T) {
+  for (int i = threadIdx.x; i < n * 8; i += AT_THREADS) {
+    const int r = i >> 3, c = (i & 7) * 8;
+    uint4 v = make_uint4(0, 0, 0, 0);
+    if (r0 + r < T) v = *reinterpret_cast<const uint4*>(src + (size_t)(r0 + r) * ld + c0 + c);
+    *reinterpret_cast<uint4*>(Y + r * LDS + c) = v;
+  }
+}
+// Yt[64][ldt] (transposed: Yt[d][row]) <- the same rows
+__device__ __forceinline__ void load_rows_t(__half* Yt, int ldt, const __half* src, int ld, int c0, int r0, int n, int T) {
+  for (int i = threadIdx.x; i < n * 8; i += AT_THREADS) {
+    const int r = i >> 3, c = (i & 7) * 8;
+    uint4 v = make_uint4(0, 0, 0, 0);
+    if (r0 + r < T) v = *reinterpret_cast<const uint4*>(src + (size_t)(r0 + r) * ld + c0 + c);
+    const __half* h = reinterpret_cast<const __half*>(&v);
 #pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    const float2 f = __half22float2(h[j]);
-    x[2 * j] = f.x;
-    x[2 * j + 1] = f.y;
+    for (int j = 0; j < 8; ++j) Yt[(c + j) * ldt + r] = h[j];
+  }
+}
+// dO rows [r0, r0 + 64) into Y (and Yt when non-null), D[r] = dO_r . O_r, lse[r] * log2(e) (zeros past T)
+__device__ __forceinline__ void load_do_block(const AttnParams& p, int b, int h, int r0, __half* Y, __half* Yt, float* D,
+                                              float* L) {
+  const int T = p.T, W = p.W;
+  for (int i = threadIdx.x; i < 64 * 8; i += AT_THREADS) {  // the 8 lanes of a row are adjacent: shuffle-reduce
+    const int r = i >> 3, c = (i & 7) * 8;
+    uint4 v = make_uint4(0, 0, 0, 0), o = make_uint4(0, 0, 0, 0);
+    if (r0 + r < T) {
+      const size_t off = (size_t)(b * T + r0 + r) * W + h * 64 + c;
+      v = *reinterpret_cast<const uint4*>(p.d_o + off);
+      o = *reinterpret_cast<const uint4*>(p.o + off);
+    }
+    *reinterpret_cast<uint4*>(Y + r * LDS + c) = v;
+    const __half* hv = reinterpret_cast<const __half*>(&v);
+    const __half* ho = reinterpret_cast<const __half*>(&o);
+    float d = 0.f;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      d += __half2float(hv[j]) * __half2float(ho[j]);
+      if (Yt) Yt[(c + j) * LDS + r] = hv[j];
+    }
+    d += __shfl_xor_sync(0xffffffffu, d, 1);
+    d += __shfl_xor_sync(0xffffffffu, d, 2);
+    d += __shfl_xor_sync(0xffffffffu, d, 4);
+    if ((i & 7) == 0) {
+      D[r] = d;
+      L[r] = (r0 + r < T) ? p.lse[(size_t)(b * p.H + h) * T + r0 + r] * LOG2E : 0.f;
+    }
   }
 }
 
-// byte offset of the 8 fp16 starting at column j0 (multiple of 8) of row r in a [128 x n] K-major operand made of
-// 128 x 64 atoms (128-byte swizzle: 16-byte chunk index XOR (row % 8))
-__device__ __forceinline__ uint32_t op_off(int r, int j0) {
-  return static_cast<uint32_t>(j0 >> 6) * ATOM + static_cast<uint32_t>(r) * 128u +
-         (static_cast<uint32_t>(((j0 & 63) >> 3) ^ (r & 7)) << 4);
-}
-
-__device__ __forceinline__ uint64_t desc_k(uint32_t addr) { return make_smem_desc_sw128(addr, 0, 1024); }
-__device__ __forceinline__ uint64_t desc_mn(uint32_t addr, uint32_t lbo) { return make_smem_desc_sw128(addr, lbo, 1024); }
-
-// Visit the 16-column blocks first, first + step, ... (< nblk) of this thread's accumulator row with the TMEM load of
-// the next block in flight while the current one is processed.  f(regs, blk).
-template <class F>
-__device__ __forceinline__ void for_blocks(uint32_t taddr, int first, int step, int nblk, F&& f) {
-  uint32_t a[16], b[16];
-  int blk = first;
-  if (blk >= nblk) return;
-  tmem_ld_x16(taddr + blk * 16, a);
-  while (true) {
-    tmem_ld_wait();
-    const int nb = blk + step;
-    if (nb < nblk) tmem_ld_x16(taddr + nb * 16, b);
-    f(a, blk);
-    if (nb >= nblk) break;
-    tmem_ld_wait();
-    blk = nb + step;
-    if (blk < nblk) tmem_ld_x16(taddr + blk * 16, a);
-    f(b, nb);
-    if (blk >= nblk) break;
-  }
-}
-
-__device__ __forceinline__ uint32_t kv_slot_bytes(int n_pad) { return (static_cast<uint32_t>(n_pad) * 128u + 1023u) & ~1023u; }
-
-// ------------------------------------------------------------------------------------------------ forward
-// smem: Q (two 128-row tiles) 32 KiB | K | V (n_pad rows each) | P tile 0 | P tile 1 (64 KiB each) | barriers | exchange.
-// TMEM: S tile mt at columns [256 mt, 256 mt + n_pad); O tile mt re-uses the first 64 columns of its S tile.
-// The next pair's Q / K are fetched as soon as both S tiles are complete, its V once both PV products are.
-__global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_kernel(const __grid_constant__ AttnParams p) {
-  pdl_launch_dependents();
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t base_u32 = smem_u32(smem_raw);
-  uint8_t* smem = smem_raw + (((base_u32 + 1023u) & ~1023u) - base_u32);
-  const int n_mt = p.n_mt, n_pad = p.n_pad, T = p.T;
-  const uint32_t kvb = kv_slot_bytes(n_pad);
-  const uint32_t F_Q = 0, F_K = 32 * KiB, F_V = F_K + kvb, F_P0 = F_V + kvb, F_P1 = F_P0 + 64 * KiB, F_BAR = F_P1 + 64 * KiB;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + F_BAR);
-  uint64_t* bar_qk = bars;        // TMA: Q, K landed
-  uint64_t* bar_v = bars + 1;     // TMA: V landed
-  uint64_t* bar_s = bars + 2;     // both S tiles complete (Q / K consumed)
-  uint64_t* bar_p = bars + 3;     // [2] P tile written by its eight warps
-  uint64_t* bar_o = bars + 5;     // [2] O tile complete (P tile / V consumed)
-  uint64_t* bar_free = bars + 7;  // all epilogue warps done with TMEM
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 8);
-  float* xmax = reinterpret_cast<float*>(smem + F_BAR + 256);  // [2 tiles][2 halves][128 rows]
-  float* xsum = xmax + 512;
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) {
-    prefetch_tmap(&p.tm_q);
-    prefetch_tmap(&p.tm_kv);
-    mbar_init(bar_qk, 1);
-    mbar_init(bar_v, 1);
-    mbar_init(bar_s, 1);
-    mbar_init(&bar_p[0], 8);
-    mbar_init(&bar_p[1], 8);
-    mbar_init(&bar_o[0], 1);
-    mbar_init(&bar_o[1], 1);
-    mbar_init(bar_free, ATT_EPI_WARPS);
-    fence_barrier_init();
-  }
-  if (warp == 1) tmem_alloc(tmem_ptr, 512);
-  tc_fence_before();
+// ------------------------------------------------------------------------------------------------------------ forward
+// CTA = (64-query block, head, image).  Warp w: query rows 16 w.. of the block; online softmax over 64-key blocks.
+__global__ void __launch_bounds__(AT_THREADS) attn_fwd_kernel(const __grid_constant__ AttnParams p) {
+  pdl_prologue();
+  extern __shared__ uint4 smem_at[];
+  const int qb = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+  const int T = p.T, TP = (T + 63) / 64 * 64, ld3 = 3 * p.W, ldv = TP + 8;
+  __half* Qs = reinterpret_cast<__half*>(smem_at);
+  __half* Ks = Qs + 64 * LDS;
+  __half* Vt = Ks + TP * LDS;  // [64][TP + 8]: V transposed (the PV product's B operand is key-contiguous)
+  const __half* base = p.qkv + (size_t)b * T * ld3;
+  load_rows(Qs, base, ld3, h * 64, qb * 64, 64, T);
+  load_rows(Ks, base, ld3, p.W + h * 64, 0, TP, T);
+  load_rows_t(Vt, ldv, base, ld3, 2 * p.W + h * 64, 0, TP, T);
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-  const uint32_t s_base = smem_u32(smem);
-  pdl_wait();  // above: parameters, shared memory, TMEM only
-
-  if (warp == 0) {
-    if (lane == 0) {
-      const uint32_t kv_bytes = static_cast<uint32_t>(n_pad) * 128u;
-      int it = 0;
-      for (int item = blockIdx.x; item < p.items; item += gridDim.x, ++it) {
-        const int b = item / p.H, h = item % p.H;
-        if (it > 0) mbar_wait(bar_s, (it - 1) & 1);  // the previous pair's S products have consumed Q and K
-        mbar_arrive_expect_tx(bar_qk, static_cast<uint32_t>(n_mt) * ATOM + kv_bytes);
-        for (int mt = 0; mt < n_mt; ++mt) tma_load_4d(&p.tm_q, bar_qk, smem + F_Q + mt * ATOM, h * 64, mt * 128, b, 0);
-        tma_load_4d(&p.tm_kv, bar_qk, smem + F_K, p.W + h * 64, 0, b, 0);
-        if (it > 0)
-          for (int mt = 0; mt < n_mt; ++mt) mbar_wait(&bar_o[mt], (it - 1) & 1);  // ... and its PV products V
-        mbar_arrive_expect_tx(bar_v, kv_bytes);
-        tma_load_4d(&p.tm_kv, bar_v, smem + F_V, 2 * p.W + h * 64, 0, b, 0);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3, r0 = warp * 16;
+  uint32_t qa[4][4];
+#pragma unroll
+  for (int kc = 0; kc < 4; ++kc) load_a(qa[kc], Qs, LDS, r0, kc * 16, g, t);
+  float o[8][4] = {};
+  float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
+  const float c = p.scale * LOG2E;
+  for (int kb = 0; kb * 64 < T; ++kb) {
+    float s[8][4] = {};
+#pragma unroll
+    for (int kc = 0; kc < 4; ++kc)
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const __half* kr = Ks + (kb * 64 + j * 8 + g) * LDS + kc * 16 + 2 * t;
+        mma16816(s[j], qa[kc], ld32(kr), ld32(kr + 8));
       }
+    float x0 = -INFINITY, x1 = -INFINITY;
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int key = kb * 64 + j * 8 + 2 * t + (e & 1);
+        s[j][e] = key < T ? s[j][e] * c : -INFINITY;
+        if (e < 2) x0 = fmaxf(x0, s[j][e]);
+        else x1 = fmaxf(x1, s[j][e]);
+      }
+#pragma unroll
+    for (int off = 1; off < 4; off <<= 1) {
+      x0 = fmaxf(x0, __shfl_xor_sync(0xffffffffu, x0, off));
+      x1 = fmaxf(x1, __shfl_xor_sync(0xffffffffu, x1, off));
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t id_s = make_idesc_f16(128, n_pad, 0, 0, 0);
-      const uint32_t id_pv = make_idesc_f16(128, 64, 0, 0, 1);
-      // descriptors are built once; advancing an operand by X bytes adds X >> 4 to the address field (the single issuing
-      // thread is on the critical path of every phase: keep its instruction count down)
-      constexpr uint64_t AT = ATOM >> 4;
-      const uint64_t d_q = desc_k(s_base + F_Q), d_k = desc_k(s_base + F_K), d_v = desc_mn(s_base + F_V, 8192);
-      const uint64_t d_p0 = desc_k(s_base + F_P0), d_p1 = desc_k(s_base + F_P1);
-      const int n_k = n_pad / 16;
-      int it = 0;
-      for (int item = blockIdx.x; item < p.items; item += gridDim.x, ++it) {
-        mbar_wait(bar_qk, it & 1);
-        if (it > 0) mbar_wait(bar_free, (it - 1) & 1);
-        tc_fence_after();
-        for (int mt = 0; mt < n_mt; ++mt) {
+    const float n0 = fmaxf(m0, x0), n1 = fmaxf(m1, x1);  // every key block holds a key < T: finite
+    const float a0 = exp2f(m0 - n0), a1 = exp2f(m1 - n1);
+    m0 = n0;
+    m1 = n1;
+    l0 *= a0;
+    l1 *= a1;
 #pragma unroll
-          for (int k = 0; k < 4; ++k) umma_f16(tmem_base + mt * 256, d_q + mt * AT + 2 * k, d_k + 2 * k, id_s, k ? 1u : 0u);
-        }
-        umma_commit(bar_s);
-        mbar_wait(bar_v, it & 1);
-        for (int mt = 0; mt < n_mt; ++mt) {
-          mbar_wait(&bar_p[mt], it & 1);
-          tc_fence_after();
-          const uint64_t pa = mt ? d_p1 : d_p0;
-          const uint32_t d_o = tmem_base + mt * 256;
-#pragma unroll 4
-          for (int k = 0; k < n_k; ++k)
-            umma_f16(d_o, pa + (k >> 2) * AT + (k & 3) * 2, d_v + k * 128, id_pv, k ? 1u : 0u);
-          umma_commit(&bar_o[mt]);
-        }
-      }
+    for (int j = 0; j < 8; ++j) {
+      s[j][0] = exp2f(s[j][0] - n0);
+      s[j][1] = exp2f(s[j][1] - n0);
+      s[j][2] = exp2f(s[j][2] - n1);
+      s[j][3] = exp2f(s[j][3] - n1);
+      l0 += s[j][0] + s[j][1];
+      l1 += s[j][2] + s[j][3];
+      o[j][0] *= a0;
+      o[j][1] *= a0;
+      o[j][2] *= a1;
+      o[j][3] *= a1;
     }
-  } else {
-    const int q = warp & 3, sub = (warp - 2) >> 2;
-    const int mt = sub >> 1, half = sub & 1;  // tile, and which of the two warps sharing this tile's lane quarter
-    const int row = q * 32 + lane;
-    const float sc = p.scale * LOG2E;
-    const int nblk = n_pad / 16;  // 16-column blocks
-    const int pair_bar = 1 + mt * 4 + q;
-    float* my_max = xmax + (mt * 2 + half) * 128 + row;
-    float* other_max = xmax + (mt * 2 + (half ^ 1)) * 128 + row;
-    float* my_sum = xsum + (mt * 2 + half) * 128 + row;
-    float* other_sum = xsum + (mt * 2 + (half ^ 1)) * 128 + row;
-    uint8_t* prow = smem + (mt ? F_P1 : F_P0);
-    const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>(mt * 256);
-    int it = 0;
-    for (int item = blockIdx.x; item < p.items; item += gridDim.x, ++it) {
-      const int b = item / p.H, h = item % p.H;
-      // EVERY warp paces itself on the item's S barrier, also the eight that own the second query tile when there is
-      // none (T <= 128): without it they would run through all their items at once and arrive on bar_free ahead of
-      // the phases those arrivals belong to (a CTA with more than one item then deadlocks: B x heads > #SMs at T <= 128,
-      // e.g. ViT-B/32 with cutn = 128)
-      mbar_wait(bar_s, it & 1);
-      if (mt < n_mt) {
-        const int i = mt * 128 + row;
-        tc_fence_after();
-        // ---- row maximum (columns split between the two warps of the pair)
-        float m4[4] = {-3.0e38f, -3.0e38f, -3.0e38f, -3.0e38f};
-        for_blocks(taddr, half, 2, nblk, [&](const uint32_t(&r)[16], int blk) {
-          const int c0 = blk * 16;
-          if (c0 + 16 <= T) {
 #pragma unroll
-            for (int j = 0; j < 16; ++j) m4[j & 3] = fmaxf(m4[j & 3], __uint_as_float(r[j]));
-          } else {
+    for (int kc = 0; kc < 4; ++kc) {  // 16 keys of the block
+      uint32_t pa[4];
+      acc_to_a(pa, s[2 * kc], s[2 * kc + 1]);
 #pragma unroll
-            for (int j = 0; j < 16; ++j)
-              if (c0 + j < T) m4[j & 3] = fmaxf(m4[j & 3], __uint_as_float(r[j]));
-          }
-        });
-        float mx = fmaxf(fmaxf(m4[0], m4[1]), fmaxf(m4[2], m4[3]));
-        *my_max = mx;
-        named_bar_sync(pair_bar, 64);
-        mx = fmaxf(mx, *other_max);
-        const float mxs = mx * sc;
-        // ---- P~ = exp(S - max) as fp16 into the operand layout; partial row sums
-        float s4[4] = {0.f, 0.f, 0.f, 0.f};
-        for_blocks(taddr, half, 2, nblk, [&](const uint32_t(&r)[16], int blk) {
-          const int c0 = blk * 16;
-          const bool full = c0 + 16 <= T;
-#pragma unroll
-          for (int g = 0; g < 2; ++g) {
-            float e[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              float x = ex2_approx(fmaf(__uint_as_float(r[8 * g + j]), sc, -mxs));
-              if (!full && c0 + 8 * g + j >= T) x = 0.f;
-              e[j] = x;
-              s4[j & 3] += x;
-            }
-            *reinterpret_cast<uint4*>(prow + op_off(row, c0 + 8 * g)) = pack8h(e);
-          }
-        });
-        const float sum_part = (s4[0] + s4[1]) + (s4[2] + s4[3]);
-        *my_sum = sum_part;
-        tc_fence_before();
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&bar_p[mt]);
-        // ---- O = (P~ V) / sum : this warp writes 32 of the 64 head channels
-        mbar_wait(&bar_o[mt], it & 1);
-        tc_fence_after();
-        named_bar_sync(pair_bar, 64);
-        const float sum = sum_part + *other_sum;
-        const float inv = __fdividef(1.f, sum);
-        uint32_t o[32];
-        tmem_ld_x32(taddr + half * 32, o);
-        tmem_ld_wait();
-        if (i < T) {
-          __half* dst = p.o + (static_cast<size_t>(b) * T + i) * p.W + h * 64 + half * 32;
-#pragma unroll
-          for (int c = 0; c < 4; ++c) reinterpret_cast<uint4*>(dst)[c] = pack8h_acc(o + 8 * c, inv);
-          if (half == 0) p.lse[(static_cast<size_t>(b) * p.H + h) * T + i] = mx * p.scale + __logf(sum);
-        }
+      for (int j = 0; j < 8; ++j) {
+        const __half* vr = Vt + (j * 8 + g) * ldv + kb * 64 + kc * 16 + 2 * t;
+        mma16816(o[j], pa, ld32(vr), ld32(vr + 8));
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_free);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    __syncwarp();
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+#pragma unroll
+  for (int off = 1; off < 4; off <<= 1) {
+    l0 += __shfl_xor_sync(0xffffffffu, l0, off);
+    l1 += __shfl_xor_sync(0xffffffffu, l1, off);
+  }
+  const int q0 = qb * 64 + r0 + g, q1 = q0 + 8;
+  const float i0 = 1.f / l0, i1 = 1.f / l1;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const int col = h * 64 + j * 8 + 2 * t;
+    if (q0 < T) *reinterpret_cast<uint32_t*>(p.o + (size_t)(b * T + q0) * p.W + col) = pack(o[j][0] * i0, o[j][1] * i0);
+    if (q1 < T) *reinterpret_cast<uint32_t*>(p.o + (size_t)(b * T + q1) * p.W + col) = pack(o[j][2] * i1, o[j][3] * i1);
+  }
+  if (t == 0) {
+    float* lse = p.lse + (size_t)(b * p.H + h) * T;
+    if (q0 < T) lse[q0] = (m0 + log2f(l0)) * LN2;
+    if (q1 < T) lse[q1] = (m1 + log2f(l1)) * LN2;
   }
 }
 
-// ------------------------------------------------------------------------------------------------ backward
-// smem: Q 32 KiB (two 128-row tiles) | K | V (n_pad rows each) | dO 32 KiB | PS 64 KiB (P, then dS in place).
-// TMEM: region A = columns [0, 256): S, then dP, then dQ (first 64 columns) of the current 128 query rows;
-//       dK key tile jt at [256 + 64 jt, +64), dV at [384 + 64 jt, +64) -- accumulated over both query tiles.
-// Per query tile:  S -> P (threads) -> {dP, dV += P^T dO} -> dS (threads) -> {dQ, dK += dS^T Q} -> dQ out (threads).
-// The four warps of a TMEM lane quarter split the 32-column blocks of their rows.
-constexpr uint32_t TM_DK = 256, TM_DV = 384;
-
-__global__ void __launch_bounds__(ATT_THREADS, 1) attn_bwd_kernel(const __grid_constant__ AttnParams p) {
-  pdl_launch_dependents();
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t base_u32 = smem_u32(smem_raw);
-  uint8_t* smem = smem_raw + (((base_u32 + 1023u) & ~1023u) - base_u32);
-  const int n_mt = p.n_mt, n_pad = p.n_pad, T = p.T;
-  const uint32_t kvb = kv_slot_bytes(n_pad);
-  const uint32_t B_Q = 0, B_K = 32 * KiB, B_V = B_K + kvb, B_DO = B_V + kvb, B_PS = B_DO + 32 * KiB, B_BAR = B_PS + 64 * KiB;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + B_BAR);
-  uint64_t* bar_load = bars;        // per pair: Q, K, V, dO landed
-  uint64_t* bar_s = bars + 1;       // per query tile: S complete
-  uint64_t* bar_p = bars + 2;       // P written (16 warps)
-  uint64_t* bar_dp = bars + 3;      // dP complete
-  uint64_t* bar_pfree = bars + 4;   // dV products have consumed P
-  uint64_t* bar_ds = bars + 5;      // dS written (16 warps)
-  uint64_t* bar_dq = bars + 6;      // dQ complete
-  uint64_t* bar_dsfree = bars + 7;  // dK products have consumed dS
-  uint64_t* bar_afree = bars + 8;   // region A read out (16 warps)
-  uint64_t* bar_done = bars + 9;    // per pair: dK / dV read out (16 warps)
-  uint64_t* bar_smem = bars + 10;   // per pair: every product has consumed its operands
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 12);
-  float* xd = reinterpret_cast<float*>(smem + B_BAR + 256);  // [2 buffers][4 column quarters][128 rows] partial D
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) {
-    prefetch_tmap(&p.tm_q);
-    prefetch_tmap(&p.tm_kv);
-    prefetch_tmap(&p.tm_do);
-    mbar_init(bar_load, 1);
-    mbar_init(bar_s, 1);
-    mbar_init(bar_p, ATT_EPI_WARPS);
-    mbar_init(bar_dp, 1);
-    mbar_init(bar_pfree, 1);
-    mbar_init(bar_ds, ATT_EPI_WARPS);
-    mbar_init(bar_dq, 1);
-    mbar_init(bar_dsfree, 1);
-    mbar_init(bar_afree, ATT_EPI_WARPS);
-    mbar_init(bar_done, ATT_EPI_WARPS);
-    mbar_init(bar_smem, 1);
-    fence_barrier_init();
-  }
-  if (warp == 1) tmem_alloc(tmem_ptr, 512);
-  tc_fence_before();
+// ------------------------------------------------------------------------------------------------------------ dQ
+// CTA = (64-query block, head, image).  dQ_i = scale * sum_j P_ij (dP_ij - D_i) K_j with dP = dO V^T.
+__global__ void __launch_bounds__(AT_THREADS) attn_bwd_dq_kernel(const __grid_constant__ AttnParams p) {
+  pdl_prologue();
+  extern __shared__ uint4 smem_at[];
+  const int qb = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+  const int T = p.T, TP = (T + 63) / 64 * 64, ld3 = 3 * p.W, ldk = TP + 8;
+  __half* Qs = reinterpret_cast<__half*>(smem_at);
+  __half* dOs = Qs + 64 * LDS;
+  __half* Ks = dOs + 64 * LDS;
+  __half* Vs = Ks + TP * LDS;
+  __half* Kt = Vs + TP * LDS;  // [64][TP + 8]
+  float* Ds = reinterpret_cast<float*>(Kt + 64 * ldk);
+  float* Ls = Ds + 64;
+  const __half* base = p.qkv + (size_t)b * T * ld3;
+  load_rows(Qs, base, ld3, h * 64, qb * 64, 64, T);
+  load_rows(Ks, base, ld3, p.W + h * 64, 0, TP, T);
+  load_rows(Vs, base, ld3, 2 * p.W + h * 64, 0, TP, T);
+  load_rows_t(Kt, ldk, base, ld3, p.W + h * 64, 0, TP, T);
+  load_do_block(p, b, h, qb * 64, dOs, nullptr, Ds, Ls);
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-  const uint32_t s_base = smem_u32(smem);
-  pdl_wait();  // above: parameters, shared memory, TMEM only
-
-  if (warp == 0) {
-    if (lane == 0) {
-      const uint32_t bytes = 2u * static_cast<uint32_t>(n_mt) * ATOM + 2u * static_cast<uint32_t>(n_pad) * 128u;
-      int it = 0;
-      for (int item = blockIdx.x; item < p.items; item += gridDim.x, ++it) {
-        const int b = item / p.H, h = item % p.H;
-        if (it > 0) mbar_wait(bar_smem, (it - 1) & 1);
-        mbar_arrive_expect_tx(bar_load, bytes);
-        for (int mt = 0; mt < n_mt; ++mt) {
-          tma_load_4d(&p.tm_q, bar_load, smem + B_Q + mt * ATOM, h * 64, mt * 128, b, 0);
-          tma_load_4d(&p.tm_do, bar_load, smem + B_DO + mt * ATOM, h * 64, mt * 128, b, 0);
-        }
-        tma_load_4d(&p.tm_kv, bar_load, smem + B_K, p.W + h * 64, 0, b, 0);
-        tma_load_4d(&p.tm_kv, bar_load, smem + B_V, 2 * p.W + h * 64, 0, b, 0);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3, r0 = warp * 16;
+  uint32_t qa[4][4], da[4][4];
+#pragma unroll
+  for (int kc = 0; kc < 4; ++kc) {
+    load_a(qa[kc], Qs, LDS, r0, kc * 16, g, t);
+    load_a(da[kc], dOs, LDS, r0, kc * 16, g, t);
+  }
+  const float L0 = Ls[r0 + g], L1 = Ls[r0 + g + 8], D0 = Ds[r0 + g], D1 = Ds[r0 + g + 8];
+  const float c = p.scale * LOG2E;
+  float dq[8][4] = {};
+  for (int kb = 0; kb * 64 < T; ++kb) {
+    float s[8][4] = {}, dp[8][4] = {};
+#pragma unroll
+    for (int kc = 0; kc < 4; ++kc)
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const int row = (kb * 64 + j * 8 + g) * LDS + kc * 16 + 2 * t;
+        mma16816(s[j], qa[kc], ld32(Ks + row), ld32(Ks + row + 8));
+        mma16816(dp[j], da[kc], ld32(Vs + row), ld32(Vs + row + 8));
       }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t id_s = make_idesc_f16(128, n_pad, 0, 0, 0);   // S, dP: both operands K-major
-      const uint32_t id_dq = make_idesc_f16(128, 64, 0, 0, 1);     // dQ = dS K: A K-major, B MN-major
-      const uint32_t id_t = make_idesc_f16(128, 64, 0, 1, 1);      // dV = P^T dO, dK = dS^T Q: both MN-major
-      const uint32_t tA = tmem_base;
-      // descriptors built once, advanced by adds on the address field (see the forward kernel)
-      constexpr uint64_t AT = ATOM >> 4;
-      const uint64_t dk_q = desc_k(s_base + B_Q), dk_k = desc_k(s_base + B_K), dk_v = desc_k(s_base + B_V),
-                     dk_do = desc_k(s_base + B_DO), dk_ps = desc_k(s_base + B_PS);
-      const uint64_t dm_ps = desc_mn(s_base + B_PS, ATOM), dm_do = desc_mn(s_base + B_DO, 8192),
-                     dm_q = desc_mn(s_base + B_Q, 8192), dm_k = desc_mn(s_base + B_K, 8192);
-      const int n_k = n_pad / 16;
-      int it = 0, cnt = 0;
-      for (int item = blockIdx.x; item < p.items; item += gridDim.x, ++it) {
-        mbar_wait(bar_load, it & 1);
-        if (it > 0) mbar_wait(bar_done, (it - 1) & 1);
-        tc_fence_after();
-        for (int mt = 0; mt < n_mt; ++mt, ++cnt) {
-          if (cnt > 0) {
-            mbar_wait(bar_afree, (cnt - 1) & 1);
-            tc_fence_after();
-          }
-          const int rows_left = T - mt * 128;
-          const int ksi = rows_left >= 128 ? 8 : (rows_left + 15) / 16;  // 16-row reduction steps over this tile's queries
 #pragma unroll
-          for (int k = 0; k < 4; ++k) umma_f16(tA, dk_q + mt * AT + 2 * k, dk_k + 2 * k, id_s, k ? 1u : 0u);
-          umma_commit(bar_s);
-          mbar_wait(bar_p, cnt & 1);
-          tc_fence_after();
+    for (int j = 0; j < 8; ++j)
 #pragma unroll
-          for (int k = 0; k < 4; ++k) umma_f16(tA, dk_do + mt * AT + 2 * k, dk_v + 2 * k, id_s, k ? 1u : 0u);
-          umma_commit(bar_dp);
-          for (int jt = 0; jt < n_mt; ++jt) {
-            const uint64_t a0 = dm_ps + 2 * jt * AT, b0 = dm_do + mt * AT;
-#pragma unroll 4
-            for (int ks = 0; ks < ksi; ++ks)
-              umma_f16(tmem_base + TM_DV + jt * 64, a0 + ks * 128, b0 + ks * 128, id_t, (mt | ks) ? 1u : 0u);
-          }
-          umma_commit(bar_pfree);
-          mbar_wait(bar_ds, cnt & 1);
-          tc_fence_after();
-#pragma unroll 4
-          for (int k = 0; k < n_k; ++k)
-            umma_f16(tA, dk_ps + (k >> 2) * AT + (k & 3) * 2, dm_k + k * 128, id_dq, k ? 1u : 0u);
-          umma_commit(bar_dq);
-          for (int jt = 0; jt < n_mt; ++jt) {
-            const uint64_t a0 = dm_ps + 2 * jt * AT, b0 = dm_q + mt * AT;
-#pragma unroll 4
-            for (int ks = 0; ks < ksi; ++ks)
-              umma_f16(tmem_base + TM_DK + jt * 64, a0 + ks * 128, b0 + ks * 128, id_t, (mt | ks) ? 1u : 0u);
-          }
-          umma_commit(bar_dsfree);
-        }
-        umma_commit(bar_smem);
+      for (int e = 0; e < 4; ++e) {
+        const int key = kb * 64 + j * 8 + 2 * t + (e & 1);
+        const float pv = key < T ? exp2f(s[j][e] * c - (e < 2 ? L0 : L1)) : 0.f;
+        s[j][e] = pv * (dp[j][e] - (e < 2 ? D0 : D1));
       }
-    }
-  } else {
-    const int q = warp & 3, cq = (warp - 2) >> 2;  // lane quarter; which of its four warps (column blocks cq, cq + 4)
-    const int row = q * 32 + lane;
-    const float sc = p.scale * LOG2E;
-    const int nblk = n_pad / 16;  // 16-column blocks
-    const uint32_t lane_addr = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
-    uint8_t* ps = smem + B_PS;
-    int it = 0, cnt = 0;
-    for (int item = blockIdx.x; item < p.items; item += gridDim.x, ++it) {
-      const int b = item / p.H, h = item % p.H;
-      mbar_wait(bar_load, it & 1);
-      for (int mt = 0; mt < n_mt; ++mt, ++cnt) {
-        const int i = mt * 128 + row;
-        const bool valid = i < T;
-        // D_i = dO_i . O_i : each of the quarter's four warps takes 16 of the 64 channels
-        float dpart = 0.f;
-        float lse2 = 3.0e38f;  // invalid rows: exp2(x - huge) = 0
-        if (valid) {
-          lse2 = p.lse[(static_cast<size_t>(b) * p.H + h) * T + i] * LOG2E;
-          const uint4* orow = reinterpret_cast<const uint4*>(p.o + (static_cast<size_t>(b) * T + i) * p.W + h * 64);
-          const uint8_t* drow = smem + B_DO + mt * ATOM;
 #pragma unroll
-          for (int c = 0; c < 2; ++c) {
-            float a[8], g[8];
-            unpack8h(__ldg(orow + 2 * cq + c), a);
-            unpack8h(*reinterpret_cast<const uint4*>(drow + op_off(row, 8 * (2 * cq + c))), g);
+    for (int kc = 0; kc < 4; ++kc) {
+      uint32_t a[4];
+      acc_to_a(a, s[2 * kc], s[2 * kc + 1]);
 #pragma unroll
-            for (int j = 0; j < 8; ++j) dpart += a[j] * g[j];
-          }
-        }
-        float* xb = xd + (cnt & 1) * 512;  // double-buffered: the next tile's partials never meet this tile's readers
-        xb[cq * 128 + row] = dpart;
-        named_bar_sync(1 + q, 128);
-        const float D = (xb[row] + xb[128 + row]) + (xb[256 + row] + xb[384 + row]);
-        mbar_wait(bar_s, cnt & 1);
-        tc_fence_after();
-        if (mt > 0) mbar_wait(bar_dsfree, (cnt - 1) & 1);  // the previous tile's dS is consumed: PS may be rewritten
-        for_blocks(lane_addr, cq, 4, nblk, [&](const uint32_t(&r)[16], int blk) {
-          const int c0 = blk * 16;
-          const bool full = c0 + 16 <= T;
-#pragma unroll
-          for (int g = 0; g < 2; ++g) {
-            float e[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              float x = ex2_approx(fmaf(__uint_as_float(r[8 * g + j]), sc, -lse2));
-              if (!full && c0 + 8 * g + j >= T) x = 0.f;
-              e[j] = x;
-            }
-            *reinterpret_cast<uint4*>(ps + op_off(row, c0 + 8 * g)) = pack8h(e);
-          }
-        });
-        tc_fence_before();
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar_p);
-        // ---- dS = scale * P * (dP - D), in place over P
-        mbar_wait(bar_dp, cnt & 1);
-        tc_fence_after();
-        mbar_wait(bar_pfree, cnt & 1);
-        for_blocks(lane_addr, cq, 4, nblk, [&](const uint32_t(&r)[16], int blk) {
-          const int c0 = blk * 16;
-#pragma unroll
-          for (int g = 0; g < 2; ++g) {
-            uint4* ptr = reinterpret_cast<uint4*>(ps + op_off(row, c0 + 8 * g));
-            float e[8];
-            unpack8h(*ptr, e);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) e[j] = p.scale * e[j] * (__uint_as_float(r[8 * g + j]) - D);
-            *ptr = pack8h(e);
-          }
-        });
-        tc_fence_before();
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar_ds);
-        // ---- dQ rows out (this warp: 16 of the 64 head channels)
-        mbar_wait(bar_dq, cnt & 1);
-        tc_fence_after();
-        {
-          uint32_t u[16];
-          tmem_ld_x16(lane_addr + cq * 16, u);
-          tmem_ld_wait();
-          if (valid) {
-            uint4* dst = reinterpret_cast<uint4*>(p.gqkv + (static_cast<size_t>(b) * T + i) * 3 * p.W + h * 64 + cq * 16);
-            dst[0] = pack8h_acc(u, 1.f);
-            dst[1] = pack8h_acc(u + 8, 1.f);
-          }
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar_afree);
+      for (int j = 0; j < 8; ++j) {
+        const __half* kr = Kt + (j * 8 + g) * ldk + kb * 64 + kc * 16 + 2 * t;
+        mma16816(dq[j], a, ld32(kr), ld32(kr + 8));
       }
-      // ---- dK (cq 0, 1) / dV (cq 2, 3) rows of key tile cq & 1
-      mbar_wait(bar_dsfree, (cnt - 1) & 1);
-      tc_fence_after();
-      {
-        const int jt = cq & 1, which = cq >> 1;
-        if (jt < n_mt) {
-          const int j = jt * 128 + row;
-          const uint32_t src = lane_addr + (which ? TM_DV : TM_DK) + jt * 64;
-          uint4* dst = reinterpret_cast<uint4*>(p.gqkv + (static_cast<size_t>(b) * T + (j < T ? j : 0)) * 3 * p.W + (which + 1) * p.W + h * 64);
-#pragma unroll
-          for (int hh = 0; hh < 2; ++hh) {
-            uint32_t a0[32];
-            tmem_ld_x32(src + hh * 32, a0);
-            tmem_ld_wait();
-            if (j < T) {
-#pragma unroll
-              for (int c = 0; c < 4; ++c) dst[hh * 4 + c] = pack8h_acc(a0 + 8 * c, 1.f);
-            }
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_done);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    __syncwarp();
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+  const int q0 = qb * 64 + r0 + g, q1 = q0 + 8;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const int col = h * 64 + j * 8 + 2 * t;
+    if (q0 < T) *reinterpret_cast<uint32_t*>(p.gqkv + (size_t)(b * T + q0) * ld3 + col) = pack(dq[j][0] * p.scale, dq[j][1] * p.scale);
+    if (q1 < T) *reinterpret_cast<uint32_t*>(p.gqkv + (size_t)(b * T + q1) * ld3 + col) = pack(dq[j][2] * p.scale, dq[j][3] * p.scale);
   }
 }
 
-// ------------------------------------------------------------------------------------------------ backward, version 2
-// Key-tile-outer order with ONE threads<->tensor-pipe hand-off per 128 x 128 score block (the first version above makes
-// six serial MMA <-> softmax round trips per query tile and leaves the tensor pipe idle 86 % of the time,
-// profiles/r01_ncu_attn_full_summary.txt).  For key tile jt (outer) and query tile mt (inner):
-//     phase 1 (tensor):  S  = Q_mt K_jt^T          dP = dO_mt V_jt^T                       -> TMEM
-//     threads         :  P  = exp2(S sc - lse)     dS = scale P (dP - D)                   -> shared memory (fp16 operands)
-//     phase 2 (tensor):  dV_jt += P^T dO_mt        dK_jt += dS^T Q_mt      dQ_mt += dS K_jt
-// S and dP sit side by side in TMEM, so the threads produce P and dS in one pass over both.  The MMA thread issues
-// phase 1 of block n+1 BEFORE phase 2 of block n (the S / dP columns are free as soon as the threads have loaded block
-// n into registers), so while the threads work on block n+1 the tensor pipe runs phase 2 of block n: one hand-off each
-// way per block, software-pipelined inside an (image, head) item.
-// smem: Q 32 KiB | dO 32 KiB | K | V (n_pad rows each) | P 32 KiB | dS 32 KiB | barriers | D exchange.
-// TMEM: S [0,128) | dP [128,256) | dQ tile 0 / 1 [256,320) [320,384) | dK_jt [384,448) | dV_jt [448,512).
-constexpr uint32_t T2_S = 0, T2_DP = 128, T2_DQ = 256, T2_DK = 384, T2_DV = 448;
-
-__global__ void __launch_bounds__(ATT_THREADS, 1) attn_bwd2_kernel(const __grid_constant__ AttnParams p) {
-  pdl_launch_dependents();
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t base_u32 = smem_u32(smem_raw);
-  uint8_t* smem = smem_raw + (((base_u32 + 1023u) & ~1023u) - base_u32);
-  const int n_mt = p.n_mt, n_pad = p.n_pad, T = p.T;
-  const uint32_t kvb = kv_slot_bytes(n_pad);
-  const uint32_t B_Q = 0, B_DO = 32 * KiB, B_K = 64 * KiB, B_V = B_K + kvb, B_P = B_V + kvb, B_DS = B_P + 32 * KiB,
-                 B_BAR = B_DS + 32 * KiB;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + B_BAR);
-  uint64_t* bar_load = bars;      // per item: Q, dO, K, V landed
-  uint64_t* bar_p1 = bars + 1;    // per block: S and dP complete
-  uint64_t* bar_free = bars + 2;  // per block: every warp has loaded its S / dP columns (16 warps)
-  uint64_t* bar_pds = bars + 3;   // per block: P and dS written (16 warps)
-  uint64_t* bar_p2 = bars + 4;    // per block: dV / dK / dQ products complete (P / dS consumed, accumulators current)
-  uint64_t* bar_smem = bars + 5;  // per item: every product has consumed Q / dO / K / V
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 8);
-  float* xd = reinterpret_cast<float*>(smem + B_BAR + 256);  // [2 query tiles][4 channel quarters][128 rows] partial D
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) {
-    prefetch_tmap(&p.tm_q);
-    prefetch_tmap(&p.tm_kv);
-    prefetch_tmap(&p.tm_do);
-    mbar_init(bar_load, 1);
-    mbar_init(bar_p1, 1);
-    mbar_init(bar_free, ATT_EPI_WARPS);
-    mbar_init(bar_pds, ATT_EPI_WARPS);
-    mbar_init(bar_p2, 1);
-    mbar_init(bar_smem, 1);
-    fence_barrier_init();
-  }
-  if (warp == 1) tmem_alloc(tmem_ptr, 512);
-  tc_fence_before();
+// ------------------------------------------------------------------------------------------------------------ dK, dV
+// CTA = (64-key block, head, image), loop over 64-query blocks.  Transposed scores: S^T = K Q^T, dP^T = V dO^T;
+// dV_j = sum_i P_ij dO_i, dK_j = scale * sum_i P_ij (dP_ij - D_i) Q_i.
+__global__ void __launch_bounds__(AT_THREADS) attn_bwd_dkv_kernel(const __grid_constant__ AttnParams p) {
+  pdl_prologue();
+  extern __shared__ uint4 smem_at[];
+  const int kb0 = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+  const int T = p.T, ld3 = 3 * p.W;
+  __half* Ks = reinterpret_cast<__half*>(smem_at);
+  __half* Vs = Ks + 64 * LDS;
+  __half* Qs = Vs + 64 * LDS;
+  __half* dOs = Qs + 64 * LDS;
+  __half* Qt = dOs + 64 * LDS;  // [64][LDS]: Q^T of the query block
+  __half* dOt = Qt + 64 * LDS;
+  float* Ds = reinterpret_cast<float*>(dOt + 64 * LDS);
+  float* Ls = Ds + 64;
+  const __half* base = p.qkv + (size_t)b * T * ld3;
+  load_rows(Ks, base, ld3, p.W + h * 64, kb0 * 64, 64, T);
+  load_rows(Vs, base, ld3, 2 * p.W + h * 64, kb0 * 64, 64, T);
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-  const uint32_t s_base = smem_u32(smem);
-  pdl_wait();  // above: parameters, shared memory, TMEM only
-  const int n_blocks = n_mt * n_mt;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      const uint32_t bytes = 2u * static_cast<uint32_t>(n_mt) * ATOM + 2u * static_cast<uint32_t>(n_pad) * 128u;
-      int it = 0;
-      for (int item = blockIdx.x; item < p.items; item += gridDim.x, ++it) {
-        const int b = item / p.H, h = item % p.H;
-        if (it > 0) mbar_wait(bar_smem, (it - 1) & 1);
-        mbar_arrive_expect_tx(bar_load, bytes);
-        for (int mt = 0; mt < n_mt; ++mt) {
-          tma_load_4d(&p.tm_q, bar_load, smem + B_Q + mt * ATOM, h * 64, mt * 128, b, 0);
-          tma_load_4d(&p.tm_do, bar_load, smem + B_DO + mt * ATOM, h * 64, mt * 128, b, 0);
-        }
-        tma_load_4d(&p.tm_kv, bar_load, smem + B_K, p.W + h * 64, 0, b, 0);
-        tma_load_4d(&p.tm_kv, bar_load, smem + B_V, 2 * p.W + h * 64, 0, b, 0);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3, r0 = warp * 16;
+  uint32_t ka[4][4], va[4][4];
+#pragma unroll
+  for (int kc = 0; kc < 4; ++kc) {
+    load_a(ka[kc], Ks, LDS, r0, kc * 16, g, t);
+    load_a(va[kc], Vs, LDS, r0, kc * 16, g, t);
+  }
+  const float c = p.scale * LOG2E;
+  float dk[8][4] = {}, dv[8][4] = {};
+  for (int qb = 0; qb * 64 < T; ++qb) {
+    __syncthreads();  // the previous query block's tiles are consumed
+    load_rows(Qs, base, ld3, h * 64, qb * 64, 64, T);
+    load_rows_t(Qt, LDS, base, ld3, h * 64, qb * 64, 64, T);
+    load_do_block(p, b, h, qb * 64, dOs, dOt, Ds, Ls);
+    __syncthreads();
+    float s[8][4] = {}, dp[8][4] = {};
+#pragma unroll
+    for (int kc = 0; kc < 4; ++kc)
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const int row = (j * 8 + g) * LDS + kc * 16 + 2 * t;
+        mma16816(s[j], ka[kc], ld32(Qs + row), ld32(Qs + row + 8));
+        mma16816(dp[j], va[kc], ld32(dOs + row), ld32(dOs + row + 8));
       }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t id_dq = make_idesc_f16(128, 64, 0, 0, 1);  // dQ = dS K: A K-major, B MN-major
-      const uint32_t id_t = make_idesc_f16(128, 64, 0, 1, 1);   // dV = P^T dO, dK = dS^T Q: both MN-major
-      constexpr uint64_t AT = ATOM >> 4;
-      const uint64_t dk_q = desc_k(s_base + B_Q), dk_k = desc_k(s_base + B_K), dk_v = desc_k(s_base + B_V),
-                     dk_do = desc_k(s_base + B_DO), dk_ds = desc_k(s_base + B_DS);
-      const uint64_t dm_p = desc_mn(s_base + B_P, ATOM), dm_ds = desc_mn(s_base + B_DS, ATOM),
-                     dm_do = desc_mn(s_base + B_DO, 8192), dm_q = desc_mn(s_base + B_Q, 8192),
-                     dm_k = desc_mn(s_base + B_K, 8192);
-      int it = 0, cnt = 0;  // cnt: blocks issued so far (all items) = parity source of the per-block barriers
-      auto phase2 = [&](int jt, int mt, int nk) {
-        const int rows_left = T - mt * 128;
-        const int ksi = rows_left >= 128 ? 8 : (rows_left + 15) / 16;  // 16-row reduction steps over this tile's queries
-#pragma unroll 4
-        for (int ks = 0; ks < ksi; ++ks)
-          umma_f16(tmem_base + T2_DV, dm_p + ks * 128, dm_do + mt * AT + ks * 128, id_t, (mt | ks) ? 1u : 0u);
-#pragma unroll 4
-        for (int ks = 0; ks < ksi; ++ks)
-          umma_f16(tmem_base + T2_DK, dm_ds + ks * 128, dm_q + mt * AT + ks * 128, id_t, (mt | ks) ? 1u : 0u);
-        const int n_k = nk / 16;
-#pragma unroll 4
-        for (int k = 0; k < n_k; ++k)
-          umma_f16(tmem_base + T2_DQ + mt * 64, dk_ds + (k >> 2) * AT + (k & 3) * 2, dm_k + (jt * 8 + k) * 128, id_dq,
-                   (jt | k) ? 1u : 0u);
-      };
-      for (int item = blockIdx.x; item < p.items; item += gridDim.x, ++it) {
-        mbar_wait(bar_load, it & 1);
-        tc_fence_after();
-        int pj = 0, pm = 0, pnk = 0;  // the block whose phase 2 is pending
-        for (int n = 0; n < n_blocks; ++n, ++cnt) {
-          const int jt = n / n_mt, mt = n % n_mt;
-          const int nk = min(128, n_pad - jt * 128);
-          if (cnt > 0) {  // S / dP columns: every warp has loaded the previous block into registers
-            mbar_wait(bar_free, (cnt - 1) & 1);
-            tc_fence_after();
-          }
-          const uint32_t id_s = make_idesc_f16(128, nk, 0, 0, 0);  // S, dP: both operands K-major
 #pragma unroll
-          for (int k = 0; k < 4; ++k)
-            umma_f16(tmem_base + T2_S, dk_q + mt * AT + 2 * k, dk_k + jt * AT + 2 * k, id_s, k ? 1u : 0u);
+    for (int j = 0; j < 8; ++j)
 #pragma unroll
-          for (int k = 0; k < 4; ++k)
-            umma_f16(tmem_base + T2_DP, dk_do + mt * AT + 2 * k, dk_v + jt * AT + 2 * k, id_s, k ? 1u : 0u);
-          umma_commit(bar_p1);
-          if (n > 0) {
-            mbar_wait(bar_pds, (cnt - 1) & 1);
-            tc_fence_after();
-            phase2(pj, pm, pnk);
-            umma_commit(bar_p2);
-          }
-          pj = jt;
-          pm = mt;
-          pnk = nk;
-        }
-        // drain at the item boundary: the next item's operands can only be fetched once these products have run
-        mbar_wait(bar_pds, (cnt - 1) & 1);
-        tc_fence_after();
-        phase2(pj, pm, pnk);
-        umma_commit(bar_p2);
-        umma_commit(bar_smem);
+      for (int e = 0; e < 4; ++e) {
+        const int ql = j * 8 + 2 * t + (e & 1);
+        const float pv = qb * 64 + ql < T ? exp2f(s[j][e] * c - Ls[ql]) : 0.f;
+        s[j][e] = pv;
+        dp[j][e] = pv * (dp[j][e] - Ds[ql]);
       }
-    }
-  } else {
-    const int q = warp & 3, cq = (warp - 2) >> 2;  // lane quarter; which of its four warps (32-column slice cq of a block)
-    const int row = q * 32 + lane;
-    const float sc = p.scale * LOG2E;
-    const uint32_t lane_addr = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
-    uint8_t* pbuf = smem + B_P;
-    uint8_t* dsbuf = smem + B_DS;
-    int it = 0, cnt = 0;
-    int pb = 0, ph = 0;  // (image, head) of the previous item: its dQ leaves after its last block's phase 2
-    // dK / dV rows of key tile jt (this warp: dK for cq 0, 1 / dV for cq 2, 3; 32 of the 64 channels) and, after an
-    // item's last block, its dQ rows (16 of the 64 channels of both query tiles).  Call after bar_p2 of that block.
-    auto read_out = [&](int b, int h, int jt, bool item_done) {
-      tc_fence_after();
-      {
-        const int which = cq >> 1, half = cq & 1;
-        const int j = jt * 128 + row;
-        uint32_t a0[16], a1[16];
-        tmem_ld_x16(lane_addr + (which ? T2_DV : T2_DK) + half * 32, a0);
-        tmem_ld_x16(lane_addr + (which ? T2_DV : T2_DK) + half * 32 + 16, a1);
-        tmem_ld_wait();
-        if (j < T) {
-          uint4* dst = reinterpret_cast<uint4*>(p.gqkv + (static_cast<size_t>(b) * T + j) * 3 * p.W + (which + 1) * p.W + h * 64 + half * 32);
-          dst[0] = pack8h_acc(a0, 1.f);
-          dst[1] = pack8h_acc(a0 + 8, 1.f);
-          dst[2] = pack8h_acc(a1, 1.f);
-          dst[3] = pack8h_acc(a1 + 8, 1.f);
-        }
+#pragma unroll
+    for (int kc = 0; kc < 4; ++kc) {  // 16 queries
+      uint32_t pa[4], sa[4];
+      acc_to_a(pa, s[2 * kc], s[2 * kc + 1]);
+      acc_to_a(sa, dp[2 * kc], dp[2 * kc + 1]);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const int row = (j * 8 + g) * LDS + kc * 16 + 2 * t;
+        mma16816(dv[j], pa, ld32(dOt + row), ld32(dOt + row + 8));
+        mma16816(dk[j], sa, ld32(Qt + row), ld32(Qt + row + 8));
       }
-      if (item_done) {
-        for (int mt = 0; mt < n_mt; ++mt) {
-          const int i = mt * 128 + row;
-          uint32_t u[16];
-          tmem_ld_x16(lane_addr + T2_DQ + mt * 64 + cq * 16, u);
-          tmem_ld_wait();
-          if (i < T) {
-            uint4* dst = reinterpret_cast<uint4*>(p.gqkv + (static_cast<size_t>(b) * T + i) * 3 * p.W + h * 64 + cq * 16);
-            dst[0] = pack8h_acc(u, 1.f);
-            dst[1] = pack8h_acc(u + 8, 1.f);
-          }
-        }
-      }
-      tc_fence_before();
-    };
-    for (int item = blockIdx.x; item < p.items; item += gridDim.x, ++it) {
-      const int b = item / p.H, h = item % p.H;
-      mbar_wait(bar_load, it & 1);
-      // D_i = dO_i . O_i and the row log-sum-exp for both query tiles (each of the quarter's four warps: 16 channels)
-      float Dv0 = 0.f, Dv1 = 0.f, lse2_0 = 3.0e38f, lse2_1 = 3.0e38f;  // invalid rows: exp2(x - huge) = 0
-      for (int mt = 0; mt < n_mt; ++mt) {
-        const int i = mt * 128 + row;
-        float dpart = 0.f;
-        if (i < T) {
-          const float l2 = p.lse[(static_cast<size_t>(b) * p.H + h) * T + i] * LOG2E;
-          if (mt == 0) lse2_0 = l2;
-          else lse2_1 = l2;
-          const uint4* orow = reinterpret_cast<const uint4*>(p.o + (static_cast<size_t>(b) * T + i) * p.W + h * 64);
-          const uint8_t* drow = smem + B_DO + mt * ATOM;
-#pragma unroll
-          for (int c = 0; c < 2; ++c) {
-            float a[8], g[8];
-            unpack8h(__ldg(orow + 2 * cq + c), a);
-            unpack8h(*reinterpret_cast<const uint4*>(drow + op_off(row, 8 * (2 * cq + c))), g);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) dpart += a[j] * g[j];
-          }
-        }
-        xd[(mt * 4 + cq) * 128 + row] = dpart;
-      }
-      named_bar_sync(1 + q, 128);
-      Dv0 = (xd[0 * 128 + row] + xd[1 * 128 + row]) + (xd[2 * 128 + row] + xd[3 * 128 + row]);
-      if (n_mt > 1) Dv1 = (xd[4 * 128 + row] + xd[5 * 128 + row]) + (xd[6 * 128 + row] + xd[7 * 128 + row]);
-      // the next item's partials overwrite xd: its writers are ordered behind these reads by the per-block mbarrier
-      // chain anyway, but a second barrier makes the exchange self-contained (and visible to compute-sanitizer)
-      named_bar_sync(1 + q, 128);
-      for (int n = 0; n < n_blocks; ++n, ++cnt) {
-        const int jt = n / n_mt, mt = n % n_mt;
-        const int nk = min(128, n_pad - jt * 128);
-        const int c_lo = cq * 32;
-        const int ncol = max(0, min(32, nk - c_lo));  // this warp's columns of the block: 32, 16 or 0
-        mbar_wait(bar_p1, cnt & 1);
-        tc_fence_after();
-        // Sixteen columns at a time (S and dP of the same columns side by side: 32 live accumulator registers + the packed
-        // results; the 96-register budget of a 576-thread block has no room for all 64 at once).  ~7 instructions per score:
-        // FFMA + EX2 for p, FADD + 2 FMUL for dS, half a cvt.pack each -- the threads, not the tensor pipe, pace this kernel
-        // (ncu: 830 instructions per thread and block before this rewrite, profiles/r02_ncu_attn_summary.txt), so the
-        // key-padding mask is only evaluated in the one slice that straddles T.
-        uint4 pv[4], dv[4];
-        const float lz = mt ? lse2_1 : lse2_0, Dm = mt ? Dv1 : Dv0;
-        const int key0 = jt * 128 + c_lo;
-        const bool all_keys_valid = key0 + 32 <= T;
-        const float ps = p.scale;
-#pragma unroll
-        for (int hf = 0; hf < 2; ++hf) {
-          uint32_t sr[16], dr[16];
-          const bool live = ncol > 16 * hf;
-          if (live) {
-            tmem_ld_x16(lane_addr + T2_S + c_lo + 16 * hf, sr);
-            tmem_ld_x16(lane_addr + T2_DP + c_lo + 16 * hf, dr);
-          }
-          tmem_ld_wait();
-          if (hf == 1) {  // both halves are in registers: phase 1 of the next block may overwrite S / dP
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(bar_free);
-          }
-          if (!live) continue;
-#pragma unroll
-          for (int g = 0; g < 2; ++g) {
-            float e[8], f[8];
-            if (all_keys_valid) {
-#pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                const float x = ex2_approx(fmaf(__uint_as_float(sr[8 * g + j]), sc, -lz));
-                e[j] = x;
-                f[j] = ps * x * (__uint_as_float(dr[8 * g + j]) - Dm);
-              }
-            } else {
-#pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                float x = ex2_approx(fmaf(__uint_as_float(sr[8 * g + j]), sc, -lz));
-                if (key0 + 16 * hf + 8 * g + j >= T) x = 0.f;  // keys past the sequence: P = 0, and so dS = 0
-                e[j] = x;
-                f[j] = ps * x * (__uint_as_float(dr[8 * g + j]) - Dm);
-              }
-            }
-            pv[2 * hf + g] = pack8h(e);
-            dv[2 * hf + g] = pack8h(f);
-          }
-        }
-        // the previous block's products have consumed P / dS (and its accumulators are current)
-        if (cnt > 0) {
-          mbar_wait(bar_p2, (cnt - 1) & 1);
-          if (n == 0) read_out(pb, ph, n_mt - 1, true);            // previous item: last key tile + its dQ
-          else if (mt == 0) read_out(b, h, jt - 1, false);         // previous key tile of this item is complete
-        }
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          if (8 * g < ncol) {
-            *reinterpret_cast<uint4*>(pbuf + op_off(row, c_lo + 8 * g)) = pv[g];
-            *reinterpret_cast<uint4*>(dsbuf + op_off(row, c_lo + 8 * g)) = dv[g];
-          }
-        }
-        tc_fence_before();
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar_pds);
-      }
-      pb = b;
-      ph = h;
-    }
-    if (cnt > 0) {  // the last item's last key tile and its dQ
-      mbar_wait(bar_p2, (cnt - 1) & 1);
-      read_out(pb, ph, n_mt - 1, true);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    __syncwarp();
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+  const int k0 = kb0 * 64 + r0 + g, k1 = k0 + 8;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const int col = h * 64 + j * 8 + 2 * t;
+    if (k0 < T) {
+      __half* row = p.gqkv + (size_t)(b * T + k0) * ld3 + col;
+      *reinterpret_cast<uint32_t*>(row + p.W) = pack(dk[j][0] * p.scale, dk[j][1] * p.scale);
+      *reinterpret_cast<uint32_t*>(row + 2 * p.W) = pack(dv[j][0], dv[j][1]);
+    }
+    if (k1 < T) {
+      __half* row = p.gqkv + (size_t)(b * T + k1) * ld3 + col;
+      *reinterpret_cast<uint32_t*>(row + p.W) = pack(dk[j][2] * p.scale, dk[j][3] * p.scale);
+      *reinterpret_cast<uint32_t*>(row + 2 * p.W) = pack(dv[j][2], dv[j][3]);
+    }
   }
 }
 
-int fwd_smem_bytes(int n_pad) { return 32 * 1024 + 2 * (int)((n_pad * 128 + 1023) / 1024 * 1024) + 128 * 1024 + 256 + 4096 + 1024; }
-int bwd_smem_bytes(int n_pad) { return 64 * 1024 + 2 * (int)((n_pad * 128 + 1023) / 1024 * 1024) + 64 * 1024 + 256 + 4096 + 1024; }
-int bwd2_smem_bytes(int n_pad) { return 64 * 1024 + 2 * (int)((n_pad * 128 + 1023) / 1024 * 1024) + 64 * 1024 + 256 + 4096 + 1024; }
+int fwd_smem(int TP) { return (64 * LDS + TP * LDS + 64 * (TP + 8)) * 2; }
+int dq_smem(int TP) { return (2 * 64 * LDS + 2 * TP * LDS + 64 * (TP + 8)) * 2 + 2 * 64 * 4; }
+int dkv_smem() { return 6 * 64 * LDS * 2 + 2 * 64 * 4; }
 
 }  // namespace
 
-// T <= 240: the forward keeps Q, K, V and both P tiles resident (<= 227 KiB of shared memory)
 bool attn_supported(int T, int head_dim, int W) { return head_dim == 64 && T >= 1 && T <= 240 && W % 64 == 0; }
 
 int attn_plan_make(AttnPlan* plan, const __half* qkv, __half* o, const __half* d_o, __half* gqkv, float* lse, int B,
                    int T, int H, int W, float scale, int num_sms, char* err, int errlen) {
+  (void)num_sms;
   *plan = AttnPlan{};
-  if (!attn_supported(T, W / H, W)) {
+  if (!attn_supported(T, W / H, W) || W != 64 * H) {
     if (err && errlen > 0) snprintf(err, errlen, "fused attention needs 64-wide heads and T <= 240");
     return -1;
   }
   AttnParams& p = plan->p;
+  p.qkv = qkv;
+  p.o = o;
+  p.lse = lse;
+  p.d_o = d_o;
+  p.gqkv = gqkv;
   p.T = T;
-  p.n_pad = (T + 15) / 16 * 16;
   p.H = H;
   p.B = B;
   p.W = W;
-  p.n_mt = (T + 127) / 128;
-  p.items = B * H;
   p.scale = scale;
-  p.o = o;
-  p.lse = lse;
-  p.gqkv = gqkv;
-  const uint64_t qd[4] = {(uint64_t)3 * W, (uint64_t)T, (uint64_t)B, 1};
-  const uint64_t qs[3] = {(uint64_t)3 * W, (uint64_t)T * 3 * W, (uint64_t)T * 3 * W * B};
-  const uint32_t box_q[4] = {64, 128, 1, 1};
-  const uint32_t box_kv[4] = {64, (uint32_t)p.n_pad, 1, 1};
-  int rc = tmap_encode_4d(&p.tm_q, qkv, 0, qd, qs, box_q, err, errlen);
-  if (!rc) rc = tmap_encode_4d(&p.tm_kv, qkv, 0, qd, qs, box_kv, err, errlen);
-  if (!rc && d_o) {
-    const uint64_t dd[4] = {(uint64_t)W, (uint64_t)T, (uint64_t)B, 1};
-    const uint64_t ds[3] = {(uint64_t)W, (uint64_t)T * W, (uint64_t)T * W * B};
-    rc = tmap_encode_4d(&p.tm_do, d_o, 0, dd, ds, box_q, err, errlen);
-  }
-  if (rc) return rc;
-  plan->grid = p.items < num_sms ? p.items : num_sms;
-  plan->smem_fwd = fwd_smem_bytes(p.n_pad);
-  plan->smem_bwd = bwd_smem_bytes(p.n_pad);
-  plan->smem_bwd2 = bwd2_smem_bytes(p.n_pad);
-  const double tt = (double)T * T * 64 * 2 * p.items;
+  const int TP = (T + 63) / 64 * 64;
+  plan->smem_fwd = fwd_smem(TP);
+  plan->smem_dq = dq_smem(TP);
+  plan->smem_dkv = dkv_smem();
+  const double tt = (double)T * T * 64 * 2 * B * H;
   plan->flops_fwd = 2 * tt;  // QK^T, PV
   plan->flops_bwd = 4 * tt;  // dP, dQ, dK, dV (the recomputed S is not algorithmic work)
   const double mw = (double)B * T * W * 2.0;  // one [B*T, W] fp16 tensor
@@ -883,25 +377,22 @@ int attn_plan_make(AttnPlan* plan, const __half* qkv, __half* o, const __half* d
   plan->bytes_bwd = 3 * mw + mw + mw + 3 * mw + 4.0 * B * H * T;
   static std::once_flag once;
   std::call_once(once, [] {
-    cudaFuncSetAttribute(attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, fwd_smem_bytes(240));
-    cudaFuncSetAttribute(attn_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bwd_smem_bytes(240));
-    cudaFuncSetAttribute(attn_bwd2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bwd2_smem_bytes(240));
+    cudaFuncSetAttribute(attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, fwd_smem(256));
+    cudaFuncSetAttribute(attn_bwd_dq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dq_smem(256));
+    cudaFuncSetAttribute(attn_bwd_dkv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dkv_smem());
   });
   return 0;
 }
 
 void attn_forward_launch(const AttnPlan& plan, cudaStream_t st) {
-  launch_pdl(attn_fwd_kernel, dim3(plan.grid), dim3(ATT_THREADS), plan.smem_fwd, st, plan.p);
+  const AttnParams& p = plan.p;
+  launch_pdl(attn_fwd_kernel, dim3((p.T + 63) / 64, p.H, p.B), dim3(AT_THREADS), plan.smem_fwd, st, p);
 }
-// Measured in the config-2 iteration (profiles/README.md, round 2): the first backward kernel 106 us per layer, the
-// key-tile-outer one 151 us -- so the first one stays the default; PXR_ATTN_BWD=2 selects the second for A/B runs.
+
 void attn_backward_launch(const AttnPlan& plan, cudaStream_t st) {
-  static const bool v1 = [] {
-    const char* e = getenv("PXR_ATTN_BWD");
-    return !(e && atoi(e) == 2);
-  }();
-  if (v1) launch_pdl(attn_bwd_kernel, dim3(plan.grid), dim3(ATT_THREADS), plan.smem_bwd, st, plan.p);
-  else launch_pdl(attn_bwd2_kernel, dim3(plan.grid), dim3(ATT_THREADS), plan.smem_bwd2, st, plan.p);
+  const AttnParams& p = plan.p;
+  launch_pdl(attn_bwd_dq_kernel, dim3((p.T + 63) / 64, p.H, p.B), dim3(AT_THREADS), plan.smem_dq, st, p);
+  launch_pdl(attn_bwd_dkv_kernel, dim3((p.T + 63) / 64, p.H, p.B), dim3(AT_THREADS), plan.smem_dkv, st, p);
 }
 
 }  // namespace pxr

@@ -1,12 +1,14 @@
 // Fused multi-head self-attention of the CLIP ViT (nn.MultiheadAttention inside SLIP/models.py:18-64 residual blocks;
-// openai-CLIP VisionTransformer) for sm_100a: one kernel for the forward, one for the backward, both on tcgen05 with
-// the accumulators in TMEM.  Replaces, per layer, {QK^T GEMM, softmax, PV GEMM} and {dP GEMM, softmax backward,
-// dQ / dK / dV GEMMs} of the unfused path (which stays as the fallback for sequences longer than 256 tokens).
+// openai-CLIP VisionTransformer) and of the v-diffusion U-Net for sm_90a: one kernel for the forward, two for the
+// backward, all on the tensor cores (warp-level mma.sync m16n8k16, fp16 operands, fp32 accumulators in registers).
+// Replaces, per layer, {QK^T GEMM, softmax, PV GEMM} and {dP GEMM, softmax backward, dQ / dK / dV GEMMs} of the unfused
+// path (which stays for sequences longer than 240 tokens).
 //
-// One CTA owns one (image, head) pair at a time: T <= 256 tokens, head width 64, so the whole score matrix of the pair
-// (two 128-row accumulator tiles of N = round_up(T, 16) columns) lives in TMEM and is never written to memory.
-// Forward keeps only the row log-sum-exp; backward recomputes P = exp(S - lse) from Q, K (flash-attention style) and
-// uses D_i = dO_i . O_i for the softmax backward.
+// Flash-attention style: a CTA owns 64 query rows (forward, dQ) or 64 key rows (dK / dV) of one (image, head) pair and
+// stages that pair's K, V (or Q, dO) in shared memory; the scores of a warp's 16 rows live in registers and are never
+// written to memory.  Forward keeps only the row log-sum-exp; backward recomputes P = exp(S - lse) from Q, K and uses
+// D_i = dO_i . O_i for the softmax backward.  Every output element is written by exactly one thread (no atomics), so
+// results are deterministic.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -16,25 +18,23 @@
 namespace pxr {
 
 struct AttnParams {
-  CUtensorMap tm_q;   // qkv [B][T][3W] fp16, box 64 x 128 rows
-  CUtensorMap tm_kv;  // same tensor, box 64 x n_pad rows
-  CUtensorMap tm_do;  // dO [B][T][W] fp16, box 64 x 128 rows (backward only)
-  int T, n_pad, H, B, W, n_mt, items;
-  float scale;            // 1 / sqrt(64): S = scale * q k^T
-  __half* o;              // forward out / backward in: [B*T, W] (head h at columns h*64)
+  const __half* qkv;      // [B*T, 3W]: q | k | v, head h at columns h*64 of each third
+  __half* o;              // forward out / backward in: [B*T, W]
   float* lse;             // [B*H, T] natural-log sum-exp of the scaled scores
+  const __half* d_o;      // backward in [B*T, W]
   __half* gqkv;           // backward out [B*T, 3W]: dq | dk | dv
+  int T, H, B, W;
+  float scale;            // S = scale * q k^T
 };
 
 struct AttnPlan {
   AttnParams p;
-  int grid = 0;
-  int smem_fwd = 0, smem_bwd = 0, smem_bwd2 = 0;
+  int smem_fwd = 0, smem_dq = 0, smem_dkv = 0;
   double flops_fwd = 0, flops_bwd = 0;
   double bytes_fwd = 0, bytes_bwd = 0;  // compulsory traffic: qkv in, o out (+ lse) / qkv, o, dO in, dqkv out
 };
 
-// true when the fused kernels cover this shape (head width 64, T <= 256, 16-byte aligned rows)
+// true when the fused kernels cover this shape (head width 64, T <= 240, 16-byte aligned rows)
 bool attn_supported(int T, int head_dim, int W);
 // qkv: [B*T, 3W]; o: [B*T, W]; d_o: [B*T, W]; gqkv: [B*T, 3W]; lse: [B*H*T]
 int attn_plan_make(AttnPlan* plan, const __half* qkv, __half* o, const __half* d_o, __half* gqkv, float* lse, int B,

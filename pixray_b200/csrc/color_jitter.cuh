@@ -22,7 +22,7 @@
 // (1, 1, x) have a hue of exactly 60 degrees, i.e. exactly on the sector boundary of hsv_to_rgb, and whether
 // floor(6 h) comes out as 0 or 1 there is decided by the last bit of h / 2pi.  Round 1 used __fdividef and let the
 // compiler contract: forward values agreed to 2e-6, but ~2e-4 of the pixels of a clamped image took the other
-// one-sided Jacobian, which showed up as a 2.5e-2 error of d loss / d image (profiles/r02_jitter_gap_diagnosis.log).
+// one-sided Jacobian, which showed up as a 2.5e-2 error of d loss / d image.
 // Derivative parts carry no such constraint.
 #pragma once
 #include <cmath>

@@ -31,13 +31,13 @@ class Engine {
   cudaStream_t st = nullptr;
   std::string err;
   int64_t launches = 0;
-  int num_sms = 148;
+  int num_sms = 132;
   int fmt = 0;
   float S = 4096.f;  // grad scale
   bool fuse_softmax = false;  // PXR_FUSE_SOFTMAX=1: attention softmax inside the GEMM epilogue (see DESIGN.md 4)
   bool gn_coop = true;        // PXR_GN_COOP=0: three-kernel GroupNorm instead of the cooperative single-kernel one
   bool stream16 = true;       // the ViT residual stream and its gradient in fp16, like the reference's CUDA path (clip.load gives a half model, slip.py:176); PXR_CLIP_STREAM=32 keeps them in fp32
-  bool fused_attn = true;     // PXR_FUSED_ATTN=0: fall back to the batched-GEMM attention (attn_tc.cu covers T <= 256)
+  bool fused_attn = true;     // PXR_FUSED_ATTN=0: fall back to the batched-GEMM attention (attn_tc.cu covers T <= 240)
   std::map<std::string, HostWeight> weights[3];
   std::vector<void*> allocs;
   bool finalized = false;
@@ -385,18 +385,16 @@ class Engine {
       auto it = forced.find(N);
       if (it != forced.end() && it->second % step == 0 && m_tiles > 16) return it->second;
     }
-    if (N <= 256 && m_tiles * 1 >= num_sms / 2) return round_up(N, step);
+    // N <= 128: one tile column.  Above 32 columns round up to 64 / 128, the widths with a compile-time wgmma chain
+    // (gemm_tc.cu, mma_tile); the extra columns read zero-filled rows of B and are not stored.
+    auto narrow = [step](int n) { const int b = round_up(n, step); return b <= 32 ? b : round_up(n, 64); };
+    if (N <= 128 && m_tiles * 1 >= num_sms / 2) return narrow(N);
     int best = 0;
     double best_cost = 1e30;
-    // CTA pairs (cta_group::2) schedule 256-row tile pairs over num_sms / 2 clusters
-    const bool paired = m_tiles >= 2 && gemm_default_cta_group() == 2;
-    const long long m_units = paired ? (m_tiles + 1) / 2 : m_tiles;
-    const long long sm_units = paired ? num_sms / 2 : num_sms;
-    for (int bn = 256; bn >= 64; bn -= 64) {
+    for (int bn = 128; bn >= 64; bn -= 64) {  // gemm_tc.cu: plain-epilogue tiles are at most 128 wide
       if (bn % step) continue;
-      if (paired && b_mn && bn % 128) continue;
-      const long long tiles = m_units * ((N + bn - 1) / bn);
-      const long long waves = (tiles + sm_units - 1) / sm_units;
+      const long long tiles = m_tiles * ((N + bn - 1) / bn);
+      const long long waves = (tiles + num_sms - 1) / num_sms;
       // narrower tiles re-read A more often and sit closer to the smem-bandwidth limit: mild penalty
       const double cost = (double)waves * (bn + 40.0) * (bn >= 192 ? 1.0 : (bn == 128 ? 1.06 : 1.2));
       if (cost < best_cost - 1e-9) {
@@ -404,7 +402,7 @@ class Engine {
         best = bn;
       }
     }
-    if (N < best) best = round_up(N, step);
+    if (N < best) best = narrow(N);
     return best;
   }
   void add_gemm(OpList& l, const GemmOperand& A, const GemmOperand& B, int M, int N, int K, const GemmEpilogue& e,
@@ -419,8 +417,8 @@ class Engine {
   }
   static std::string gemm_label(const char* kind, const GemmPlan& p, int am, int bm, const GemmEpilogue& e) {
     char b[256];
-    snprintf(b, sizeof b, "%s M=%d N=%d K=%d batch=%d bn=%d cg=%d A%s B%s act=%d%s%s%s%s%s%s", kind, p.p.M, p.p.N,
-             p.p.num_k_blocks * GEMM_BLOCK_K, p.p.total_tiles / (p.p.tiles_m * p.p.tiles_n), p.p.block_n, p.p.cta_group, am == OP_MNMAJOR ? "mn" : "k", bm == OP_MNMAJOR ? "mn" : "k",
+    snprintf(b, sizeof b, "%s M=%d N=%d K=%d batch=%d bn=%d A%s B%s act=%d%s%s%s%s%s%s", kind, p.p.M, p.p.N,
+             p.p.num_k_blocks * GEMM_BLOCK_K, p.p.total_tiles / (p.p.tiles_m * p.p.tiles_n), p.p.block_n, am == OP_MNMAJOR ? "mn" : "k", bm == OP_MNMAJOR ? "mn" : "k",
              e.act, e.bias ? " bias" : "", e.res_f32 ? " res32" : "", e.res_f16 ? " res16" : "", e.out_f32 ? " o32" : "",
              e.out_f16 ? " o16" : "", e.aux_out ? " aux" : "");
     return b;
@@ -663,7 +661,7 @@ void Engine::create() {
   PXR_CUDA(cudaSetDevice(cfg.device));
   cudaDeviceProp prop;
   PXR_CUDA(cudaGetDeviceProperties(&prop, cfg.device));
-  if (prop.major != 10) throw EngineError(-3, std::string("pixray_b200 needs an sm_100 GPU (B200); found ") + prop.name);
+  if (prop.major != 9) throw EngineError(-3, std::string("pixray_b200 needs an sm_90 GPU (H100); found ") + prop.name);
   num_sms = prop.multiProcessorCount;
   PXR_CUDA(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
   if (cfg.world < 1) cfg.world = 1;
@@ -1558,7 +1556,7 @@ void Engine::build_clip(int i) {
   C.gh = dalloc<act_t>((size_t)M * Wd);
   C.go = dalloc<act_t>((size_t)M * Wd);
   C.gqkv = dalloc<act_t>((size_t)M * 3 * Wd);
-  const bool fuse_attn = fused_attn && attn_supported(T, d, Wd);  // attn_tc.cu: one kernel per direction, T <= 256
+  const bool fuse_attn = fused_attn && attn_supported(T, d, Wd);  // attn_tc.cu: T <= 240
   C.dP = fuse_attn ? nullptr : dalloc<act_t>((size_t)B * Hh * T * ldT);
   const bool s16 = stream16;
   const size_t xbytes = (size_t)M * Wd * (s16 ? sizeof(act_t) : sizeof(float));
@@ -1786,7 +1784,7 @@ void Engine::build_clip(int i) {
       std::shared_ptr<AttnPlan> ap = ly.attn;
       char lab[96];
       snprintf(lab, sizeof lab, "attn_bwd B=%d T=%d heads=%d", B, T, Hh);
-      C.bwd.add(1, [ap, cs] { attn_backward_launch(*ap, cs); }, ap->flops_bwd, lab, ap->bytes_bwd);
+      C.bwd.add(2, [ap, cs] { attn_backward_launch(*ap, cs); }, ap->flops_bwd, lab, ap->bytes_bwd);
     } else {
     {  // dP = go v^T ; fused: dS = scale * P * (dP - <P, dP>)
       GemmEpilogue e;
@@ -2450,7 +2448,7 @@ static thread_local std::string g_create_err;
 
 extern "C" {
 
-const char* pxr_version(void) { return "pixray_b200 0.1 (sm_100a)"; }
+const char* pxr_version(void) { return "pixray_b200 0.1 (sm_90a)"; }
 const char* pxr_last_error(pxr_handle h) { return h ? h->e->err.c_str() : g_create_err.c_str(); }
 
 int pxr_create(const pxr_config* cfg, pxr_handle* out) {

@@ -1,4 +1,4 @@
-// See gemm_tc.cuh for the contract.  sm_100a only (tcgen05 + TMA + TMEM).
+// See gemm_tc.cuh for the contract.  sm_90a only (wgmma + TMA + mbarrier).
 #include "gemm_tc.cuh"
 #include "launch.cuh"
 #include "ptx.cuh"
@@ -68,7 +68,7 @@ constexpr int TB_WARP_BYTES = TB_FLOATS * 4 + 32 * 8 + 32 * 4;  // + per-row off
 constexpr int GEMM_EPI_WARPS = 8;
 
 // Row <-> column layout exchange through the warp-private smem block.
-//   row layout   : thread = accumulator row (TMEM lane), registers = columns     (what tcgen05.ld delivers)
+//   row layout   : thread = accumulator row, registers = columns                 (one row of the staged tile)
 //   store layout : lane = (row_sub, 16-byte chunk of the row)                    (what coalesced global access wants)
 struct RowInfo {
   long long off;  // element offset of this thread's row in the output tensors, -1 if the row is out of range
@@ -92,17 +92,15 @@ __device__ __forceinline__ RowInfo row_info(const GemmParams& p, const TileCoord
   return ri;
 }
 
-// Load `width` (16 or 32) accumulator columns of this thread's row, starting at TMEM address `taddr`.
-// Both 16-column loads are issued before the single tcgen05.wait::ld (the wait, not the load, is the expensive part).
-__device__ __forceinline__ void load_acc(uint32_t taddr, int width, float (&v)[32]) {
-  uint32_t u0[16], u1[16];
-  tmem_ld_x16(taddr, u0);
-  if (width > 16) tmem_ld_x16(taddr + 16, u1);
-  tmem_ld_wait();
+// Load `width` (16 or 32) accumulator columns of this thread's row of the staged tile (shared memory, 16-byte aligned).
+__device__ __forceinline__ void load_acc(const float* src, int width, float (&v)[32]) {
 #pragma unroll
-  for (int j = 0; j < 16; ++j) {
-    v[j] = __uint_as_float(u0[j]);
-    v[16 + j] = (width > 16) ? __uint_as_float(u1[j]) : 0.f;
+  for (int j = 0; j < 8; ++j) {
+    const float4 f = (j < 4 || width > 16) ? reinterpret_cast<const float4*>(src)[j] : make_float4(0.f, 0.f, 0.f, 0.f);
+    v[4 * j] = f.x;
+    v[4 * j + 1] = f.y;
+    v[4 * j + 2] = f.z;
+    v[4 * j + 3] = f.w;
   }
 }
 
@@ -203,7 +201,7 @@ __device__ __forceinline__ int prefetch_kind(const GemmParams& p) {
   return p.res_f32 ? 1 : (p.res_f16 ? 2 : (p.act == ACT_QUICKGELU_BWD ? 3 : 0));
 }
 
-// Issue the global loads of the block's input tensor BEFORE the TMEM load / smem transpose, so their DRAM latency
+// Issue the global loads of the block's input tensor BEFORE the accumulator block is read, so their DRAM latency
 // overlaps it (a load-use chain per row made the fp32-residual GEMMs latency-bound).
 template <int E>
 __device__ __forceinline__ void prefetch_block(const GemmParams& p, const long long* s_off, int lane, int col_base,
@@ -253,7 +251,7 @@ __device__ __forceinline__ void unpack_pf(const uint4& u, int kind, float (&x)[E
 // Generic epilogue of one staged 32 x 32 block.  E elements per lane: 8 when every tensor is fp16 (16-byte accesses,
 // 8 rows per warp instruction), 4 when an fp32 tensor takes part (16-byte accesses on the fp32 side, 4 rows).
 template <int E>
-__device__ __forceinline__ void epilogue_block(const GemmParams& p, const float* tb, const long long* s_off,
+__device__ __forceinline__ void epilogue_block(const GemmParams& p, const float* tb, int ld, const long long* s_off,
                                                const int* s_row, int lane, int col_base, int col_limit, int kind,
                                                const uint4 (&pf)[BlockMap<E>::NIT]) {
   using M = BlockMap<E>;
@@ -275,7 +273,7 @@ __device__ __forceinline__ void epilogue_block(const GemmParams& p, const float*
     const long long o = off_r + col;
     float x[E];
 #pragma unroll
-    for (int j = 0; j < E; ++j) x[j] = tb[r * TB_LD + c0 + j] * p.alpha + bias[j];
+    for (int j = 0; j < E; ++j) x[j] = tb[r * ld + c0 + j] * p.alpha + bias[j];
     if (p.bias && p.bias_per_row) {
       const float b = p.bias[s_row[r]];
 #pragma unroll
@@ -336,26 +334,26 @@ __device__ __forceinline__ void store_block_f16(const GemmParams& p, const float
 // taming AttnBlock): requires the whole row in one tile (tiles_n == 1).  Thread = row.  Columns [N, n_store) are
 // written as zeros so the result can be consumed as a K-major operand with a padded row pitch.
 __device__ __forceinline__ void epilogue_softmax_fwd(const GemmParams& p, float* tb, const long long* s_off,
-                                                     uint32_t taddr, int lane) {
+                                                     const float* arow, int lane) {
   const int nslab = (p.block_n + 31) / 32;
   float v[32];
   float mx = -3.0e38f;
   for (int s = 0; s < nslab; ++s) {
-    load_acc(taddr + s * 32, min(32, p.block_n - s * 32), v);
+    load_acc(arow + s * 32, min(32, p.block_n - s * 32), v);
 #pragma unroll
     for (int j = 0; j < 32; ++j)
       if (s * 32 + j < p.N) mx = fmaxf(mx, v[j] * p.alpha);
   }
   float sum = 0.f;
   for (int s = 0; s < nslab; ++s) {
-    load_acc(taddr + s * 32, min(32, p.block_n - s * 32), v);
+    load_acc(arow + s * 32, min(32, p.block_n - s * 32), v);
 #pragma unroll
     for (int j = 0; j < 32; ++j)
       if (s * 32 + j < p.N) sum += __expf(v[j] * p.alpha - mx);
   }
   const float inv = __fdividef(1.f, sum);
   for (int s = 0; s < nslab; ++s) {
-    load_acc(taddr + s * 32, min(32, p.block_n - s * 32), v);
+    load_acc(arow + s * 32, min(32, p.block_n - s * 32), v);
 #pragma unroll
     for (int j = 0; j < 32; ++j) v[j] = (s * 32 + j < p.N) ? __expf(v[j] * p.alpha - mx) * inv : 0.f;
     stage_rows(tb, v, lane);
@@ -367,7 +365,7 @@ __device__ __forceinline__ void epilogue_softmax_fwd(const GemmParams& p, float*
 // Fused softmax backward: accumulator = dP row, aux_in = P (fp16, same indexing as the output);
 // dS = alpha * P * (dP - sum_j P_j dP_j).
 __device__ __forceinline__ void epilogue_softmax_bwd(const GemmParams& p, float* tb, const long long* s_off,
-                                                     uint32_t taddr, int lane) {
+                                                     const float* arow, int lane) {
   const int nslab = (p.block_n + 31) / 32;
   const int chunk = lane & 3, rsub = lane >> 2;
   float v[32];
@@ -394,7 +392,7 @@ __device__ __forceinline__ void epilogue_softmax_bwd(const GemmParams& p, float*
         for (int j = 0; j < 8; ++j) tb[r * TB_LD + chunk * 8 + j] = x[j];
       }
       __syncwarp();
-      load_acc(taddr + s * 32, min(32, p.block_n - s * 32), v);
+      load_acc(arow + s * 32, min(32, p.block_n - s * 32), v);
       if (pass == 0) {
 #pragma unroll
         for (int j = 0; j < 32; ++j) dot += tb[lane * TB_LD + j] * v[j];
@@ -412,11 +410,8 @@ __device__ __forceinline__ void epilogue_softmax_bwd(const GemmParams& p, float*
 }
 
 // TMA producer (one lane): walks this CTA's tiles and fills the stage ring.
-// This single thread paces the whole kernel (one k-block of MMA work is ~512 cycles at block_n = 256): ncu showed the MMA
-// thread finding its stage not yet full on 93 % of the k-blocks while the producer never waited for a free slot -- the
-// loop body was ~160 dependent integer instructions (runtime divisions for the tap / k offset, operand-mode branches,
-// generic->shared address conversions).  The body below is specialised on the operand modes, carries (tap, kk) as
-// running counters and works on 32-bit shared addresses: ~25 instructions per k-block.
+// This single thread paces the whole kernel, so its loop body is kept short: specialised on the operand modes (no runtime
+// divisions for the tap / k offset, no mode branches), (tap, kk) carried as running counters, 32-bit shared addresses.
 template <int AM, int BM>
 __device__ __forceinline__ void producer_tiles(const GemmParams& p, uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar,
                                                uint32_t stage_bytes) {
@@ -494,173 +489,99 @@ __device__ __forceinline__ void producer_loop(const GemmParams& p, uint8_t* smem
   }
 }
 
-// MMA issuer (one lane): tcgen05.mma over the stage ring into the double-buffered TMEM accumulator.  The shared-memory
-// descriptors are built once; a stage / k-step advance is an add on their address field (bits [0,14) = address >> 4,
-// and the whole ring sits below 256 KiB, so the add never carries out of the field).
-__device__ __forceinline__ void mma_loop(const GemmParams& p, uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar,
-                                         uint64_t* tmem_full_bar, uint64_t* tmem_empty_bar, uint32_t tmem_base,
-                                         uint32_t stage_bytes) {
-  const uint32_t idesc =
-      make_idesc_f16(GEMM_BLOCK_M, p.block_n, p.fmt, p.a_mode == OP_MNMAJOR, p.b_mode == OP_MNMAJOR);
-  // K-major: 8-row groups 1024 B apart; K advance = 32 B inside the swizzled row.
+// Accumulator of one warpgroup: 64 rows x NCH 64-column wgmma fragments (sized per kernel, so that the fragments of a
+// 64- or 128-wide tile do not carry the registers of a 256-wide one).
+template <int NCH>
+struct WgAcc {
+  float d[NCH][32];
+};
+template <int NF>
+using AccFor = WgAcc<NF ? NF : 4>;
+
+// MMA warpgroup `wg` (0 or 1: tile rows [64 wg, 64 wg + 64)): wgmma over the k-blocks of one tile.  A k-block is four
+// k16 steps; each step issues block_n / 64 m64n64 instructions and, for block_n % 64, up to three m64n16 ones.  The
+// shared-memory descriptors are built once; a stage / k-step advance is an add on their address field (bits [0,14) =
+// address >> 4, and the whole ring sits below 256 KiB, so the add never carries out of the field).  The stage read by
+// k-block kb is released once kb's wgmma group has completed (checked after k-block kb + 1 has been issued).
+// NF > 0: fp16 operands and block_n == 64 NF, so every instruction of a k-step is known at compile time and the fragments
+// take 32 NF registers (runtime-guarded wgmma or a larger live fragment make ptxas serialise the chain); NF == 0 covers
+// every other width and bf16.  With a single stage the k-block's slot is released as soon as its group completes.
+template <int TA, int TB, int NF>
+__device__ __forceinline__ void mma_tile(const GemmParams& p, AccFor<NF>& acc, int wg, int n_kb, uint32_t smem0, uint32_t full0,
+                                         uint64_t* empty_bar, uint32_t stage_bytes, int& stage, uint32_t& phase) {
+  // K-major: 8-row groups 1024 B apart, a 64-row slab is 8 KiB; K advance = 32 B inside the swizzled row.
   // MN-major: 64-wide MN atoms 8192 B apart (LBO), 8-deep K groups 1024 B apart (SBO); K advance = 2048 B.
-  const uint32_t a_lbo = (p.a_mode == OP_MNMAJOR) ? MN_ATOM_BYTES : 0;
-  const uint32_t b_lbo = (p.b_mode == OP_MNMAJOR) ? MN_ATOM_BYTES : 0;
-  const uint64_t a_kstep = ((p.a_mode == OP_MNMAJOR) ? 2048 : 32) >> 4;
-  const uint64_t b_kstep = ((p.b_mode == OP_MNMAJOR) ? 2048 : 32) >> 4;
-  const uint32_t smem0 = smem_u32(smem), full0 = smem_u32(full_bar), empty0 = smem_u32(empty_bar);
-  const uint64_t a_desc0 = make_smem_desc_sw128(smem0, a_lbo, 1024);
-  const uint64_t b_desc0 = make_smem_desc_sw128(smem0 + A_TILE_BYTES, b_lbo, 1024);
+  const uint64_t a_kstep = (TA ? 2048 : 32) >> 4, b_kstep = (TB ? 2048 : 32) >> 4;
+  const uint64_t a_desc0 = make_smem_desc_sw128(smem0 + wg * 8192, TA ? MN_ATOM_BYTES : 0, 1024);
+  const uint64_t b_desc0 = make_smem_desc_sw128(smem0 + A_TILE_BYTES, TB ? MN_ATOM_BYTES : 0, 1024);
   const uint64_t stage_step = stage_bytes >> 4;
-  const int tiles_mn = p.tiles_m * p.tiles_n;
-  int stage = 0;
-  uint32_t phase = 0;
-  int it = 0;
-  for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++it) {
-    const int as = it & 1;
-    const uint32_t aphase = (it >> 1) & 1;
-    mbar_wait(&tmem_empty_bar[as], aphase ^ 1);
-    tc_fence_after();
-    const uint32_t d_tmem = tmem_base + static_cast<uint32_t>(as * p.block_n);
-    int n_kb = p.num_k_blocks;
-    if (p.k_splits > 1) {
-      const int kb_begin = (tile / tiles_mn) * p.kb_per_split;
-      n_kb = min(p.num_k_blocks, kb_begin + p.kb_per_split) - kb_begin;
-    }
-    uint32_t acc = 0;
-    for (int kb = 0; kb < n_kb; ++kb) {
-      mbar_wait_s(full0 + stage * 8, phase);
-      tc_fence_after();
-      const uint64_t ad = a_desc0 + stage * stage_step, bd = b_desc0 + stage * stage_step;
-      umma_f16(d_tmem, ad, bd, idesc, acc);
-      umma_f16(d_tmem, ad + a_kstep, bd + b_kstep, idesc, 1u);
-      umma_f16(d_tmem, ad + 2 * a_kstep, bd + 2 * b_kstep, idesc, 1u);
-      umma_f16(d_tmem, ad + 3 * a_kstep, bd + 3 * b_kstep, idesc, 1u);
-      acc = 1u;
-      umma_commit_s(empty0 + stage * 8);
-      if (++stage == p.stages) {
-        stage = 0;
-        phase ^= 1;
-      }
-    }
-    umma_commit(&tmem_full_bar[as]);
-  }
-}
-
-// EPI: 0 generic epilogue, 1 fused softmax forward, 2 fused softmax backward.  HAS_IN: the generic epilogue reads an
-// input tensor (residual / saved pre-activation) that is prefetched; kept out of the input-free kernel so that one
-// stays lean (the prefetch registers cost the plain GEMMs ~25 %).
-template <int EPI, bool HAS_IN>
-__device__ __forceinline__ void gemm_tc_body(const GemmParams& p) {
-  pdl_launch_dependents();
-  extern __shared__ uint8_t smem_raw[];
-  // keep the pointer derived from the __shared__ symbol (offset arithmetic only) so smem accesses compile to LDS/STS
-  const uint32_t smem_base_u32 = smem_u32(smem_raw);
-  uint8_t* smem = smem_raw + (((smem_base_u32 + 1023u) & ~1023u) - smem_base_u32);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t b_bytes = static_cast<uint32_t>(p.block_n) * GEMM_BLOCK_K * 2;
-  const uint32_t stage_bytes = A_TILE_BYTES + b_bytes;
-
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + static_cast<size_t>(p.stages) * stage_bytes);
-  uint64_t* empty_bar = full_bar + GEMM_MAX_STAGES;
-  uint64_t* tmem_full_bar = empty_bar + GEMM_MAX_STAGES;
-  uint64_t* tmem_empty_bar = tmem_full_bar + 2;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tmem_empty_bar + 2);
-  float* tbuf_base = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(full_bar) + 256);
-
-  if (threadIdx.x == 0) {
-    prefetch_tmap(&p.tma_a);
-    prefetch_tmap(&p.tma_b);
-    for (int i = 0; i < p.stages; ++i) {
-      mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full_bar[i], 1);
-      mbar_init(&tmem_empty_bar[i], GEMM_EPI_WARPS);
-    }
-    fence_barrier_init();
-  }
-  if (warp == 1) tmem_alloc(tmem_ptr_smem, static_cast<uint32_t>(p.tmem_cols));
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  pdl_wait();  // everything above touched only parameters, shared memory and TMEM
-
-  if (warp == 0) {
-    if (lane == 0) producer_loop(p, smem, full_bar, empty_bar, stage_bytes);
-  } else if (warp == 1) {
-    if (lane == 0) mma_loop(p, smem, full_bar, empty_bar, tmem_full_bar, tmem_empty_bar, tmem_base, stage_bytes);
-  } else {
-    // ------------------------------------------------------------ epilogue (TMEM -> regs -> smem transpose -> global)
-    const int ew = warp - 2;          // 0..7
-    const int q = warp & 3;           // TMEM lane quarter this warp may access
-    const int half = ew >> 2;         // two warps share a quarter and split the 32-column slabs
-    uint8_t* wbase = reinterpret_cast<uint8_t*>(tbuf_base) + static_cast<size_t>(ew) * TB_WARP_BYTES;
-    float* tb = reinterpret_cast<float*>(wbase);
-    long long* s_off = reinterpret_cast<long long*>(wbase + TB_FLOATS * 4);
-    int* s_row = reinterpret_cast<int*>(wbase + TB_FLOATS * 4 + 32 * 8);
-    const bool wide = (p.out_f32 != nullptr) || (p.res_f32 != nullptr);
-    int it = 0;
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++it) {
-      const TileCoord t = decode_tile(p, tile);
-      const int as = it & 1;
-      const uint32_t aphase = (it >> 1) & 1;
-      const RowInfo ri = row_info(p, t, q * 32 + lane);
-      s_off[lane] = ri.off;
-      s_row[lane] = ri.row;
-      __syncwarp();
-      mbar_wait(&tmem_full_bar[as], aphase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>(as * p.block_n);
-      if (EPI == 1) {
-        if (half == 0) epilogue_softmax_fwd(p, tb, s_off, taddr, lane);
-      } else if (EPI == 2) {
-        if (half == 0) epilogue_softmax_bwd(p, tb, s_off, taddr, lane);
-      } else {
-        const int nslab = (p.block_n + 31) / 32;
-        const int col_limit = min(p.N, t.n0 + p.block_n);
-        const int kind = HAS_IN ? prefetch_kind(p) : 0;
-        for (int s = half; s < nslab; s += 2) {
-          float v[32];
-          if (wide) {
-            uint4 pf[BlockMap<4>::NIT];
-            if (HAS_IN) prefetch_block<4>(p, s_off, lane, t.n0 + s * 32, col_limit, kind, pf);
-            load_acc(taddr + s * 32, min(32, p.block_n - s * 32), v);
-            stage_rows(tb, v, lane);
-            epilogue_block<4>(p, tb, s_off, s_row, lane, t.n0 + s * 32, col_limit, kind, pf);
-          } else {
-            uint4 pf[BlockMap<8>::NIT];
-            if (HAS_IN) prefetch_block<8>(p, s_off, lane, t.n0 + s * 32, col_limit, kind, pf);
-            load_acc(taddr + s * 32, min(32, p.block_n - s * 32), v);
-            stage_rows(tb, v, lane);
-            epilogue_block<8>(p, tb, s_off, s_row, lane, t.n0 + s * 32, col_limit, kind, pf);
-          }
-          __syncwarp();
+  const int nfull = NF ? NF : p.block_n / 64, ntail = NF ? 0 : (p.block_n % 64) / 16;
+  const int bf16 = NF ? 0 : p.fmt;
+  constexpr int NCH = NF ? NF : 4;
+  const bool elected = (threadIdx.x & 127) == 0;
+  int prev = -1;
+  for (int kb = 0; kb < n_kb; ++kb) {
+    mbar_wait_s(full0 + stage * 8, phase);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const uint64_t ad = a_desc0 + stage * stage_step + k * a_kstep, bd = b_desc0 + stage * stage_step + k * b_kstep;
+      const uint32_t scale_d = (kb | k) ? 1u : 0u;
+#pragma unroll
+      for (int j = 0; j < NCH; ++j) {
+        if (j < nfull) wgmma_m64n64<TA, TB>(acc.d[j], ad, bd + j * (8192 >> 4), scale_d, bf16);
+        if (!NF && j == nfull) {  // 16-column tail (K-major B only: MN-major B tiles are multiples of 64 wide)
+#pragma unroll
+          for (int t = 0; t < 3; ++t)
+            if (t < ntail) wgmma_m64n16<TA, TB>(acc.d[j] + 8 * t, ad, bd + (j * 8192 + t * 2048) / 16, scale_d, bf16);
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty_bar[as]);
+    }
+    wgmma_commit();
+    if (p.stages == 1) {  // the producer cannot run ahead: free the only slot now
+      wgmma_wait<0>();
+      if (elected) mbar_arrive(&empty_bar[stage]);
+    } else {
+      wgmma_wait<1>();
+      if (prev >= 0 && elected) mbar_arrive(&empty_bar[prev]);
+      prev = stage;
+    }
+    if (++stage == p.stages) {
+      stage = 0;
+      phase ^= 1;
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    __syncwarp();
-    tc_fence_after();
-    tmem_dealloc(tmem_base, static_cast<uint32_t>(p.tmem_cols));
+  wgmma_wait<0>();
+  if (prev >= 0 && elected) mbar_arrive(&empty_bar[prev]);
+}
+
+// Write this warpgroup's fragments into the staged tile: row-major fp32, row pitch ld floats.
+template <int NCH>
+__device__ __forceinline__ void dump_acc(const WgAcc<NCH>& acc, float* tile, int ld, int block_n) {
+  const int t = threadIdx.x & 127;
+  const int r0 = (threadIdx.x >> 7) * 64 + (t >> 5) * 16 + ((t & 31) >> 2), c0 = 2 * (t & 3);
+#pragma unroll
+  for (int j = 0; j < NCH; ++j) {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const int c = 64 * j + 8 * i + c0;
+      if (64 * j + 8 * i < block_n) {
+        *reinterpret_cast<float2*>(tile + r0 * ld + c) = make_float2(acc.d[j][4 * i], acc.d[j][4 * i + 1]);
+        *reinterpret_cast<float2*>(tile + (r0 + 8) * ld + c) = make_float2(acc.d[j][4 * i + 2], acc.d[j][4 * i + 3]);
+      }
+    }
   }
 }
 
+__device__ __forceinline__ int tile_k_blocks(const GemmParams& p, int tile) {
+  if (p.k_splits <= 1) return p.num_k_blocks;
+  const int kb_begin = (tile / (p.tiles_m * p.tiles_n)) * p.kb_per_split;
+  return min(p.num_k_blocks, kb_begin + p.kb_per_split) - kb_begin;
+}
 
 // ------------------------------------------------------------------------------------------------ tensor-map epilogue
-// The generic epilogue above is instruction- and latency-bound (ncu: 8 epilogue warps busy ~85 % of the time, tensor pipe
-// 43 % on the plain 12608 x 3072 x 768 GEMM, 20 % with the QuickGELU-backward epilogue): transposing every 32 x 32 block
-// through shared memory costs ~10 instructions per element and every input tensor is a dependent global load.
+// The generic epilogue above is instruction- and latency-bound: every element goes through a row-to-column exchange and
+// every input tensor is a dependent global load.
 // Here each lane keeps its accumulator ROW: it writes 64 contiguous bytes (32 fp16 / 16 fp32 columns) of that row into a
 // 32-row x 64-byte box in shared memory (64B-swizzled, conflict-free), and one lane hands the box to a TMA store.
 // Input tensors (residual, saved pre-activation) come in through TMA loads into the same box, two blocks ahead, and the
@@ -668,7 +589,7 @@ __device__ __forceinline__ void gemm_tc_body(const GemmParams& p) {
 constexpr int TE_BUF_BYTES = 2048;  // 32 rows x 64 bytes
 constexpr int TE_BUFS = 4;          // boxes per epilogue warp
 constexpr int TE_WARP_BYTES = TE_BUFS * TE_BUF_BYTES;
-constexpr int TE_BAR_BYTES = 1024;  // barrier block (stage ring, TMEM, per-warp input barriers)
+constexpr int TE_BAR_BYTES = 1024;  // barrier block (stage ring, per-warp input barriers)
 
 // byte offset of 16-byte chunk c (0..3) of row r (0..31) in a CU_TENSOR_MAP_SWIZZLE_64B box (chunk ^= address bits 7..8)
 __device__ __forceinline__ uint32_t te_off(int r, int c) {
@@ -692,8 +613,7 @@ __device__ __forceinline__ void unpack8(const uint4& u, float* x) {
 }
 
 // QuickGELU and its derivative on packed fp16 pairs for the tensor-map epilogue (the fp32 form costs ~8 instructions per
-// element with two MUFU ops and made the fc1 / fc2-dgrad epilogues ALU-bound: ncu showed the 8 epilogue warps pacing
-// the tile loop at 1.6x the MMA time).  sigmoid(z) = 0.5 tanh(z / 2) + 0.5 with tanh.approx.f16x2: one MUFU per pair.
+// element with two MUFU ops and makes the fc1 / fc2-dgrad epilogues ALU-bound).  sigmoid(z) = 0.5 tanh(z / 2) + 0.5 with tanh.approx.f16x2: one MUFU per pair.
 // The operands are already fp16 here (u is stored as fp16; the reference runs its CLIP in fp16 on CUDA, slip.py:176).
 __device__ __forceinline__ __half2 tanh_h2(__half2 x) {
   uint32_t r, a = *reinterpret_cast<uint32_t*>(&x);
@@ -712,40 +632,18 @@ __device__ __forceinline__ __half2 quickgelu_grad_h2(__half2 u) {
   return __hfma2(s, b, s);                       // s (1 + 1.702 u (1 - s))
 }
 
-template <int MODE, bool PAIR>
-__device__ __forceinline__ void tma_epilogue_loop(const GemmParams& p, uint8_t* wbuf, uint64_t* in_bar,
-                                                  uint64_t* tmem_full_bar, uint64_t* tmem_empty_bar, uint32_t tmem_base,
-                                                  int warp, int lane) {
+// One tile of the tensor-map epilogue for warp `warp` (rows [32 q, 32 q + 32) of the tile, column blocks half, half + 2,
+// ...).  `cnt` counts the blocks this warp has processed: box rotation and input-barrier parity.
+template <int MODE>
+__device__ __forceinline__ void tma_epilogue_tile(const GemmParams& p, const TileCoord& t, uint8_t* wbuf,
+                                                  uint64_t* in_bar, const float* arow, int warp, int lane,
+                                                  uint32_t& cnt) {
   constexpr bool F32 = (MODE == TE_RES32);
   constexpr bool IN = (MODE == TE_GELU_BWD || MODE == TE_RES32 || MODE == TE_RES16);
   constexpr int BW = F32 ? 16 : 32;  // columns per 64-byte box row
-  const int q = warp & 3;            // TMEM lane quarter
-  const int half = (warp - 2) >> 2;  // the two warps of a quarter alternate over the column blocks
-  uint32_t cnt = 0;                  // blocks this warp has processed: box rotation and input-barrier parity
-  int it = 0;
-  // work items: tiles of this CTA, or (PAIR) this CTA's half of the tile pairs of its cluster
-  uint32_t rank = 0;
-  int w_begin = blockIdx.x, w_step = gridDim.x, w_end = p.total_tiles, pairs_m = 1;
-  if (PAIR) {
-    rank = cluster_ctarank();
-    w_begin = blockIdx.x >> 1;
-    w_step = gridDim.x >> 1;
-    pairs_m = (p.tiles_m + 1) / 2;
-    w_end = pairs_m * p.tiles_n * (p.total_tiles / (p.tiles_m * p.tiles_n));
-  }
-  for (int w = w_begin; w < w_end; w += w_step, ++it) {
-    TileCoord t;
-    bool exists = true;
-    if (PAIR) {
-      const int tn = w % p.tiles_n, r = w / p.tiles_n;
-      const int tm = 2 * (r % pairs_m) + static_cast<int>(rank);
-      t = make_coord(p, tn, tm, r / pairs_m);
-      exists = tm < p.tiles_m;  // odd tile count: the peer's last tile does not exist
-    } else {
-      t = decode_tile(p, w);
-    }
-    const int as = it & 1;
-    const uint32_t aphase = (it >> 1) & 1;
+  const int q = warp & 3;            // row quarter of the tile
+  const int half = warp >> 2;        // the two warps of a quarter alternate over the column blocks
+  {
     // tensor-map coordinates of this warp's 32 rows: (col, row, b0, b1) or, for conv, (col, w, h, image)
     int c1, c2, c3;
     if (p.a_mode == OP_CONV) {
@@ -760,7 +658,7 @@ __device__ __forceinline__ void tma_epilogue_loop(const GemmParams& p, uint8_t* 
     // blocks with at least one column inside N; this warp takes s = half, half + 2, ...
     const int ncols = min(p.N - t.n0, p.block_n);
     const int nblk = (ncols + BW - 1) / BW;
-    const int my = exists ? (nblk - half + 1) / 2 : 0;
+    const int my = (nblk - half + 1) / 2;
     if (IN && lane == 0) {
       bulk_wait_group_read<1>();
       for (int j = 0; j < 2 && j < my; ++j) {
@@ -769,9 +667,6 @@ __device__ __forceinline__ void tma_epilogue_loop(const GemmParams& p, uint8_t* 
         tma_load_4d(&p.tma_d, &in_bar[b], wbuf + b * TE_BUF_BYTES, t.n0 + (half + 2 * j) * BW, c1, c2, c3);
       }
     }
-    mbar_wait(&tmem_full_bar[as], aphase);
-    tc_fence_after();
-    const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>(as * p.block_n);
     for (int j = 0; j < my; ++j) {
       const int s = half + 2 * j;
       const int col = t.n0 + s * BW;
@@ -795,17 +690,10 @@ __device__ __forceinline__ void tma_epilogue_loop(const GemmParams& p, uint8_t* 
       // accumulator columns of this row
       float x[BW];
       {
-        uint32_t a0[16], a1[16];
-        const bool second = !F32 && (p.block_n - s * BW > 16);  // block_n % 32 == 16: the last block is half wide
-        tmem_ld_x16(taddr + s * BW, a0);
-        if (second) tmem_ld_x16(taddr + s * BW + 16, a1);
-        tmem_ld_wait();
+        float a[32];
+        load_acc(arow + s * BW, (!F32 && p.block_n - s * BW > 16) ? 32 : 16, a);  // block_n % 32 == 16: last block half wide
 #pragma unroll
-        for (int i = 0; i < 16; ++i) x[i] = __uint_as_float(a0[i]) * p.alpha;
-        if constexpr (!F32) {
-#pragma unroll
-          for (int i = 0; i < 16; ++i) x[16 + i] = second ? __uint_as_float(a1[i]) * p.alpha : 0.f;
-        }
+        for (int i = 0; i < BW; ++i) x[i] = a[i] * p.alpha;
       }
       if (p.bias) {
         const float4* bp = reinterpret_cast<const float4*>(p.bias + col);
@@ -878,21 +766,26 @@ __device__ __forceinline__ void tma_epilogue_loop(const GemmParams& p, uint8_t* 
       }
     }
     cnt += my;
-    tc_fence_before();
-    __syncwarp();
-    if (lane == 0) {
-      if (!PAIR || rank == 0) mbar_arrive(&tmem_empty_bar[as]);
-      else mbar_arrive_cluster(&tmem_empty_bar[as], 0);
-    }
   }
-  if (lane == 0) bulk_wait_group<0>();
-  __syncwarp();
 }
 
-template <int MODE>
-__device__ __forceinline__ void gemm_tce_body(const GemmParams& p) {
+constexpr int GEMM_BAR_BYTES = 1024;  // stage-ring barriers, per-warp input barriers (tensor-map epilogue)
+
+// Row pitch (floats) of the staged accumulator tile: a multiple of 4 (16-byte row reads) that is 4 mod 32, so the
+// epilogue's thread-per-row 16-byte reads hit distinct banks within each quarter warp.
+__host__ __device__ __forceinline__ int acc_ld(int block_n) { return (block_n + 31) / 32 * 32 + 4; }
+
+// Warps 0..7 = two MMA warpgroups (tile rows 0..63, 64..127) that afterwards run the epilogue, warp 8 = TMA producer.
+// Per tile: wgmma into registers, fragments -> staged fp32 tile in shared memory, epilogue from there.  The producer runs
+// ahead through the stage ring, so the next tile's operands stream in while the epilogue of this one runs.
+// EPI: 0 generic or tensor-map epilogue (TE = its mode), 1 fused softmax forward, 2 fused softmax backward.  HAS_IN: the
+// generic epilogue reads an input tensor (residual / saved pre-activation) that is prefetched; kept out of the
+// input-free kernel so that one stays lean.
+template <int EPI, bool HAS_IN, int TE, int NF>
+__device__ __forceinline__ void gemm_body(const GemmParams& p) {
   pdl_launch_dependents();
   extern __shared__ uint8_t smem_raw[];
+  // keep the pointer derived from the __shared__ symbol (offset arithmetic only) so smem accesses compile to LDS/STS
   const uint32_t smem_base_u32 = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + (((smem_base_u32 + 1023u) & ~1023u) - smem_base_u32);
 
@@ -903,390 +796,128 @@ __device__ __forceinline__ void gemm_tce_body(const GemmParams& p) {
   uint8_t* bar_block = smem + static_cast<size_t>(p.stages) * stage_bytes;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(bar_block);
   uint64_t* empty_bar = full_bar + GEMM_MAX_STAGES;
-  uint64_t* tmem_full_bar = empty_bar + GEMM_MAX_STAGES;
-  uint64_t* tmem_empty_bar = tmem_full_bar + 2;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tmem_empty_bar + 2);
   uint64_t* in_bars = reinterpret_cast<uint64_t*>(bar_block + 256);  // [GEMM_EPI_WARPS][TE_BUFS]
-  uint8_t* boxes = bar_block + TE_BAR_BYTES;                          // 1024-byte aligned
+  const int ald = acc_ld(p.block_n);
+  float* acc_tile = reinterpret_cast<float*>(bar_block + GEMM_BAR_BYTES);
+  uint8_t* epi_base = reinterpret_cast<uint8_t*>(acc_tile + GEMM_BLOCK_M * ald);  // 1024-byte aligned
 
   if (threadIdx.x == 0) {
     prefetch_tmap(&p.tma_a);
     prefetch_tmap(&p.tma_b);
-    prefetch_tmap(&p.tma_c);
-    if (MODE != TE_F16) prefetch_tmap(&p.tma_d);
+    if (TE != TE_NONE) prefetch_tmap(&p.tma_c);
+    if (TE != TE_NONE && TE != TE_F16) prefetch_tmap(&p.tma_d);
     for (int i = 0; i < p.stages; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
+      mbar_init(&empty_bar[i], 2);  // one arrive per MMA warpgroup
     }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full_bar[i], 1);
-      mbar_init(&tmem_empty_bar[i], GEMM_EPI_WARPS);
-    }
-    for (int i = 0; i < GEMM_EPI_WARPS * TE_BUFS; ++i) mbar_init(&in_bars[i], 1);
+    if (TE != TE_NONE)
+      for (int i = 0; i < GEMM_EPI_WARPS * TE_BUFS; ++i) mbar_init(&in_bars[i], 1);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_ptr_smem, static_cast<uint32_t>(p.tmem_cols));
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  pdl_wait();  // everything above touched only parameters, shared memory and TMEM
+  pdl_wait();  // everything above touched only parameters and shared memory
 
-  if (warp == 0) {
+  if (warp == GEMM_EPI_WARPS) {
     if (lane == 0) producer_loop(p, smem, full_bar, empty_bar, stage_bytes);
-  } else if (warp == 1) {
-    if (lane == 0) mma_loop(p, smem, full_bar, empty_bar, tmem_full_bar, tmem_empty_bar, tmem_base, stage_bytes);
-  } else {
-    const int ew = warp - 2;
-    tma_epilogue_loop<MODE, false>(p, boxes + static_cast<size_t>(ew) * TE_WARP_BYTES, in_bars + ew * TE_BUFS,
-                                   tmem_full_bar, tmem_empty_bar, tmem_base, warp, lane);
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    __syncwarp();
-    tc_fence_after();
-    tmem_dealloc(tmem_base, static_cast<uint32_t>(p.tmem_cols));
-  }
-}
-
-
-// ------------------------------------------------------------------------------------------------ cta_group::2
-// Two CTAs of a cluster (one TPC) cooperate on a 256 x block_n tile pair: each CTA holds its own 128 rows of A and
-// HALF of the B tile, one tcgen05.mma.cta_group::2 (issued by the rank-0 CTA) consumes both CTAs' shared memory and
-// writes each CTA's 128 x block_n accumulator into its own TMEM.  Per k-block a CTA loads 16 KB + block_n/2 * 128 B
-// instead of 16 KB + block_n * 128 B: with 128 x 256 tiles per SM the single-CTA kernel needs ~96 B/clk/SM of L2->SM
-// traffic at tensor peak, more than the ~43 B/clk/SM the L2 can deliver, so it is L2-bound at < 50 % of peak.
-// Pair geometry shared by the three roles of the cta_group::2 kernels.
-struct PairInfo {
-  uint32_t rank;
-  bool leader;
-  int cluster_id, num_clusters, pairs_m, total_pairs, half_n;
-};
-__device__ __forceinline__ PairInfo pair_info(const GemmParams& p) {
-  PairInfo pi;
-  pi.rank = cluster_ctarank();
-  pi.leader = pi.rank == 0;
-  pi.cluster_id = blockIdx.x >> 1;
-  pi.num_clusters = gridDim.x >> 1;
-  pi.pairs_m = (p.tiles_m + 1) / 2;
-  pi.total_pairs = pi.pairs_m * p.tiles_n * (p.total_tiles / (p.tiles_m * p.tiles_n));
-  pi.half_n = p.block_n / 2;
-  return pi;
-}
-
-template <int AM, int BM>
-__device__ __forceinline__ void producer2_tiles(const GemmParams& p, const PairInfo& pi, uint8_t* smem, uint64_t* full_bar,
-                                                uint64_t* empty_bar, uint32_t stage_bytes) {
-  const uint32_t rank = pi.rank;
-  const bool leader = pi.leader;
-  const int half_n = pi.half_n, n_atoms = half_n / 64;
-  const uint32_t smem0 = smem_u32(smem), full0 = smem_u32(full_bar), empty0 = smem_u32(empty_bar);
-  const int k_per_tap = p.k_blocks_per_tap * GEMM_BLOCK_K;
+  const int wg = warp >> 2;
+  const int q = warp & 3, half = warp >> 2;  // epilogue: row quarter, and which column slabs of it
+  const float* arow = acc_tile + (q * 32 + lane) * ald;
+  uint8_t* wbase = epi_base + static_cast<size_t>(warp) * (TE != TE_NONE ? TE_WARP_BYTES : TB_WARP_BYTES);
+  float* tb = reinterpret_cast<float*>(wbase);
+  long long* s_off = reinterpret_cast<long long*>(wbase + TB_FLOATS * 4);
+  int* s_row = reinterpret_cast<int*>(wbase + TB_FLOATS * 4 + 32 * 8);
+  const bool wide = (p.out_f32 != nullptr) || (p.res_f32 != nullptr);
+  const uint32_t smem0 = smem_u32(smem), full0 = smem_u32(full_bar);
   int stage = 0;
-  uint32_t phase = 0;
-  for (int tp = pi.cluster_id; tp < pi.total_pairs; tp += pi.num_clusters) {
-    const int tn = tp % p.tiles_n, r = tp / p.tiles_n;
-    const TileCoord t = make_coord(p, tn, 2 * (r % pi.pairs_m) + (int)rank, r / pi.pairs_m);
-    const int bb0 = p.b_batched ? t.b0 : 0, bb1 = p.b_batched ? t.b1 : 0;
-    const int nb = t.n0 + (int)rank * half_n;  // this CTA's half of the B tile
-    int kk = 0, ty = p.num_taps == 9 ? -1 : 0, tx = ty, b_row = nb;
-    for (int kb = 0; kb < p.num_k_blocks; ++kb) {
-      const uint32_t fb = full0 + stage * 8, sa = smem0 + stage * stage_bytes, sb = sa + A_TILE_BYTES;
-      mbar_wait_s(empty0 + stage * 8, phase ^ 1);
-      if (leader) mbar_arrive_expect_tx_s(fb, 2 * stage_bytes);
-      if (AM == OP_KMAJOR) {
-        tma_load_4d_2sm_s(&p.tma_a, fb, sa, kk, t.m0, t.b0, t.b1);
-      } else if (AM == OP_MNMAJOR) {
-        tma_load_4d_2sm_s(&p.tma_a, fb, sa, t.m0, kk, t.b0, t.b1);
-        tma_load_4d_2sm_s(&p.tma_a, fb, sa + MN_ATOM_BYTES, t.m0 + 64, kk, t.b0, t.b1);
-      } else {
-        tma_load_4d_2sm_s(&p.tma_a, fb, sa, kk, t.w0 + tx, t.h0 + ty, t.z);
-      }
-      if (BM == OP_KMAJOR) {
-        tma_load_4d_2sm_s(&p.tma_b, fb, sb, kk, b_row, bb0, bb1);
-      } else {
-        for (int j = 0; j < n_atoms; ++j)
-          tma_load_4d_2sm_s(&p.tma_b, fb, sb + j * MN_ATOM_BYTES, nb + 64 * j, kk, bb0, bb1);
-      }
-      kk += GEMM_BLOCK_K;
-      if (AM == OP_CONV && kk == k_per_tap) {
-        kk = 0;
-        b_row += p.b_tap_rows;
-        if (++tx == 2) {
-          tx = -1;
-          ++ty;
-        }
-      }
-      if (++stage == p.stages) {
-        stage = 0;
-        phase ^= 1;
-      }
+  uint32_t phase = 0, cnt = 0;
+  AccFor<NF> acc;
+  for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+    const TileCoord t = decode_tile(p, tile);
+    const int n_kb = tile_k_blocks(p, tile);
+    if (p.a_mode == OP_MNMAJOR) {
+      if (p.b_mode == OP_MNMAJOR) mma_tile<1, 1, NF>(p, acc, wg, n_kb, smem0, full0, empty_bar, stage_bytes, stage, phase);
+      else mma_tile<1, 0, NF>(p, acc, wg, n_kb, smem0, full0, empty_bar, stage_bytes, stage, phase);
+    } else {
+      if (p.b_mode == OP_MNMAJOR) mma_tile<0, 1, NF>(p, acc, wg, n_kb, smem0, full0, empty_bar, stage_bytes, stage, phase);
+      else mma_tile<0, 0, NF>(p, acc, wg, n_kb, smem0, full0, empty_bar, stage_bytes, stage, phase);
     }
-  }
-}
-
-__device__ __forceinline__ void producer2_loop(const GemmParams& p, const PairInfo& pi, uint8_t* smem, uint64_t* full_bar,
-                                               uint64_t* empty_bar, uint32_t stage_bytes) {
-  if (p.a_mode == OP_CONV) {
-    producer2_tiles<OP_CONV, OP_KMAJOR>(p, pi, smem, full_bar, empty_bar, stage_bytes);
-  } else if (p.a_mode == OP_KMAJOR) {
-    if (p.b_mode == OP_KMAJOR) producer2_tiles<OP_KMAJOR, OP_KMAJOR>(p, pi, smem, full_bar, empty_bar, stage_bytes);
-    else producer2_tiles<OP_KMAJOR, OP_MNMAJOR>(p, pi, smem, full_bar, empty_bar, stage_bytes);
-  } else {
-    if (p.b_mode == OP_KMAJOR) producer2_tiles<OP_MNMAJOR, OP_KMAJOR>(p, pi, smem, full_bar, empty_bar, stage_bytes);
-    else producer2_tiles<OP_MNMAJOR, OP_MNMAJOR>(p, pi, smem, full_bar, empty_bar, stage_bytes);
-  }
-}
-
-__device__ __forceinline__ void mma2_loop(const GemmParams& p, const PairInfo& pi, uint8_t* smem, uint64_t* full_bar,
-                                          uint64_t* empty_bar, uint64_t* tmem_full_bar, uint64_t* tmem_empty_bar,
-                                          uint32_t tmem_base, uint32_t stage_bytes) {
-  const int cluster_id = pi.cluster_id, num_clusters = pi.num_clusters, total_pairs = pi.total_pairs;
-  const uint32_t idesc = make_idesc_f16(2 * GEMM_BLOCK_M, p.block_n, p.fmt, p.a_mode == OP_MNMAJOR,
-                                        p.b_mode == OP_MNMAJOR);
-  const uint32_t a_lbo = (p.a_mode == OP_MNMAJOR) ? MN_ATOM_BYTES : 0;
-  const uint32_t b_lbo = (p.b_mode == OP_MNMAJOR) ? MN_ATOM_BYTES : 0;
-  const uint64_t a_kstep = ((p.a_mode == OP_MNMAJOR) ? 2048 : 32) >> 4;
-  const uint64_t b_kstep = ((p.b_mode == OP_MNMAJOR) ? 2048 : 32) >> 4;
-  const uint32_t smem0 = smem_u32(smem), full0 = smem_u32(full_bar), empty0 = smem_u32(empty_bar);
-  const uint64_t a_desc0 = make_smem_desc_sw128(smem0, a_lbo, 1024);
-  const uint64_t b_desc0 = make_smem_desc_sw128(smem0 + A_TILE_BYTES, b_lbo, 1024);
-  const uint64_t stage_step = stage_bytes >> 4;
-  int stage = 0;
-  uint32_t phase = 0;
-  int it = 0;
-  for (int tp = cluster_id; tp < total_pairs; tp += num_clusters, ++it) {
-    const int as = it & 1;
-    const uint32_t aphase = (it >> 1) & 1;
-    mbar_wait(&tmem_empty_bar[as], aphase ^ 1);
-    tc_fence_after();
-    const uint32_t d_tmem = tmem_base + static_cast<uint32_t>(as * p.block_n);
-    uint32_t acc = 0;
-    for (int kb = 0; kb < p.num_k_blocks; ++kb) {
-      mbar_wait_s(full0 + stage * 8, phase);
-      tc_fence_after();
-      const uint64_t ad = a_desc0 + stage * stage_step, bd = b_desc0 + stage * stage_step;
-      umma_f16_2sm(d_tmem, ad, bd, idesc, acc);
-      umma_f16_2sm(d_tmem, ad + a_kstep, bd + b_kstep, idesc, 1u);
-      umma_f16_2sm(d_tmem, ad + 2 * a_kstep, bd + 2 * b_kstep, idesc, 1u);
-      umma_f16_2sm(d_tmem, ad + 3 * a_kstep, bd + 3 * b_kstep, idesc, 1u);
-      acc = 1u;
-      umma_commit_2sm_s(empty0 + stage * 8, 3);  // frees the smem slot in both CTAs
-      if (++stage == p.stages) {
-        stage = 0;
-        phase ^= 1;
-      }
-    }
-    umma_commit_2sm(&tmem_full_bar[as], 3);
-  }
-}
-
-template <bool HAS_IN>
-__device__ __forceinline__ void gemm_tc2_body(const GemmParams& p) {
-  pdl_launch_dependents();
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base_u32 = smem_u32(smem_raw);
-  uint8_t* smem = smem_raw + (((smem_base_u32 + 1023u) & ~1023u) - smem_base_u32);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  const int half_n = p.block_n / 2;
-  const uint32_t b_bytes = static_cast<uint32_t>(half_n) * GEMM_BLOCK_K * 2;
-  const uint32_t stage_bytes = A_TILE_BYTES + b_bytes;
-
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + static_cast<size_t>(p.stages) * stage_bytes);
-  uint64_t* empty_bar = full_bar + GEMM_MAX_STAGES;
-  uint64_t* tmem_full_bar = empty_bar + GEMM_MAX_STAGES;
-  uint64_t* tmem_empty_bar = tmem_full_bar + 2;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tmem_empty_bar + 2);
-  float* tbuf_base = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(full_bar) + 256);
-
-  if (threadIdx.x == 0) {
-    prefetch_tmap(&p.tma_a);
-    prefetch_tmap(&p.tma_b);
-    for (int i = 0; i < p.stages; ++i) {
-      mbar_init(&full_bar[i], 1);   // leader's copy is the live one: one arrive.expect_tx covering both CTAs' bytes
-      mbar_init(&empty_bar[i], 1);  // one multicast tcgen05.commit per CTA
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full_bar[i], 1);
-      mbar_init(&tmem_empty_bar[i], 2 * GEMM_EPI_WARPS);  // leader's copy: epilogue warps of BOTH CTAs
-    }
-    fence_barrier_init();
-  }
-  if (warp == 1) tmem_alloc_2sm(tmem_ptr_smem, static_cast<uint32_t>(p.tmem_cols));
-  tc_fence_before();
-  cluster_sync_all();  // peer barriers initialised before any remote arrive / TMA signal
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  pdl_wait();
-
-  const PairInfo pinfo = pair_info(p);
-  const int cluster_id = pinfo.cluster_id, num_clusters = pinfo.num_clusters, pairs_m = pinfo.pairs_m,
-            total_pairs = pinfo.total_pairs;
-
-  if (warp == 0) {
-    if (lane == 0) producer2_loop(p, pinfo, smem, full_bar, empty_bar, stage_bytes);
-  } else if (warp == 1) {
-    if (lane == 0 && leader)
-      mma2_loop(p, pinfo, smem, full_bar, empty_bar, tmem_full_bar, tmem_empty_bar, tmem_base, stage_bytes);
-  } else {
-    const int ew = warp - 2;
-    const int q = warp & 3;
-    const int half = ew >> 2;
-    uint8_t* wbase = reinterpret_cast<uint8_t*>(tbuf_base) + static_cast<size_t>(ew) * TB_WARP_BYTES;
-    float* tb = reinterpret_cast<float*>(wbase);
-    long long* s_off = reinterpret_cast<long long*>(wbase + TB_FLOATS * 4);
-    int* s_row = reinterpret_cast<int*>(wbase + TB_FLOATS * 4 + 32 * 8);
-    const bool wide = (p.out_f32 != nullptr) || (p.res_f32 != nullptr);
-    int it = 0;
-    for (int tp = cluster_id; tp < total_pairs; tp += num_clusters, ++it) {
-      const int tn = tp % p.tiles_n, r = tp / p.tiles_n;
-      const int tm = 2 * (r % pairs_m) + (int)rank;
-      const TileCoord t = make_coord(p, tn, tm, r / pairs_m);
-      const int as = it & 1;
-      const uint32_t aphase = (it >> 1) & 1;
-      RowInfo ri = row_info(p, t, q * 32 + lane);
-      if (tm >= p.tiles_m) ri.off = -1;  // odd tile count: the peer's last tile does not exist
+    dump_acc(acc, acc_tile, ald, p.block_n);
+    named_bar_sync(1, GEMM_EPI_WARPS * 32);
+    if (TE != TE_NONE) {
+      tma_epilogue_tile<TE>(p, t, wbase, in_bars + warp * TE_BUFS, arow, warp, lane, cnt);
+    } else {
+      const RowInfo ri = row_info(p, t, q * 32 + lane);
       s_off[lane] = ri.off;
       s_row[lane] = ri.row;
       __syncwarp();
-      mbar_wait(&tmem_full_bar[as], aphase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>(as * p.block_n);
-      const int nslab = (p.block_n + 31) / 32;
-      const int col_limit = min(p.N, t.n0 + p.block_n);
-      const int kind = HAS_IN ? prefetch_kind(p) : 0;
-      for (int s = half; s < nslab; s += 2) {
-        float v[32];
-        if (wide) {
-          uint4 pf[BlockMap<4>::NIT];
-          if (HAS_IN) prefetch_block<4>(p, s_off, lane, t.n0 + s * 32, col_limit, kind, pf);
-          load_acc(taddr + s * 32, min(32, p.block_n - s * 32), v);
-          stage_rows(tb, v, lane);
-          epilogue_block<4>(p, tb, s_off, s_row, lane, t.n0 + s * 32, col_limit, kind, pf);
-        } else {
-          uint4 pf[BlockMap<8>::NIT];
-          if (HAS_IN) prefetch_block<8>(p, s_off, lane, t.n0 + s * 32, col_limit, kind, pf);
-          load_acc(taddr + s * 32, min(32, p.block_n - s * 32), v);
-          stage_rows(tb, v, lane);
-          epilogue_block<8>(p, tb, s_off, s_row, lane, t.n0 + s * 32, col_limit, kind, pf);
+      if (EPI == 1) {
+        if (half == 0) epilogue_softmax_fwd(p, tb, s_off, arow, lane);
+      } else if (EPI == 2) {
+        if (half == 0) epilogue_softmax_bwd(p, tb, s_off, arow, lane);
+      } else {
+        const int nslab = (p.block_n + 31) / 32;
+        const int col_limit = min(p.N, t.n0 + p.block_n);
+        const int kind = HAS_IN ? prefetch_kind(p) : 0;
+        const float* blk = acc_tile + q * 32 * ald;
+        for (int s = half; s < nslab; s += 2) {
+          if (wide) {
+            uint4 pf[BlockMap<4>::NIT];
+            if (HAS_IN) prefetch_block<4>(p, s_off, lane, t.n0 + s * 32, col_limit, kind, pf);
+            epilogue_block<4>(p, blk + s * 32, ald, s_off, s_row, lane, t.n0 + s * 32, col_limit, kind, pf);
+          } else {
+            uint4 pf[BlockMap<8>::NIT];
+            if (HAS_IN) prefetch_block<8>(p, s_off, lane, t.n0 + s * 32, col_limit, kind, pf);
+            epilogue_block<8>(p, blk + s * 32, ald, s_off, s_row, lane, t.n0 + s * 32, col_limit, kind, pf);
+          }
         }
-        __syncwarp();
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if (leader) mbar_arrive(&tmem_empty_bar[as]);
-        else mbar_arrive_cluster(&tmem_empty_bar[as], 0);
       }
     }
+    named_bar_sync(1, GEMM_EPI_WARPS * 32);  // the staged tile is free for the next tile's fragments
   }
-  tc_fence_before();
-  cluster_sync_all();  // the leader's MMAs read the peer's smem: nobody leaves before everything is consumed
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc_2sm(tmem_base, static_cast<uint32_t>(p.tmem_cols));
-  }
+  if (TE != TE_NONE && lane == 0) bulk_wait_group<0>();
 }
 
-// CTA pairs with the tensor-map epilogue: the pair halves the L2 -> SM operand traffic per FLOP (the single-CTA 128 x 256
-// tile is capped near 45 % of tensor peak by the ~43 B/clk/SM the L2 delivers), the epilogue keeps out of its way.
-template <int MODE>
-__device__ __forceinline__ void gemm_tce2_body(const GemmParams& p) {
-  pdl_launch_dependents();
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base_u32 = smem_u32(smem_raw);
-  uint8_t* smem = smem_raw + (((smem_base_u32 + 1023u) & ~1023u) - smem_base_u32);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const PairInfo pinfo = pair_info(p);
-  const uint32_t stage_bytes = A_TILE_BYTES + static_cast<uint32_t>(pinfo.half_n) * GEMM_BLOCK_K * 2;
-
-  uint8_t* bar_block = smem + static_cast<size_t>(p.stages) * stage_bytes;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(bar_block);
-  uint64_t* empty_bar = full_bar + GEMM_MAX_STAGES;
-  uint64_t* tmem_full_bar = empty_bar + GEMM_MAX_STAGES;
-  uint64_t* tmem_empty_bar = tmem_full_bar + 2;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tmem_empty_bar + 2);
-  uint64_t* in_bars = reinterpret_cast<uint64_t*>(bar_block + 256);
-  uint8_t* boxes = bar_block + TE_BAR_BYTES;
-
-  if (threadIdx.x == 0) {
-    prefetch_tmap(&p.tma_a);
-    prefetch_tmap(&p.tma_b);
-    prefetch_tmap(&p.tma_c);
-    if (MODE != TE_F16) prefetch_tmap(&p.tma_d);
-    for (int i = 0; i < p.stages; ++i) {
-      mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full_bar[i], 1);
-      mbar_init(&tmem_empty_bar[i], 2 * GEMM_EPI_WARPS);
-    }
-    for (int i = 0; i < GEMM_EPI_WARPS * TE_BUFS; ++i) mbar_init(&in_bars[i], 1);
-    fence_barrier_init();
-  }
-  if (warp == 1) tmem_alloc_2sm(tmem_ptr_smem, static_cast<uint32_t>(p.tmem_cols));
-  tc_fence_before();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  pdl_wait();
-
-  if (warp == 0) {
-    if (lane == 0) producer2_loop(p, pinfo, smem, full_bar, empty_bar, stage_bytes);
-  } else if (warp == 1) {
-    if (lane == 0 && pinfo.leader)
-      mma2_loop(p, pinfo, smem, full_bar, empty_bar, tmem_full_bar, tmem_empty_bar, tmem_base, stage_bytes);
-  } else {
-    const int ew = warp - 2;
-    tma_epilogue_loop<MODE, true>(p, boxes + static_cast<size_t>(ew) * TE_WARP_BYTES, in_bars + ew * TE_BUFS,
-                                  tmem_full_bar, tmem_empty_bar, tmem_base, warp, lane);
-  }
-  tc_fence_before();
-  cluster_sync_all();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc_2sm(tmem_base, static_cast<uint32_t>(p.tmem_cols));
-  }
-}
-
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GEMM_THREADS, 1)
-    gemm_tc2_kernel(const __grid_constant__ GemmParams p) {
-  gemm_tc2_body<false>(p);
-}
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GEMM_THREADS, 1)
-    gemm_tc2_in_kernel(const __grid_constant__ GemmParams p) {
-  gemm_tc2_body<true>(p);
-}
-
+template <int NF>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_constant__ GemmParams p) {
-  gemm_tc_body<0, false>(p);
+  gemm_body<0, false, TE_NONE, NF>(p);
 }
+template <int NF>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_in_kernel(const __grid_constant__ GemmParams p) {
-  gemm_tc_body<0, true>(p);
+  gemm_body<0, true, TE_NONE, NF>(p);
 }
 __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_softmax_fwd_kernel(const __grid_constant__ GemmParams p) {
-  gemm_tc_body<1, false>(p);
+  gemm_body<1, false, TE_NONE, 0>(p);
 }
 __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_softmax_bwd_kernel(const __grid_constant__ GemmParams p) {
-  gemm_tc_body<2, false>(p);
+  gemm_body<2, false, TE_NONE, 0>(p);
+}
+template <int MODE, int NF>
+__global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tce_kernel(const __grid_constant__ GemmParams p) {
+  gemm_body<0, false, MODE, NF>(p);
 }
 
-template <int MODE>
-__global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tce_kernel(const __grid_constant__ GemmParams p) {
-  gemm_tce_body<MODE>(p);
+// The kernel for a plan: fragment width NF (see mma_tile) and epilogue.
+template <int NF>
+void (*plain_kernel(const GemmParams& p))(GemmParams) {
+  switch (p.tma_epi) {
+    case TE_F16: return gemm_tce_kernel<TE_F16, NF>;
+    case TE_GELU: return gemm_tce_kernel<TE_GELU, NF>;
+    case TE_GELU_BWD: return gemm_tce_kernel<TE_GELU_BWD, NF>;
+    case TE_RES32: return gemm_tce_kernel<TE_RES32, NF>;
+    case TE_RES16: return gemm_tce_kernel<TE_RES16, NF>;
+    default: break;
+  }
+  if (p.res_f32 || p.res_f16 || p.act == ACT_QUICKGELU_BWD) return gemm_tc_in_kernel<NF>;
+  return gemm_tc_kernel<NF>;
 }
-template <int MODE>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GEMM_THREADS, 1)
-    gemm_tce2_kernel(const __grid_constant__ GemmParams p) {
-  gemm_tce2_body<MODE>(p);
+void (*kernel_for(const GemmParams& p))(GemmParams) {
+  if (p.tma_epi == TE_NONE && p.act == ACT_SOFTMAX) return gemm_tc_softmax_fwd_kernel;
+  if (p.tma_epi == TE_NONE && p.act == ACT_SOFTMAX_BWD) return gemm_tc_softmax_bwd_kernel;
+  if (p.fmt == 0 && p.block_n == 128) return plain_kernel<2>(p);
+  if (p.fmt == 0 && p.block_n == 64) return plain_kernel<1>(p);
+  return plain_kernel<0>(p);
 }
 
 // ------------------------------------------------------------------ host side
@@ -1387,28 +1018,18 @@ int tmap_encode_4d(CUtensorMap* out, const void* ptr, int fmt, const uint64_t di
   return encode_tmap4(out, ptr, fmt, dims, strides_elems, box, err, errlen);
 }
 
-// Measured on B200 (tests/test_gemm_gpu.py::test_gemm_throughput_report): CTA pairs are within +-8% of single-CTA tiles
-// on the CLIP GEMM shapes (ahead only at K = 3072), so single-CTA tiles stay the default; PXR_GEMM_CTA_GROUP=2 turns
-// pairs on wherever the tile shape allows it.
-int gemm_default_cta_group() {
-  static const int env_cg = [] {
-    const char* e = getenv("PXR_GEMM_CTA_GROUP");
-    return e && atoi(e) == 2 ? 2 : 1;
-  }();
-  return env_cg;
-}
-
 namespace {
-// CTA pairs need (see gemm_tc2_body): a generic epilogue, an even split of the B tile, at least two M tiles.
-int decide_cta_group(const GemmParams& p, const GemmEpilogue& epi, int block_n, int num_sms) {
+// Widest tile of the plain / tensor-map epilogue kernels: the staged fp32 accumulator tile (128 x block_n) shares the
+// 227 KiB of shared memory with the stage ring and the epilogue buffers, and at 128 columns three stages still fit.
+// The fused softmax epilogues need the whole row in one tile and may go to 256 columns (with a shorter ring).
+constexpr int GEMM_MAX_BN_PLAIN = 128;
+
+int effective_block_n(int block_n, const GemmEpilogue& epi) {
   const bool softmax_epi = epi.act == ACT_SOFTMAX || epi.act == ACT_SOFTMAX_BWD;
-  const bool can_pair = p.k_splits <= 1 && !softmax_epi && block_n % 32 == 0 && (p.b_mode != OP_MNMAJOR || block_n % 128 == 0) &&
-                        p.tiles_m >= 2 && num_sms >= 2;
-  const int want = epi.cta_group ? epi.cta_group : gemm_default_cta_group();
-  return (want == 1 || !can_pair) ? 1 : 2;
+  return (!softmax_epi && block_n > GEMM_MAX_BN_PLAIN) ? GEMM_MAX_BN_PLAIN : block_n;
 }
 
-// Tensor-map epilogue (see tma_epilogue_loop) when the epilogue is one of its shapes and every tensor can be described
+// Tensor-map epilogue (see tma_epilogue_tile) when the epilogue is one of its shapes and every tensor can be described
 // by a tensor map; anything else keeps the generic epilogue.  PXR_GEMM_TMA_EPI=0 disables it globally.
 int decide_tma_epi(const GemmParams& p, const GemmEpilogue& e, int block_n) {
   static const bool enabled = [] {
@@ -1506,16 +1127,16 @@ int finish_plan(GemmPlan* plan, const GemmEpilogue& epi, int block_n, int num_sm
     if (!rc && second) rc = encode_epilogue_map(&p.tma_d, second, f32, p, epi, err, errlen);
     if (rc) p.tma_epi = TE_NONE;  // a stride the tensor map cannot express: generic epilogue
   }
-  const int stage_bytes = A_TILE_BYTES + (p.cta_group == 2 ? block_n / 2 : block_n) * GEMM_BLOCK_K * 2;
-  const int epi_smem = p.tma_epi != TE_NONE ? TE_BAR_BYTES + GEMM_EPI_WARPS * TE_WARP_BYTES
-                                             : 256 + GEMM_EPI_WARPS * TB_WARP_BYTES;
+  const int stage_bytes = A_TILE_BYTES + block_n * GEMM_BLOCK_K * 2;
+  const int epi_smem = GEMM_BAR_BYTES + GEMM_BLOCK_M * acc_ld(block_n) * 4 +
+                       GEMM_EPI_WARPS * (p.tma_epi != TE_NONE ? TE_WARP_BYTES : TB_WARP_BYTES);
   int stages = (227 * 1024 - 1024 - epi_smem) / stage_bytes;
   if (stages > GEMM_MAX_STAGES) stages = GEMM_MAX_STAGES;
-  if (stages < 2) stages = 2;
+  if (stages < 1) {
+    set_err(err, errlen, "block_n too wide for shared memory");
+    return -13;
+  }
   p.stages = stages;
-  int cols = 32;
-  while (cols < 2 * block_n) cols <<= 1;
-  p.tmem_cols = cols;
   p.alpha = epi.alpha;
   p.n_store = epi.n_store > 0 ? epi.n_store : p.N;
   if ((epi.act == ACT_SOFTMAX || epi.act == ACT_SOFTMAX_BWD) && (p.tiles_n != 1 || !epi.out_f16)) {
@@ -1537,33 +1158,22 @@ int finish_plan(GemmPlan* plan, const GemmEpilogue& epi, int block_n, int num_sm
   p.vec_ok = (epi.ldc % 8 == 0) && (epi.bs0 % 8 == 0) && (epi.bs1 % 8 == 0) && aligned16(epi.aux_in) &&
              aligned16(epi.aux_out) && aligned16(epi.res_f32) && aligned16(epi.res_f16) && aligned16(epi.out_f32) &&
              aligned16(epi.out_f16);
-  if (p.cta_group == 2) {
-    const int batches = p.total_tiles / (p.tiles_m * p.tiles_n);
-    const int pairs = ((p.tiles_m + 1) / 2) * p.tiles_n * batches;
-    const int max_clusters = num_sms / 2;
-    plan->grid = 2 * (pairs < max_clusters ? pairs : max_clusters);
-  } else {
-    plan->grid = p.total_tiles < num_sms ? p.total_tiles : num_sms;
-  }
+  plan->grid = p.total_tiles < num_sms ? p.total_tiles : num_sms;
   plan->smem_bytes = stages * stage_bytes + 1024 + epi_smem;
   static std::once_flag once;
   std::call_once(once, [] {
-    cudaFuncSetAttribute(gemm_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    cudaFuncSetAttribute(gemm_tc_in_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    cudaFuncSetAttribute(gemm_tc2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    cudaFuncSetAttribute(gemm_tc2_in_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    for (int nf = 0; nf < 3; ++nf)
+      for (int te = TE_NONE; te <= TE_RES16; ++te)
+        for (int in = 0; in < 2; ++in) {
+          GemmParams q{};
+          q.fmt = 0;
+          q.block_n = nf == 2 ? 128 : (nf == 1 ? 64 : 16);
+          q.tma_epi = te;
+          q.act = in ? ACT_QUICKGELU_BWD : ACT_NONE;
+          cudaFuncSetAttribute(kernel_for(q), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+        }
     cudaFuncSetAttribute(gemm_tc_softmax_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     cudaFuncSetAttribute(gemm_tc_softmax_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    cudaFuncSetAttribute(gemm_tce_kernel<TE_F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    cudaFuncSetAttribute(gemm_tce_kernel<TE_GELU>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    cudaFuncSetAttribute(gemm_tce_kernel<TE_GELU_BWD>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    cudaFuncSetAttribute(gemm_tce_kernel<TE_RES32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    cudaFuncSetAttribute(gemm_tce_kernel<TE_RES16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    cudaFuncSetAttribute(gemm_tce2_kernel<TE_F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    cudaFuncSetAttribute(gemm_tce2_kernel<TE_GELU>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    cudaFuncSetAttribute(gemm_tce2_kernel<TE_GELU_BWD>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    cudaFuncSetAttribute(gemm_tce2_kernel<TE_RES32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    cudaFuncSetAttribute(gemm_tce2_kernel<TE_RES16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
   });
   return 0;
 }
@@ -1578,6 +1188,7 @@ int gemm_plan_make(GemmPlan* plan, const GemmOperand& A, const GemmOperand& B, i
     set_err(err, errlen, "use conv_plan_make for conv operands");
     return -20;
   }
+  block_n = effective_block_n(block_n, epi);
   p.M = M;
   p.N = N;
   p.fmt = fmt;
@@ -1612,8 +1223,7 @@ int gemm_plan_make(GemmPlan* plan, const GemmOperand& A, const GemmOperand& B, i
   }
   int rc = encode_operand(&p.tma_a, A, GEMM_BLOCK_M, fmt, err, errlen);
   if (rc) return rc;
-  p.cta_group = decide_cta_group(p, epi, block_n, num_sms);
-  rc = encode_operand(&p.tma_b, B, p.cta_group == 2 ? block_n / 2 : block_n, fmt, err, errlen);
+  rc = encode_operand(&p.tma_b, B, block_n, fmt, err, errlen);
   if (rc) return rc;
   plan->flops = 2.0 * M * N * K * nb0 * nb1;
   {
@@ -1639,6 +1249,7 @@ int conv_plan_make(GemmPlan* plan, const void* in, long long in_ld, int batch, i
   // M tile = tile_h x tile_w pixels (8 x 16 or 16 x 8).  Any W works: columns past the image are zero-filled by the
   // TMA loads and clipped by the stores (tensor-map epilogue) / predicated off (generic epilogue); pick the width that
   // wastes the fewest columns (pixray's presets give latents such as 9 x 9, 18 x 18, 12 x 6: pixray.py:1864-1878)
+  block_n = effective_block_n(block_n, epi);
   const int waste16 = (W + 15) / 16 * 16, waste8 = (W + 7) / 8 * 8;
   int tile_w = (waste16 <= waste8) ? 16 : 8;
   int tile_h = GEMM_BLOCK_M / tile_w;
@@ -1687,8 +1298,7 @@ int conv_plan_make(GemmPlan* plan, const void* in, long long in_ld, int batch, i
     B.ld = c_in;
     B.mn_extent = (long long)p.num_taps * cout_pad;
     B.k_extent = c_in;
-    p.cta_group = decide_cta_group(p, epi, block_n, num_sms);
-    int rc = encode_operand(&p.tma_b, B, p.cta_group == 2 ? block_n / 2 : block_n, fmt, err, errlen);
+    int rc = encode_operand(&p.tma_b, B, block_n, fmt, err, errlen);
     if (rc) return rc;
   }
   plan->flops = 2.0 * H * W * (double)n_out * c_in * p.num_taps * batch;
@@ -1764,46 +1374,12 @@ void splitk_reduce(const float* ws, int splits, long long pixels, int N, int ld_
                    const __half* res, __half* out, int ld_out, cudaStream_t stream) {
   const long long n = pixels * (N / 8);
   long long g = (n + 255) / 256;
-  if (g > 148 * 8) g = 148 * 8;
+  if (g > 132 * 8) g = 132 * 8;
   launch_pdl(splitk_reduce_kernel, dim3(static_cast<int>(g)), dim3(256), 0, stream, ws, splits, pixels, N, ld_ws, bias, res, out, ld_out);
 }
 
-#define PXR_LAUNCH_TCE2(MODE) \
-  launch_pdl(gemm_tce2_kernel<MODE>, dim3(plan.grid), dim3(GEMM_THREADS), plan.smem_bytes, stream, plan.p)
-
 void gemm_launch(const GemmPlan& plan, cudaStream_t stream) {
-  if (plan.p.tma_epi != TE_NONE && plan.p.cta_group == 2) {
-    switch (plan.p.tma_epi) {
-      case TE_F16: PXR_LAUNCH_TCE2(TE_F16); break;
-      case TE_GELU: PXR_LAUNCH_TCE2(TE_GELU); break;
-      case TE_GELU_BWD: PXR_LAUNCH_TCE2(TE_GELU_BWD); break;
-      case TE_RES32: PXR_LAUNCH_TCE2(TE_RES32); break;
-      default: PXR_LAUNCH_TCE2(TE_RES16); break;
-    }
-    return;
-  }
-  if (plan.p.tma_epi == TE_F16)
-    launch_pdl(gemm_tce_kernel<TE_F16>, dim3(plan.grid), dim3(GEMM_THREADS), plan.smem_bytes, stream, plan.p);
-  else if (plan.p.tma_epi == TE_GELU)
-    launch_pdl(gemm_tce_kernel<TE_GELU>, dim3(plan.grid), dim3(GEMM_THREADS), plan.smem_bytes, stream, plan.p);
-  else if (plan.p.tma_epi == TE_GELU_BWD)
-    launch_pdl(gemm_tce_kernel<TE_GELU_BWD>, dim3(plan.grid), dim3(GEMM_THREADS), plan.smem_bytes, stream, plan.p);
-  else if (plan.p.tma_epi == TE_RES32)
-    launch_pdl(gemm_tce_kernel<TE_RES32>, dim3(plan.grid), dim3(GEMM_THREADS), plan.smem_bytes, stream, plan.p);
-  else if (plan.p.tma_epi == TE_RES16)
-    launch_pdl(gemm_tce_kernel<TE_RES16>, dim3(plan.grid), dim3(GEMM_THREADS), plan.smem_bytes, stream, plan.p);
-  else if (plan.p.act == ACT_SOFTMAX)
-    launch_pdl(gemm_tc_softmax_fwd_kernel, dim3(plan.grid), dim3(GEMM_THREADS), plan.smem_bytes, stream, plan.p);
-  else if (plan.p.act == ACT_SOFTMAX_BWD)
-    launch_pdl(gemm_tc_softmax_bwd_kernel, dim3(plan.grid), dim3(GEMM_THREADS), plan.smem_bytes, stream, plan.p);
-  else if (plan.p.cta_group == 2 && (plan.p.res_f32 || plan.p.res_f16 || plan.p.act == ACT_QUICKGELU_BWD))
-    launch_pdl(gemm_tc2_in_kernel, dim3(plan.grid), dim3(GEMM_THREADS), plan.smem_bytes, stream, plan.p);
-  else if (plan.p.cta_group == 2)
-    launch_pdl(gemm_tc2_kernel, dim3(plan.grid), dim3(GEMM_THREADS), plan.smem_bytes, stream, plan.p);
-  else if (plan.p.res_f32 || plan.p.res_f16 || plan.p.act == ACT_QUICKGELU_BWD)
-    launch_pdl(gemm_tc_in_kernel, dim3(plan.grid), dim3(GEMM_THREADS), plan.smem_bytes, stream, plan.p);
-  else
-    launch_pdl(gemm_tc_kernel, dim3(plan.grid), dim3(GEMM_THREADS), plan.smem_bytes, stream, plan.p);
+  launch_pdl(kernel_for(plan.p), dim3(plan.grid), dim3(GEMM_THREADS), plan.smem_bytes, stream, plan.p);
 }
 
 }  // namespace pxr

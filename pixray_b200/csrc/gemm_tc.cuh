@@ -1,4 +1,4 @@
-// tcgen05 / TMA / TMEM GEMM for sm_100a: the one dense-contraction kernel of the engine.
+// wgmma / TMA GEMM for sm_90a: the one dense-contraction kernel of the engine.
 //
 //   D[m, n] = epilogue( alpha * sum_k A[m, k] * B[n, k] )          fp16 (or bf16) operands, fp32 accumulate
 //
@@ -9,10 +9,10 @@
 //   * 3x3 / 1x1 convolutions of the VQGAN decoder as implicit GEMM: the A operand is fetched by a 4-D TMA
 //     box (C, W, H, B) shifted per filter tap, out-of-image halo zero-filled by TMA.
 //
-// Structure: warp 0 = TMA producer, warp 1 = MMA issuer (+TMEM owner), warps 2..9 = epilogue (two per TMEM lane
-// quarter; accumulators are transposed through warp-private smem so every global access is coalesced).  smem ring of
-// `stages` {A 128x64, B block_n x 64} tiles (128-byte swizzle), two TMEM accumulator buffers so the epilogue of
-// tile i overlaps the main loop of tile i+1.
+// Structure: warps 0..7 = two MMA warpgroups (64 tile rows each, fp32 accumulators in registers) that then run the
+// epilogue, warp 8 = TMA producer.  smem ring of `stages` {A 128x64, B block_n x 64} tiles (128-byte swizzle); after the
+// main loop the fragments are staged as a row-major fp32 tile in shared memory, from which the epilogue warps read whole
+// rows and write coalesced, while the producer already streams the next tile's operands into the ring.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -27,7 +27,7 @@ enum EpiAct : int { ACT_NONE = 0, ACT_QUICKGELU = 1, ACT_QUICKGELU_BWD = 2, ACT_
 constexpr int GEMM_BLOCK_M = 128;
 constexpr int GEMM_BLOCK_K = 64;
 constexpr int GEMM_MAX_STAGES = 8;
-constexpr int GEMM_THREADS = 320;  // warp 0 TMA, warp 1 MMA, warps 2..9 epilogue
+constexpr int GEMM_THREADS = 288;  // warps 0..7 MMA + epilogue, warp 8 TMA
 
 struct GemmParams {
   CUtensorMap tma_a;
@@ -35,9 +35,8 @@ struct GemmParams {
   // tiling
   int M, N;            // logical output extent per batch (predication)
   int n_store;         // softmax epilogues: columns [N, n_store) are written as zeros (padded row pitch)
-  int block_n;         // multiple of 16, <= 256 (multiple of 64 when B is MN-major)
+  int block_n;         // multiple of 16, <= 128 (<= 256 for the softmax epilogues; multiple of 64 when B is MN-major)
   int stages;
-  int tmem_cols;       // power of two >= 2 * block_n
   int num_k_blocks;    // taps * k_blocks_per_tap
   int k_blocks_per_tap;
   int num_taps;        // 1 or 9
@@ -61,7 +60,6 @@ struct GemmParams {
   __half* out_f16;
   long long ldc, out_bs0, out_bs1;
   int vec_ok;          // 16-byte vector epilogue accesses allowed (alignment checked on host)
-  int cta_group;       // 1: one CTA per tile; 2: CTA pairs (cta_group::2) on 256 x block_n tile pairs
   // split-K (conv only): the "batch" index of a tile selects the k-block range [z * kb_per_split, ...) and the fp32
   // partial-sum slab z of the output workspace; k_splits == 1 otherwise
   int k_splits, kb_per_split;
@@ -98,7 +96,6 @@ struct GemmEpilogue {
   __half* out_f16 = nullptr;
   long long ldc = 0, bs0 = 0, bs1 = 0;
   int n_store = 0;  // softmax modes: zero-fill columns [N, n_store)
-  int cta_group = 0;  // 0 = auto, 1 / 2 = force
   int tma_epi = 0;    // 0 = auto (tensor-map epilogue when the tensors allow it), -1 = force the generic epilogue
   int k_splits = 1;   // conv_plan_make only: > 1 writes fp32 partial sums [k_splits][pixels][ldc] to out_f32
 };
@@ -131,11 +128,8 @@ void splitk_reduce(const float* ws, int splits, long long pixels, int N, int ld_
                    const __half* res, __half* out, int ld_out, cudaStream_t stream);
 
 // 4-D tiled tensor map, zero fill out of bounds, 128-byte swizzle (fmt 0 = fp16, 1 = bf16, 2 = fp32); strides in elements.
-// Shared with attn_tc.cu.  Returns 0 on success, otherwise writes a message to err.
+// Returns 0 on success, otherwise writes a message to err.
 int tmap_encode_4d(CUtensorMap* out, const void* ptr, int fmt, const uint64_t dims[4], const uint64_t strides_elems[3],
                    const uint32_t box[4], char* err, int errlen);
-
-// 1 (single-CTA tiles) unless PXR_GEMM_CTA_GROUP=2 asks for CTA pairs where the shape allows them.
-int gemm_default_cta_group();
 
 }  // namespace pxr

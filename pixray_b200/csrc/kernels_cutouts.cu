@@ -405,7 +405,7 @@ __global__ void __launch_bounds__(256) minmax_partial_kernel(const float* __rest
 // One block folds the per-block partial extremes.  (value, then the smaller element index on ties) is a total order, so the
 // fold is associative and commutative: any tree gives the same result.  1024 threads keep <= 4 partials each in flight
 // (all loads issued before the first compare) and finish with warp shuffles; the previous 256-thread version walked the
-// partials with dependent loads and folded 256 shared-memory slots serially in thread 0 (30 us under ncu, now ~4).
+// partials with dependent loads and folded 256 shared-memory slots serially in thread 0.
 constexpr int MMR_THREADS = 1024;
 __device__ __forceinline__ void mmr_take_min(float& v, int& i, float ov, int oi) {
   if (ov < v || (ov == v && oi < i)) {

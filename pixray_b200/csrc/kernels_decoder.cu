@@ -353,8 +353,8 @@ constexpr int GNC_THREADS = 1024;
 // an SM forever runs on the device -- the engine's stream runs one kernel at a time; under programmatic dependent launch the
 // previous kernel's blocks may still hold SMs when the first blocks of this one start, but they finish on their own, and
 // this kernel's own dependents are only released once every one of its blocks is resident (griddepcontrol.launch_dependents
-// is issued per block).  A plain launch plus this barrier is ~6 us cheaper per call than cudaLaunchCooperativeKernel +
-// grid.sync() (measured per op with CUDA events), which matters at 78 GroupNorm calls per iteration.  `counter` only ever
+// is issued per block).  A plain launch plus this barrier avoids the extra launch cost of cudaLaunchCooperativeKernel +
+// grid.sync(), which matters at 78 GroupNorm calls per iteration.  `counter` only ever
 // grows: the launcher passes the value it must reach (count before the launch + gridDim.x), so no reset and no generation
 // bit is needed.  The spin is bounded: ~2 s of SM clocks (2^32) without progress traps the kernel, so a violated invariant
 // (a debugger or sanitizer serialising blocks, a foreign persistent kernel on the device) surfaces as a launch failure on
@@ -378,7 +378,7 @@ __device__ __forceinline__ void gnc_grid_barrier(unsigned long long* counter, un
 // per-block fixed-order reduction of the thread partials s[half][a/b] to part_out[32 groups][2].
 // Threads (vc, pl) hold the sums of vector column vc over the pixels of plane pl: a fixed-shape binary tree over the
 // planes (plane = GNC_THREADS / vecs is a power of two for every supported C) -- log2(plane) barriers instead of a
-// serial walk over up to 64 planes by `vecs` threads (which was ~3 us of dependent shared-memory loads per call).
+// serial walk over up to 64 planes by `vecs` threads (a chain of dependent shared-memory loads).
 __device__ __forceinline__ void gnc_block_partials(const float (&s)[2][2], float* red, int vecs, int cpg,
                                                    float* __restrict__ part_out) {
   const int tid = threadIdx.x, vc = tid % vecs, pl = tid / vecs, plane = GNC_THREADS / vecs;
@@ -565,7 +565,7 @@ __global__ void __launch_bounds__(GNC_THREADS, 1)
   float* red = reinterpret_cast<float*>(gnc_smem);
   // The slab kept in shared memory between the two phases is dxh = dy * act'(a) * gamma (fp16), NOT x: the activation's
   // derivative (exp + reciprocal per element) is then evaluated once instead of once per phase -- at the 256^2 level the
-  // kernel was bound by exactly those instructions (33 us for 64 MB of L2 traffic) -- and phase 2 re-reads x from L2
+  // kernel is bound by exactly those instructions -- and phase 2 re-reads x from L2
   // in place of dy: the same bytes.  (cache_dy is ignored; kept in the signature for the launcher.)
   act_t* cg = reinterpret_cast<act_t*>(gnc_smem + 4 * GNC_THREADS * 4);
   __shared__ double acc4[GNC_THREADS];  // gnc_fold: [16 lanes][64 slots]

@@ -1,7 +1,7 @@
 // GroupNorm(32, C) for the small-spatial decoder levels, one thread-block CLUSTER per group (no grid-wide barrier).
 //
 // The single-kernel GroupNorm of kernels_decoder.cu splits the PIXELS over the grid, so every block owns a piece of every
-// group and the statistics need a grid-wide barrier (~9 us of launch + barrier latency per call; 52 such calls per config-2
+// group and the statistics need a grid-wide barrier (launch + barrier latency on every call; 52 such calls per config-2
 // iteration on tensors of 256 KB ... 2 MB).  Here the split is by GROUP: the cluster (1 ... 8 CTAs) of group g reads only
 // that group's channels, reduces (sum, sum of squares) over its own CTAs through distributed shared memory and applies --
 // nothing crosses clusters, so there is no global synchronisation at all.
@@ -310,10 +310,9 @@ GgLaunch gg_plan(int px, int C, bool any_size) {
   const int vpg = C / GG_G / 8;
   if (vpg != 1 && vpg != 2 && vpg != 4) return l;
   const long long upg = (long long)px * vpg;
-  // Measured on B200 (tests/test_groupnorm_gpu.py::test_groupnorm_timing_report, profiles/r02_gn_group_timing.log): the
-  // group split wins while a group is <= 2048 units (16^2 / 32^2 latents: 5.6 us per call against ~10 us for the
-  // grid-barrier kernel); beyond that the 16-byte reads at a pixel stride of C and the scheduling of 8-CTA clusters of
-  // 512 threads cost more than the barrier saves (px = 4096: 15 vs 11 us, px = 16384: 40 vs 16 us).
+  // The group split is used while a group is <= 2048 units (16^2 / 32^2 latents); beyond that the 16-byte reads at a
+  // pixel stride of C and the scheduling of 8-CTA clusters of 512 threads cost more than the grid barrier saves
+  // (tests/test_groupnorm_gpu.py::test_groupnorm_timing_report times both).
   static const long long max_units = [] {
     const char* e = getenv("PXR_GN_GROUP_MAX_UNITS");
     const long long v = e ? atoll(e) : 0;

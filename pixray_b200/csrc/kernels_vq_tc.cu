@@ -1,10 +1,10 @@
 // Nearest codebook row (vqgan.py:60-64) with the distance matrix on the tensor cores and the decision in exact fp32.
 //
 // vq_partial_kernel (kernels_decoder.cu) evaluates |x|^2 + |c|^2 - 2 x.c for all hw x n_e pairs with fp32 FMAs: 1.07 G FMAs =
-// 122 us at config 2 (256 positions, 16384 codes, 256 channels) for 2 GFLOP.  Here:
+// slow at config 2 (256 positions, 16384 codes, 256 channels) for 2 GFLOP.  Here:
 //   1. vq_prep: z [C, hw] fp32 -> zh [hw, C] fp16, each position scaled by a power of two into fp16's normal range;
 //      |x|^2 and the error-bound terms |x|_2, |x|_1 per position;
-//   2. one tcgen05 GEMM (gemm_tc.cu): scores[p, j] = zh[p, :] . cbh[j, :]  (fp16 operands, fp32 accumulate, 2 GFLOP);
+//   2. one wgmma GEMM (gemm_tc.cu): scores[p, j] = zh[p, :] . cbh[j, :]  (fp16 operands, fp32 accumulate, 2 GFLOP);
 //   3. vq_select: per position the approximate distances d~ = |c|^2 - 2 x.c~, their minimum, every code whose d~ lies
 //      within the ROUNDING BOUND of that minimum (a handful), and for those candidates the exact fp32 evaluation -- the
 //      same FMA chain over k = 0 .. C-1 and the same expression as vq_partial_kernel -- with first-index ties.  The true

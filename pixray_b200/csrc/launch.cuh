@@ -1,8 +1,8 @@
 // Programmatic dependent launch (PDL) for the engine's one-stream kernel chain.
 //
-// An iteration is ~450 dependent launches on ONE stream (profiles/r01_ncu_launches_c2_summary.txt); with plain
+// An iteration is ~450 dependent launches on ONE stream; with plain
 // stream order kernel N+1 is only scheduled once kernel N has fully drained, and its own prologue (block scheduling,
-// barrier init, TMEM allocation, tensor-map prefetch, parameter loads) then runs on an idle GPU.  With the
+// barrier init, tensor-map prefetch, parameter loads) then runs on an idle GPU.  With the
 // programmatic-serialization launch attribute the blocks of kernel N+1 are scheduled as soon as every block of kernel N
 // has STARTED (each kernel issues griddepcontrol.launch_dependents first thing) and SM resources free up; they run
 // their prologue and park at griddepcontrol.wait, which returns when kernel N has completed and flushed its memory.
@@ -10,7 +10,7 @@
 // Rules every kernel launched through launch_pdl() follows:
 //   * pdl_launch_dependents() at the top (the dependents' own griddepcontrol.wait keeps them correct);
 //   * pdl_wait() before the first access (read OR write) to memory another kernel of the chain produces or consumes;
-//     only kernel parameters, constant weights and the kernel's own shared memory / TMEM may be touched before it.
+//     only kernel parameters, constant weights and the kernel's own shared memory may be touched before it.
 // Kernels that are launched the plain way interoperate: they simply serialise fully.  PXR_PDL=0 turns the attribute off.
 #pragma once
 #include <cuda_runtime.h>

@@ -1,6 +1,6 @@
-// Thin inline-PTX wrappers for sm_100a: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (MMA / TMEM).
+// Thin inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), wgmma.
 // Everything here is device-side and header-only.  No CUTLASS dependency: the descriptor bit layouts
-// below restate the PTX ISA "tcgen05 shared-memory / instruction descriptor" tables.
+// below restate the PTX ISA "wgmma matrix descriptor" table.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -47,7 +47,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   }
 }
 
-// shared-space (u32 address) variants for the single-thread producer / MMA loops, where every instruction counts
+// shared-space (u32 address) variants for the single-thread producer loop, where every instruction counts
 __device__ __forceinline__ void mbar_wait_s(uint32_t bar, uint32_t parity) {
   uint32_t ok;
   do {
@@ -71,9 +71,6 @@ __device__ __forceinline__ void tma_load_4d_s(const CUtensorMap* m, uint32_t bar
       "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
-__device__ __forceinline__ void umma_commit_s(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
 
 // ---------------------------------------------------------------- TMA
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* m) {
@@ -94,59 +91,57 @@ __device__ __forceinline__ void tma_load_4d(const CUtensorMap* m, uint64_t* bar,
       : "memory");
 }
 
-// ---------------------------------------------------------------- tcgen05
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+// ---------------------------------------------------------------- wgmma (sm_90a warpgroup MMA)
+// Issued by all 128 threads of a warpgroup; D (fp32) lives in registers in the m64nNk16 fragment layout: register r of
+// thread t holds row 16 (t / 32) + (t % 32) / 4 + 8 ((r / 2) % 2), column 8 (r / 4) + 2 (t % 4) + r % 2.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// D (+)= A[smem desc] * B[smem desc]; TA / TB = 1: that operand is MN-major in shared memory.  scale_d = 0 overwrites D.
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n64(float* d, uint64_t adesc, uint64_t bdesc, uint32_t scale_d, int bf16) {
+  if (bf16) {
+      asm volatile(
+          "{\n\t.reg .pred p;\n\t"
+          "setp.ne.b32 p, %34, 0;\n\t"
+          "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+          "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n\t}"
+          : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+          : "l"(adesc), "l"(bdesc), "r"(scale_d), "n"(TA), "n"(TB));
+  } else {
+      asm volatile(
+          "{\n\t.reg .pred p;\n\t"
+          "setp.ne.b32 p, %34, 0;\n\t"
+          "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+          "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n\t}"
+          : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+          : "l"(adesc), "l"(bdesc), "r"(scale_d), "n"(TA), "n"(TB));
+  }
+}
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n16(float* d, uint64_t adesc, uint64_t bdesc, uint32_t scale_d, int bf16) {
+  if (bf16) {
+      asm volatile(
+          "{\n\t.reg .pred p;\n\t"
+          "setp.ne.b32 p, %10, 0;\n\t"
+          "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 "
+          "{%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, %11, %12;\n\t}"
+          : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+          : "l"(adesc), "l"(bdesc), "r"(scale_d), "n"(TA), "n"(TB));
+  } else {
+      asm volatile(
+          "{\n\t.reg .pred p;\n\t"
+          "setp.ne.b32 p, %10, 0;\n\t"
+          "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 "
+          "{%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, %11, %12;\n\t}"
+          : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+          : "l"(adesc), "l"(bdesc), "r"(scale_d), "n"(TA), "n"(TB));
+  }
+}
 
-// Whole warp. Writes the TMEM base address (lane<<16 | column) to *dst_smem.
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
-// D[tmem] (+)= A[smem desc] * B[smem desc], fp16/bf16 inputs, fp32 accumulate. One thread issues.
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                         uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier once all previously issued tcgen05.mma of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// TMEM -> registers: 32 lanes x 16 consecutive 32-bit columns; thread i gets lane (base+i).
-__device__ __forceinline__ void tmem_ld_x16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
-      "[%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-// 32 lanes x 32 consecutive 32-bit columns
-__device__ __forceinline__ void tmem_ld_x32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
@@ -156,34 +151,16 @@ __device__ __forceinline__ float ex2_approx(float x) {
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
-// Shared-memory matrix descriptor (sm_100 "version 1"), 128-byte swizzle.
+// Shared-memory matrix descriptor (sm_90 wgmma), 128-byte swizzle.
 //   bits [0,14)  start address >> 4        bits [16,30) leading-dim byte offset >> 4
-//   bits [32,46) stride-dim byte offset>>4 bits [46,48) version = 1
-//   bits [61,64) layout type (2 = SWIZZLE_128B)
+//   bits [32,46) stride-dim byte offset>>4 bits [62,64) layout type (1 = SWIZZLE_128B)
 __device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
-  return d;
-}
-
-// Instruction descriptor for kind::f16: fp32 accumulate, A/B both `fmt` (0 = f16, 1 = bf16).
-//   bits [4,6) c_format (1 = F32)   bits [7,10) a_format   bits [10,13) b_format
-//   bit 15 a_major (1 = MN-major)   bit 16 b_major          bits [17,23) N>>3   bits [24,29) M>>4
-__host__ __device__ __forceinline__ uint32_t make_idesc_f16(int m, int n, int fmt, int a_mn_major, int b_mn_major) {
-  uint32_t d = 0;
-  d |= 1u << 4;
-  d |= static_cast<uint32_t>(fmt & 7) << 7;
-  d |= static_cast<uint32_t>(fmt & 7) << 10;
-  d |= static_cast<uint32_t>(a_mn_major & 1) << 15;
-  d |= static_cast<uint32_t>(b_mn_major & 1) << 16;
-  d |= static_cast<uint32_t>((n >> 3) & 0x3F) << 17;
-  d |= static_cast<uint32_t>((m >> 4) & 0x1F) << 24;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
 
@@ -204,77 +181,6 @@ __device__ __forceinline__ void bulk_wait_group() {
   asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
 }
 
-
-// ---------------------------------------------------------------- 2-CTA (cta_group::2) variants
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// TMA load executed by either CTA of the pair; the transaction bytes are signalled on the LEADER's mbarrier
-// (shared::cluster address with the CTA-rank bit cleared, as CUTLASS' SM100_TMA_2SM_LOAD does).
-__device__ __forceinline__ void tma_load_4d_2sm(const CUtensorMap* m, uint64_t* bar_local, void* dst, int c0, int c1,
-                                                int c2, int c3) {
-  const uint32_t bar = smem_u32(bar_local) & 0xFEFFFFFFu;
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, "
-      "%5, %6}], [%2];" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_2sm_s(const CUtensorMap* m, uint32_t bar_local, uint32_t dst, int c0, int c1,
-                                                  int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, "
-      "%5, %6}], [%2];" ::"r"(dst),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_local & 0xFEFFFFFFu), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_2sm_s(uint32_t bar, uint16_t mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-      "h"(mask)
-      : "memory");
-}
-__device__ __forceinline__ void umma_f16_2sm(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive (once all prior MMAs of this thread are done) on the barrier at the same smem offset in every CTA of `mask`
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar, uint16_t mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(mask)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// arrive on the barrier at the same smem offset in CTA `rank` of the cluster
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar_local, uint32_t rank) {
-  asm volatile(
-      "{\n\t.reg .b32 r;\n\t"
-      "mapa.shared::cluster.u32 r, %0, %1;\n\t"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [r];\n\t}" ::"r"(smem_u32(bar_local)),
-      "r"(rank)
-      : "memory");
-}
 
 }  // namespace ptx
 }  // namespace pxr

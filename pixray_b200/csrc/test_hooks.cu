@@ -17,7 +17,7 @@ static int num_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (g_num_sms <= 0) g_num_sms = 148;
+    if (g_num_sms <= 0) g_num_sms = 132;
   }
   return g_num_sms;
 }
@@ -37,7 +37,6 @@ static void fill_epilogue(GemmEpilogue& e, const pxr_test_gemm_desc* d) {
   e.bs0 = d->c_bs0;
   e.bs1 = d->c_bs1;
   e.n_store = d->n_store;
-  e.cta_group = d->cta_group;
   e.tma_epi = d->tma_epi;
 }
 

@@ -35,7 +35,7 @@ class B200Engine:
                  clip=(), noise_fac=0.1, seed=0, device=0, rank=0, world=1, grad_scale=0.0, lr_betas=(0.9, 0.999),
                  adam_eps=1e-8, fft_decay=0.0, fft_colors=0.0, fft_contrast=0.0, cut_aspect=1.0):
         if not torch.cuda.is_available():
-            raise EngineError("pixray_b200 needs a CUDA device (B200); there is no CPU fallback")
+            raise EngineError("pixray_b200 needs a CUDA device (H100); there is no CPU fallback")
         self.lib = _lib.load()
         cfg = _lib.Config()
         cfg.device, cfg.rank, cfg.world = device, rank, world

@@ -1,4 +1,4 @@
-"""pixray's filter plugins (filters/FilterInterface.py:4-16 and filters/{tiler,wallpaper,colorlookup}.py) on the B200 engine.
+"""pixray's filter plugins (filters/FilterInterface.py:4-16 and filters/{tiler,wallpaper,colorlookup}.py) on the H100 engine.
 
 The reference applies them to drawer.synth's output before MakeCutouts (do_synth_and_filter, pixray.py:1203-1222): each is an
 nn.Module whose forward(img) returns (img, loss).  Here a filter instance describes itself to the engine (pxr_add_filter): the

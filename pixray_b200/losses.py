@@ -1,4 +1,4 @@
-"""The reference's auxiliary losses (Losses/*.py, registered in pixray.loss_class_table, pixray.py:131-140) on the B200
+"""The reference's auxiliary losses (Losses/*.py, registered in pixray.loss_class_table, pixray.py:131-140) on the H100
 engine.  Same class names, `add_settings` arguments and `parse_settings` behaviour as the reference; the difference is
 where the arithmetic runs: the reference's `get_loss` returns an autograd tensor, here `attach()` installs the loss
 inside the engine (one fused loss + gradient kernel per loss, pixray_b200/csrc/kernels_losses.cu) and `get_loss`

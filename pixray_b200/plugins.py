@@ -1,4 +1,4 @@
-"""pixray's plugin surface (SURVEY.md 8b) on top of the B200 engine.
+"""pixray's plugin surface (SURVEY.md 8b) on top of the H100 engine.
 
 Same class / method names, argument meaning and error behaviour as the reference, so a pixray loop written against
 `drawer.synth`, `MakeCutouts.__call__`, `perceptor.encode_image`, `Prompt.__call__`, `opt.step()` / `drawer.clip_z()`

@@ -1,4 +1,4 @@
-"""Fused tcgen05 attention (pixray_b200/csrc/attn_tc.cu) against a torch fp32 restatement of nn.MultiheadAttention's
+"""Fused tensor-core attention (pixray_b200/csrc/attn_tc.cu) against a torch fp32 restatement of nn.MultiheadAttention's
 core (SLIP/models.py:18-64 residual blocks call it with need_weights=False): S = q k^T / sqrt(d), P = softmax(S),
 O = P v, and its backward.  Tolerances: fp16 operands / fp32 accumulate vs fp32 math on the same fp16 inputs."""
 import ctypes as C

@@ -214,7 +214,7 @@ def test_iteration_gradient_with_color_jitter():
     channel, hue sector, the saturation clamp).  The device body uses exactly-rounded fp32 operations, so it lands on the
     same piece as the oracle whenever it sees the same colour (test_zz_host_paths: device vs host body, 0 pixels off-piece;
     round 1's 2.5e-2 gap was __fdividef / FMA contraction flipping the sector at saturated-channel ties, see
-    profiles/r02_jitter_gap_diagnosis.log).
+    tests/diag_color_jitter.py).
       (a) decisive: the ORACLE's image goes into the engine's cutouts -> the jittered batch matches to 2e-4 and d loss / d
           image to 5e-3 of max (measured 1.6e-3, the level of the un-jittered path);
       (b) whole chain from z: the engine's fp16 decoder image differs from the oracle's by ~1e-3 before the clamp, which

@@ -1,4 +1,9 @@
-"""GPU parity of the tcgen05 GEMM / implicit-GEMM conv kernel against torch fp32 matmul of the same fp16 inputs."""
+"""GPU parity of the wgmma GEMM / implicit-GEMM conv kernel against torch fp32 matmul of the same fp16 inputs.
+
+`cg` is the C ABI's cta_group request: sm_90 has no CTA-pair MMA, so cg=2 must be accepted and runs the same single-CTA
+tiles as cg=1 (the axis checks that the request stays harmless).  Plain-epilogue tiles are at most 128 columns wide: a
+requested block_n of 192 or 256 runs as 128.  Widths other than 64 / 128 (e.g. 16, 80, 112, 208) take the generic
+fragment path."""
 import pytest
 import torch
 import torch.nn.functional as F
@@ -21,10 +26,10 @@ def _check(out, ref, tol, name):
 
 @pytest.mark.parametrize("cg", [1, 2])
 @pytest.mark.parametrize("M,N,K,bn", [(300, 256, 192, 128), (128, 64, 64, 64), (197, 197, 64, 208), (1000, 768, 768, 256),
-                                      (1000, 768, 768, 192), (2000, 100, 320, 64)])
+                                      (1000, 768, 768, 192), (2000, 100, 320, 64), (700, 400, 448, 80),
+                                      (500, 336, 320, 112)])
 def test_gemm_kmajor(M, N, K, bn, cg):
-    """cg=1: one CTA per 128 x bn tile; cg=2: CTA pairs on 256 x bn tile pairs (tcgen05 cta_group::2) where the shape
-    allows it (falls back to single-CTA tiles otherwise, e.g. one M tile or bn % 32 != 0)."""
+    """One CTA per 128 x bn tile (bn clamped to 128 for this epilogue); cg=2 runs the same tiles."""
     torch.manual_seed(0)
     A, B = _rand(M, K), _rand(N, K)
     out = torch.full((M, N), 7.0, device="cuda")
@@ -158,6 +163,26 @@ def test_gemm_fused_softmax_forward_and_backward():
     dSref = 0.125 * Pf * (dP - (Pf * dP).sum(-1, keepdim=True))
     _check(dS[..., :T], dSref, 4e-3, "fused softmax bwd")
     assert dS[..., T:].abs().max().item() == 0.0
+
+
+def test_gemm_fused_softmax_with_several_k_blocks():
+    """Softmax epilogues on 256-wide rows, where the staged accumulator tile leaves room for a single stage, with
+    K = 192 (three k-blocks through that one slot)."""
+    torch.manual_seed(10)
+    heads, T, K, ldp = 2, 256, 192, 256
+    A, B = _rand(heads, T, K, scale=0.3), _rand(heads, T, K, scale=0.3)
+    P = torch.full((heads, T, ldp), 7.0, device="cuda", dtype=torch.half)
+    run_gemm(A, B, T, T, K, lda=K, ldb=K, nb0=heads, a_bs=(T * K, 0), b_bs=(T * K, 0), b_batched=1, block_n=256,
+             alpha=0.125, act=3, n_store=ldp, out_f16=P, ldc=ldp, c_bs=(T * ldp, 0))
+    Pref = torch.softmax(0.125 * A.float() @ B.float().transpose(-1, -2), dim=-1)
+    _check(P, Pref, 2e-3, "fused softmax fwd, 3 k-blocks")
+    G = _rand(heads, T, K, scale=0.3)
+    dS = torch.full((heads, T, ldp), 7.0, device="cuda", dtype=torch.half)
+    run_gemm(G, B, T, T, K, lda=K, ldb=K, nb0=heads, a_bs=(T * K, 0), b_bs=(T * K, 0), b_batched=1, block_n=256,
+             alpha=0.125, act=4, aux_in=P, n_store=ldp, out_f16=dS, ldc=ldp, c_bs=(T * ldp, 0))
+    dP = G.float() @ B.float().transpose(-1, -2)
+    Pf = P.float()
+    _check(dS, 0.125 * Pf * (dP - (Pf * dP).sum(-1, keepdim=True)), 4e-3, "fused softmax bwd, 3 k-blocks")
 
 
 @pytest.mark.parametrize("cg", [1, 2])

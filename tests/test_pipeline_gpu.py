@@ -88,8 +88,8 @@ class _ClampSided(torch.autograd.Function):
 def vqgan_synth_with_engine_clamp_sides(vq, eng, image_hw):
     """ClampWithGrad's backward is discontinuous in the unclamped image: a pixel within the engine's fp16 forward error
     (~1.5e-3) of 0 or 1 can sit on the other side of the clamp in the engine, and then a whole pixel's gradient is kept
-    on one side and dropped on the other (measured on the 48x32 canvas: ONE such pixel moves z.grad by 3e-2 of its maximum;
-    profiles/r02_aspect_diag_clamp.log).  Returns (synth, n_flipped): the oracle's synth evaluated on the piece of the
+    on one side and dropped on the other (on the 48x32 canvas ONE such pixel moves z.grad by 3e-2 of its maximum;
+    tests/diag_aspect.py).  Returns (synth, n_flipped): the oracle's synth evaluated on the piece of the
     function the engine is on -- identical to R.vqgan_synth wherever the sides agree."""
     H, W = image_hw
     pre_e = eng.debug_read("img_pre", (1, 3, H, W)).cpu()

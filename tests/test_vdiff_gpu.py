@@ -8,7 +8,7 @@ checkpoint's keys.  Tolerances (fp16 tensor-core operands / fp32 accumulation vs
 
 z.grad: the U-Net's 111 ReLUs make its backward DISCONTINUOUS in the forward activations: a pre-activation within the
 fp16 forward error (~1e-3 of the activation scale) of zero takes the other branch than in the fp32 oracle, and every such
-element changes its gradient entry by O(1).  profiles/r01_vdiff_layer_parity.log shows this entering block by block
+element changes its gradient entry by O(1).  tools/vdiff_layers.py shows this entering block by block
 (forward taps agree to 1e-3 everywhere; gradient taps drift to ~5e-2 rel-L2 through the 56 blocks), independent of the
 gradient scale.  The smooth drawers (swish / QuickGELU) do not have this effect and keep 3e-2; here the stated bound is
 max-abs-err <= 8e-2 max|z.grad|, relative L2 error <= 0.12 and cosine similarity >= 0.99 -- the reference's own CUDA path

@@ -1,5 +1,5 @@
 """BASELINE configs 3 and 5 on the GPUs the launcher gives it (informational; bench.py measures config 2, the
-configuration BASELINE.json's metric is quoted on).  NOT yet run on a B200 -- written after round 1's GPU budget.
+configuration BASELINE.json's metric is quoted on).
 
     python tools/bench_configs.py c3 [steps]        # vqgan 512x512, ViT-B/16 + ViT-B/32, cutn=128 (cutouts sharded over ranks)
     python tools/bench_configs.py c5 [steps]        # fft 512x512, ViT-L/14, cutn=256 (one problem per GPU: replicas)

@@ -1,5 +1,5 @@
 """The CLIP ViT-B/16 cutn=64 GEMM shapes with their pipeline epilogues, one launch each through the pxr_test_gemm hook
--- the target for `ncu --set full -k regex:gemm_tc` (see profiles/README.md).  Prints the launch order."""
+-- the target for `ncu --set full -k regex:gemm_tc`.  Prints the launch order."""
 import os
 import sys
 

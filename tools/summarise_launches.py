@@ -1,7 +1,7 @@
 """Aggregate an ncu launch list (`--metrics gpu__time_duration.sum,dram__bytes_read.sum,dram__bytes_write.sum --csv`) of
-tools/profile_c2.py into the per-kernel summary and the tcgen05-family DRAM traffic bench.py reports as roofline.traffic.
+tools/profile_c2.py into the per-kernel summary and the GEMM-family DRAM traffic per launch.
 
-    python tools/summarise_launches.py gpurun_out/launches.csv profiles/r02_ncu_launches_c2
+    python tools/summarise_launches.py launches.csv out_prefix
 
 Keeps the LAST complete iteration (from the last-but-one vq_prep_kernel / vq_partial_kernel launch to the last one)."""
 import csv
