@@ -319,6 +319,19 @@ int pxr_test_groupnorm(int variant, const void* x, const float* ws, int splits, 
                        float* stats, const void* dy, const float* ws_dy, int splits_dy, const void* dres, void* dx,
                        float* scratch, int repeat);
 
+/* the row softmax of the unfused attention on DEVICE fp16 [rows, ld] (ld % 8 == 0, cols <= ld; pad columns come back
+ * 0): backward == 0 turns the scores in p_or_s into probabilities in place; backward != 0 overwrites dp (dP) with
+ * dS = P * (dP - <P, dP>), P in p_or_s.  Synchronous on the default stream. */
+int pxr_test_softmax(int backward, void* p_or_s, void* dp, int rows, int cols, int ld);
+
+/* one CLIP LayerNorm kernel chosen explicitly -- variant 0: fp32 residual stream, 1: fp16 stream with 8-byte vectors,
+ * 2: fp16 stream with 16-byte vectors (W % 256 == 0, no pos, fp16 output only) -- forward, or backward (accumulate
+ * adds into gx / gx16).  Arguments as the engine's layernorm_forward / layernorm_backward; x is fp32 for variant 0 and
+ * fp16 otherwise; y16, dy, gx16 fp16; all DEVICE.  Returns -1 when the variant has no kernel for the width. */
+int pxr_test_layernorm(int variant, int backward, const void* x, long long x_stride, const float* pos, int T,
+                       const float* gamma, const float* beta, int rows, int W, float eps, void* y16, float* y32,
+                       float* stats, const void* dy, int accumulate, float* gx, void* gx16);
+
 #ifdef __cplusplus
 }
 #endif

@@ -1512,7 +1512,11 @@ void Engine::build_clip(int i) {
   const int mod = PXR_MOD_CLIP0 + i;
   const int Wd = C.c.width, L = C.c.layers, Hh = C.c.heads, P = C.c.patch, D = C.c.out_dim;
   if (C.c.image_res != cfg.cut_size) throw EngineError(-50, "clip image_res must equal cut_size");
-  if (Wd % 64 || Wd > 1024 || Wd / Hh != 64) throw EngineError(-51, "ViT width must be a multiple of 64 (<=1024) with 64-wide heads");
+  // a LayerNorm warp gives each lane whole 4-element vectors of every 128-column slice of the row
+  if (Wd % 128 || Wd > 1024 || Wd != 64 * Hh)
+    throw EngineError(-51, "ViT width " + std::to_string(Wd) + " with " + std::to_string(Hh) +
+                               " heads: the width must be a multiple of 128 (the LayerNorm granularity), <= 1024, "
+                               "with 64-wide heads");
   if (P < 2 || cfg.cut_size % P) throw EngineError(-52, "patch size must divide cut_size");
   const int gp = cfg.cut_size / P, np = gp * gp, T = np + 1, B = n_local, M = B * T, d = 64;
   const int Kp = round_up(3 * P * P, 64), ldT = round_up(T, 8);

@@ -180,24 +180,35 @@ void cutout_backward(const CutoutArgs& a, const float* g_batch, const float* ran
 
 // ------------------------------------------------------------------ CLIP ViT (slip.py:62-66; SLIP/models.py:18-64)
 // y = LN(x [+ pos[row % T]]) * gamma + beta ; x fp32 [rows, W]; outputs optional fp16 / fp32; stats [rows][2]
-// W in {128, 256, 512, 768, 1024}; row r of x starts at x + r * x_stride (class-token rows: stride T * W)
-void layernorm_forward(const float* x, long long x_stride, const float* pos, int T, const float* gamma,
-                       const float* beta, int rows, int W, float eps, act_t* y16, float* y32, float* stats,
-                       cudaStream_t st);
+// W = 128 * k, k in [1, 8]; row r of x starts at x + r * x_stride (class-token rows: stride T * W).
+// All four return 0, or -1 without launching anything when W has no kernel.
+int layernorm_forward(const float* x, long long x_stride, const float* pos, int T, const float* gamma,
+                      const float* beta, int rows, int W, float eps, act_t* y16, float* y32, float* stats,
+                      cudaStream_t st);
 // the same on an fp16 residual stream (x fp16)
-void layernorm_forward(const act_t* x, long long x_stride, const float* pos, int T, const float* gamma,
-                       const float* beta, int rows, int W, float eps, act_t* y16, float* y32, float* stats,
-                       cudaStream_t st);
+int layernorm_forward(const act_t* x, long long x_stride, const float* pos, int T, const float* gamma,
+                      const float* beta, int rows, int W, float eps, act_t* y16, float* y32, float* stats,
+                      cudaStream_t st);
 // gx (+)= LN'(x) applied to dy (fp16, scaled); also writes gx16 = fp16(gx).  accumulate=0 overwrites gx.
 // dy is compact [rows, W]; x, gx, gx16 rows are x_stride apart
-void layernorm_backward(const act_t* dy, const float* x, long long x_stride, const float* pos, int T,
-                        const float* stats, const float* gamma, int rows, int W, int accumulate, float* gx,
-                        act_t* gx16, cudaStream_t st);
+int layernorm_backward(const act_t* dy, const float* x, long long x_stride, const float* pos, int T,
+                       const float* stats, const float* gamma, int rows, int W, int accumulate, float* gx,
+                       act_t* gx16, cudaStream_t st);
 // fp16 residual stream: x fp16; with gx == nullptr the stream gradient lives in gx16 alone (accumulate reads it there)
-void layernorm_backward(const act_t* dy, const act_t* x, long long x_stride, const float* pos, int T,
-                        const float* stats, const float* gamma, int rows, int W, int accumulate, float* gx,
-                        act_t* gx16, cudaStream_t st);
-// in-place row softmax over the first `cols` of each row of length ld (pad columns zeroed); rows total
+int layernorm_backward(const act_t* dy, const act_t* x, long long x_stride, const float* pos, int T,
+                       const float* stats, const float* gamma, int rows, int W, int accumulate, float* gx,
+                       act_t* gx16, cudaStream_t st);
+// One LayerNorm kernel family chosen explicitly (the functions above choose by stream type and PXR_LN16_WIDE):
+//   LN_F32_STREAM: fp32 x; LN_F16_VEC4: fp16 x, 8-byte vectors; LN_F16_VEC8: fp16 x, 16-byte vectors (W % 256 == 0,
+//   no pos, fp16 output / gradient only).  -1 when the variant has no kernel for these arguments.
+enum { LN_F32_STREAM = 0, LN_F16_VEC4 = 1, LN_F16_VEC8 = 2 };
+int layernorm_forward_variant(int variant, const void* x, long long x_stride, const float* pos, int T, const float* gamma,
+                              const float* beta, int rows, int W, float eps, act_t* y16, float* y32, float* stats,
+                              cudaStream_t st);
+int layernorm_backward_variant(int variant, const act_t* dy, const void* x, long long x_stride, const float* pos, int T,
+                               const float* stats, const float* gamma, int rows, int W, int accumulate, float* gx,
+                               act_t* gx16, cudaStream_t st);
+// in-place row softmax over the first `cols` of each row of length ld (pad columns zeroed); rows total; any ld % 8 == 0
 void softmax_forward(act_t* s, int rows, int cols, int ld, cudaStream_t st);
 void softmax_backward(const act_t* p, act_t* dp_to_ds, int rows, int cols, int ld, cudaStream_t st);
 // Prompt.forward for all prompts of one perceptor + its gradient w.r.t. the un-normalised embeds.

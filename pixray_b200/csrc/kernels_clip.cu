@@ -386,6 +386,74 @@ __global__ void __launch_bounds__(256) softmax_bwd_kernel(const act_t* __restric
   }
 }
 
+__device__ __forceinline__ void ld_half8(const act_t* p, float (&f)[8]) { ln_unpack8(*reinterpret_cast<const uint4*>(p), f); }
+
+// rows longer than the register-resident kernels above hold (ld > 1024): the warp walks the row in 256-column steps (one
+// 16-byte vector per lane) keeping a per-lane running max and a sum rescaled to it, combines the lanes, then reads the
+// row again to write the probabilities.  Any ld % 8 == 0.
+__global__ void __launch_bounds__(256) softmax_fwd_long_kernel(act_t* __restrict__ s, long long rows, int cols, int ld) {
+  pdl_prologue();
+  const long long row = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (row >= rows) return;
+  act_t* r = s + row * ld;
+  const int nvec = ld / 8;
+  float m = -FLT_MAX, sum = 0.f;
+  for (int vi = lane; vi < nvec; vi += 32) {
+    float v[8];
+    ld_half8(r + vi * 8, v);
+    float cm = -FLT_MAX;
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+      if (vi * 8 + j < cols) cm = fmaxf(cm, v[j]);
+    if (cm > m) {
+      sum *= __expf(m - cm);
+      m = cm;
+    }
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+      if (vi * 8 + j < cols) sum += __expf(v[j] - m);
+  }
+  const float mx = warp_max(m);
+  const float inv = 1.f / warp_sum(sum > 0.f ? sum * __expf(m - mx) : 0.f);
+  for (int vi = lane; vi < nvec; vi += 32) {
+    float v[8];
+    ld_half8(r + vi * 8, v);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) v[j] = (vi * 8 + j < cols) ? __expf(v[j] - mx) * inv : 0.f;
+    *reinterpret_cast<uint4*>(r + vi * 8) = ln_pack8(v);
+  }
+}
+
+__global__ void __launch_bounds__(256) softmax_bwd_long_kernel(const act_t* __restrict__ p, act_t* __restrict__ dp,
+                                                               long long rows, int cols, int ld) {
+  pdl_prologue();
+  const long long row = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (row >= rows) return;
+  const act_t* pr = p + row * ld;
+  act_t* dr = dp + row * ld;
+  const int nvec = ld / 8;
+  float dot = 0.f;
+  for (int vi = lane; vi < nvec; vi += 32) {
+    float a[8], b[8];
+    ld_half8(pr + vi * 8, a);
+    ld_half8(dr + vi * 8, b);
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+      if (vi * 8 + j < cols) dot += a[j] * b[j];
+  }
+  dot = warp_sum(dot);
+  for (int vi = lane; vi < nvec; vi += 32) {
+    float a[8], b[8];
+    ld_half8(pr + vi * 8, a);
+    ld_half8(dr + vi * 8, b);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) a[j] = (vi * 8 + j < cols) ? a[j] * (b[j] - dot) : 0.f;
+    *reinterpret_cast<uint4*>(dr + vi * 8) = ln_pack8(a);
+  }
+}
+
 // one block (128 threads) per cutout row.  Accumulates losses with atomics (n prompts).
 __global__ void __launch_bounds__(128) prompt_loss_kernel(const float* __restrict__ e, int D,
                                                           const float* __restrict__ prompts,
@@ -599,69 +667,123 @@ static bool ln16_wide_ok() {
   return on;
 }
 
-#define LN_DISPATCH(KERNEL, XT, ...)                                                   \
-  switch (W / 128) {                                                              \
-    case 1: launch_pdl(KERNEL<1, XT>, dim3((rows + 7) / 8), dim3(256), 0, st, __VA_ARGS__); break;        \
-    case 2: launch_pdl(KERNEL<2, XT>, dim3((rows + 7) / 8), dim3(256), 0, st, __VA_ARGS__); break;        \
-    case 4: launch_pdl(KERNEL<4, XT>, dim3((rows + 7) / 8), dim3(256), 0, st, __VA_ARGS__); break;        \
-    case 6: launch_pdl(KERNEL<6, XT>, dim3((rows + 7) / 8), dim3(256), 0, st, __VA_ARGS__); break;        \
-    case 8: launch_pdl(KERNEL<8, XT>, dim3((rows + 7) / 8), dim3(256), 0, st, __VA_ARGS__); break;        \
-    default: break;                                                               \
+// every W = 128 * k, k in [1, 8]; any other width has no kernel and returns -1 (nothing launched)
+#define LN_DISPATCH(KERNEL, XT, ...)                                                                       \
+  if (W % 128) return -1;                                                                                  \
+  switch (W / 128) {                                                                                       \
+    case 1: launch_pdl(KERNEL<1, XT>, dim3((rows + 7) / 8), dim3(256), 0, st, __VA_ARGS__); return 0;      \
+    case 2: launch_pdl(KERNEL<2, XT>, dim3((rows + 7) / 8), dim3(256), 0, st, __VA_ARGS__); return 0;      \
+    case 3: launch_pdl(KERNEL<3, XT>, dim3((rows + 7) / 8), dim3(256), 0, st, __VA_ARGS__); return 0;      \
+    case 4: launch_pdl(KERNEL<4, XT>, dim3((rows + 7) / 8), dim3(256), 0, st, __VA_ARGS__); return 0;      \
+    case 5: launch_pdl(KERNEL<5, XT>, dim3((rows + 7) / 8), dim3(256), 0, st, __VA_ARGS__); return 0;      \
+    case 6: launch_pdl(KERNEL<6, XT>, dim3((rows + 7) / 8), dim3(256), 0, st, __VA_ARGS__); return 0;      \
+    case 7: launch_pdl(KERNEL<7, XT>, dim3((rows + 7) / 8), dim3(256), 0, st, __VA_ARGS__); return 0;      \
+    case 8: launch_pdl(KERNEL<8, XT>, dim3((rows + 7) / 8), dim3(256), 0, st, __VA_ARGS__); return 0;      \
+    default: return -1;                                                                                    \
   }
 
-void layernorm_forward(const float* x, long long x_stride, const float* pos, int T, const float* gamma,
-                       const float* beta, int rows, int W, float eps, act_t* y16, float* y32, float* stats,
-                       cudaStream_t st) {
-  LN_DISPATCH(layernorm_fwd_kernel, float, x, x_stride, pos, T, gamma, beta, rows, W, eps, y16, y32, stats)
+template <typename XT>
+static int ln_forward_vec4(const XT* x, long long x_stride, const float* pos, int T, const float* gamma, const float* beta,
+                           int rows, int W, float eps, act_t* y16, float* y32, float* stats, cudaStream_t st) {
+  LN_DISPATCH(layernorm_fwd_kernel, XT, x, x_stride, pos, T, gamma, beta, rows, W, eps, y16, y32, stats)
 }
-void layernorm_forward(const act_t* x, long long x_stride, const float* pos, int T, const float* gamma,
-                       const float* beta, int rows, int W, float eps, act_t* y16, float* y32, float* stats,
-                       cudaStream_t st) {
-  if (ln16_wide_ok() && !pos && !y32 && y16 && W % 256 == 0 && x_stride % 8 == 0) {
-    const dim3 grid((rows + 7) / 8), block(256);
-    switch (W / 256) {
-      case 1: launch_pdl(layernorm_fwd16_kernel<1>, grid, block, 0, st, x, x_stride, gamma, beta, rows, W, eps, y16, stats); return;
-      case 2: launch_pdl(layernorm_fwd16_kernel<2>, grid, block, 0, st, x, x_stride, gamma, beta, rows, W, eps, y16, stats); return;
-      case 3: launch_pdl(layernorm_fwd16_kernel<3>, grid, block, 0, st, x, x_stride, gamma, beta, rows, W, eps, y16, stats); return;
-      case 4: launch_pdl(layernorm_fwd16_kernel<4>, grid, block, 0, st, x, x_stride, gamma, beta, rows, W, eps, y16, stats); return;
-      default: break;
-    }
+template <typename XT>
+static int ln_backward_vec4(const act_t* dy, const XT* x, long long x_stride, const float* pos, int T, const float* stats,
+                            const float* gamma, int rows, int W, int accumulate, float* gx, act_t* gx16, cudaStream_t st) {
+  LN_DISPATCH(layernorm_bwd_kernel, XT, dy, x, x_stride, pos, T, stats, gamma, rows, W, accumulate, gx, gx16)
+}
+// the 16-byte fp16 kernels: W in {256, 512, 768, 1024}, rows 16-byte aligned, no pos, fp16 output only
+static int ln_forward_vec8(const act_t* x, long long x_stride, const float* gamma, const float* beta, int rows, int W,
+                           float eps, act_t* y16, float* stats, cudaStream_t st) {
+  if (W % 256 || x_stride % 8 || !y16) return -1;
+  const dim3 grid((rows + 7) / 8), block(256);
+  switch (W / 256) {
+    case 1: launch_pdl(layernorm_fwd16_kernel<1>, grid, block, 0, st, x, x_stride, gamma, beta, rows, W, eps, y16, stats); return 0;
+    case 2: launch_pdl(layernorm_fwd16_kernel<2>, grid, block, 0, st, x, x_stride, gamma, beta, rows, W, eps, y16, stats); return 0;
+    case 3: launch_pdl(layernorm_fwd16_kernel<3>, grid, block, 0, st, x, x_stride, gamma, beta, rows, W, eps, y16, stats); return 0;
+    case 4: launch_pdl(layernorm_fwd16_kernel<4>, grid, block, 0, st, x, x_stride, gamma, beta, rows, W, eps, y16, stats); return 0;
+    default: return -1;
   }
-  LN_DISPATCH(layernorm_fwd_kernel, act_t, x, x_stride, pos, T, gamma, beta, rows, W, eps, y16, y32, stats)
 }
-void layernorm_backward(const act_t* dy, const float* x, long long x_stride, const float* pos, int T,
-                        const float* stats, const float* gamma, int rows, int W, int accumulate, float* gx,
-                        act_t* gx16, cudaStream_t st) {
-  LN_DISPATCH(layernorm_bwd_kernel, float, dy, x, x_stride, pos, T, stats, gamma, rows, W, accumulate, gx, gx16)
-}
-void layernorm_backward(const act_t* dy, const act_t* x, long long x_stride, const float* pos, int T,
-                        const float* stats, const float* gamma, int rows, int W, int accumulate, float* gx,
-                        act_t* gx16, cudaStream_t st) {
-  if (ln16_wide_ok() && !pos && !gx && gx16 && W % 256 == 0 && x_stride % 8 == 0) {
-    const dim3 grid((rows + 7) / 8), block(256);
-    switch (W / 256) {
-      case 1: launch_pdl(layernorm_bwd16_kernel<1>, grid, block, 0, st, dy, x, x_stride, stats, gamma, rows, W, accumulate, gx16); return;
-      case 2: launch_pdl(layernorm_bwd16_kernel<2>, grid, block, 0, st, dy, x, x_stride, stats, gamma, rows, W, accumulate, gx16); return;
-      case 3: launch_pdl(layernorm_bwd16_kernel<3>, grid, block, 0, st, dy, x, x_stride, stats, gamma, rows, W, accumulate, gx16); return;
-      case 4: launch_pdl(layernorm_bwd16_kernel<4>, grid, block, 0, st, dy, x, x_stride, stats, gamma, rows, W, accumulate, gx16); return;
-      default: break;
-    }
+static int ln_backward_vec8(const act_t* dy, const act_t* x, long long x_stride, const float* stats, const float* gamma,
+                            int rows, int W, int accumulate, act_t* gx16, cudaStream_t st) {
+  if (W % 256 || x_stride % 8 || !gx16) return -1;
+  const dim3 grid((rows + 7) / 8), block(256);
+  switch (W / 256) {
+    case 1: launch_pdl(layernorm_bwd16_kernel<1>, grid, block, 0, st, dy, x, x_stride, stats, gamma, rows, W, accumulate, gx16); return 0;
+    case 2: launch_pdl(layernorm_bwd16_kernel<2>, grid, block, 0, st, dy, x, x_stride, stats, gamma, rows, W, accumulate, gx16); return 0;
+    case 3: launch_pdl(layernorm_bwd16_kernel<3>, grid, block, 0, st, dy, x, x_stride, stats, gamma, rows, W, accumulate, gx16); return 0;
+    case 4: launch_pdl(layernorm_bwd16_kernel<4>, grid, block, 0, st, dy, x, x_stride, stats, gamma, rows, W, accumulate, gx16); return 0;
+    default: return -1;
   }
-  LN_DISPATCH(layernorm_bwd_kernel, act_t, dy, x, x_stride, pos, T, stats, gamma, rows, W, accumulate, gx, gx16)
+}
+
+int layernorm_forward(const float* x, long long x_stride, const float* pos, int T, const float* gamma,
+                      const float* beta, int rows, int W, float eps, act_t* y16, float* y32, float* stats,
+                      cudaStream_t st) {
+  return ln_forward_vec4(x, x_stride, pos, T, gamma, beta, rows, W, eps, y16, y32, stats, st);
+}
+int layernorm_forward(const act_t* x, long long x_stride, const float* pos, int T, const float* gamma,
+                      const float* beta, int rows, int W, float eps, act_t* y16, float* y32, float* stats,
+                      cudaStream_t st) {
+  if (ln16_wide_ok() && !pos && !y32 && ln_forward_vec8(x, x_stride, gamma, beta, rows, W, eps, y16, stats, st) == 0) return 0;
+  return ln_forward_vec4(x, x_stride, pos, T, gamma, beta, rows, W, eps, y16, y32, stats, st);
+}
+int layernorm_backward(const act_t* dy, const float* x, long long x_stride, const float* pos, int T,
+                       const float* stats, const float* gamma, int rows, int W, int accumulate, float* gx,
+                       act_t* gx16, cudaStream_t st) {
+  return ln_backward_vec4(dy, x, x_stride, pos, T, stats, gamma, rows, W, accumulate, gx, gx16, st);
+}
+int layernorm_backward(const act_t* dy, const act_t* x, long long x_stride, const float* pos, int T,
+                       const float* stats, const float* gamma, int rows, int W, int accumulate, float* gx,
+                       act_t* gx16, cudaStream_t st) {
+  if (ln16_wide_ok() && !pos && !gx && ln_backward_vec8(dy, x, x_stride, stats, gamma, rows, W, accumulate, gx16, st) == 0)
+    return 0;
+  return ln_backward_vec4(dy, x, x_stride, pos, T, stats, gamma, rows, W, accumulate, gx, gx16, st);
+}
+int layernorm_forward_variant(int variant, const void* x, long long x_stride, const float* pos, int T, const float* gamma,
+                              const float* beta, int rows, int W, float eps, act_t* y16, float* y32, float* stats,
+                              cudaStream_t st) {
+  switch (variant) {
+    case LN_F32_STREAM:
+      return ln_forward_vec4(static_cast<const float*>(x), x_stride, pos, T, gamma, beta, rows, W, eps, y16, y32, stats, st);
+    case LN_F16_VEC4:
+      return ln_forward_vec4(static_cast<const act_t*>(x), x_stride, pos, T, gamma, beta, rows, W, eps, y16, y32, stats, st);
+    case LN_F16_VEC8:
+      if (pos || y32) return -1;
+      return ln_forward_vec8(static_cast<const act_t*>(x), x_stride, gamma, beta, rows, W, eps, y16, stats, st);
+    default: return -1;
+  }
+}
+int layernorm_backward_variant(int variant, const act_t* dy, const void* x, long long x_stride, const float* pos, int T,
+                               const float* stats, const float* gamma, int rows, int W, int accumulate, float* gx,
+                               act_t* gx16, cudaStream_t st) {
+  switch (variant) {
+    case LN_F32_STREAM:
+      return ln_backward_vec4(dy, static_cast<const float*>(x), x_stride, pos, T, stats, gamma, rows, W, accumulate, gx, gx16, st);
+    case LN_F16_VEC4:
+      return ln_backward_vec4(dy, static_cast<const act_t*>(x), x_stride, pos, T, stats, gamma, rows, W, accumulate, gx, gx16, st);
+    case LN_F16_VEC8:
+      if (pos || gx) return -1;
+      return ln_backward_vec8(dy, static_cast<const act_t*>(x), x_stride, stats, gamma, rows, W, accumulate, gx16, st);
+    default: return -1;
+  }
 }
 void softmax_forward(act_t* s, int rows, int cols, int ld, cudaStream_t st) {
   const int nv = (ld / 8 + 31) / 32;
   const int grid = (rows + 7) / 8;
   if (nv <= 1) launch_pdl(softmax_fwd_kernel<1>, dim3(grid), dim3(256), 0, st, s, rows, cols, ld);
   else if (nv == 2) launch_pdl(softmax_fwd_kernel<2>, dim3(grid), dim3(256), 0, st, s, rows, cols, ld);
-  else launch_pdl(softmax_fwd_kernel<4>, dim3(grid), dim3(256), 0, st, s, rows, cols, ld);
+  else if (nv <= 4) launch_pdl(softmax_fwd_kernel<4>, dim3(grid), dim3(256), 0, st, s, rows, cols, ld);
+  else launch_pdl(softmax_fwd_long_kernel, dim3(grid), dim3(256), 0, st, s, rows, cols, ld);
 }
 void softmax_backward(const act_t* p, act_t* dp_to_ds, int rows, int cols, int ld, cudaStream_t st) {
   const int nv = (ld / 8 + 31) / 32;
   const int grid = (rows + 7) / 8;
   if (nv <= 1) launch_pdl(softmax_bwd_kernel<1>, dim3(grid), dim3(256), 0, st, p, dp_to_ds, rows, cols, ld);
   else if (nv == 2) launch_pdl(softmax_bwd_kernel<2>, dim3(grid), dim3(256), 0, st, p, dp_to_ds, rows, cols, ld);
-  else launch_pdl(softmax_bwd_kernel<4>, dim3(grid), dim3(256), 0, st, p, dp_to_ds, rows, cols, ld);
+  else if (nv <= 4) launch_pdl(softmax_bwd_kernel<4>, dim3(grid), dim3(256), 0, st, p, dp_to_ds, rows, cols, ld);
+  else launch_pdl(softmax_bwd_long_kernel, dim3(grid), dim3(256), 0, st, p, dp_to_ds, rows, cols, ld);
 }
 void prompt_loss(const float* e, int B, int D, const float* prompts, const float* weights, const float* stops,
                  const int* slots, const float* inv_rows, int n, int cutn_global, float grad_scale, float* e_unit,

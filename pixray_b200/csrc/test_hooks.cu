@@ -112,6 +112,39 @@ extern "C" int pxr_test_attention(const void* qkv, void* o, float* lse, const vo
   return 0;
 }
 
+// The engine's row softmax (softmax_forward / softmax_backward, unfused attention) on caller DEVICE fp16 [rows, ld]:
+// backward == 0: p_or_s holds the scores and is overwritten with the probabilities; backward != 0: p_or_s holds P and
+// dp holds dP, overwritten with dS = P * (dP - <P, dP>).
+extern "C" int pxr_test_softmax(int backward, void* p_or_s, void* dp, int rows, int cols, int ld) {
+  if (!p_or_s || rows < 1 || cols < 1 || ld < cols || ld % 8 || (backward && !dp)) return -1;
+  if (backward) softmax_backward(static_cast<const act_t*>(p_or_s), static_cast<act_t*>(dp), rows, cols, ld, nullptr);
+  else softmax_forward(static_cast<act_t*>(p_or_s), rows, cols, ld, nullptr);
+  cudaError_t ce = cudaDeviceSynchronize();
+  if (ce == cudaSuccess) ce = cudaGetLastError();
+  return ce == cudaSuccess ? 0 : -100;
+}
+
+// One LayerNorm kernel chosen by `variant` (0: fp32 stream, 1: fp16 stream 8-byte vectors, 2: fp16 stream 16-byte
+// vectors) whatever PXR_LN16_WIDE says, forward (x, pos, gamma, beta -> y16 / y32, stats) or backward (dy, x, pos, stats,
+// gamma -> gx / gx16, accumulate adds to what they hold).  All DEVICE; x is fp32 for variant 0 and fp16 otherwise.
+// -1 when that variant has no kernel for the width or the arguments.
+extern "C" int pxr_test_layernorm(int variant, int backward, const void* x, long long x_stride, const float* pos, int T,
+                                  const float* gamma, const float* beta, int rows, int W, float eps, void* y16, float* y32,
+                                  float* stats, const void* dy, int accumulate, float* gx, void* gx16) {
+  if (!x || !gamma || !stats || rows < 1 || (pos && T < 1)) return -2;
+  int rc;
+  if (backward)
+    rc = layernorm_backward_variant(variant, static_cast<const act_t*>(dy), x, x_stride, pos, T, stats, gamma, rows, W,
+                                    accumulate, gx, static_cast<act_t*>(gx16), nullptr);
+  else
+    rc = layernorm_forward_variant(variant, x, x_stride, pos, T, gamma, beta, rows, W, eps, static_cast<act_t*>(y16), y32,
+                                   stats, nullptr);
+  if (rc) return rc;
+  cudaError_t ce = cudaDeviceSynchronize();
+  if (ce == cudaSuccess) ce = cudaGetLastError();
+  return ce == cudaSuccess ? 0 : -100;
+}
+
 // Host evaluation of the per-pixel ColorJitter body the cutout kernels run (color_jitter.cuh is host+device code):
 // lets the CPU suite compare the arithmetic and its Jacobian with the oracle without a GPU.  rgb / g_out / out / g_in
 // are HOST [n, 3]; g_out and g_in may be NULL.

@@ -356,3 +356,101 @@ def test_fft_drawer_and_patch14_perceptor():
     exp = R.AdamState(z).step(z, zg.cpu(), 0.3)
     e_z, _ = report("fft z after Adam", zc, exp)
     assert e_z < 1e-5
+
+
+def _stagewise(vq, clip, eng, prompts, z, image, seed):
+    """synth -> cutouts -> embeds -> losses -> z.grad on the engine, against the oracle evaluated on the engine's side of
+    the clamp (vqgan_synth_with_engine_clamp_sides: the same forward).  Returns the engine's (image, embeds, losses,
+    z.grad) and the errors against the stated tolerances' quantities."""
+    cutn, cs = 8, 224
+    T = random_transforms(cutn, cs, seed)
+    g = torch.Generator().manual_seed(seed + 9)
+    facs, noise = plant_extremes(torch.rand(cutn, generator=g) * 0.1, torch.randn(cutn, 3, cs, cs, generator=g))
+    img = eng.synth(z)
+    synth, _ = vqgan_synth_with_engine_clamp_sides(vq, eng, (image, image))
+    ref = R.iterate(synth, z, [clip], [prompts], torch.from_numpy(T), cs, "reflection", 0.37, facs, noise)
+    eng.make_cutouts(img, transforms=T, zoom_padding=E.PAD_REFLECTION, fill=0.37, noise_facs=facs.numpy(), noise=noise)
+    emb = eng.encode_image(0).clone()
+    losses = eng.prompt_loss(0).clone()
+    zg = eng.backward().clone()
+    assert torch.isfinite(zg).all()
+    err = dict(image=report(f"{image}x{image} image", img, ref["image"])[0],
+               embeds=report("unit embeds", emb, ref["embeds"][0])[0],
+               losses=report("prompt losses", losses, torch.stack([l.reshape(()) for l in ref["losses"]]))[0])
+    err["z_grad"], err["z_grad_max"] = report("z.grad", zg, ref["z_grad"])
+    return (img, emb, losses, zg), err
+
+
+def _assert_pipeline_tolerances(err):
+    assert err["image"] < 5e-3
+    assert err["embeds"] < 5e-3
+    assert err["losses"] < 2e-3
+    assert err["z_grad"] <= 3e-2 * err["z_grad_max"]
+
+
+def test_decoder_attention_rows_longer_than_1024():
+    """A 96 x 96 canvas: the 48 x 48 latent gives T = 2304 tokens in the decoder's mid and up-block attention, rows the
+    unfused row softmax must cover in full (a 640 x 480 or 1024 x 1024 canvas of the full-size model has T = 1200 / 4096)."""
+    vq, clip, eng, prompts, z = build(image=96, seed=13)
+    assert z.shape[-1] * z.shape[-2] == 2304
+    _, err = _stagewise(vq, clip, eng, prompts, z, 96, 13)
+    eng.close()
+    _assert_pipeline_tolerances(err)
+
+
+ATTENTION_PATHS = {
+    "fused": {},
+    "batched_gemms_row_softmax": {"PXR_FUSED_ATTN": "0", "PXR_FUSE_SOFTMAX": "0"},
+    "softmax_in_gemm_epilogue": {"PXR_FUSED_ATTN": "0", "PXR_FUSE_SOFTMAX": "1"},
+    "fp32_stream": {"PXR_CLIP_STREAM": "32"},
+}
+
+
+@pytest.mark.parametrize("path", sorted(ATTENTION_PATHS))
+def test_every_attention_path_matches_the_oracle(path, monkeypatch):
+    """Each attention / residual-stream path a session can select (read at session create) on the small pipeline."""
+    for k in ("PXR_FUSED_ATTN", "PXR_FUSE_SOFTMAX", "PXR_CLIP_STREAM", "PXR_CLIP_LAST_CLS"):
+        monkeypatch.delenv(k, raising=False)
+    for k, v in ATTENTION_PATHS[path].items():
+        monkeypatch.setenv(k, v)
+    vq, clip, eng, prompts, z = build(seed=21)
+    _, err = _stagewise(vq, clip, eng, prompts, z, 32, 21)
+    eng.close()
+    _assert_pipeline_tolerances(err)
+
+
+def test_last_layer_on_all_rows_is_bit_identical(monkeypatch):
+    """The last ViT layer restricted to the class rows (default) and run on all rows (PXR_CLIP_LAST_CLS=0) compute the
+    class rows with the same operations: embeddings and z.grad are bit-identical.  (The loss values are not compared
+    bit for bit: the prompt-loss kernel sums them over the cutouts with atomics, so their last bits vary from call to
+    call in either session.)"""
+    outs = {}
+    for last_cls in ("1", "0"):
+        for k in ("PXR_FUSED_ATTN", "PXR_FUSE_SOFTMAX", "PXR_CLIP_STREAM"):
+            monkeypatch.delenv(k, raising=False)
+        monkeypatch.setenv("PXR_CLIP_LAST_CLS", last_cls)
+        vq, clip, eng, prompts, z = build(seed=23)
+        outs[last_cls], err = _stagewise(vq, clip, eng, prompts, z, 32, 23)
+        eng.close()
+        _assert_pipeline_tolerances(err)
+    (img1, emb1, _, g1), (img0, emb0, _, g0) = outs["1"], outs["0"]
+    assert torch.equal(img1, img0)
+    assert torch.equal(emb1, emb0)
+    assert torch.equal(g1, g0)
+
+
+@pytest.mark.parametrize("width", [384, 640])
+def test_vit_width_not_a_multiple_of_256(width):
+    """Widths 128 k with odd k have LayerNorm kernels (8-byte vectors only) and match the oracle."""
+    clip_cfg = dict(width=width, layers=1, heads=width // 64, patch=32, image_res=224, out_dim=64)
+    vq, clip, eng, prompts, z = build(seed=width, clip_cfg=clip_cfg)
+    _, err = _stagewise(vq, clip, eng, prompts, z, 32, width)
+    eng.close()
+    _assert_pipeline_tolerances(err)
+
+
+@pytest.mark.parametrize("width", [320, 576])
+def test_vit_width_without_layernorm_kernel_is_refused(width):
+    clip_cfg = dict(width=width, layers=1, heads=width // 64, patch=32, image_res=224, out_dim=64)
+    with pytest.raises(E.EngineError, match="multiple of 128"):
+        build(clip_cfg=clip_cfg)

@@ -58,6 +58,12 @@ def test_encoder_small_matches_the_oracle():
     _check(SMALL_VQ, (32, 48), 4, SMALL_CLIP)   # non-square latent
 
 
+def test_encoder_attention_rows_longer_than_1024():
+    """96 x 96: the encoder's mid and down-block attention run at the 48 x 48 latent, T = 2304 tokens per row."""
+    from test_pipeline_gpu import SMALL_CLIP, SMALL_VQ
+    _check(SMALL_VQ, (96, 96), 6, SMALL_CLIP)
+
+
 def test_encoder_full_size_and_drawer_init():
     """imagenet_f16_16384 at 256 x 256, then VqganDrawer.init_from_tensor -> synth round trip through the plugin classes."""
     from test_pipeline_gpu import SMALL_CLIP
