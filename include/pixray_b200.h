@@ -30,7 +30,7 @@ extern "C" {
 
 typedef struct pxr_engine* pxr_handle;
 
-enum { PXR_DRAWER_VQGAN = 0, PXR_DRAWER_PIXEL = 1, PXR_DRAWER_FFT = 2, PXR_DRAWER_VDIFF = 3 };
+enum { PXR_DRAWER_VQGAN = 0, PXR_DRAWER_PIXEL = 1, PXR_DRAWER_FFT = 2, PXR_DRAWER_VDIFF = 3, PXR_DRAWER_POLYGON = 4 };
 enum { PXR_PAD_REFLECTION = 0, PXR_PAD_BORDER = 1, PXR_PAD_ZEROS = 2 };
 enum { PXR_DTYPE_F16 = 0, PXR_DTYPE_BF16 = 1 };
 /* module ids for pxr_load_weight */
@@ -140,6 +140,17 @@ int pxr_set_comm(pxr_handle h, const void* nccl_unique_id, int rank, int world);
 int pxr_get_unique_id(void* out128);
 
 int pxr_synth(pxr_handle h, const float* z, float* out_img /* [3,H,W] */);
+/* Polygon drawer (PXR_DRAWER_POLYGON; PixelDrawer with pixel_type hex / tri / diamond / knit / rectshift,
+ * pixeldrawer.py:200-367): n fixed polygons, each filled with one RGBA colour; z = [n, 4] (the reference's get_z layout).
+ * xy: host [total_vertices, 2] canvas coordinates, polygon k = vertices offsets[k] .. offsets[k+1]-1 (offsets host [n+1],
+ * offsets[0] = 0), in draw order: later polygons cover earlier ones.  3 to 8 vertices each (8 = knit), finite
+ * coordinates.  Before pxr_finalize.  The render takes 2 x 2 stratified jittered samples per pixel (Philox keyed by seed
+ * and iteration), even-odd fill, topmost polygon wins, pixel = mean of its samples, no clamp; clip_z keeps RGB in [0, 1]
+ * and alpha at 1. */
+int pxr_set_polygons(pxr_handle h, const float* xy, const int* offsets, int n);
+/* The iteration the per-op pxr_synth renders (drawer.synth(cur_iteration)): keys the polygon drawer's sample positions,
+ * ignored by the other drawers.  pxr_iterate uses its own `iter` (and leaves it set). */
+int pxr_set_synth_iteration(pxr_handle h, int iter);
 /* z = model.encode(img)[0]: VqganDrawer.init_from_tensor / reapply_from_tensor / get_z_from_tensor (vqgan.py:174-185) --
  * taming Encoder + quant_conv + nearest codebook row.  img device [3,H,W] in [-1,1]; z_out device [z_channels,h,w].
  * Available when the weights loaded before pxr_finalize include the checkpoint's encoder.* and quant_conv.* tensors. */
@@ -304,6 +315,10 @@ int pxr_test_color_jitter_device(const float* rgb, int n, int code, float satura
 
 /* adaptive-pool window bounds as the device computes them (pool_fwd / pool_bwd): DEVICE int [out_size] each */
 int pxr_test_pool_bounds(int in_size, int out_size, int* starts, int* ends);
+
+/* the polygon drawer's sample positions as the device computes them (raster_samples.cuh): out DEVICE float
+ * [H, W, 4, 2], sample s = dx + 2 dy of pixel (x, y) as (x, y) canvas coordinates */
+int pxr_test_raster_samples(uint64_t seed, int iter, int H, int W, float* out);
 
 /* fused ViT attention (attn_tc.cu): forward, and backward when d_o != NULL.  qkv [B*T, 3W], o / d_o [B*T, W],
  * gqkv [B*T, 3W] fp16 device tensors, lse [B*H*T] fp32; heads are 64 wide (W = 64 H), T <= 240 */

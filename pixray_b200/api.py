@@ -30,13 +30,15 @@ import torch
 from . import engine as E
 from . import filters as FL
 from . import losses as L
+from . import pixel_shapes as PS
 from . import plugins as P
 from . import synthetic as S
 from .util import apply_overlay, get_learning_rate_drops, parse_unit, split_pipes
 
-# pixray.class_table (pixray.py:74-113) restricted to the drawers of the BASELINE configs; "pixel" is the rect grid the
-# reference renders through diffvg, which fast_pixel reproduces (SURVEY.md 2, row 6)
-class_table = {"vqgan": P.VqganDrawer, "fast_pixel": P.FastPixelDrawer, "pixel": P.FastPixelDrawer, "fft": P.FftDrawer,
+# pixray.class_table (pixray.py:74-113) restricted to the drawers of the BASELINE configs.  "pixel" contributes the reference
+# PixelDrawer's five options; its default rect grid runs as fast_pixel (the square cells diffvg renders, SURVEY.md 2,
+# row 6), every other pixel_type on the polygon rasteriser (do_init)
+class_table = {"vqgan": P.VqganDrawer, "fast_pixel": P.FastPixelDrawer, "pixel": P.PixelDrawer, "fft": P.FftDrawer,
                "vdiff": P.VdiffDrawer}
 _DRAWER_KIND = {"vqgan": E.DRAWER_VQGAN, "fast_pixel": E.DRAWER_PIXEL, "pixel": E.DRAWER_PIXEL, "fft": E.DRAWER_FFT,
                 "vdiff": E.DRAWER_VDIFF}
@@ -325,6 +327,13 @@ def do_init(args):
         raise NotImplementedError("at most two perceptors per session")
     st.seed = _seed_everything(args)
     kind = _DRAWER_KIND[args.drawer]
+    drawer_class = class_table[args.drawer]
+    if args.drawer == "pixel":
+        if args.pixel_type == "rect":
+            drawer_class = P.FastPixelDrawer  # nearest-upsampled colour grid at the global learning rate
+        else:
+            PS.check_pixel_type(args.pixel_type)
+            kind = E.DRAWER_POLYGON
     n_levels = len(E.VQGAN_F16_16384["ch_mult"]) if kind == E.DRAWER_VQGAN else None
     sideX, sideY = _side(args, n_levels)
     # global_aspect_width = args.size[0] / args.size[1] (pixray.py:1931: the REQUESTED size, before the drawer rounds it):
@@ -341,6 +350,9 @@ def do_init(args):
     if kind == E.DRAWER_PIXEL:  # fast_pixeldrawer.py:37-63: 40x40 / 40x50 / 80x45 default grid, pixel_scale, clamp to canvas
         kw["grid"] = P.FastPixelDrawer.grid_for((sideX, sideY), getattr(args, "pixel_size", None), getattr(args, "pixel_scale", None))
         print(f"Running fast pixeldrawer with {kw['grid'][1]}x{kw['grid'][0]} grid")
+    if kind == E.DRAWER_POLYGON:  # pixeldrawer.py:123-177 (prints "Running pixeldrawer with CxR grid"), 234-291
+        rows, cols = P.PixelDrawer.grid_for(args, (sideX, sideY))
+        kw["polygons"] = PS.polygons((sideX, sideY), rows, cols, args.pixel_type)
     if kind == E.DRAWER_FFT:
         kw.update(fft_decay=args.fft_decay, fft_colors=args.fft_colors)
     eng = _engine_factory(**kw)
@@ -364,12 +376,12 @@ def do_init(args):
     if world > 1:
         eng.init_comm()
     st.engine, st.session = eng, P.Session(eng)
-    drawer = class_table[args.drawer](args, st.session)
+    drawer = drawer_class(args, st.session)
     drawer.load_model(args, eng.device)
     # ---- image initialisation (pixray.py:674-727): a noise / gradient / blank start image, optionally an init image, into
     # drawer.init_from_tensor(t * 2 - 1) -- for the VQGAN drawer that is model.encode on the engine (pxr_vqgan_encode)
     st.init_image_tensor, st.z_orig = None, None
-    if kind in (E.DRAWER_VQGAN, E.DRAWER_PIXEL) and (args.init_image or args.init_noise):
+    if kind in (E.DRAWER_VQGAN, E.DRAWER_PIXEL, E.DRAWER_POLYGON) and (args.init_image or args.init_noise):
         from PIL import Image
         from .util import random_gradient_image, random_noise_image
         rng = np.random.default_rng(st.seed)

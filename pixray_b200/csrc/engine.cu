@@ -560,6 +560,14 @@ class Engine {
   void finalize();
   void build_vqgan();
   void build_pixel();
+  void build_polygon();
+  // polygon drawer: host copies from pxr_set_polygons ([total_vertices, 2] and [n + 1] offsets), the binned scene, the
+  // per-sample winners of the last render, and the iteration that keys the render's sample positions
+  std::vector<float> poly_xy;
+  std::vector<int> poly_off;
+  RasterScene scene{};
+  int* poly_winner = nullptr;
+  int synth_iter = 0;
   void build_fft();
   FftPlans* fft = nullptr;
   void build_cutouts();
@@ -633,6 +641,7 @@ class Engine {
   void forward_clip(int i);
   void loss_clip(int i);
   void backward_all();
+  int clip_mode() const;
   void step(float lr);
   void step_managed(int iter);
   void write_initial_drop_state();
@@ -1314,6 +1323,68 @@ void Engine::build_pixel() {
   float inv = 1.f / S;
   drawer_fwd.add(1, [=] { pixel_synth(zb, rows, cols, H, Wd, ip, im, cs); }, 0.0, "pixel_synth");
   drawer_bwd.add(1, [=] { pixel_synth_backward(gi, ip, rows, cols, H, Wd, inv, zg, cs); }, 0.0, "pixel_synth_backward");
+}
+
+// PixelDrawer with shaped cells (pixeldrawer.py:200-304, 330-367): fixed polygons from pxr_set_polygons, z = [n, 4] RGBA
+// fill colours.  The tile grid is built here once, on the host (kernels.cuh RasterScene).
+void Engine::build_polygon() {
+  const int n = (int)poly_off.size() - 1, H = cfg.image_h, Wd = cfg.image_w;
+  if (n < 1) throw EngineError(-75, "polygon drawer: call pxr_set_polygons before pxr_finalize");
+  z_numel = (int64_t)4 * n;
+  z_buf = dalloc<float>(z_numel);
+  z_grad = dalloc<float>(z_numel);
+  img = dalloc<float>((size_t)3 * H * Wd);
+  img_pre = img;  // no clamp in the render (pixeldrawer.py:342-355): the image is its own pre-activation
+  g_img = dalloc<float>((size_t)3 * H * Wd);
+  poly_winner = dalloc<int>((size_t)4 * H * Wd);
+  const int T = RASTER_TILE, tx = (Wd + T - 1) / T, ty = (H + T - 1) / T;
+  std::vector<float4> bbox(n);
+  std::vector<int> tx0(n), tx1(n), ty0(n), ty1(n), count((size_t)tx * ty + 1, 0);
+  for (int k = 0; k < n; ++k) {
+    float4 b = make_float4(INFINITY, INFINITY, -INFINITY, -INFINITY);
+    for (int i = poly_off[k]; i < poly_off[k + 1]; ++i) {
+      const float x = poly_xy[2 * i], y = poly_xy[2 * i + 1];
+      b.x = std::min(b.x, x);
+      b.y = std::min(b.y, y);
+      b.z = std::max(b.z, x);
+      b.w = std::max(b.w, y);
+    }
+    bbox[k] = b;
+    // tile j covers the closed interval [j T, (j + 1) T]: it meets [lo, hi] for ceil(lo / T) - 1 <= j <= floor(hi / T).
+    // The box is clamped to one tile around the canvas first, so far-away (finite) coordinates convert to int safely;
+    // a polygon entirely off the canvas gets an empty tile range.
+    auto tile_lo = [T](double v, int n) { return (int)std::ceil(std::min(std::max(v, -(double)T), (double)n * T + T) / T) - 1; };
+    auto tile_hi = [T](double v, int n) { return (int)std::floor(std::min(std::max(v, -(double)T), (double)n * T + T) / T); };
+    tx0[k] = std::max(0, tile_lo(b.x, tx));
+    tx1[k] = std::min(tx - 1, tile_hi(b.z, tx));
+    ty0[k] = std::max(0, tile_lo(b.y, ty));
+    ty1[k] = std::min(ty - 1, tile_hi(b.w, ty));
+    for (int j = ty0[k]; j <= ty1[k]; ++j)
+      for (int i = tx0[k]; i <= tx1[k]; ++i) ++count[(size_t)j * tx + i + 1];
+  }
+  for (size_t t = 1; t < count.size(); ++t) count[t] += count[t - 1];
+  std::vector<int> fill(count.begin(), count.end() - 1), list(count.back() > 0 ? count.back() : 1, 0);
+  for (int k = n - 1; k >= 0; --k)  // topmost first: shapes are drawn in index order, later over earlier
+    for (int j = ty0[k]; j <= ty1[k]; ++j)
+      for (int i = tx0[k]; i <= tx1[k]; ++i) list[fill[(size_t)j * tx + i]++] = k;
+  std::vector<float2> xy(poly_xy.size() / 2);
+  for (size_t i = 0; i < xy.size(); ++i) xy[i] = make_float2(poly_xy[2 * i], poly_xy[2 * i + 1]);
+  scene.xy = upload(xy);
+  scene.off = upload(poly_off);
+  scene.bbox = upload(bbox);
+  scene.tile_start = upload(count);
+  scene.tile_list = upload(list);
+  scene.n = n;
+  scene.tiles_x = tx;
+  cudaStream_t cs = st;
+  float *zb = z_buf, *im = img, *gi = g_img, *zg = z_grad;
+  int* win = poly_winner;
+  const RasterScene sc = scene;
+  const uint64_t seed = cfg.seed;
+  const float inv = 1.f / S;
+  const int* iter = &synth_iter;  // read when the op runs: pxr_iterate's iteration, or pxr_set_synth_iteration's
+  drawer_fwd.add(1, [=] { raster_forward(sc, zb, H, Wd, seed, *iter, win, im, cs); }, 0.0, "raster_forward");
+  drawer_bwd.add(1, [=] { raster_backward(sc, win, gi, H, Wd, inv, zg, cs); }, 0.0, "raster_backward");
 }
 
 // FftDrawer.synth (fftdrawer.py:78-84): params = rfft2 spectrum [1,3,H,W/2+1,2]; see kernels_fft.cu
@@ -2170,11 +2241,18 @@ bool Engine::spot_pass(int which, bool accumulate_img) {
   return true;
 }
 
+// clip_z without per-channel bounds: the fast pixel grid clamps to [0, 1], the polygon fills RGB to [0, 1] and alpha to 1
+int Engine::clip_mode() const {
+  if (cfg.drawer == PXR_DRAWER_PIXEL) return CLIP_01;
+  if (cfg.drawer == PXR_DRAWER_POLYGON) return CLIP_RGBA;
+  return CLIP_NONE;
+}
+
 void Engine::step(float lr) {
   ++adam_t;
   const int per_channel = (cfg.drawer == PXR_DRAWER_VQGAN) ? (int)(z_numel / cfg.z_channels) : 1;
   adam_clip_step(z_buf, adam_m, adam_v, batches > 1 ? z_grad_acc : z_grad, 1.f, (int)z_numel, per_channel, zmin, zmax,
-                 cfg.drawer == PXR_DRAWER_PIXEL, lr, cfg.beta1, cfg.beta2, cfg.adam_eps, adam_t, st);
+                 clip_mode(), lr, cfg.beta1, cfg.beta2, cfg.adam_eps, adam_t, st);
   launches += 1;
 }
 
@@ -2338,7 +2416,7 @@ void Engine::step_managed(int iter) {
   const int per_channel = (cfg.drawer == PXR_DRAWER_VQGAN) ? (int)(z_numel / cfg.z_channels) : 1;
   const float* g = batches > 1 ? z_grad_acc : z_grad;
   adam_clip_managed(z_buf, adam_m, adam_v, g, best_z, 1.f, (int)z_numel, per_channel, zmin, zmax,
-                    cfg.drawer == PXR_DRAWER_PIXEL, cfg.beta1, cfg.beta2, cfg.adam_eps, losses_dev, num_losses(), iter,
+                    clip_mode(), cfg.beta1, cfg.beta2, cfg.adam_eps, losses_dev, num_losses(), iter,
                     drop_cfg, drop_state + drop_parity, drop_state + (drop_parity ^ 1), drop_status_dev, st);
   drop_parity ^= 1;
   launches += 1;
@@ -2350,6 +2428,7 @@ void Engine::finalize() {
   else if (cfg.drawer == PXR_DRAWER_PIXEL) build_pixel();
   else if (cfg.drawer == PXR_DRAWER_FFT) build_fft();
   else if (cfg.drawer == PXR_DRAWER_VDIFF) build_vdiff();
+  else if (cfg.drawer == PXR_DRAWER_POLYGON) build_polygon();
   else throw EngineError(-47, "unknown drawer kind");
   adam_m = dalloc<float>(z_numel);
   adam_v = dalloc<float>(z_numel);
@@ -2397,6 +2476,7 @@ void Engine::finalize() {
     reg("best_z", best_z, z_numel * 4);
     reg("z", z_buf, z_numel * 4);
     reg("losses", losses_dev, 64 * 4);
+    if (poly_winner) reg("poly_winner", poly_winner, npx / 3 * 4 * sizeof(int));
     if (vd_pred) {
       reg("vd_pred", vd_pred, npx * 4);
       reg("vd_v", vd_v, npx * 4);
@@ -2607,6 +2687,35 @@ int pxr_set_image_prompts(pxr_handle h, const float* imgs, int n, const float* w
   return pxr_set_image_prompts_sized(h, ptrs.data(), hs.data(), ws.data(), n, weights);
 }
 
+// The polygon drawer's shapes (PixelDrawer.encode_image, pixeldrawer.py:200-304): polygon k has the vertices
+// xy[offsets[k] .. offsets[k + 1]) (host [total_vertices, 2]), in draw order.  Copied; before pxr_finalize.
+int pxr_set_polygons(pxr_handle h, const float* xy, const int* offsets, int n) {
+  PXR_TRY(h, {
+    Engine* e = h->e;
+    if (e->cfg.drawer != PXR_DRAWER_POLYGON) throw EngineError(-76, "pxr_set_polygons: not a polygon-drawer engine");
+    if (e->finalized) throw EngineError(-12, "pxr_set_polygons: the polygons cannot change after pxr_finalize");
+    if (n < 1) throw EngineError(-77, "pxr_set_polygons: n = " + std::to_string(n) + ", at least one polygon is needed");
+    if (!xy || !offsets) throw EngineError(-10, "pxr_set_polygons: null pointer");
+    if (offsets[0] != 0) throw EngineError(-77, "pxr_set_polygons: offsets[0] must be 0");
+    for (int k = 0; k < n; ++k) {
+      const int nv = offsets[k + 1] - offsets[k];
+      if (nv < 3 || nv > 8)
+        throw EngineError(-77, "pxr_set_polygons: polygon " + std::to_string(k) + " has " + std::to_string(nv) +
+                                   " vertices; 3 to 8 are supported");
+    }
+    const int nv = offsets[n];
+    for (int i = 0; i < 2 * nv; ++i)
+      if (!std::isfinite(xy[i]))
+        throw EngineError(-77, "pxr_set_polygons: vertex " + std::to_string(i / 2) + " has a non-finite coordinate");
+    e->poly_xy.assign(xy, xy + 2 * nv);
+    e->poly_off.assign(offsets, offsets + n + 1);
+  });
+}
+
+int pxr_set_synth_iteration(pxr_handle h, int iter) {
+  PXR_TRY(h, h->e->synth_iter = iter);
+}
+
 int pxr_synth(pxr_handle h, const float* z, float* out_img) {
   PXR_TRY(h, {
     Engine* e = h->e;
@@ -2747,6 +2856,7 @@ int pxr_iterate(pxr_handle h, float* z, float lr, int iter, const pxr_cut_params
     if (z) PXR_CUDA(cudaMemcpyAsync(e->z_buf, z, e->z_numel * sizeof(float), cudaMemcpyDeviceToDevice, e->st));
     if (e->batches > 1 && p) throw EngineError(-63, "batches > 1 draws its cutout parameters in the engine: pass p = NULL");
     e->vd_iter_request = iter;
+    e->synth_iter = iter;
     for (int b = 0; b < e->batches; ++b) {
       // every pass is one ascend_txt + backward (pixray.py:1464-1482): fresh augmentations, gradients accumulate in z.grad;
       // checkdrop and the reported loss vector use the FIRST pass (`if i == 0`, pixray.py:1466)

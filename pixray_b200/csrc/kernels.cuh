@@ -105,6 +105,28 @@ void pixel_synth(const float* z, int rows, int cols, int H, int W, float* pre, f
 void pixel_synth_backward(const float* g_img, const float* pre, int rows, int cols, int H, int W, float inv_scale,
                           float* z_grad, cudaStream_t st);
 
+// ------------------------------------------------------------------ polygon drawer (kernels_raster.cu; PixelDrawer.synth,
+// pixeldrawer.py:330-367).  Fixed polygons with one RGBA fill each, z = [n, 4]; 2 x 2 jittered samples per pixel
+// (raster_samples.cuh), even-odd fill, the topmost polygon containing a sample wins, pixel = mean of its samples.
+// The shapes are binned once into a uniform grid of RASTER_TILE-pixel tiles; each tile lists the polygons whose bounding
+// box meets it (closed intervals), topmost first.
+constexpr int RASTER_TILE = 16;
+struct RasterScene {
+  const float2* xy;       // [total_vertices] vertices, polygon k = xy[off[k] .. off[k+1])
+  const int* off;         // [n + 1]
+  const float4* bbox;     // [n] {xmin, ymin, xmax, ymax} of the vertices
+  const int* tile_start;  // [tiles_x * tiles_y + 1]
+  const int* tile_list;   // polygon indices per tile, topmost (highest index) first
+  int n, tiles_x;
+};
+// winner [4, H, W] int32 (-1: no polygon covers the sample); img [3, H, W] = sum of the winners' RGB / 4
+void raster_forward(const RasterScene& s, const float* z, int H, int W, uint64_t seed, int iter, int* winner, float* img,
+                    cudaStream_t st);
+// z_grad[k, c] = 0.25 * inv_scale * sum of g_img[c, p] over the samples k won (c < 3); z_grad[k, 3] = 0.  One warp per
+// polygon over its bounding box: one writer per element, fixed order, no atomics.
+void raster_backward(const RasterScene& s, const int* winner, const float* g_img, int H, int W, float inv_scale,
+                     float* z_grad, cudaStream_t st);
+
 // ------------------------------------------------------------------ FFT drawer (fftdrawer.py:78-84)
 struct FftPlans;  // cuFFT C2R / R2C plans (3 planes of H x W), resolved through dlopen
 FftPlans* fft_plans_create(int H, int W, cudaStream_t st, const char** err);
@@ -220,9 +242,20 @@ void prompt_loss(const float* e, int B, int D, const float* prompts, const float
 
 // ------------------------------------------------------------------ optimiser (pixray.py:538-539, 1484-1487)
 // Adam (bias-corrected, torch.optim.Adam semantics) on z with gradient g * inv_scale, then clip_z to per-channel
-// [zmin, zmax] (vqgan.py:202-204) or [0,1] when zmin == nullptr && clip01.
+// [zmin, zmax] (vqgan.py:202-204) or, when zmin == nullptr, by clip_mode:
+//   CLIP_NONE  no clamp
+//   CLIP_01    [0, 1] (fast_pixeldrawer.py:98-100)
+//   CLIP_RGBA  z is [n, 4] RGBA fill colours: RGB to [0, 1], alpha to [1, 1] (pixeldrawer.py:378-382)
+enum { CLIP_NONE = 0, CLIP_01 = 1, CLIP_RGBA = 2 };
+#ifdef __CUDACC__
+__device__ __forceinline__ float clip_mode_apply(int clip_mode, int i, float zi) {
+  if (clip_mode == CLIP_01) return fminf(fmaxf(zi, 0.f), 1.f);
+  if (clip_mode == CLIP_RGBA) return (i & 3) == 3 ? 1.f : fminf(fmaxf(zi, 0.f), 1.f);
+  return zi;
+}
+#endif
 void adam_clip_step(float* z, float* m, float* v, const float* g, float inv_scale, int n, int per_channel,
-                    const float* zmin, const float* zmax, int clip01, float lr, float b1, float b2, float eps, int t,
+                    const float* zmin, const float* zmax, int clip_mode, float lr, float b1, float b2, float eps, int t,
                     cudaStream_t st);
 
 // ------------------------------------------------------------------ device-side checkdrop + Adam (pixray.py:1090-1109, 1464-1512)
@@ -262,7 +295,7 @@ struct DropStatus {
   volatile int seq_end;
 };
 void adam_clip_managed(float* z, float* m, float* v, const float* g, float* best_z, float inv_scale, int n,
-                       int per_channel, const float* zmin, const float* zmax, int clip01, float b1, float b2,
+                       int per_channel, const float* zmin, const float* zmax, int clip_mode, float b1, float b2,
                        float eps, const float* losses, int n_losses, int iter, const DropConfig& cfg,
                        const DropState* cur, DropState* next, DropStatus* status_mapped, cudaStream_t st);
 // acc (=|+=) g: gradient accumulation over the `batches` passes of one iteration (pixray.py:1464-1482)

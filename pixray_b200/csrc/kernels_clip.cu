@@ -531,7 +531,7 @@ __global__ void __launch_bounds__(128) prompt_loss_kernel(const float* __restric
 
 __global__ void adam_clip_kernel(float* __restrict__ z, float* __restrict__ m, float* __restrict__ v,
                                  const float* __restrict__ g, float inv_scale, int n, int per_channel,
-                                 const float* __restrict__ zmin, const float* __restrict__ zmax, int clip01,
+                                 const float* __restrict__ zmin, const float* __restrict__ zmax, int clip_mode,
                                  float step_size, float b1, float b2, float eps, float inv_sqrt_bc2) {
   pdl_prologue();
   int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -546,8 +546,8 @@ __global__ void adam_clip_kernel(float* __restrict__ z, float* __restrict__ m, f
   if (zmin) {
     int c = i / per_channel;
     zi = fminf(fmaxf(zi, zmin[c]), zmax[c]);  // vqgan.py:202-204
-  } else if (clip01) {
-    zi = fminf(fmaxf(zi, 0.f), 1.f);  // fast_pixeldrawer.py:98-100
+  } else {
+    zi = clip_mode_apply(clip_mode, i, zi);
   }
   z[i] = zi;
 }
@@ -556,7 +556,7 @@ __global__ void adam_clip_kernel(float* __restrict__ z, float* __restrict__ m, f
 __global__ void adam_clip_managed_kernel(float* __restrict__ z, float* __restrict__ m, float* __restrict__ v,
                                          const float* __restrict__ g, float* __restrict__ best_z, float inv_scale, int n,
                                          int per_channel, const float* __restrict__ zmin, const float* __restrict__ zmax,
-                                         int clip01, float b1, float b2, float eps, const float* __restrict__ losses,
+                                         int clip_mode, float b1, float b2, float eps, const float* __restrict__ losses,
                                          int n_losses, int iter, DropConfig cfg, const DropState* __restrict__ cur,
                                          DropState* __restrict__ next, DropStatus* status) {
   pdl_prologue();
@@ -612,8 +612,8 @@ __global__ void adam_clip_managed_kernel(float* __restrict__ z, float* __restric
       if (zmin) {
         const int c = i / per_channel;
         zi = fminf(fmaxf(zi, zmin[c]), zmax[c]);
-      } else if (clip01) {
-        zi = fminf(fmaxf(zi, 0.f), 1.f);
+      } else {
+        zi = clip_mode_apply(clip_mode, i, zi);
       }
       z[i] = zi;
     }
@@ -794,22 +794,22 @@ void prompt_loss(const float* e, int B, int D, const float* prompts, const float
 }
 
 void adam_clip_step(float* z, float* m, float* v, const float* g, float inv_scale, int n, int per_channel,
-                    const float* zmin, const float* zmax, int clip01, float lr, float b1, float b2, float eps, int t,
+                    const float* zmin, const float* zmax, int clip_mode, float lr, float b1, float b2, float eps, int t,
                     cudaStream_t st) {
   // torch.optim.Adam: step_size = lr / (1 - b1^t); denom = sqrt(v) / sqrt(1 - b2^t) + eps
   const double bc1 = 1.0 - pow((double)b1, t), bc2 = 1.0 - pow((double)b2, t);
-  launch_pdl(adam_clip_kernel, dim3((n + 255) / 256), dim3(256), 0, st, z, m, v, g, inv_scale, n, per_channel, zmin, zmax, clip01,
+  launch_pdl(adam_clip_kernel, dim3((n + 255) / 256), dim3(256), 0, st, z, m, v, g, inv_scale, n, per_channel, zmin, zmax, clip_mode,
                                                     (float)(lr / bc1), b1, b2, eps, (float)(1.0 / sqrt(bc2)));
 }
 
 void adam_clip_managed(float* z, float* m, float* v, const float* g, float* best_z, float inv_scale, int n,
-                       int per_channel, const float* zmin, const float* zmax, int clip01, float b1, float b2,
+                       int per_channel, const float* zmin, const float* zmax, int clip_mode, float b1, float b2,
                        float eps, const float* losses, int n_losses, int iter, const DropConfig& cfg,
                        const DropState* cur, DropState* next, DropStatus* status_mapped, cudaStream_t st) {
   int grid = (n + 255) / 256;
   if (grid > 148 * 4) grid = 148 * 4;
   launch_pdl(adam_clip_managed_kernel, dim3(grid), dim3(256), 0, st, z, m, v, g, best_z, inv_scale, n, per_channel, zmin,
-             zmax, clip01, b1, b2, eps, losses, n_losses, iter, cfg, cur, next, status_mapped);
+             zmax, clip_mode, b1, b2, eps, losses, n_losses, iter, cfg, cur, next, status_mapped);
 }
 
 void accumulate_f32(const float* g, float* acc, long long n, int accumulate, cudaStream_t st) {

@@ -5,6 +5,7 @@
 #include "attn_tc.cuh"
 #include "color_jitter.cuh"
 #include "pool_bounds.cuh"
+#include "raster_samples.cuh"
 #include "kernels.cuh"
 #include <cstdio>
 #include <cstring>
@@ -202,6 +203,22 @@ __global__ void pool_bounds_kernel(int in_size, int out_size, int* starts, int* 
 extern "C" int pxr_test_pool_bounds(int in_size, int out_size, int* starts, int* ends) {
   if (in_size < 1 || out_size < 1 || !starts || !ends) return -1;
   pool_bounds_kernel<<<(out_size + 255) / 256, 256>>>(in_size, out_size, starts, ends);
+  return cudaDeviceSynchronize() == cudaSuccess ? 0 : -2;
+}
+
+// The polygon rasteriser's sample positions from the function its kernels call (raster_samples.cuh): DEVICE float
+// [H, W, 4, 2].
+namespace {
+__global__ void raster_samples_kernel(uint64_t seed, int iter, int H, int W, float* out) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= H * W) return;
+  for (int s = 0; s < 4; ++s) pxr::raster_sample(seed, iter, p % W, p / W, W, s, out[(size_t)p * 8 + 2 * s], out[(size_t)p * 8 + 2 * s + 1]);
+}
+}  // namespace
+
+extern "C" int pxr_test_raster_samples(uint64_t seed, int iter, int H, int W, float* out) {
+  if (H < 1 || W < 1 || !out) return -1;
+  raster_samples_kernel<<<(H * W + 255) / 256, 256>>>(seed, iter, H, W, out);
   return cudaDeviceSynchronize() == cudaSuccess ? 0 : -2;
 }
 

@@ -10,7 +10,7 @@ import torch
 
 from . import _lib
 
-DRAWER_VQGAN, DRAWER_PIXEL, DRAWER_FFT, DRAWER_VDIFF = 0, 1, 2, 3
+DRAWER_VQGAN, DRAWER_PIXEL, DRAWER_FFT, DRAWER_VDIFF, DRAWER_POLYGON = 0, 1, 2, 3, 4
 LOSS_SYMMETRY, LOSS_SATURATION, LOSS_PALETTE, LOSS_SMOOTHNESS, LOSS_EDGE, LOSS_GAUSSIAN, LOSS_AESTHETIC = range(7)
 ANCHOR_SPHERICAL, ANCHOR_MSE, ANCHOR_COS, ANCHOR_PIX = 0, 1, 2, 3
 FILTER_TILER, FILTER_WALLPAPER, FILTER_LOOKUP = range(3)
@@ -33,7 +33,7 @@ class EngineError(RuntimeError):
 class B200Engine:
     def __init__(self, *, drawer=DRAWER_VQGAN, image_hw=(256, 256), vqgan=None, grid=None, cutn=64, cut_size=224,
                  clip=(), noise_fac=0.1, seed=0, device=0, rank=0, world=1, grad_scale=0.0, lr_betas=(0.9, 0.999),
-                 adam_eps=1e-8, fft_decay=0.0, fft_colors=0.0, fft_contrast=0.0, cut_aspect=1.0):
+                 adam_eps=1e-8, fft_decay=0.0, fft_colors=0.0, fft_contrast=0.0, cut_aspect=1.0, polygons=None):
         if not torch.cuda.is_available():
             raise EngineError("pixray_b200 needs a CUDA device (H100); there is no CPU fallback")
         self.lib = _lib.load()
@@ -56,6 +56,14 @@ class B200Engine:
         elif drawer == DRAWER_FFT:
             # FftDrawer params (fftdrawer.py:57-61): rfft2 spectrum [1, 3, H, W/2+1, 2]
             self.z_shape = (1, 3, image_hw[0], image_hw[1] // 2 + 1, 2)
+        elif drawer == DRAWER_POLYGON:
+            # PixelDrawer's shaped cells (pixeldrawer.py:200-304): polygons = (xy [total_vertices, 2], offsets [n + 1]) from
+            # pixel_shapes.polygons; z = the [n, 4] RGBA fill colours, get_z's layout (pixeldrawer.py:384-390)
+            if polygons is None:
+                raise EngineError("drawer=DRAWER_POLYGON needs polygons=(xy, offsets)")
+            xy = np.ascontiguousarray(np.asarray(polygons[0], dtype=np.float32).reshape(-1, 2))
+            off = np.ascontiguousarray(np.asarray(polygons[1], dtype=np.int32).reshape(-1))
+            self.z_shape = (int(off.size) - 1, 4)
         else:
             cfg.grid_rows, cfg.grid_cols = grid
             self.z_shape = (1, 3, grid[0], grid[1])
@@ -89,6 +97,10 @@ class B200Engine:
             raise EngineError(f"pxr_create failed ({rc}): {self.lib.pxr_last_error(None).decode()}")
         self.h = h
         self._keep = []
+        if drawer == DRAWER_POLYGON:
+            rc = self.lib.pxr_set_polygons(self.h, xy.ctypes.data_as(C.c_void_p), off.ctypes.data_as(C.c_void_p),
+                                           int(off.size) - 1)
+            self._check(rc, "pxr_set_polygons")
         self._ext = None  # torch view of the engine's stream (ordering against torch-side producers of z / noise)
 
     # ------------------------------------------------------------------ plumbing
@@ -349,6 +361,10 @@ class B200Engine:
         self._check(self.lib.pxr_synth(self.h, self._p(z), self._p(out)), "pxr_synth")
         self.sync()
         return out
+
+    def set_synth_iteration(self, it):
+        """The iteration the next synth() renders (drawer.synth(cur_iteration)): keys the polygon drawer's samples."""
+        self._check(self.lib.pxr_set_synth_iteration(self.h, int(it)), "pxr_set_synth_iteration")
 
     def vqgan_encode(self, img):
         """z = model.encode(img)[0] (vqgan.py:174-185): img [1, 3, H, W] in [-1, 1] -> z [1, C, h, w] (codebook rows)."""

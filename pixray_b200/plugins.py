@@ -194,6 +194,104 @@ class FastPixelDrawer(DrawingInterface):
         return self.z.clone()
 
 
+class PixelDrawer(DrawingInterface):
+    """pixeldrawer.py:110-406 for the shaped cells (pixel_type rectshift / hex / tri / diamond / knit): fixed polygons
+    (pixel_shapes.py), z = their [n, 4] RGBA fill colours, rendered by the engine's polygon rasteriser
+    (PXR_DRAWER_POLYGON).  The drawer owns its Adam rate, 0.03 / decay_divisor, which get_opts reports for the engine's
+    fused Adam like FftDrawer does.  pixel_type rect keeps the square-grid fast path (FastPixelDrawer, chosen in
+    api.do_init)."""
+
+    @staticmethod
+    def add_settings(parser):
+        from .api import str2bool
+        parser.add_argument("--pixel_size", nargs=2, type=int, help="Pixel size (width height)", default=None, dest="pixel_size")
+        parser.add_argument("--pixel_scale", type=float, help="Pixel scale", default=None, dest="pixel_scale")
+        parser.add_argument("--pixel_type", type=str, help="rect, rectshift, hex, tri, diamond, knit", default="rect", dest="pixel_type")
+        parser.add_argument("--pixel_edge_check", type=str2bool, help="ensure grid is symmetric", default=True, dest="pixel_edge_check")
+        parser.add_argument("--pixel_iso_check", type=str2bool, help="ensure tri and hex shapes are w/h scaled", default=True, dest="pixel_iso_check")
+        return parser
+
+    @staticmethod
+    def grid_for(settings, size, verbose=True):
+        """(num_rows, num_cols) of the settings on a canvas of size (width, height) (pixeldrawer.py:123-177)."""
+        from . import pixel_shapes
+        return pixel_shapes.grid_for(size, settings.pixel_type, getattr(settings, "pixel_size", None),
+                                     getattr(settings, "pixel_scale", None), getattr(settings, "pixel_edge_check", True),
+                                     getattr(settings, "pixel_iso_check", True), verbose=verbose)
+
+    def __init__(self, settings, session: Session):
+        super().__init__(settings)
+        from . import pixel_shapes
+        self.session = session
+        self.pixel_type = pixel_shapes.check_pixel_type(settings.pixel_type)
+        self.canvas_height, self.canvas_width = session.engine.image_hw
+        self.num_rows, self.num_cols = PixelDrawer.grid_for(settings, (self.canvas_width, self.canvas_height), verbose=False)
+        self.z = None
+        self.img = None
+
+    def load_model(self, settings, device):
+        self.device = device
+
+    def get_opts(self, decay_divisor=1):
+        return [{"lr": 0.03 / decay_divisor}]
+
+    def get_num_resolutions(self):
+        return None
+
+    def _colours(self, tensor):
+        from . import pixel_shapes
+        c = pixel_shapes.init_colours(tensor, self.num_rows, self.num_cols, self.pixel_type)
+        return torch.from_numpy(c).to(self.session.engine.device, torch.float32).contiguous()
+
+    def init_from_tensor(self, init_tensor):
+        """encode_image (pixeldrawer.py:200-304): every cell averages up to 4 x 4 pixels of (init_tensor + 1) / 2.  A start
+        image is required: init_tensor None raises ValueError."""
+        self.z = self._colours(init_tensor)
+
+    def reapply_from_tensor(self, new_tensor):
+        new_z = self._colours(new_tensor)
+        with torch.no_grad():
+            self.z.copy_(new_z)
+
+    def get_z_from_tensor(self, ref_tensor):
+        return None
+
+    def synth(self, cur_iteration):
+        """The render of cur_iteration's sample positions, [1, 3, H, W] (RGB: the background is transparent black)."""
+        eng = self.session.engine
+        eng.set_synth_iteration(cur_iteration)
+        self.img = eng.synth(self.z)
+        return self.img
+
+    @torch.no_grad()
+    def to_image(self):
+        """The current colours rendered with the session's iteration, clipped to [0, 1] (pixeldrawer.py:369-376).  The
+        reference shows its last render, which its loop refreshes every iteration through synth; here the fused iteration
+        renders inside the engine, so the image is rendered afresh from the current z."""
+        from PIL import Image
+        img = self.synth(self.session.cur_iteration)
+        arr = np.uint8(np.clip(img[0].detach().cpu().numpy().transpose(1, 2, 0), 0, 1) * 255)
+        return Image.fromarray(arr, mode="RGB")
+
+    def clip_z(self):
+        with torch.no_grad():
+            self.z[:, :3].clamp_(0.0, 1.0)
+            self.z[:, 3].clamp_(1.0, 1.0)
+
+    def get_z(self):
+        return self.z
+
+    def set_z(self, new_z):
+        if self.z is None:
+            self.z = new_z.detach().to(self.session.engine.device, torch.float32).contiguous().clone()
+            return self.z
+        with torch.no_grad():
+            return self.z.copy_(new_z)
+
+    def get_z_copy(self):
+        return self.z.clone()
+
+
 class VdiffDrawer(DrawingInterface):
     """vdiff.py:58-190 (cc12m_1): z = the noisy image x; synth = one v-prediction step + ClampWithGrad; after every
     optimiser step the loop re-noises x (`makenoise`, pixray.py:1489-1495) and builds a fresh Adam."""
