@@ -286,7 +286,7 @@ typedef struct {
   int M, N, K, block_n, fmt;
   float alpha;
   const float* bias;
-  int bias_per_row, act;
+  int bias_per_row, act; /* act: 0 none, 1 QuickGELU (+ pre-activation to aux_out), 2 QuickGELU backward; others are refused */
   const void* aux_in;
   void* aux_out;
   const float* res_f32;
@@ -296,7 +296,6 @@ typedef struct {
   long long ldc, c_bs0, c_bs1;
   void* stream;
   int repeat;
-  int n_store; /* fused-softmax epilogues (act 3 / 4): zero-fill columns [N, n_store) */
   int cta_group; /* ignored: sm_90 has no CTA-pair MMA, every GEMM runs single-CTA tiles (kept for the struct layout) */
   int tma_epi;   /* 0 auto (tensor-map epilogue when the tensors allow it), -1 force the generic epilogue */
 } pxr_test_gemm_desc;

@@ -58,7 +58,7 @@ class TestGemmDesc(C.Structure):
         ("aux_in", C.c_void_p), ("aux_out", C.c_void_p), ("res_f32", C.c_void_p), ("res_f16", C.c_void_p),
         ("out_f32", C.c_void_p), ("out_f16", C.c_void_p),
         ("ldc", C.c_longlong), ("c_bs0", C.c_longlong), ("c_bs1", C.c_longlong),
-        ("stream", C.c_void_p), ("repeat", C.c_int), ("n_store", C.c_int), ("cta_group", C.c_int), ("tma_epi", C.c_int),
+        ("stream", C.c_void_p), ("repeat", C.c_int), ("cta_group", C.c_int), ("tma_epi", C.c_int),
     ]
 
 

@@ -34,7 +34,6 @@ class Engine {
   int num_sms = 132;
   int fmt = 0;
   float S = 4096.f;  // grad scale
-  bool fuse_softmax = false;  // PXR_FUSE_SOFTMAX=1: attention softmax inside the GEMM epilogue (see DESIGN.md 4)
   bool gn_coop = true;        // PXR_GN_COOP=0: three-kernel GroupNorm instead of the cooperative single-kernel one
   bool stream16 = true;       // the ViT residual stream and its gradient in fp16, like the reference's CUDA path (clip.load gives a half model, slip.py:176); PXR_CLIP_STREAM=32 keeps them in fp32
   bool fused_attn = true;     // PXR_FUSED_ATTN=0: fall back to the batched-GEMM attention (attn_tc.cu covers T <= 240)
@@ -155,8 +154,6 @@ class Engine {
       float *stats1, *stats2;
       act_t *qkv, *P, *u;
       act_t* o = nullptr;     // fused attention: per-layer attention output (backward needs D = dO . O)
-      float* lse = nullptr;   // fused attention: row log-sum-exp [B, heads, T]
-      std::shared_ptr<AttnPlan> attn;
     };
     std::vector<Layer> layers;
     // buffers
@@ -391,7 +388,7 @@ class Engine {
     if (N <= 128 && m_tiles * 1 >= num_sms / 2) return narrow(N);
     int best = 0;
     double best_cost = 1e30;
-    for (int bn = 128; bn >= 64; bn -= 64) {  // gemm_tc.cu: plain-epilogue tiles are at most 128 wide
+    for (int bn = 128; bn >= 64; bn -= 64) {  // gemm_tc.cu: tiles are at most 128 wide
       if (bn % step) continue;
       const long long tiles = m_tiles * ((N + bn - 1) / bn);
       const long long waves = (tiles + num_sms - 1) / num_sms;
@@ -453,6 +450,21 @@ class Engine {
   }
   float* splitk_ws = nullptr;
   size_t splitk_ws_elems = 0;
+  // Split count for an output of `rows` x N in `tiles` tiles over nkb k-blocks: enough splits to fill the idle SMs with at
+  // least four k-blocks each; 1 (no split) unless the epilogue is an fp16 store the reduce can apply (bias, fp16 residual)
+  // and the partial sums fit the workspace.
+  int splitk_count(const GemmEpilogue& e, long long rows, int N, int nkb, long long tiles) const {
+    if (!conv_splitk || !splitk_ws || !e.out_f16 || e.out_f32 || e.res_f32 || e.aux_out || e.act != ACT_NONE || N % 8 ||
+        e.ldc % 8 || tiles * 2 > num_sms || nkb < 8)
+      return 1;
+    int splits = 1;
+    const int want = (int)std::min<long long>(num_sms / tiles, nkb / 4);
+    if (want >= 2) {
+      const int kbps = (nkb + want - 1) / want;
+      splits = (nkb + kbps - 1) / kbps;
+    }
+    return (size_t)splits * rows * N > splitk_ws_elems ? 1 : splits;
+  }
   void add_conv(OpList& l, const act_t* in, int H, int Wd, int cin, const act_t* wt, int cout_pad, int n_out, int ks,
                 const GemmEpilogue& e) {
     const long long m_tiles = (long long)(H * Wd + 127) / 128;
@@ -462,17 +474,7 @@ class Engine {
     char kind[32];
     snprintf(kind, sizeof kind, "conv%dx%d", ks, ks);
     const int nkb = ks * ks * cin / 64;
-    const long long tiles = m_tiles * ((n_out + bn - 1) / bn);
-    int splits = 1;
-    if (conv_splitk && splitk_ws && e.out_f16 && !e.out_f32 && !e.res_f32 && !e.aux_out && e.act == ACT_NONE &&
-        n_out % 8 == 0 && e.ldc % 8 == 0 && tiles * 2 <= num_sms && nkb >= 8) {
-      const int want = (int)std::min<long long>(num_sms / tiles, nkb / 4);
-      if (want >= 2) {
-        const int kbps = (nkb + want - 1) / want;
-        splits = (nkb + kbps - 1) / kbps;
-      }
-      if ((size_t)splits * H * Wd * n_out > splitk_ws_elems) splits = 1;
-    }
+    const int splits = splitk_count(e, (long long)H * Wd, n_out, nkb, m_tiles * ((n_out + bn - 1) / bn));
     auto plan = std::make_shared<GemmPlan>();
     char buf[256] = {0};
     if (splits > 1) {
@@ -519,16 +521,7 @@ class Engine {
     const int bn = pick_bn(N, false, (M + 127) / 128);
     const int nkb = (K + GEMM_BLOCK_K - 1) / GEMM_BLOCK_K;
     const long long tiles = (long long)((M + 127) / 128) * ((N + bn - 1) / bn);
-    int splits = 1;
-    if (conv_splitk && splitk_ws && e.out_f16 && !e.out_f32 && !e.res_f32 && !e.aux_out && e.act == ACT_NONE && e.alpha == 1.f &&
-        N % 8 == 0 && e.ldc % 8 == 0 && tiles * 2 <= num_sms && nkb >= 8) {
-      const int want = (int)std::min<long long>(num_sms / tiles, nkb / 4);
-      if (want >= 2) {
-        const int kbps = (nkb + want - 1) / want;
-        splits = (nkb + kbps - 1) / kbps;
-      }
-      if ((size_t)splits * M * N > splitk_ws_elems) splits = 1;
-    }
+    const int splits = e.alpha == 1.f ? splitk_count(e, M, N, nkb, tiles) : 1;  // the reduce applies no alpha
     if (splits <= 1) {
       add_gemm(l, A, B, M, N, K, e);
       return;
@@ -581,27 +574,60 @@ class Engine {
   float* enc_z = nullptr;     // [C, hw] result
   void build_vqgan_encoder();
   NormW load_norm(int mod, const std::string& prefix, int c);
-  Act new_act(int H, int Wd, int C) {
+  Act new_act(int H, int Wd, int C, bool grad = true) {
     Act a;
     a.H = H;
     a.W = Wd;
     a.C = C;
     a.p = dalloc<act_t>((size_t)H * Wd * C);
-    a.g = dalloc<act_t>((size_t)H * Wd * C);
+    if (grad) a.g = dalloc<act_t>((size_t)H * Wd * C);
     return a;
   }
+  // the codebook [n_embed, z_channels], its transpose and squared row norms, as the nearest-code search reads them
+  // (build_vqgan; the encoder's quantiser reads the same copies)
+  float *vq_cb = nullptr, *vq_cbT = nullptr, *vq_c2 = nullptr;
   // decoder blocks: append forward ops to drawer_fwd, push the backward closure list (reverse order) to bwd_stack
   std::vector<OpList> bwd_stack;
   float* gn_part = nullptr;  // scratch for GN partial sums (sized for the largest layer)
   GridBarrier gn_bar;        // grid barrier state of the single-kernel GroupNorm
   Act conv_fwd_bwd(const Act& x, const ConvW& w, OpList& bwd);
-  Act resblock(const Act& x, const std::string& prefix, int cin, int cout);
-  Act attnblock(const Act& x, const std::string& prefix, int c);
   Act upsample(const Act& x, const std::string& prefix);
   struct GNSaved {
     float* stats;
     float* gstats;
   };
+  // taming ResnetBlock / AttnBlock, shared by the decoder and the encoder: the forward builder appends to `l` and returns
+  // what the backward builder needs (grad = false allocates no gradient buffers: the encoder); the backward builder
+  // pushes its op list onto bwd_stack
+  struct ResBlock {
+    NormW n1, n2;
+    ConvW c1, c2, sc;
+    Act x, a1, h1, a2, out;
+    GNSaved s1, s2;
+  };
+  struct AttnBlock {
+    NormW n;
+    act_t* wqkv;
+    ConvW po;
+    Act x, a, O, out;
+    act_t* gqkv;
+    GNSaved s;
+    OpList attn_bwd;  // dO -> gqkv, from add_attention
+  };
+  ResBlock resblock_fwd(OpList& l, const Act& x, const std::string& prefix, int cin, int cout, bool grad);
+  void resblock_bwd(const ResBlock& r);
+  AttnBlock attnblock_fwd(OpList& l, const Act& x, const std::string& prefix, int c, bool grad);
+  void attnblock_bwd(const AttnBlock& a);
+  // Self-attention O = softmax(scale q k^T) v of `images` x `heads` heads of width d over T tokens, in attn_tc.cuh's
+  // layout: qkv and gqkv [images T, 3 heads d] (q | k | v, head h at column h d of each third), o and d_o
+  // [images T, heads d].  Appends the forward to `fwd` and, when `bwd` is given, the backward (d_o -> gqkv) to *bwd.
+  // multihead (the ViT, the U-Net): the fused kernels when attn_fused() holds, else the batched-GEMM chain with tile
+  // widths fixed for the head-batched shapes; otherwise (taming's AttnBlock) always the chain, tile widths by add_gemm.
+  // The chain's P is allocated here (and returned; nullptr on the fused path), its dP too unless the caller passes a
+  // scratch that several calls share.
+  act_t* add_attention(OpList& fwd, OpList* bwd, const act_t* qkv, act_t* o, const act_t* d_o, act_t* gqkv, int images,
+                       int heads, int T, int d, float scale, bool multihead, act_t* dP = nullptr);
+  bool attn_fused(int T, int d, int heads) const { return fused_attn && attn_supported(T, d, heads * d); }
   GNSaved add_gn(OpList& l, const Act& x, const NormW& n, int swish, act_t* y);
   void add_gn_bwd(OpList& l, const act_t* dy, const act_t* x, const GNSaved& s, const NormW& n, int px, int C, int swish,
                   const act_t* dres, act_t* dx);
@@ -680,7 +706,6 @@ void Engine::create() {
   fmt = cfg.op_dtype;
   if (fmt != PXR_DTYPE_F16) throw EngineError(-5, "only PXR_DTYPE_F16 operands are wired through the pointwise kernels");
   if (cfg.grad_scale > 0) S = cfg.grad_scale;
-  if (const char* fs = getenv("PXR_FUSE_SOFTMAX")) fuse_softmax = atoi(fs) != 0;
   if (const char* fa = getenv("PXR_FUSED_ATTN")) fused_attn = atoi(fa) != 0;
   if (const char* cs16 = getenv("PXR_CLIP_STREAM")) stream16 = atoi(cs16) != 32;
   if (const char* gc = getenv("PXR_GN_COOP")) gn_coop = atoi(gc) != 0;
@@ -813,70 +838,79 @@ Act Engine::conv_fwd_bwd(const Act& x, const ConvW& w, OpList& bwd) {
   return y;
 }
 
-Act Engine::resblock(const Act& x, const std::string& prefix, int cin, int cout) {
-  NormW n1 = load_norm(PXR_MOD_VQGAN, prefix + ".norm1", cin), n2 = load_norm(PXR_MOD_VQGAN, prefix + ".norm2", cout);
-  ConvW c1 = load_conv(prefix + ".conv1", cin, cout, 3), c2 = load_conv(prefix + ".conv2", cout, cout, 3);
-  const int H = x.H, Wd = x.W, px = x.pixels();
-  Act a1 = new_act(H, Wd, cin), h1 = new_act(H, Wd, cout), a2 = new_act(H, Wd, cout), out = new_act(H, Wd, cout);
-  cudaStream_t cs = st;
-  float* part = gn_part;
-  // ---- forward
-  GNSaved s1 = add_gn(drawer_fwd, x, n1, 1, a1.p);
+Engine::ResBlock Engine::resblock_fwd(OpList& l, const Act& x, const std::string& prefix, int cin, int cout, bool grad) {
+  ResBlock r;
+  r.x = x;
+  r.n1 = load_norm(PXR_MOD_VQGAN, prefix + ".norm1", cin);
+  r.n2 = load_norm(PXR_MOD_VQGAN, prefix + ".norm2", cout);
+  r.c1 = load_conv(prefix + ".conv1", cin, cout, 3);
+  r.c2 = load_conv(prefix + ".conv2", cout, cout, 3);
+  const int H = x.H, Wd = x.W;
+  r.a1 = new_act(H, Wd, cin, grad);
+  r.h1 = new_act(H, Wd, cout, grad);
+  r.a2 = new_act(H, Wd, cout, grad);
+  r.out = new_act(H, Wd, cout, grad);
+  r.s1 = add_gn(l, x, r.n1, 1, r.a1.p);
   {
     GemmEpilogue e;
-    e.bias = c1.bias;
-    e.out_f16 = h1.p;
+    e.bias = r.c1.bias;
+    e.out_f16 = r.h1.p;
     e.ldc = cout;
-    add_conv(drawer_fwd, a1.p, H, Wd, cin, c1.w, c1.cout_pad, cout, 3, e);
+    add_conv(l, r.a1.p, H, Wd, cin, r.c1.w, r.c1.cout_pad, cout, 3, e);
   }
-  GNSaved s2 = add_gn(drawer_fwd, h1, n2, 1, a2.p);
-  ConvW sc;
+  r.s2 = add_gn(l, r.h1, r.n2, 1, r.a2.p);
   if (cin != cout) {
-    sc = load_conv(prefix + ".nin_shortcut", cin, cout, 1);
+    r.sc = load_conv(prefix + ".nin_shortcut", cin, cout, 1);
     GemmEpilogue e;
-    e.bias = sc.bias;
-    e.out_f16 = out.p;
+    e.bias = r.sc.bias;
+    e.out_f16 = r.out.p;
     e.ldc = cout;
-    add_conv(drawer_fwd, x.p, H, Wd, cin, sc.w, sc.cout_pad, cout, 1, e);
+    add_conv(l, x.p, H, Wd, cin, r.sc.w, r.sc.cout_pad, cout, 1, e);
   }
   {
     GemmEpilogue e;
-    e.bias = c2.bias;
-    e.res_f16 = (cin != cout) ? out.p : x.p;
-    e.out_f16 = out.p;
+    e.bias = r.c2.bias;
+    e.res_f16 = (cin != cout) ? r.out.p : x.p;
+    e.out_f16 = r.out.p;
     e.ldc = cout;
-    add_conv(drawer_fwd, a2.p, H, Wd, cout, c2.w, c2.cout_pad, cout, 3, e);
+    add_conv(l, r.a2.p, H, Wd, cout, r.c2.w, r.c2.cout_pad, cout, 3, e);
   }
-  // ---- backward (execution order)
-  OpList b;
+  return r;
+}
+
+void Engine::resblock_bwd(const ResBlock& r) {
+  const Act& x = r.x;
+  const int H = x.H, Wd = x.W, px = x.pixels(), cin = r.c1.cin, cout = r.c1.cout;
+  OpList b;  // execution order
   {
     GemmEpilogue e;
-    e.out_f16 = a2.g;
+    e.out_f16 = r.a2.g;
     e.ldc = cout;
-    add_conv(b, out.g, H, Wd, c2.cout_k, c2.wd, c2.cin_rows, cout, 3, e);
+    add_conv(b, r.out.g, H, Wd, r.c2.cout_k, r.c2.wd, r.c2.cin_rows, cout, 3, e);
   }
-  add_gn_bwd(b, a2.g, h1.p, s2, n2, px, cout, 1, nullptr, h1.g);
+  add_gn_bwd(b, r.a2.g, r.h1.p, r.s2, r.n2, px, cout, 1, nullptr, r.h1.g);
   {
     GemmEpilogue e;
-    e.out_f16 = a1.g;
+    e.out_f16 = r.a1.g;
     e.ldc = cin;
-    add_conv(b, h1.g, H, Wd, c1.cout_k, c1.wd, c1.cin_rows, cin, 3, e);
+    add_conv(b, r.h1.g, H, Wd, r.c1.cout_k, r.c1.wd, r.c1.cin_rows, cin, 3, e);
   }
   if (cin != cout) {
     GemmEpilogue e;
     e.out_f16 = x.g;
     e.ldc = cin;
-    add_conv(b, out.g, H, Wd, sc.cout_k, sc.wd, sc.cin_rows, cin, 1, e);
-    add_gn_bwd(b, a1.g, x.p, s1, n1, px, cin, 1, x.g, x.g);
+    add_conv(b, r.out.g, H, Wd, r.sc.cout_k, r.sc.wd, r.sc.cin_rows, cin, 1, e);
+    add_gn_bwd(b, r.a1.g, x.p, r.s1, r.n1, px, cin, 1, x.g, x.g);
   } else {
-    add_gn_bwd(b, a1.g, x.p, s1, n1, px, cin, 1, out.g, x.g);
+    add_gn_bwd(b, r.a1.g, x.p, r.s1, r.n1, px, cin, 1, r.out.g, x.g);
   }
   bwd_stack.push_back(std::move(b));
-  return out;
 }
 
-Act Engine::attnblock(const Act& x, const std::string& prefix, int c) {
-  NormW n = load_norm(PXR_MOD_VQGAN, prefix + ".norm", c);
+Engine::AttnBlock Engine::attnblock_fwd(OpList& l, const Act& x, const std::string& prefix, int c, bool grad) {
+  AttnBlock a;
+  a.x = x;
+  a.n = load_norm(PXR_MOD_VQGAN, prefix + ".norm", c);
   // fused q/k/v 1x1 convs: weight [3c, c]
   std::vector<float> wq, bq;
   for (const char* nm : {".q", ".k", ".v"}) {
@@ -885,105 +919,144 @@ Act Engine::attnblock(const Act& x, const std::string& prefix, int c) {
     wq.insert(wq.end(), w.data.begin(), w.data.end());
     bq.insert(bq.end(), b.data.begin(), b.data.end());
   }
-  act_t* wqkv = upload_f16(wq);
+  a.wqkv = upload_f16(wq);
   float* bqkv = upload(bq);
-  ConvW po = load_conv(prefix + ".proj_out", c, c, 1);
-  const int T = x.pixels(), ldT = round_up(T, 8);
-  const float alpha = 1.f / std::sqrt((float)c);
-  Act a = new_act(x.H, x.W, c), O = new_act(x.H, x.W, c), out = new_act(x.H, x.W, c);
+  a.po = load_conv(prefix + ".proj_out", c, c, 1);
+  const int T = x.pixels();
+  a.a = new_act(x.H, x.W, c, grad);
+  a.O = new_act(x.H, x.W, c, grad);
+  a.out = new_act(x.H, x.W, c, grad);
   act_t* qkv = dalloc<act_t>((size_t)T * 3 * c);
-  act_t* gqkv = dalloc<act_t>((size_t)T * 3 * c);
-  act_t* P = dalloc<act_t>((size_t)T * ldT);
-  act_t* dP = dalloc<act_t>((size_t)T * ldT);
-  cudaStream_t cs = st;
-  float* part = gn_part;
-  // ---- forward
-  GNSaved s = add_gn(drawer_fwd, x, n, 0, a.p);
+  a.gqkv = grad ? dalloc<act_t>((size_t)T * 3 * c) : nullptr;
+  a.s = add_gn(l, x, a.n, 0, a.a.p);
   {
     GemmEpilogue e;
     e.bias = bqkv;
     e.out_f16 = qkv;
     e.ldc = 3 * c;
-    add_gemm(drawer_fwd, opK(a.p, c, T, c), opK(wqkv, c, 3 * c, c), T, 3 * c, c, e);
+    add_gemm(l, opK(a.a.p, c, T, c), opK(a.wqkv, c, 3 * c, c), T, 3 * c, c, e);
   }
-  const bool fuse_sm = fuse_softmax && T <= 256;  // whole row in one accumulator tile -> softmax in the GEMM epilogue
+  add_attention(l, grad ? &a.attn_bwd : nullptr, qkv, a.O.p, a.O.g, a.gqkv, 1, 1, T, c, 1.f / std::sqrt((float)c), false);
   {
     GemmEpilogue e;
-    e.alpha = alpha;
-    e.out_f16 = P;
-    e.ldc = ldT;
-    if (fuse_sm) {
-      e.act = ACT_SOFTMAX;
-      e.n_store = ldT;
-    }
-    add_gemm(drawer_fwd, opK(qkv, 3 * c, T, c), opK(qkv + c, 3 * c, T, c), T, T, c, e, fuse_sm ? round_up(T, 16) : 0);
-  }
-  if (!fuse_sm) drawer_fwd.add(1, [=] { softmax_forward(P, T, T, ldT, cs); }, 0.0, "softmax_forward");
-  {
-    GemmEpilogue e;
-    e.out_f16 = O.p;
-    e.ldc = c;
-    add_gemm(drawer_fwd, opK(P, ldT, T, ldT), opMN(qkv + 2 * c, 3 * c, c, T), T, c, T, e);
-  }
-  {
-    GemmEpilogue e;
-    e.bias = po.bias;
+    e.bias = a.po.bias;
     e.res_f16 = x.p;
-    e.out_f16 = out.p;
+    e.out_f16 = a.out.p;
     e.ldc = c;
-    add_conv(drawer_fwd, O.p, x.H, x.W, c, po.w, po.cout_pad, c, 1, e);
+    add_conv(l, a.O.p, x.H, x.W, c, a.po.w, a.po.cout_pad, c, 1, e);
   }
-  // ---- backward
+  return a;
+}
+
+void Engine::attnblock_bwd(const AttnBlock& a) {
+  const Act& x = a.x;
+  const int T = x.pixels(), c = x.C;
   OpList b;
   {
     GemmEpilogue e;
-    e.out_f16 = O.g;
+    e.out_f16 = a.O.g;
     e.ldc = c;
-    add_conv(b, out.g, x.H, x.W, po.cout_k, po.wd, po.cin_rows, c, 1, e);
+    add_conv(b, a.out.g, x.H, x.W, a.po.cout_k, a.po.wd, a.po.cin_rows, c, 1, e);
   }
-  {  // dP = dO v^T ; dS = alpha * P * (dP - <P, dP>) fused in the epilogue when the row fits one tile
+  b.append(a.attn_bwd);
+  {  // da = dqkv Wqkv   (B = Wqkv stored [3c (k), c (n)] -> MN-major)
+    GemmEpilogue e;
+    e.out_f16 = a.a.g;
+    e.ldc = c;
+    add_gemm(b, opK(a.gqkv, 3 * c, T, 3 * c), opMN(a.wqkv, c, c, 3 * c), T, c, 3 * c, e);
+  }
+  add_gn_bwd(b, a.a.g, x.p, a.s, a.n, T, c, 0, a.out.g, x.g);
+  bwd_stack.push_back(std::move(b));
+}
+
+act_t* Engine::add_attention(OpList& fwd, OpList* bwd, const act_t* qkv, act_t* o, const act_t* d_o, act_t* gqkv,
+                             int images, int heads, int T, int d, float scale, bool multihead, act_t* dP) {
+  const int W = heads * d, ldT = round_up(T, 8);
+  cudaStream_t cs = st;
+  if (multihead && attn_fused(T, d, heads)) {  // S, softmax and PV in one kernel; S / P never leave the SM
+    float* lse = dalloc<float>((size_t)images * heads * T);
+    auto ap = std::make_shared<AttnPlan>();
+    char buf[256] = {0};
+    int rc = attn_plan_make(ap.get(), qkv, o, d_o, gqkv, lse, images, T, heads, W, scale, num_sms, buf, sizeof buf);
+    if (rc) throw EngineError(rc, std::string("attention plan: ") + buf);
+    char lab[96];
+    snprintf(lab, sizeof lab, "attn_fwd B=%d T=%d heads=%d", images, T, heads);
+    fwd.add(1, [ap, cs] { attn_forward_launch(*ap, cs); }, ap->flops_fwd, lab, ap->bytes_fwd);
+    if (bwd) {  // dQ, dK, dV in one kernel (recomputes P from Q, K and the saved log-sum-exp)
+      snprintf(lab, sizeof lab, "attn_bwd B=%d T=%d heads=%d", images, T, heads);
+      bwd->add(2, [ap, cs] { attn_backward_launch(*ap, cs); }, ap->flops_bwd, lab, ap->bytes_bwd);
+    }
+    return nullptr;
+  }
+  // batched GEMMs over (head, image) around the row softmax; P and dP have a padded row pitch
+  const int bn_s = multihead ? pick_bn(T, false, 1000) : 0, bn_d = multihead ? 64 : 0;  // T- / d-wide outputs
+  const long long qs0 = d, qs1 = (long long)T * 3 * W;                          // (head, image) strides in qkv / gqkv
+  const long long os0 = d, os1 = (long long)T * W;                              // ... in o / d_o
+  const long long ps0 = (long long)T * ldT, ps1 = (long long)heads * T * ldT;   // ... in P / dP
+  const int rows = images * heads * T;
+  act_t* P = dalloc<act_t>((size_t)rows * ldT);
+  {  // S = scale q k^T
+    GemmEpilogue e;
+    e.alpha = scale;
+    e.out_f16 = P;
+    e.ldc = ldT;
+    e.bs0 = ps0;
+    e.bs1 = ps1;
+    add_gemm(fwd, opK(qkv, 3 * W, T, d, heads, qs0, images, qs1), opK(qkv + W, 3 * W, T, d, heads, qs0, images, qs1), T,
+             T, d, e, bn_s);
+  }
+  fwd.add(1, [=] { softmax_forward(P, rows, T, ldT, cs); }, 0.0, "softmax_forward");
+  {  // O = P v
+    GemmEpilogue e;
+    e.out_f16 = o;
+    e.ldc = W;
+    e.bs0 = os0;
+    e.bs1 = os1;
+    add_gemm(fwd, opK(P, ldT, T, ldT, heads, ps0, images, ps1), opMN(qkv + 2 * W, 3 * W, d, T, heads, qs0, images, qs1),
+             T, d, T, e, bn_d);
+  }
+  if (!bwd) return P;
+  if (!dP) dP = dalloc<act_t>((size_t)rows * ldT);
+  {  // dP = dO v^T
     GemmEpilogue e;
     e.out_f16 = dP;
     e.ldc = ldT;
-    if (fuse_sm) {
-      e.act = ACT_SOFTMAX_BWD;
-      e.aux_in = P;
-      e.alpha = alpha;
-      e.n_store = ldT;
-    }
-    add_gemm(b, opK(O.g, c, T, c), opK(qkv + 2 * c, 3 * c, T, c), T, T, c, e, fuse_sm ? round_up(T, 16) : 0);
+    e.bs0 = ps0;
+    e.bs1 = ps1;
+    add_gemm(*bwd, opK(d_o, W, T, d, heads, os0, images, os1), opK(qkv + 2 * W, 3 * W, T, d, heads, qs0, images, qs1), T,
+             T, d, e, bn_s);
   }
-  if (!fuse_sm) b.add(1, [=] { softmax_backward(P, dP, T, T, ldT, cs); }, 0.0, "softmax_backward");
-  const float alpha_b = fuse_sm ? 1.f : alpha;  // fused path already carries alpha in dS
-  {  // dq = alpha dS k
+  bwd->add(1, [=] { softmax_backward(P, dP, rows, T, ldT, cs); }, 0.0, "softmax_backward");  // dS, in place of dP
+  {  // dq = scale dS k
     GemmEpilogue e;
-    e.alpha = alpha_b;
+    e.alpha = scale;
     e.out_f16 = gqkv;
-    e.ldc = 3 * c;
-    add_gemm(b, opK(dP, ldT, T, ldT), opMN(qkv + c, 3 * c, c, T), T, c, T, e);
+    e.ldc = 3 * W;
+    e.bs0 = qs0;
+    e.bs1 = qs1;
+    add_gemm(*bwd, opK(dP, ldT, T, ldT, heads, ps0, images, ps1), opMN(qkv + W, 3 * W, d, T, heads, qs0, images, qs1), T,
+             d, T, e, bn_d);
   }
-  {  // dk = alpha dS^T q
+  {  // dk = scale dS^T q
     GemmEpilogue e;
-    e.alpha = alpha_b;
-    e.out_f16 = gqkv + c;
-    e.ldc = 3 * c;
-    add_gemm(b, opMN(dP, ldT, T, T), opMN(qkv, 3 * c, c, T), T, c, T, e);
+    e.alpha = scale;
+    e.out_f16 = gqkv + W;
+    e.ldc = 3 * W;
+    e.bs0 = qs0;
+    e.bs1 = qs1;
+    add_gemm(*bwd, opMN(dP, ldT, T, T, heads, ps0, images, ps1), opMN(qkv, 3 * W, d, T, heads, qs0, images, qs1), T, d,
+             T, e, bn_d);
   }
   {  // dv = P^T dO
     GemmEpilogue e;
-    e.out_f16 = gqkv + 2 * c;
-    e.ldc = 3 * c;
-    add_gemm(b, opMN(P, ldT, T, T), opMN(O.g, c, c, T), T, c, T, e);
+    e.out_f16 = gqkv + 2 * W;
+    e.ldc = 3 * W;
+    e.bs0 = qs0;
+    e.bs1 = qs1;
+    add_gemm(*bwd, opMN(P, ldT, T, T, heads, ps0, images, ps1), opMN(d_o, W, d, T, heads, os0, images, os1), T, d, T, e,
+             bn_d);
   }
-  {  // da = dqkv Wqkv   (B = Wqkv stored [3c (k), c (n)] -> MN-major)
-    GemmEpilogue e;
-    e.out_f16 = a.g;
-    e.ldc = c;
-    add_gemm(b, opK(gqkv, 3 * c, T, 3 * c), opMN(wqkv, c, c, 3 * c), T, c, 3 * c, e);
-  }
-  add_gn_bwd(b, a.g, x.p, s, n, T, c, 0, out.g, x.g);
-  bwd_stack.push_back(std::move(b));
-  return out;
+  return P;
 }
 
 Act Engine::upsample(const Act& x, const std::string& prefix) {
@@ -1026,9 +1099,9 @@ void Engine::build_vqgan() {
     }
     c2[j] = s;
   }
-  float* d_cb = upload(cb.data);
-  float* d_cbT = upload(cbT);
-  float* d_c2 = upload(c2);
+  float* d_cb = vq_cb = upload(cb.data);
+  float* d_cbT = vq_cbT = upload(cbT);
+  float* d_c2 = vq_c2 = upload(c2);
   zmin = upload(mn);  // vqgan.py:141-142
   zmax = upload(mx);
   const int n_chunks = (ne + 1023) / 1024;
@@ -1097,6 +1170,16 @@ void Engine::build_vqgan() {
     b.add(1, [=] { vq_backward(zq.g, inv, zc, hw, zg, cs); }, 0.0, "vq_backward");
     bwd_stack.push_back(std::move(b));
   }
+  auto resblock = [&](const Act& x, const std::string& prefix, int cin, int cout) {
+    const ResBlock r = resblock_fwd(drawer_fwd, x, prefix, cin, cout, true);
+    resblock_bwd(r);
+    return r.out;
+  };
+  auto attnblock = [&](const Act& x, const std::string& prefix, int c) {
+    const AttnBlock a = attnblock_fwd(drawer_fwd, x, prefix, c, true);
+    attnblock_bwd(a);
+    return a.out;
+  };
   hcur = resblock(hcur, "decoder.mid.block_1", block_in, block_in);
   hcur = attnblock(hcur, "decoder.mid.attn_1", block_in);
   hcur = resblock(hcur, "decoder.mid.block_2", block_in, block_in);
@@ -1160,82 +1243,27 @@ void Engine::build_vqgan() {
 
 // taming Encoder (un-vendored: taming/modules/diffusionmodules/model.py, restated in oracle/ref_path.py): conv_in, per level
 // num_res_blocks x ResnetBlock (+ AttnBlock at attn_resolution) and a strided Downsample, mid block_1 / attn_1 / block_2,
-// norm_out + swish + conv_out; then VQModel.encode's quant_conv and the quantiser's nearest code.  Same kernels as the
-// decoder's forward; no backward (the encoder only runs at init / overlay time, never inside the gradient path).
+// norm_out + swish + conv_out; then VQModel.encode's quant_conv and the quantiser's nearest code.  The blocks are the
+// decoder's forward builders; no backward and no gradient buffers (the encoder only runs at init / overlay time, never
+// inside the gradient path).
 void Engine::build_vqgan_encoder() {
   const int zc = cfg.z_channels, ne = cfg.n_embed, L = cfg.n_levels, H = cfg.image_h, Wd = cfg.image_w;
   cudaStream_t cs = st;
-  auto act = [&](int h, int w, int c) {
-    Act a;
-    a.H = h;
-    a.W = w;
-    a.C = c;
-    a.p = dalloc<act_t>((size_t)h * w * c);
-    return a;
-  };
-  auto conv = [&](const Act& x, const ConvW& w, const act_t* res) {
+  auto act = [&](int h, int w, int c) { return new_act(h, w, c, false); };
+  auto conv = [&](const Act& x, const ConvW& w) {
     Act y = act(x.H, x.W, w.cout);
     GemmEpilogue e;
     e.bias = w.bias;
-    e.res_f16 = res;
     e.out_f16 = y.p;
     e.ldc = y.C;
     add_conv(enc_fwd, x.p, x.H, x.W, x.C, w.w, w.cout_pad, w.cout, w.ks, e);
     return y;
   };
-  auto resblock_fwd = [&](const Act& x, const std::string& prefix, int cin, int cout) {
-    NormW n1 = load_norm(PXR_MOD_VQGAN, prefix + ".norm1", cin), n2 = load_norm(PXR_MOD_VQGAN, prefix + ".norm2", cout);
-    ConvW c1 = load_conv(prefix + ".conv1", cin, cout, 3), c2 = load_conv(prefix + ".conv2", cout, cout, 3);
-    Act a1 = act(x.H, x.W, cin), a2 = act(x.H, x.W, cout);
-    add_gn(enc_fwd, x, n1, 1, a1.p);
-    Act h1 = conv(a1, c1, nullptr);
-    add_gn(enc_fwd, h1, n2, 1, a2.p);
-    const act_t* shortcut = x.p;
-    if (cin != cout) {
-      ConvW sc = load_conv(prefix + ".nin_shortcut", cin, cout, 1);
-      shortcut = conv(x, sc, nullptr).p;
-    }
-    return conv(a2, c2, shortcut);
+  auto resblock = [&](const Act& x, const std::string& prefix, int cin, int cout) {
+    return resblock_fwd(enc_fwd, x, prefix, cin, cout, false).out;
   };
-  auto attn_fwd = [&](const Act& x, const std::string& prefix, int c) {
-    NormW n = load_norm(PXR_MOD_VQGAN, prefix + ".norm", c);
-    std::vector<float> wq, bq;
-    for (const char* nm : {".q", ".k", ".v"}) {
-      const HostWeight& w = W(PXR_MOD_VQGAN, prefix + nm + ".weight", {c, c, 1, 1});
-      const HostWeight& b = W(PXR_MOD_VQGAN, prefix + nm + ".bias", {c});
-      wq.insert(wq.end(), w.data.begin(), w.data.end());
-      bq.insert(bq.end(), b.data.begin(), b.data.end());
-    }
-    act_t* wqkv = upload_f16(wq);
-    float* bqkv = upload(bq);
-    ConvW po = load_conv(prefix + ".proj_out", c, c, 1);
-    const int T = x.pixels(), ldT = round_up(T, 8);
-    Act a = act(x.H, x.W, c), O = act(x.H, x.W, c);
-    act_t* qkv = dalloc<act_t>((size_t)T * 3 * c);
-    act_t* P = dalloc<act_t>((size_t)T * ldT);
-    add_gn(enc_fwd, x, n, 0, a.p);
-    {
-      GemmEpilogue e;
-      e.bias = bqkv;
-      e.out_f16 = qkv;
-      e.ldc = 3 * c;
-      add_gemm(enc_fwd, opK(a.p, c, T, c), opK(wqkv, c, 3 * c, c), T, 3 * c, c, e);
-    }
-    {
-      GemmEpilogue e;
-      e.alpha = 1.f / std::sqrt((float)c);
-      e.out_f16 = P;
-      e.ldc = ldT;
-      add_gemm(enc_fwd, opK(qkv, 3 * c, T, c), opK(qkv + c, 3 * c, T, c), T, T, c, e);
-    }
-    enc_fwd.add(1, [=] { softmax_forward(P, T, T, ldT, cs); }, 0.0, "softmax_forward");
-    {
-      GemmEpilogue e;
-      e.out_f16 = O.p;
-      e.ldc = c;
-      add_gemm(enc_fwd, opK(P, ldT, T, ldT), opMN(qkv + 2 * c, 3 * c, c, T), T, c, T, e);
-    }
-    return conv(O, po, x.p);
+  auto attnblock = [&](const Act& x, const std::string& prefix, int c) {
+    return attnblock_fwd(enc_fwd, x, prefix, c, false).out;
   };
   enc_img = dalloc<float>((size_t)3 * H * Wd);
   Act x0 = act(H, Wd, 64);
@@ -1245,20 +1273,20 @@ void Engine::build_vqgan_encoder() {
     enc_fwd.add(1, [=] { image_to_nhwc64(im, px, x0.p, cs); }, 0.0, "image_to_nhwc64");
   }
   ConvW cin_w = load_conv("encoder.conv_in", 64, cfg.ch, 3, 3);
-  Act hcur = conv(x0, cin_w, nullptr);
+  Act hcur = conv(x0, cin_w);
   int curr_res = cfg.resolution, block_in = cfg.ch;
   for (int lv = 0; lv < L; ++lv) {
     const int block_out = cfg.ch * cfg.ch_mult[lv];
     for (int ib = 0; ib < cfg.num_res_blocks; ++ib) {
       const std::string p = "encoder.down." + std::to_string(lv) + ".block." + std::to_string(ib);
-      hcur = resblock_fwd(hcur, p, block_in, block_out);
+      hcur = resblock(hcur, p, block_in, block_out);
       block_in = block_out;
       if (curr_res == cfg.attn_resolution)
-        hcur = attn_fwd(hcur, "encoder.down." + std::to_string(lv) + ".attn." + std::to_string(ib), block_in);
+        hcur = attnblock(hcur, "encoder.down." + std::to_string(lv) + ".attn." + std::to_string(ib), block_in);
     }
     if (lv != L - 1) {
       ConvW dw = load_conv("encoder.down." + std::to_string(lv) + ".downsample.conv", block_in, block_in, 3);
-      Act full = conv(hcur, dw, nullptr);
+      Act full = conv(hcur, dw);
       Act half = act(hcur.H / 2, hcur.W / 2, block_in);
       const int fh = hcur.H, fw = hcur.W, fc = block_in;
       enc_fwd.add(1, [=] { subsample_odd(full.p, fh, fw, fc, half.p, cs); }, 0.0, "subsample_odd");
@@ -1266,31 +1294,20 @@ void Engine::build_vqgan_encoder() {
       curr_res /= 2;
     }
   }
-  hcur = resblock_fwd(hcur, "encoder.mid.block_1", block_in, block_in);
-  hcur = attn_fwd(hcur, "encoder.mid.attn_1", block_in);
-  hcur = resblock_fwd(hcur, "encoder.mid.block_2", block_in, block_in);
+  hcur = resblock(hcur, "encoder.mid.block_1", block_in, block_in);
+  hcur = attnblock(hcur, "encoder.mid.attn_1", block_in);
+  hcur = resblock(hcur, "encoder.mid.block_2", block_in, block_in);
   NormW no = load_norm(PXR_MOD_VQGAN, "encoder.norm_out", block_in);
   Act a = act(hcur.H, hcur.W, block_in);
   add_gn(enc_fwd, hcur, no, 1, a.p);
   ConvW co = load_conv("encoder.conv_out", block_in, zc, 3);  // double_z = False for the VQ models
-  Act hz = conv(a, co, nullptr);
+  Act hz = conv(a, co);
   ConvW qc = load_conv("quant_conv", zc, zc, 1);
-  Act hq = conv(hz, qc, nullptr);
+  Act hq = conv(hz, qc);
   const int hw = hq.pixels();
   if ((int64_t)zc * hw != z_numel) throw EngineError(-44, "encoder output does not match the latent size");
-  // quantise: the same exact fp32 nearest-code search as synth (the codebook copies are the decoder's)
-  const HostWeight& cb = W(PXR_MOD_VQGAN, "quantize.embedding.weight", {ne, zc});
-  std::vector<float> cbT((size_t)zc * ne), c2(ne);
-  for (int j = 0; j < ne; ++j) {
-    float s2 = 0.f;
-    for (int k = 0; k < zc; ++k) {
-      const float v = cb.data[(size_t)j * zc + k];
-      cbT[(size_t)k * ne + j] = v;
-      s2 += v * v;
-    }
-    c2[j] = s2;
-  }
-  float *d_cb = upload(cb.data), *d_cbT = upload(cbT), *d_c2 = upload(c2);
+  // quantise: the same exact fp32 nearest-code search as synth, on the decoder's codebook copies
+  float *d_cb = vq_cb, *d_cbT = vq_cbT, *d_c2 = vq_c2;
   const int n_chunks = (ne + 1023) / 1024;
   float* part_d = dalloc<float>((size_t)hw * n_chunks);
   int* part_i = dalloc<int>((size_t)hw * n_chunks);
@@ -1631,7 +1648,7 @@ void Engine::build_clip(int i) {
   C.gh = dalloc<act_t>((size_t)M * Wd);
   C.go = dalloc<act_t>((size_t)M * Wd);
   C.gqkv = dalloc<act_t>((size_t)M * 3 * Wd);
-  const bool fuse_attn = fused_attn && attn_supported(T, d, Wd);  // attn_tc.cu: T <= 240
+  const bool fuse_attn = attn_fused(T, d, Hh);  // attn_tc.cu: T <= 240
   C.dP = fuse_attn ? nullptr : dalloc<act_t>((size_t)B * Hh * T * ldT);
   const bool s16 = stream16;
   const size_t xbytes = (size_t)M * Wd * (s16 ? sizeof(act_t) : sizeof(float));
@@ -1672,8 +1689,7 @@ void Engine::build_clip(int i) {
   };
   C.layers.resize(L);
   const float scale = 1.f / std::sqrt((float)d);
-  const bool fuse_sm = fuse_softmax && T <= 256;  // attention row fits one tile: softmax fused into the GEMM epilogue
-  const int bnS = fuse_sm ? round_up(T, 16) : pick_bn(T, false, 1000);
+  std::vector<OpList> attn_bwd(L);  // per layer, built with the forward, spliced into the backward
 
   // ---- forward: patch embed (conv1 as GEMM over im2col'd patches, written straight into the token rows 1..np)
   {
@@ -1710,17 +1726,8 @@ void Engine::build_clip(int i) {
     Ly.stats1 = dalloc<float>((size_t)M * 2);
     Ly.stats2 = dalloc<float>((size_t)M * 2);
     Ly.qkv = dalloc<act_t>((size_t)M * 3 * Wd);
-    Ly.P = fuse_attn ? nullptr : dalloc<act_t>((size_t)B * Hh * T * ldT);
     Ly.u = dalloc<act_t>((size_t)M * 4 * Wd);
-    if (fuse_attn) {
-      Ly.o = dalloc<act_t>((size_t)M * Wd);
-      Ly.lse = dalloc<float>((size_t)B * Hh * T);
-      Ly.attn = std::make_shared<AttnPlan>();
-      char buf[256] = {0};
-      int rc = attn_plan_make(Ly.attn.get(), Ly.qkv, Ly.o, C.go, C.gqkv, Ly.lse, B, T, Hh, Wd, scale, num_sms, buf,
-                              sizeof buf);
-      if (rc) throw EngineError(rc, std::string("attention plan: ") + buf);
-    }
+    if (fuse_attn) Ly.o = dalloc<act_t>((size_t)M * Wd);
     Clip::Layer ly = Ly;
     Clip* c = &C;
     C.fwd.add(1, [=] { ln_fwd(ly.x_in, Wd, nullptr, T, ly.ln1, M, Wd, c->h16, nullptr, ly.stats1); }, 0.0, "layernorm_forward");
@@ -1731,40 +1738,8 @@ void Engine::build_clip(int i) {
       e.ldc = 3 * Wd;
       add_gemm(C.fwd, opK(C.h16, Wd, M, Wd), opK(ly.wqkv, Wd, 3 * Wd, Wd), M, 3 * Wd, Wd, e);
     }
-    const long long qs0 = d, qs1 = (long long)T * 3 * Wd;           // (head, image) strides inside qkv
-    const long long ps0 = (long long)T * ldT, ps1 = (long long)Hh * T * ldT;  // inside P / dP
-    const long long os0 = d, os1 = (long long)T * Wd;              // inside [M, W] token-major buffers
-    if (fuse_attn) {  // S, softmax and PV in one kernel; S / P never leave the SM
-      std::shared_ptr<AttnPlan> ap = ly.attn;
-      char lab[96];
-      snprintf(lab, sizeof lab, "attn_fwd B=%d T=%d heads=%d", B, T, Hh);
-      C.fwd.add(1, [ap, cs] { attn_forward_launch(*ap, cs); }, ap->flops_fwd, lab, ap->bytes_fwd);
-    } else {
-    {  // S = scale * q k^T  (nn.MultiheadAttention scales q by d^-1/2)
-      GemmEpilogue e;
-      e.alpha = scale;
-      e.out_f16 = ly.P;
-      e.ldc = ldT;
-      e.bs0 = ps0;
-      e.bs1 = ps1;
-      if (fuse_sm) {
-        e.act = ACT_SOFTMAX;
-        e.n_store = ldT;
-      }
-      add_gemm(C.fwd, opK(ly.qkv, 3 * Wd, T, d, Hh, qs0, B, qs1), opK(ly.qkv + Wd, 3 * Wd, T, d, Hh, qs0, B, qs1), T, T,
-               d, e, bnS);
-    }
-    if (!fuse_sm) C.fwd.add(1, [=] { softmax_forward(ly.P, B * Hh * T, T, ldT, cs); }, 0.0, "softmax_forward");
-    {  // O = P v
-      GemmEpilogue e;
-      e.out_f16 = C.o16;
-      e.ldc = Wd;
-      e.bs0 = os0;
-      e.bs1 = os1;
-      add_gemm(C.fwd, opK(ly.P, ldT, T, ldT, Hh, ps0, B, ps1), opMN(ly.qkv + 2 * Wd, 3 * Wd, d, T, Hh, qs0, B, qs1), T, d,
-               T, e, 64);
-    }
-    }
+    Ly.P = add_attention(C.fwd, &attn_bwd[l], ly.qkv, fuse_attn ? ly.o : C.o16, C.go, C.gqkv, B, Hh, T, d, scale, true,
+                         C.dP);
     // Last layer: only the class token's row of every image reaches ln_post / proj (slip.py:62-66 ->
     // VisionTransformer.forward takes x[:, 0, :]), and everything after the attention is row-wise -- out_proj, ln_2, the MLP
     // and their backward run on those B rows (row pitch T * W inside the [M, W] buffers) instead of on all M = B T rows.
@@ -1825,8 +1800,6 @@ void Engine::build_clip(int i) {
   for (int l = L - 1; l >= 0; --l) {
     Clip::Layer ly = C.layers[l];
     Clip* c = &C;
-    const long long qs0 = d, qs1 = (long long)T * 3 * Wd, ps0 = (long long)T * ldT, ps1 = (long long)Hh * T * ldT;
-    const long long os0 = d, os1 = (long long)T * Wd;
     const bool cls_only = clip_last_cls && l == L - 1;  // see the forward: the row-wise tail of the last layer, class rows only
     const int Mr = cls_only ? B : M;
     const long long xld = cls_only ? (long long)T * Wd : (long long)Wd;
@@ -1855,57 +1828,7 @@ void Engine::build_clip(int i) {
       e.ldc = xld;
       add_gemm(C.bwd, opK(C.gx16, xld, Mr, Wd), opMN(ly.wo, Wd, Wd, Wd), Mr, Wd, Wd, e);
     }
-    if (fuse_attn) {  // dQ, dK, dV in one kernel (recomputes P from Q, K and the saved log-sum-exp)
-      std::shared_ptr<AttnPlan> ap = ly.attn;
-      char lab[96];
-      snprintf(lab, sizeof lab, "attn_bwd B=%d T=%d heads=%d", B, T, Hh);
-      C.bwd.add(2, [ap, cs] { attn_backward_launch(*ap, cs); }, ap->flops_bwd, lab, ap->bytes_bwd);
-    } else {
-    {  // dP = go v^T ; fused: dS = scale * P * (dP - <P, dP>)
-      GemmEpilogue e;
-      e.out_f16 = C.dP;
-      e.ldc = ldT;
-      e.bs0 = ps0;
-      e.bs1 = ps1;
-      if (fuse_sm) {
-        e.act = ACT_SOFTMAX_BWD;
-        e.aux_in = ly.P;
-        e.alpha = scale;
-        e.n_store = ldT;
-      }
-      add_gemm(C.bwd, opK(C.go, Wd, T, d, Hh, os0, B, os1), opK(ly.qkv + 2 * Wd, 3 * Wd, T, d, Hh, qs0, B, qs1), T, T, d,
-               e, bnS);
-    }
-    if (!fuse_sm) C.bwd.add(1, [=] { softmax_backward(ly.P, c->dP, B * Hh * T, T, ldT, cs); }, 0.0, "softmax_backward");
-    const float scale_b = fuse_sm ? 1.f : scale;
-    {  // dq = scale dS k
-      GemmEpilogue e;
-      e.alpha = scale_b;
-      e.out_f16 = C.gqkv;
-      e.ldc = 3 * Wd;
-      e.bs0 = qs0;
-      e.bs1 = qs1;
-      add_gemm(C.bwd, opK(C.dP, ldT, T, ldT, Hh, ps0, B, ps1), opMN(ly.qkv + Wd, 3 * Wd, d, T, Hh, qs0, B, qs1), T, d, T,
-               e, 64);
-    }
-    {  // dk = scale dS^T q
-      GemmEpilogue e;
-      e.alpha = scale_b;
-      e.out_f16 = C.gqkv + Wd;
-      e.ldc = 3 * Wd;
-      e.bs0 = qs0;
-      e.bs1 = qs1;
-      add_gemm(C.bwd, opMN(C.dP, ldT, T, T, Hh, ps0, B, ps1), opMN(ly.qkv, 3 * Wd, d, T, Hh, qs0, B, qs1), T, d, T, e, 64);
-    }
-    {  // dv = P^T go
-      GemmEpilogue e;
-      e.out_f16 = C.gqkv + 2 * Wd;
-      e.ldc = 3 * Wd;
-      e.bs0 = qs0;
-      e.bs1 = qs1;
-      add_gemm(C.bwd, opMN(ly.P, ldT, T, T, Hh, ps0, B, ps1), opMN(C.go, Wd, d, T, Hh, os0, B, os1), T, d, T, e, 64);
-    }
-    }
+    C.bwd.append(attn_bwd[l]);
     {  // gh = gqkv Wqkv
       GemmEpilogue e;
       e.out_f16 = C.gh;

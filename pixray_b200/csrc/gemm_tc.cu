@@ -104,12 +104,6 @@ __device__ __forceinline__ void load_acc(const float* src, int width, float (&v)
   }
 }
 
-__device__ __forceinline__ void stage_rows(float* tb, const float (&v)[32], int lane) {
-#pragma unroll
-  for (int j = 0; j < 32; ++j) tb[lane * TB_LD + j] = v[j];
-  __syncwarp();
-}
-
 template <int E>
 __device__ __forceinline__ void ld_f16(const __half* p, bool vec, int nv, float (&x)[E]) {
   if (vec) {
@@ -309,106 +303,6 @@ __device__ __forceinline__ void epilogue_block(const GemmParams& p, const float*
   }
 }
 
-// fp16 store of a staged block with zero fill up to n_store (softmax epilogues), lane = (8 rows, 4 chunks of 8)
-__device__ __forceinline__ void store_block_f16(const GemmParams& p, const float* tb, const long long* s_off, int lane,
-                                                int col_base) {
-  const int chunk = lane & 3, rsub = lane >> 2;
-  const int col = col_base + chunk * 8;
-  int nv = p.n_store - col;
-  nv = nv < 0 ? 0 : (nv > 8 ? 8 : nv);
-  if (nv == 0) return;
-  const bool vec = p.vec_ok && nv == 8;
-#pragma unroll
-  for (int it = 0; it < 4; ++it) {
-    const int r = it * 8 + rsub;
-    const long long off_r = s_off[r];
-    if (off_r < 0) continue;
-    float x[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) x[j] = tb[r * TB_LD + chunk * 8 + j];
-    st_f16<8>(p.out_f16 + off_r + col, vec, nv, x);
-  }
-}
-
-// Fused row softmax (attention probabilities straight out of the QK^T accumulator, nn.MultiheadAttention /
-// taming AttnBlock): requires the whole row in one tile (tiles_n == 1).  Thread = row.  Columns [N, n_store) are
-// written as zeros so the result can be consumed as a K-major operand with a padded row pitch.
-__device__ __forceinline__ void epilogue_softmax_fwd(const GemmParams& p, float* tb, const long long* s_off,
-                                                     const float* arow, int lane) {
-  const int nslab = (p.block_n + 31) / 32;
-  float v[32];
-  float mx = -3.0e38f;
-  for (int s = 0; s < nslab; ++s) {
-    load_acc(arow + s * 32, min(32, p.block_n - s * 32), v);
-#pragma unroll
-    for (int j = 0; j < 32; ++j)
-      if (s * 32 + j < p.N) mx = fmaxf(mx, v[j] * p.alpha);
-  }
-  float sum = 0.f;
-  for (int s = 0; s < nslab; ++s) {
-    load_acc(arow + s * 32, min(32, p.block_n - s * 32), v);
-#pragma unroll
-    for (int j = 0; j < 32; ++j)
-      if (s * 32 + j < p.N) sum += __expf(v[j] * p.alpha - mx);
-  }
-  const float inv = __fdividef(1.f, sum);
-  for (int s = 0; s < nslab; ++s) {
-    load_acc(arow + s * 32, min(32, p.block_n - s * 32), v);
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = (s * 32 + j < p.N) ? __expf(v[j] * p.alpha - mx) * inv : 0.f;
-    stage_rows(tb, v, lane);
-    store_block_f16(p, tb, s_off, lane, s * 32);
-    __syncwarp();
-  }
-}
-
-// Fused softmax backward: accumulator = dP row, aux_in = P (fp16, same indexing as the output);
-// dS = alpha * P * (dP - sum_j P_j dP_j).
-__device__ __forceinline__ void epilogue_softmax_bwd(const GemmParams& p, float* tb, const long long* s_off,
-                                                     const float* arow, int lane) {
-  const int nslab = (p.block_n + 31) / 32;
-  const int chunk = lane & 3, rsub = lane >> 2;
-  float v[32];
-  float dot = 0.f;
-  for (int pass = 0; pass < 2; ++pass) {
-    for (int s = 0; s < nslab; ++s) {
-      // P block: coalesced 16-byte loads (store layout) -> smem -> row layout
-      const int col = s * 32 + chunk * 8;
-      int nv = p.N - col;
-      nv = nv < 0 ? 0 : (nv > 8 ? 8 : nv);
-      const bool vec = p.vec_ok && nv == 8;
-#pragma unroll
-      for (int it = 0; it < 4; ++it) {
-        const int r = it * 8 + rsub;
-        const long long off_r = s_off[r];
-        float x[8];
-        if (off_r >= 0 && nv > 0) {
-          ld_f16<8>(p.aux_in + off_r + col, vec, nv, x);
-        } else {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) x[j] = 0.f;
-        }
-#pragma unroll
-        for (int j = 0; j < 8; ++j) tb[r * TB_LD + chunk * 8 + j] = x[j];
-      }
-      __syncwarp();
-      load_acc(arow + s * 32, min(32, p.block_n - s * 32), v);
-      if (pass == 0) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) dot += tb[lane * TB_LD + j] * v[j];
-        __syncwarp();
-      } else {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = p.alpha * tb[lane * TB_LD + j] * (v[j] - dot);
-        __syncwarp();
-        stage_rows(tb, v, lane);
-        store_block_f16(p, tb, s_off, lane, s * 32);
-        __syncwarp();
-      }
-    }
-  }
-}
-
 // TMA producer (one lane): walks this CTA's tiles and fills the stage ring.
 // This single thread paces the whole kernel, so its loop body is kept short: specialised on the operand modes (no runtime
 // divisions for the tap / k offset, no mode branches), (tap, kk) carried as running counters, 32-bit shared addresses.
@@ -489,14 +383,15 @@ __device__ __forceinline__ void producer_loop(const GemmParams& p, uint8_t* smem
   }
 }
 
-// Accumulator of one warpgroup: 64 rows x NCH 64-column wgmma fragments (sized per kernel, so that the fragments of a
-// 64- or 128-wide tile do not carry the registers of a 256-wide one).
+// Accumulator of one warpgroup: 64 rows x NCH 64-column wgmma fragments, sized per kernel: NF for the 64- / 128-wide
+// fp16 kernels, two for the generic-width kernel (tiles are at most 128 wide, so a 16-column tail always lands in the
+// first two fragments).
 template <int NCH>
 struct WgAcc {
   float d[NCH][32];
 };
 template <int NF>
-using AccFor = WgAcc<NF ? NF : 4>;
+using AccFor = WgAcc<NF ? NF : 2>;
 
 // MMA warpgroup `wg` (0 or 1: tile rows [64 wg, 64 wg + 64)): wgmma over the k-blocks of one tile.  A k-block is four
 // k16 steps; each step issues block_n / 64 m64n64 instructions and, for block_n % 64, up to three m64n16 ones.  The
@@ -505,7 +400,7 @@ using AccFor = WgAcc<NF ? NF : 4>;
 // k-block kb is released once kb's wgmma group has completed (checked after k-block kb + 1 has been issued).
 // NF > 0: fp16 operands and block_n == 64 NF, so every instruction of a k-step is known at compile time and the fragments
 // take 32 NF registers (runtime-guarded wgmma or a larger live fragment make ptxas serialise the chain); NF == 0 covers
-// every other width and bf16.  With a single stage the k-block's slot is released as soon as its group completes.
+// every other width and bf16.
 template <int TA, int TB, int NF>
 __device__ __forceinline__ void mma_tile(const GemmParams& p, AccFor<NF>& acc, int wg, int n_kb, uint32_t smem0, uint32_t full0,
                                          uint64_t* empty_bar, uint32_t stage_bytes, int& stage, uint32_t& phase) {
@@ -517,7 +412,7 @@ __device__ __forceinline__ void mma_tile(const GemmParams& p, AccFor<NF>& acc, i
   const uint64_t stage_step = stage_bytes >> 4;
   const int nfull = NF ? NF : p.block_n / 64, ntail = NF ? 0 : (p.block_n % 64) / 16;
   const int bf16 = NF ? 0 : p.fmt;
-  constexpr int NCH = NF ? NF : 4;
+  constexpr int NCH = NF ? NF : 2;
   const bool elected = (threadIdx.x & 127) == 0;
   int prev = -1;
   for (int kb = 0; kb < n_kb; ++kb) {
@@ -538,14 +433,9 @@ __device__ __forceinline__ void mma_tile(const GemmParams& p, AccFor<NF>& acc, i
       }
     }
     wgmma_commit();
-    if (p.stages == 1) {  // the producer cannot run ahead: free the only slot now
-      wgmma_wait<0>();
-      if (elected) mbar_arrive(&empty_bar[stage]);
-    } else {
-      wgmma_wait<1>();
-      if (prev >= 0 && elected) mbar_arrive(&empty_bar[prev]);
-      prev = stage;
-    }
+    wgmma_wait<1>();
+    if (prev >= 0 && elected) mbar_arrive(&empty_bar[prev]);
+    prev = stage;
     if (++stage == p.stages) {
       stage = 0;
       phase ^= 1;
@@ -778,10 +668,9 @@ __host__ __device__ __forceinline__ int acc_ld(int block_n) { return (block_n + 
 // Warps 0..7 = two MMA warpgroups (tile rows 0..63, 64..127) that afterwards run the epilogue, warp 8 = TMA producer.
 // Per tile: wgmma into registers, fragments -> staged fp32 tile in shared memory, epilogue from there.  The producer runs
 // ahead through the stage ring, so the next tile's operands stream in while the epilogue of this one runs.
-// EPI: 0 generic or tensor-map epilogue (TE = its mode), 1 fused softmax forward, 2 fused softmax backward.  HAS_IN: the
-// generic epilogue reads an input tensor (residual / saved pre-activation) that is prefetched; kept out of the
-// input-free kernel so that one stays lean.
-template <int EPI, bool HAS_IN, int TE, int NF>
+// TE: the tensor-map epilogue's mode, or TE_NONE for the generic epilogue.  HAS_IN: the generic epilogue reads an input
+// tensor (residual / saved pre-activation) that is prefetched; kept out of the input-free kernel so that one stays lean.
+template <bool HAS_IN, int TE, int NF>
 __device__ __forceinline__ void gemm_body(const GemmParams& p) {
   pdl_launch_dependents();
   extern __shared__ uint8_t smem_raw[];
@@ -825,7 +714,6 @@ __device__ __forceinline__ void gemm_body(const GemmParams& p) {
   const int q = warp & 3, half = warp >> 2;  // epilogue: row quarter, and which column slabs of it
   const float* arow = acc_tile + (q * 32 + lane) * ald;
   uint8_t* wbase = epi_base + static_cast<size_t>(warp) * (TE != TE_NONE ? TE_WARP_BYTES : TB_WARP_BYTES);
-  float* tb = reinterpret_cast<float*>(wbase);
   long long* s_off = reinterpret_cast<long long*>(wbase + TB_FLOATS * 4);
   int* s_row = reinterpret_cast<int*>(wbase + TB_FLOATS * 4 + 32 * 8);
   const bool wide = (p.out_f32 != nullptr) || (p.res_f32 != nullptr);
@@ -852,25 +740,19 @@ __device__ __forceinline__ void gemm_body(const GemmParams& p) {
       s_off[lane] = ri.off;
       s_row[lane] = ri.row;
       __syncwarp();
-      if (EPI == 1) {
-        if (half == 0) epilogue_softmax_fwd(p, tb, s_off, arow, lane);
-      } else if (EPI == 2) {
-        if (half == 0) epilogue_softmax_bwd(p, tb, s_off, arow, lane);
-      } else {
-        const int nslab = (p.block_n + 31) / 32;
-        const int col_limit = min(p.N, t.n0 + p.block_n);
-        const int kind = HAS_IN ? prefetch_kind(p) : 0;
-        const float* blk = acc_tile + q * 32 * ald;
-        for (int s = half; s < nslab; s += 2) {
-          if (wide) {
-            uint4 pf[BlockMap<4>::NIT];
-            if (HAS_IN) prefetch_block<4>(p, s_off, lane, t.n0 + s * 32, col_limit, kind, pf);
-            epilogue_block<4>(p, blk + s * 32, ald, s_off, s_row, lane, t.n0 + s * 32, col_limit, kind, pf);
-          } else {
-            uint4 pf[BlockMap<8>::NIT];
-            if (HAS_IN) prefetch_block<8>(p, s_off, lane, t.n0 + s * 32, col_limit, kind, pf);
-            epilogue_block<8>(p, blk + s * 32, ald, s_off, s_row, lane, t.n0 + s * 32, col_limit, kind, pf);
-          }
+      const int nslab = (p.block_n + 31) / 32;
+      const int col_limit = min(p.N, t.n0 + p.block_n);
+      const int kind = HAS_IN ? prefetch_kind(p) : 0;
+      const float* blk = acc_tile + q * 32 * ald;
+      for (int s = half; s < nslab; s += 2) {
+        if (wide) {
+          uint4 pf[BlockMap<4>::NIT];
+          if (HAS_IN) prefetch_block<4>(p, s_off, lane, t.n0 + s * 32, col_limit, kind, pf);
+          epilogue_block<4>(p, blk + s * 32, ald, s_off, s_row, lane, t.n0 + s * 32, col_limit, kind, pf);
+        } else {
+          uint4 pf[BlockMap<8>::NIT];
+          if (HAS_IN) prefetch_block<8>(p, s_off, lane, t.n0 + s * 32, col_limit, kind, pf);
+          epilogue_block<8>(p, blk + s * 32, ald, s_off, s_row, lane, t.n0 + s * 32, col_limit, kind, pf);
         }
       }
     }
@@ -881,21 +763,15 @@ __device__ __forceinline__ void gemm_body(const GemmParams& p) {
 
 template <int NF>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_constant__ GemmParams p) {
-  gemm_body<0, false, TE_NONE, NF>(p);
+  gemm_body<false, TE_NONE, NF>(p);
 }
 template <int NF>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_in_kernel(const __grid_constant__ GemmParams p) {
-  gemm_body<0, true, TE_NONE, NF>(p);
-}
-__global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_softmax_fwd_kernel(const __grid_constant__ GemmParams p) {
-  gemm_body<1, false, TE_NONE, 0>(p);
-}
-__global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_softmax_bwd_kernel(const __grid_constant__ GemmParams p) {
-  gemm_body<2, false, TE_NONE, 0>(p);
+  gemm_body<true, TE_NONE, NF>(p);
 }
 template <int MODE, int NF>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tce_kernel(const __grid_constant__ GemmParams p) {
-  gemm_body<0, false, MODE, NF>(p);
+  gemm_body<false, MODE, NF>(p);
 }
 
 // The kernel for a plan: fragment width NF (see mma_tile) and epilogue.
@@ -913,8 +789,6 @@ void (*plain_kernel(const GemmParams& p))(GemmParams) {
   return gemm_tc_kernel<NF>;
 }
 void (*kernel_for(const GemmParams& p))(GemmParams) {
-  if (p.tma_epi == TE_NONE && p.act == ACT_SOFTMAX) return gemm_tc_softmax_fwd_kernel;
-  if (p.tma_epi == TE_NONE && p.act == ACT_SOFTMAX_BWD) return gemm_tc_softmax_bwd_kernel;
   if (p.fmt == 0 && p.block_n == 128) return plain_kernel<2>(p);
   if (p.fmt == 0 && p.block_n == 64) return plain_kernel<1>(p);
   return plain_kernel<0>(p);
@@ -1019,15 +893,12 @@ int tmap_encode_4d(CUtensorMap* out, const void* ptr, int fmt, const uint64_t di
 }
 
 namespace {
-// Widest tile of the plain / tensor-map epilogue kernels: the staged fp32 accumulator tile (128 x block_n) shares the
-// 227 KiB of shared memory with the stage ring and the epilogue buffers, and at 128 columns three stages still fit.
-// The fused softmax epilogues need the whole row in one tile and may go to 256 columns (with a shorter ring).
+// Widest tile: the staged fp32 accumulator tile (128 x block_n) shares the 227 KiB of shared memory with the stage ring
+// and the epilogue buffers; at 128 columns two stages still fit beside the tensor-map epilogue's boxes, three beside the
+// generic epilogue's.  A wider request runs as 128.
 constexpr int GEMM_MAX_BN_PLAIN = 128;
 
-int effective_block_n(int block_n, const GemmEpilogue& epi) {
-  const bool softmax_epi = epi.act == ACT_SOFTMAX || epi.act == ACT_SOFTMAX_BWD;
-  return (!softmax_epi && block_n > GEMM_MAX_BN_PLAIN) ? GEMM_MAX_BN_PLAIN : block_n;
-}
+int effective_block_n(int block_n) { return block_n > GEMM_MAX_BN_PLAIN ? GEMM_MAX_BN_PLAIN : block_n; }
 
 // Tensor-map epilogue (see tma_epilogue_tile) when the epilogue is one of its shapes and every tensor can be described
 // by a tensor map; anything else keeps the generic epilogue.  PXR_GEMM_TMA_EPI=0 disables it globally.
@@ -1105,9 +976,13 @@ double epilogue_bytes(const GemmEpilogue& e, double mn) {
 
 int finish_plan(GemmPlan* plan, const GemmEpilogue& epi, int block_n, int num_sms, char* err, int errlen) {
   GemmParams& p = plan->p;
-  if (block_n < 16 || block_n > 256 || block_n % 16) {
-    set_err(err, errlen, "block_n must be a multiple of 16 in [16, 256]");
+  if (block_n < 16 || block_n > GEMM_MAX_BN_PLAIN || block_n % 16) {
+    set_err(err, errlen, "block_n must be a multiple of 16 in [16, 128]");
     return -10;
+  }
+  if (epi.act < ACT_NONE || epi.act > ACT_QUICKGELU_BWD) {
+    set_err(err, errlen, "unknown epilogue activation (act must be 0 none, 1 QuickGELU or 2 QuickGELU backward)");
+    return -12;
   }
   if (p.b_mode == OP_MNMAJOR && block_n % 64) {
     set_err(err, errlen, "MN-major B needs block_n % 64 == 0");
@@ -1132,17 +1007,12 @@ int finish_plan(GemmPlan* plan, const GemmEpilogue& epi, int block_n, int num_sm
                        GEMM_EPI_WARPS * (p.tma_epi != TE_NONE ? TE_WARP_BYTES : TB_WARP_BYTES);
   int stages = (227 * 1024 - 1024 - epi_smem) / stage_bytes;
   if (stages > GEMM_MAX_STAGES) stages = GEMM_MAX_STAGES;
-  if (stages < 1) {
-    set_err(err, errlen, "block_n too wide for shared memory");
+  if (stages < 2) {  // mma_tile releases a stage only after the next one has been issued
+    set_err(err, errlen, "block_n too wide for a two-stage ring in shared memory");
     return -13;
   }
   p.stages = stages;
   p.alpha = epi.alpha;
-  p.n_store = epi.n_store > 0 ? epi.n_store : p.N;
-  if ((epi.act == ACT_SOFTMAX || epi.act == ACT_SOFTMAX_BWD) && (p.tiles_n != 1 || !epi.out_f16)) {
-    set_err(err, errlen, "fused softmax epilogue needs the whole row in one tile and an fp16 output");
-    return -12;
-  }
   p.bias = epi.bias;
   p.bias_per_row = epi.bias_per_row;
   p.act = epi.act;
@@ -1172,8 +1042,6 @@ int finish_plan(GemmPlan* plan, const GemmEpilogue& epi, int block_n, int num_sm
           q.act = in ? ACT_QUICKGELU_BWD : ACT_NONE;
           cudaFuncSetAttribute(kernel_for(q), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
         }
-    cudaFuncSetAttribute(gemm_tc_softmax_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    cudaFuncSetAttribute(gemm_tc_softmax_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
   });
   return 0;
 }
@@ -1188,7 +1056,7 @@ int gemm_plan_make(GemmPlan* plan, const GemmOperand& A, const GemmOperand& B, i
     set_err(err, errlen, "use conv_plan_make for conv operands");
     return -20;
   }
-  block_n = effective_block_n(block_n, epi);
+  block_n = effective_block_n(block_n);
   p.M = M;
   p.N = N;
   p.fmt = fmt;
@@ -1249,7 +1117,7 @@ int conv_plan_make(GemmPlan* plan, const void* in, long long in_ld, int batch, i
   // M tile = tile_h x tile_w pixels (8 x 16 or 16 x 8).  Any W works: columns past the image are zero-filled by the
   // TMA loads and clipped by the stores (tensor-map epilogue) / predicated off (generic epilogue); pick the width that
   // wastes the fewest columns (pixray's presets give latents such as 9 x 9, 18 x 18, 12 x 6: pixray.py:1864-1878)
-  block_n = effective_block_n(block_n, epi);
+  block_n = effective_block_n(block_n);
   const int waste16 = (W + 15) / 16 * 16, waste8 = (W + 7) / 8 * 8;
   int tile_w = (waste16 <= waste8) ? 16 : 8;
   int tile_h = GEMM_BLOCK_M / tile_w;

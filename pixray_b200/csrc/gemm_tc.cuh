@@ -22,7 +22,7 @@
 namespace pxr {
 
 enum OperandMode : int { OP_KMAJOR = 0, OP_MNMAJOR = 1, OP_CONV = 2 };
-enum EpiAct : int { ACT_NONE = 0, ACT_QUICKGELU = 1, ACT_QUICKGELU_BWD = 2, ACT_SOFTMAX = 3, ACT_SOFTMAX_BWD = 4 };
+enum EpiAct : int { ACT_NONE = 0, ACT_QUICKGELU = 1, ACT_QUICKGELU_BWD = 2 };
 
 constexpr int GEMM_BLOCK_M = 128;
 constexpr int GEMM_BLOCK_K = 64;
@@ -34,8 +34,7 @@ struct GemmParams {
   CUtensorMap tma_b;
   // tiling
   int M, N;            // logical output extent per batch (predication)
-  int n_store;         // softmax epilogues: columns [N, n_store) are written as zeros (padded row pitch)
-  int block_n;         // multiple of 16, <= 128 (<= 256 for the softmax epilogues; multiple of 64 when B is MN-major)
+  int block_n;         // multiple of 16, <= 128 (multiple of 64 when B is MN-major)
   int stages;
   int num_k_blocks;    // taps * k_blocks_per_tap
   int k_blocks_per_tap;
@@ -95,7 +94,6 @@ struct GemmEpilogue {
   float* out_f32 = nullptr;
   __half* out_f16 = nullptr;
   long long ldc = 0, bs0 = 0, bs1 = 0;
-  int n_store = 0;  // softmax modes: zero-fill columns [N, n_store)
   int tma_epi = 0;    // 0 = auto (tensor-map epilogue when the tensors allow it), -1 = force the generic epilogue
   int k_splits = 1;   // conv_plan_make only: > 1 writes fp32 partial sums [k_splits][pixels][ldc] to out_f32
 };

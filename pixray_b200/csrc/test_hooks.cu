@@ -37,7 +37,6 @@ static void fill_epilogue(GemmEpilogue& e, const pxr_test_gemm_desc* d) {
   e.ldc = d->ldc;
   e.bs0 = d->c_bs0;
   e.bs1 = d->c_bs1;
-  e.n_store = d->n_store;
   e.tma_epi = d->tma_epi;
 }
 

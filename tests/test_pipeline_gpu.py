@@ -400,8 +400,7 @@ def test_decoder_attention_rows_longer_than_1024():
 
 ATTENTION_PATHS = {
     "fused": {},
-    "batched_gemms_row_softmax": {"PXR_FUSED_ATTN": "0", "PXR_FUSE_SOFTMAX": "0"},
-    "softmax_in_gemm_epilogue": {"PXR_FUSED_ATTN": "0", "PXR_FUSE_SOFTMAX": "1"},
+    "batched_gemms_row_softmax": {"PXR_FUSED_ATTN": "0"},
     "fp32_stream": {"PXR_CLIP_STREAM": "32"},
 }
 
@@ -409,7 +408,7 @@ ATTENTION_PATHS = {
 @pytest.mark.parametrize("path", sorted(ATTENTION_PATHS))
 def test_every_attention_path_matches_the_oracle(path, monkeypatch):
     """Each attention / residual-stream path a session can select (read at session create) on the small pipeline."""
-    for k in ("PXR_FUSED_ATTN", "PXR_FUSE_SOFTMAX", "PXR_CLIP_STREAM", "PXR_CLIP_LAST_CLS"):
+    for k in ("PXR_FUSED_ATTN", "PXR_CLIP_STREAM", "PXR_CLIP_LAST_CLS"):
         monkeypatch.delenv(k, raising=False)
     for k, v in ATTENTION_PATHS[path].items():
         monkeypatch.setenv(k, v)
@@ -426,7 +425,7 @@ def test_last_layer_on_all_rows_is_bit_identical(monkeypatch):
     call in either session.)"""
     outs = {}
     for last_cls in ("1", "0"):
-        for k in ("PXR_FUSED_ATTN", "PXR_FUSE_SOFTMAX", "PXR_CLIP_STREAM"):
+        for k in ("PXR_FUSED_ATTN", "PXR_CLIP_STREAM"):
             monkeypatch.delenv(k, raising=False)
         monkeypatch.setenv("PXR_CLIP_LAST_CLS", last_cls)
         vq, clip, eng, prompts, z = build(seed=23)
