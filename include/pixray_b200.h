@@ -30,7 +30,8 @@ extern "C" {
 
 typedef struct pxr_engine* pxr_handle;
 
-enum { PXR_DRAWER_VQGAN = 0, PXR_DRAWER_PIXEL = 1, PXR_DRAWER_FFT = 2, PXR_DRAWER_VDIFF = 3, PXR_DRAWER_POLYGON = 4 };
+enum { PXR_DRAWER_VQGAN = 0, PXR_DRAWER_PIXEL = 1, PXR_DRAWER_FFT = 2, PXR_DRAWER_VDIFF = 3, PXR_DRAWER_POLYGON = 4,
+       PXR_DRAWER_SUPERRES = 5 };
 enum { PXR_PAD_REFLECTION = 0, PXR_PAD_BORDER = 1, PXR_PAD_ZEROS = 2 };
 enum { PXR_DTYPE_F16 = 0, PXR_DTYPE_BF16 = 1 };
 /* module ids for pxr_load_weight */
@@ -51,6 +52,7 @@ typedef struct {
   int drawer;            /* PXR_DRAWER_* */
   int image_h, image_w;  /* canvas (vqgan: multiple of 16) */
   /* taming Decoder hyper-parameters (vqgan.py:122-142: model.decoder / model.quantize) */
+  /* super-resolution drawer: ch = num_feat (0 -> 64) */
   int z_channels, n_embed, ch, num_res_blocks, attn_resolution, n_levels, resolution;
   int ch_mult[8];
   /* pixel drawer grid (fast_pixeldrawer.py:37-63) */
@@ -73,7 +75,8 @@ typedef struct {
   /* the stretched size itself, int(cut_size * a) resp. int(cut_size * (1 / a)) as the reference's Python floats give it
    * (kornia rescale truncates); 0 = derive from cut_aspect (which, being a C float, can round across an integer) */
   int cut_src_h, cut_src_w;
-  int reserved[2];
+  /* super-resolution drawer (RRDBNet): RRDB blocks (0 -> 23) and dense-block growth channels (0 -> 32) */
+  int num_block, num_grow_ch;
 } pxr_config;
 
 /* Per-iteration cutout parameters (SURVEY.md Appendix A): what kornia's augmentations sample per cutout, made explicit.
@@ -210,6 +213,13 @@ int pxr_clear_filters(pxr_handle h);
 int pxr_set_filter_shifts(pxr_handle h, int filter_idx, int rand_h, int rand_w);
 int pxr_read_losses(pxr_handle h, float* out_host); /* blocking: the loss vector of the last forward / backward */
 
+/* Super-resolution drawer (PXR_DRAWER_SUPERRES; SuperResolutionDrawer, super_resolution.py, with RealESRGANer at tile 0 /
+ * pre_pad 0 / scale 4): z = the low-resolution image [1, 3, H/4, W/4] in [0, 1] (image_h, image_w multiples of 4), synth =
+ * clamp_with_grad(RRDBNet(z), 0, 1) with RRDBNet(3, 3, num_feat = ch, num_block, num_grow_ch, scale 4) (basicsr's
+ * rrdbnet_arch).  Weights under the checkpoint's own keys (conv_first, body.{i}.rdb{1,2,3}.conv{1..5}, conv_body,
+ * conv_up1, conv_up2, conv_hr, conv_last; .weight / .bias) through pxr_load_weight(PXR_MOD_VQGAN = the drawer slot).
+ * clip_z clamps z to [0, 1]. */
+
 /* vdiff drawer (PXR_DRAWER_VDIFF; VdiffDrawer, vdiff.py:58-190, over diffusion/models/cc12m_1.py).  z = x [1,3,H,W];
  * weights under the checkpoint's own keys through pxr_load_weight(module PXR_MOD_VQGAN = the drawer slot).
  *   set_schedule : sample_state's steps / alphas / sigmas (vdiff.py:113-126, sampling.py:41-51), n = iterations + 1
@@ -286,7 +296,8 @@ typedef struct {
   int M, N, K, block_n, fmt;
   float alpha;
   const float* bias;
-  int bias_per_row, act; /* act: 0 none, 1 QuickGELU (+ pre-activation to aux_out), 2 QuickGELU backward; others are refused */
+  int bias_per_row, act; /* act: 0 none, 1 QuickGELU (+ pre-activation to aux_out), 2 QuickGELU backward, 4 LeakyReLU(0.2),
+                          * 5 LeakyReLU backward (see act_col0); others are refused */
   const void* aux_in;
   void* aux_out;
   const float* res_f32;
@@ -298,6 +309,9 @@ typedef struct {
   int repeat;
   int cta_group; /* ignored: sm_90 has no CTA-pair MMA, every GEMM runs single-CTA tiles (kept for the struct layout) */
   int tma_epi;   /* 0 auto (tensor-map epilogue when the tensors allow it), -1 force the generic epilogue */
+  /* act 5: out = (alpha acc + bias + residual) * (aux_in > 0 ? 1 : 0.2) in the columns >= act_col0, aux_in = the saved
+   * post-activation (same layout as the output); the columns below act_col0 are stored unmasked */
+  int act_col0;
 } pxr_test_gemm_desc;
 
 int pxr_test_gemm(const pxr_test_gemm_desc* d, char* err, int errlen);

@@ -29,7 +29,8 @@ class Config(C.Structure):
         ("op_dtype", C.c_int), ("grad_scale", C.c_float),
         ("beta1", C.c_float), ("beta2", C.c_float), ("adam_eps", C.c_float),
         ("fft_decay", C.c_float), ("fft_colors", C.c_float), ("fft_contrast", C.c_float),
-        ("cut_aspect", C.c_float), ("cut_src_h", C.c_int), ("cut_src_w", C.c_int), ("reserved", C.c_int * 2),
+        ("cut_aspect", C.c_float), ("cut_src_h", C.c_int), ("cut_src_w", C.c_int),
+        ("num_block", C.c_int), ("num_grow_ch", C.c_int),
     ]
 
 
@@ -59,6 +60,7 @@ class TestGemmDesc(C.Structure):
         ("out_f32", C.c_void_p), ("out_f16", C.c_void_p),
         ("ldc", C.c_longlong), ("c_bs0", C.c_longlong), ("c_bs1", C.c_longlong),
         ("stream", C.c_void_p), ("repeat", C.c_int), ("cta_group", C.c_int), ("tma_epi", C.c_int),
+        ("act_col0", C.c_int),
     ]
 
 

@@ -39,9 +39,9 @@ from .util import apply_overlay, get_learning_rate_drops, parse_unit, split_pipe
 # PixelDrawer's five options; its default rect grid runs as fast_pixel (the square cells diffvg renders, SURVEY.md 2,
 # row 6), every other pixel_type on the polygon rasteriser (do_init)
 class_table = {"vqgan": P.VqganDrawer, "fast_pixel": P.FastPixelDrawer, "pixel": P.PixelDrawer, "fft": P.FftDrawer,
-               "vdiff": P.VdiffDrawer}
+               "vdiff": P.VdiffDrawer, "super_resolution": P.SuperResolutionDrawer}
 _DRAWER_KIND = {"vqgan": E.DRAWER_VQGAN, "fast_pixel": E.DRAWER_PIXEL, "pixel": E.DRAWER_PIXEL, "fft": E.DRAWER_FFT,
-                "vdiff": E.DRAWER_VDIFF}
+                "vdiff": E.DRAWER_VDIFF, "super_resolution": E.DRAWER_SUPERRES}
 loss_class_table = L.loss_class_table
 filters_class_table = FL.filters_class_table
 
@@ -280,8 +280,11 @@ def _load_state_dict(spec):
             obj = torch.load(str(spec), map_location="cpu", weights_only=False)
         if isinstance(obj, dict) and "state_dict" in obj:  # taming checkpoints (vqgan.py:128-133)
             obj = obj["state_dict"]
-        return obj
-    return spec
+    else:
+        obj = spec
+    if isinstance(obj, dict) and ("params_ema" in obj or "params" in obj):  # Real-ESRGAN (real_esrganer.py:42-48)
+        obj = obj["params_ema"] if "params_ema" in obj else obj["params"]
+    return obj
 
 
 def _vector_table(name):
@@ -336,12 +339,18 @@ def do_init(args):
             kind = E.DRAWER_POLYGON
     n_levels = len(E.VQGAN_F16_16384["ch_mult"]) if kind == E.DRAWER_VQGAN else None
     sideX, sideY = _side(args, n_levels)
+    engine_hw = (sideY, sideX)
+    if kind == E.DRAWER_SUPERRES:
+        # the start image is resized to the requested size and z is a quarter of it, rounded down; the net's x4 output,
+        # which the cutouts see, is 4 * (size // 4) (super_resolution.py:75-83)
+        P.SuperResolutionDrawer.check_model(args.super_resolution_model)
+        engine_hw = (4 * (sideY // 4), 4 * (sideX // 4))
     # global_aspect_width = args.size[0] / args.size[1] (pixray.py:1931: the REQUESTED size, before the drawer rounds it):
     # != 1 stretches the pooled image before the warps and changes the wide augmentation stack (pixray.py:420-432, 468-472)
     aspect = float(args.size[0]) / float(args.size[1])
     device = int(str(args.cuda_device).split(":")[1]) if ":" in str(args.cuda_device) else 0
     clip_cfgs = [E.CLIP_ARCH[m] for m in args.clip_models]
-    kw = dict(drawer=kind, image_hw=(sideY, sideX), cutn=args.num_cuts, clip=clip_cfgs, seed=st.seed, device=device)
+    kw = dict(drawer=kind, image_hw=engine_hw, cutn=args.num_cuts, clip=clip_cfgs, seed=st.seed, device=device)
     if aspect != 1.0:
         kw["cut_aspect"] = aspect
     world = int(getattr(args, "b200_world", 1) or 1)
@@ -357,17 +366,20 @@ def do_init(args):
         kw.update(fft_decay=args.fft_decay, fft_colors=args.fft_colors)
     eng = _engine_factory(**kw)
     weights = args.b200_weights or {}
-    if kind in (E.DRAWER_VQGAN, E.DRAWER_VDIFF):
-        key = "vqgan" if kind == E.DRAWER_VQGAN else "vdiff"
+    if kind in (E.DRAWER_VQGAN, E.DRAWER_VDIFF, E.DRAWER_SUPERRES):
+        key = {E.DRAWER_VQGAN: "vqgan", E.DRAWER_VDIFF: "vdiff", E.DRAWER_SUPERRES: "super_resolution"}[kind]
         if key in weights:
             vq_sd = _load_state_dict(weights[key])
         elif kind == E.DRAWER_VQGAN:
             vq_sd = S.vqgan_state_dict(E.VQGAN_F16_16384, 0, with_encoder=True)
-        elif args.b200_allow_synthetic:
+        elif not args.b200_allow_synthetic:
+            ckpt = "the cc12m_1 checkpoint's" if kind == E.DRAWER_VDIFF else f"the {args.super_resolution_model} checkpoint's"
+            raise ValueError(f"the {args.drawer} drawer needs b200_weights['{key}'] ({ckpt} state_dict), or "
+                             "b200_allow_synthetic=True for seeded random weights")
+        elif kind == E.DRAWER_VDIFF:
             vq_sd = S.vdiff_state_dict(0)
         else:
-            raise ValueError("the vdiff drawer needs b200_weights['vdiff'] (the cc12m_1 checkpoint's state_dict), or "
-                             "b200_allow_synthetic=True for seeded random weights")
+            vq_sd = S.rrdbnet_state_dict(0)
         eng.load_module(E.MOD_VQGAN, vq_sd)
     for i, m in enumerate(args.clip_models):
         sd = _load_state_dict(weights[m]) if m in weights else S.clip_state_dict(E.CLIP_ARCH[m], 1 + i)
@@ -381,7 +393,7 @@ def do_init(args):
     # ---- image initialisation (pixray.py:674-727): a noise / gradient / blank start image, optionally an init image, into
     # drawer.init_from_tensor(t * 2 - 1) -- for the VQGAN drawer that is model.encode on the engine (pxr_vqgan_encode)
     st.init_image_tensor, st.z_orig = None, None
-    if kind in (E.DRAWER_VQGAN, E.DRAWER_PIXEL, E.DRAWER_POLYGON) and (args.init_image or args.init_noise):
+    if kind in (E.DRAWER_VQGAN, E.DRAWER_PIXEL, E.DRAWER_POLYGON, E.DRAWER_SUPERRES) and (args.init_image or args.init_noise):
         from PIL import Image
         from .util import random_gradient_image, random_noise_image
         rng = np.random.default_rng(st.seed)

@@ -465,8 +465,10 @@ class Engine {
     }
     return (size_t)splits * rows * N > splitk_ws_elems ? 1 : splits;
   }
+  // in_ld: pixel stride of `in` (0: cin); the conv reads its first cin channels
   void add_conv(OpList& l, const act_t* in, int H, int Wd, int cin, const act_t* wt, int cout_pad, int n_out, int ks,
-                const GemmEpilogue& e) {
+                const GemmEpilogue& e, long long in_ld = 0) {
+    if (in_ld <= 0) in_ld = cin;
     const long long m_tiles = (long long)(H * Wd + 127) / 128;
     int bn = pick_bn(cout_pad < 64 ? cout_pad : n_out, false, m_tiles);
     if (bn > cout_pad) bn = cout_pad;
@@ -482,7 +484,7 @@ class Engine {
       pe.out_f32 = splitk_ws;
       pe.ldc = n_out;
       pe.k_splits = splits;
-      int rc = conv_plan_make(plan.get(), in, cin, 1, H, Wd, cin, wt, cout_pad, n_out, ks, pe, bn, fmt, num_sms, buf, sizeof buf);
+      int rc = conv_plan_make(plan.get(), in, in_ld, 1, H, Wd, cin, wt, cout_pad, n_out, ks, pe, bn, fmt, num_sms, buf, sizeof buf);
       if (rc) throw EngineError(rc, std::string("conv plan (split-K): ") + buf);
       const float* ws = splitk_ws;
       const float* bias = e.bias;
@@ -509,7 +511,7 @@ class Engine {
       q.sk.out = out;
       return;
     }
-    int rc = conv_plan_make(plan.get(), in, cin, 1, H, Wd, cin, wt, cout_pad, n_out, ks, e, bn, fmt, num_sms, buf,
+    int rc = conv_plan_make(plan.get(), in, in_ld, 1, H, Wd, cin, wt, cout_pad, n_out, ks, e, bn, fmt, num_sms, buf,
                             sizeof buf);
     if (rc) throw EngineError(rc, std::string("conv plan: ") + buf);
     l.add(1, [plan, s] { gemm_launch(*plan, s); }, plan->flops, gemm_label(kind, *plan, OP_KMAJOR, OP_KMAJOR, e), plan->bytes);
@@ -656,6 +658,11 @@ class Engine {
   float *vd_pred = nullptr, *vd_v = nullptr, *vd_gpred = nullptr, *vd_vout = nullptr, *vd_mod_out = nullptr,
         *vd_h0 = nullptr, *vd_te = nullptr, *vd_tmp[5] = {nullptr}, *vd_b[5] = {nullptr};
   act_t *vd_gv = nullptr, *vd_col = nullptr, *vd_xin = nullptr, *vd_gin = nullptr, *vd_wmod = nullptr, *vd_w[5] = {nullptr};
+
+  // ------------------------------------------------------------------ super-resolution drawer (engine_superres.inc)
+  struct SrConv;
+  void build_superres();
+  SrConv sr_load_conv(const std::string& prefix, int cin, int cout, float scale);
 
   // ------------------------------------------------------------------ execution
   void prepare_cut_params(const pxr_cut_params* p, int iter);
@@ -2164,9 +2171,10 @@ bool Engine::spot_pass(int which, bool accumulate_img) {
   return true;
 }
 
-// clip_z without per-channel bounds: the fast pixel grid clamps to [0, 1], the polygon fills RGB to [0, 1] and alpha to 1
+// clip_z without per-channel bounds: the fast pixel grid and the super-resolution latent clamp to [0, 1], the polygon fills
+// RGB to [0, 1] and alpha to 1
 int Engine::clip_mode() const {
-  if (cfg.drawer == PXR_DRAWER_PIXEL) return CLIP_01;
+  if (cfg.drawer == PXR_DRAWER_PIXEL || cfg.drawer == PXR_DRAWER_SUPERRES) return CLIP_01;
   if (cfg.drawer == PXR_DRAWER_POLYGON) return CLIP_RGBA;
   return CLIP_NONE;
 }
@@ -2352,6 +2360,7 @@ void Engine::finalize() {
   else if (cfg.drawer == PXR_DRAWER_FFT) build_fft();
   else if (cfg.drawer == PXR_DRAWER_VDIFF) build_vdiff();
   else if (cfg.drawer == PXR_DRAWER_POLYGON) build_polygon();
+  else if (cfg.drawer == PXR_DRAWER_SUPERRES) build_superres();
   else throw EngineError(-47, "unknown drawer kind");
   adam_m = dalloc<float>(z_numel);
   adam_v = dalloc<float>(z_numel);
@@ -2429,6 +2438,7 @@ void Engine::finalize() {
 }
 
 #include "engine_vdiff.inc"
+#include "engine_superres.inc"
 
 }  // namespace pxr
 

@@ -192,7 +192,7 @@ struct BlockMap {
 
 // Which input tensor (if any) is prefetched for the block: residual fp32, residual fp16 or the saved pre-activation.
 __device__ __forceinline__ int prefetch_kind(const GemmParams& p) {
-  return p.res_f32 ? 1 : (p.res_f16 ? 2 : (p.act == ACT_QUICKGELU_BWD ? 3 : 0));
+  return p.res_f32 ? 1 : (p.res_f16 ? 2 : ((p.act == ACT_QUICKGELU_BWD || p.act == ACT_LRELU_BWD) ? 3 : 0));
 }
 
 // Issue the global loads of the block's input tensor BEFORE the accumulator block is read, so their DRAM latency
@@ -273,7 +273,17 @@ __device__ __forceinline__ void epilogue_block(const GemmParams& p, const float*
 #pragma unroll
       for (int j = 0; j < E; ++j) x[j] += b;
     }
-    if (p.act == ACT_QUICKGELU) {
+    unsigned neg = 0;  // ACT_LRELU_BWD: the masked columns whose saved activation is <= 0 (applied after the residual)
+    if (p.act == ACT_LRELU) {
+#pragma unroll
+      for (int j = 0; j < E; ++j) x[j] = fmaxf(x[j], 0.2f * x[j]);
+    } else if (p.act == ACT_LRELU_BWD && col + E > p.act_col0) {
+      float u[E];
+      if (vec && kind == 3) unpack_pf<E>(pf[it], 3, u);
+      else ld_f16<E>(p.aux_in + o, vec, nv, u);
+#pragma unroll
+      for (int j = 0; j < E; ++j) neg |= (col + j >= p.act_col0 && !(u[j] > 0.f)) ? 1u << j : 0u;
+    } else if (p.act == ACT_QUICKGELU) {
       if (p.aux_out) st_f16<E>(p.aux_out + o, vec, nv, x);
 #pragma unroll
       for (int j = 0; j < E; ++j) x[j] = quickgelu(x[j]);
@@ -297,6 +307,11 @@ __device__ __forceinline__ void epilogue_block(const GemmParams& p, const float*
       else ld_f16<E>(p.res_f16 + o, vec, nv, t);
 #pragma unroll
       for (int j = 0; j < E; ++j) x[j] += t[j];
+    }
+    if (neg) {
+#pragma unroll
+      for (int j = 0; j < E; ++j)
+        if (neg & (1u << j)) x[j] *= 0.2f;
     }
     if (p.out_f32) st_f32<E>(p.out_f32 + o, vec, nv, x);
     if (p.out_f16) st_f16<E>(p.out_f16 + o, vec, nv, x);
@@ -785,7 +800,7 @@ void (*plain_kernel(const GemmParams& p))(GemmParams) {
     case TE_RES16: return gemm_tce_kernel<TE_RES16, NF>;
     default: break;
   }
-  if (p.res_f32 || p.res_f16 || p.act == ACT_QUICKGELU_BWD) return gemm_tc_in_kernel<NF>;
+  if (p.res_f32 || p.res_f16 || p.act == ACT_QUICKGELU_BWD || p.act == ACT_LRELU_BWD) return gemm_tc_in_kernel<NF>;
   return gemm_tc_kernel<NF>;
 }
 void (*kernel_for(const GemmParams& p))(GemmParams) {
@@ -980,9 +995,15 @@ int finish_plan(GemmPlan* plan, const GemmEpilogue& epi, int block_n, int num_sm
     set_err(err, errlen, "block_n must be a multiple of 16 in [16, 128]");
     return -10;
   }
-  if (epi.act < ACT_NONE || epi.act > ACT_QUICKGELU_BWD) {
-    set_err(err, errlen, "unknown epilogue activation (act must be 0 none, 1 QuickGELU or 2 QuickGELU backward)");
+  if (epi.act != ACT_NONE && epi.act != ACT_QUICKGELU && epi.act != ACT_QUICKGELU_BWD && epi.act != ACT_LRELU &&
+      epi.act != ACT_LRELU_BWD) {
+    set_err(err, errlen, "unknown epilogue activation (act must be 0 none, 1 QuickGELU, 2 QuickGELU backward, 4 LeakyReLU "
+                         "or 5 LeakyReLU backward)");
     return -12;
+  }
+  if (epi.act == ACT_LRELU_BWD && !epi.aux_in) {
+    set_err(err, errlen, "the LeakyReLU backward needs the saved post-activation (aux_in)");
+    return -14;
   }
   if (p.b_mode == OP_MNMAJOR && block_n % 64) {
     set_err(err, errlen, "MN-major B needs block_n % 64 == 0");
@@ -1016,6 +1037,7 @@ int finish_plan(GemmPlan* plan, const GemmEpilogue& epi, int block_n, int num_sm
   p.bias = epi.bias;
   p.bias_per_row = epi.bias_per_row;
   p.act = epi.act;
+  p.act_col0 = epi.act_col0;
   p.aux_in = epi.aux_in;
   p.aux_out = epi.aux_out;
   p.res_f32 = epi.res_f32;

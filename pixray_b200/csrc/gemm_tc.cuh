@@ -22,7 +22,11 @@
 namespace pxr {
 
 enum OperandMode : int { OP_KMAJOR = 0, OP_MNMAJOR = 1, OP_CONV = 2 };
-enum EpiAct : int { ACT_NONE = 0, ACT_QUICKGELU = 1, ACT_QUICKGELU_BWD = 2 };
+// Code 3 is unassigned (it named the removed softmax epilogue) and stays refused.
+// ACT_LRELU: LeakyReLU(0.2) after the bias.  ACT_LRELU_BWD: the sum (accumulator + bias + residual) times 1 where the saved
+// post-activation aux_in is > 0, else 0.2, in the columns >= act_col0 (the others pass unmasked): the dense blocks of the
+// super-resolution net mask one channel slice of a wider gradient (engine_superres.inc).
+enum EpiAct : int { ACT_NONE = 0, ACT_QUICKGELU = 1, ACT_QUICKGELU_BWD = 2, ACT_LRELU = 4, ACT_LRELU_BWD = 5 };
 
 constexpr int GEMM_BLOCK_M = 128;
 constexpr int GEMM_BLOCK_K = 64;
@@ -51,6 +55,7 @@ struct GemmParams {
   const float* bias;
   int bias_per_row;
   int act;
+  int act_col0;        // ACT_LRELU_BWD: first masked column
   const __half* aux_in;
   __half* aux_out;
   const float* res_f32;
@@ -87,6 +92,7 @@ struct GemmEpilogue {
   const float* bias = nullptr;
   int bias_per_row = 0;
   int act = ACT_NONE;
+  int act_col0 = 0;   // ACT_LRELU_BWD only: columns below it are stored unmasked
   const __half* aux_in = nullptr;
   __half* aux_out = nullptr;
   const float* res_f32 = nullptr;

@@ -92,13 +92,25 @@ void subsample_odd(const act_t* full, int H, int W, int C, act_t* y, cudaStream_
 // z[c, p] = codebook[idx[p], c] (fp32): the quantised latent model.encode returns
 void gather_codes(const float* cb, const int* idx, int C, int hw, float* z, cudaStream_t st);
 
-void upsample2x(const act_t* x, int H, int W, int C, act_t* y, cudaStream_t st);        // nearest, [H,W,C]->[2H,2W,C]
+// nearest, [H,W,C]->[2H,2W,C]; the input's pixel stride is ld_in (0: C), the output is dense
+void upsample2x(const act_t* x, int H, int W, int C, act_t* y, cudaStream_t st, int ld_in = 0);
 void downsum2x(const act_t* gy, int H, int W, int C, act_t* gx, cudaStream_t st);       // adjoint: [2H,2W,C]->[H,W,C]
 
 // conv_out result [pixels, ld] fp32 (3 valid channels) -> image [3, pixels] = clamp((x+1)/2, 0, 1); pre = unclamped.
-void image_finish(const float* conv_out, int ld, int pixels, float* pre, float* img, cudaStream_t st);
-// ClampWithGrad backward (vqgan.py:76-79) + d/dx of (x+1)/2 -> fp16 [pixels, ld] (ld >= 3; other channels untouched)
-void image_finish_backward(const float* g_img, const float* pre, int pixels, int ld, act_t* g_out, cudaStream_t st);
+// shift = 0: clamp(x, 0, 1) (the super-resolution net's output is already an image in [0, 1]).
+void image_finish(const float* conv_out, int ld, int pixels, float* pre, float* img, cudaStream_t st, int shift = 1);
+// ClampWithGrad backward (vqgan.py:76-79) + d/dx of (x+1)/2 (shift = 0: without it) -> fp16 [pixels, ld] (ld >= 3; other
+// channels untouched)
+void image_finish_backward(const float* g_img, const float* pre, int pixels, int ld, act_t* g_out, cudaStream_t st,
+                           int shift = 1);
+
+// ---- super-resolution drawer (kernels_superres.cu; RRDBNet, engine_superres.inc).  NHWC fp16 tensors with pixel strides.
+// y[p, c] = fp16(alpha a[p, c] + b[p, c]) for c < C (C % 8 == 0; b may be null; y may alias b): the RRDB's outer
+// residual x + 0.2 rdb3(...) and its adjoint
+void sr_axpy(const act_t* a, int lda, float alpha, const act_t* b, int ldb, act_t* y, int ldy, int C, long long pixels,
+             cudaStream_t st);
+// z_grad[c, p] = g[p, c] * inv_scale for c < 3: the latent's gradient out of the padded NHWC input of conv_first
+void sr_zgrad(const act_t* g, int ld, long long pixels, float inv_scale, float* z_grad, cudaStream_t st);
 
 // FastPixelDrawer.synth (fast_pixeldrawer.py:89-91): nearest upsample [3,rows,cols] -> [3,H,W] + clamp; and adjoint.
 void pixel_synth(const float* z, int rows, int cols, int H, int W, float* pre, float* img, cudaStream_t st);

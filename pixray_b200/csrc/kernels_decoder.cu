@@ -664,7 +664,7 @@ __global__ void __launch_bounds__(GNC_THREADS, 1)
   }
 }
 
-__global__ void __launch_bounds__(256) upsample2x_kernel(const act_t* __restrict__ x, int H, int W, int C,
+__global__ void __launch_bounds__(256) upsample2x_kernel(const act_t* __restrict__ x, int H, int W, int C, int ld_in,
                                                          act_t* __restrict__ y) {
   pdl_prologue();
   const int vecs = C / 8;
@@ -673,7 +673,7 @@ __global__ void __launch_bounds__(256) upsample2x_kernel(const act_t* __restrict
     int vc = (int)(v % vecs);
     long long p = v / vecs;
     int ox = (int)(p % (2 * W)), oy = (int)(p / (2 * W));
-    const uint4* src = reinterpret_cast<const uint4*>(x + ((size_t)(oy >> 1) * W + (ox >> 1)) * C) + vc;
+    const uint4* src = reinterpret_cast<const uint4*>(x + ((size_t)(oy >> 1) * W + (ox >> 1)) * ld_in) + vc;
     reinterpret_cast<uint4*>(y)[v] = *src;
   }
 }
@@ -738,20 +738,21 @@ __global__ void gather_codes_kernel(const float* __restrict__ cb, const int* __r
 }
 
 __global__ void image_finish_kernel(const float* __restrict__ conv_out, int ld, int pixels, float* __restrict__ pre,
-                                    float* __restrict__ img) {
+                                    float* __restrict__ img, int shift) {
   pdl_prologue();
   int p = blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= pixels) return;
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
-    float v = (conv_out[(size_t)p * ld + c] + 1.f) / 2.f;  // decode(z_q).add(1).div(2), vqgan.py:195
+    const float x = conv_out[(size_t)p * ld + c];
+    const float v = shift ? (x + 1.f) / 2.f : x;  // decode(z_q).add(1).div(2), vqgan.py:195
     pre[(size_t)c * pixels + p] = v;
     img[(size_t)c * pixels + p] = fminf(fmaxf(v, 0.f), 1.f);
   }
 }
 
 __global__ void image_finish_bwd_kernel(const float* __restrict__ g_img, const float* __restrict__ pre, int pixels,
-                                        int ld, act_t* __restrict__ g_out) {
+                                        int ld, act_t* __restrict__ g_out, int shift) {
   pdl_prologue();
   int p = blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= pixels) return;
@@ -761,7 +762,7 @@ __global__ void image_finish_bwd_kernel(const float* __restrict__ g_img, const f
     float v = pre[(size_t)c * pixels + p];
     float cl = fminf(fmaxf(v, 0.f), 1.f);
     float keep = (g * (v - cl) >= 0.f) ? 1.f : 0.f;  // vqgan.py:79
-    g_out[(size_t)p * ld + c] = __float2half_rn(0.5f * g * keep);
+    g_out[(size_t)p * ld + c] = __float2half_rn((shift ? 0.5f * g : g) * keep);
   }
 }
 
@@ -941,8 +942,9 @@ void gn_backward_coop(const act_t* dy, const act_t* x, const float* stats, const
   if (cudaPeekAtLastError() == cudaSuccess) gb->issued += grid;
 }
 
-void upsample2x(const act_t* x, int H, int W, int C, act_t* y, cudaStream_t st) {
-  launch_pdl(upsample2x_kernel, dim3(grid_for((long long)4 * H * W * C / 8, 256)), dim3(256), 0, st, x, H, W, C, y);
+void upsample2x(const act_t* x, int H, int W, int C, act_t* y, cudaStream_t st, int ld_in) {
+  launch_pdl(upsample2x_kernel, dim3(grid_for((long long)4 * H * W * C / 8, 256)), dim3(256), 0, st, x, H, W, C,
+             ld_in > 0 ? ld_in : C, y);
 }
 void downsum2x(const act_t* gy, int H, int W, int C, act_t* gx, cudaStream_t st) {
   launch_pdl(downsum2x_kernel, dim3(grid_for((long long)H * W * C / 8, 256)), dim3(256), 0, st, gy, H, W, C, gx);
@@ -958,11 +960,12 @@ void gather_codes(const float* cb, const int* idx, int C, int hw, float* z, cuda
   launch_pdl(gather_codes_kernel, dim3((C * hw + 255) / 256), dim3(256), 0, st, cb, idx, C, hw, z);
 }
 
-void image_finish(const float* conv_out, int ld, int pixels, float* pre, float* img, cudaStream_t st) {
-  launch_pdl(image_finish_kernel, dim3((pixels + 255) / 256), dim3(256), 0, st, conv_out, ld, pixels, pre, img);
+void image_finish(const float* conv_out, int ld, int pixels, float* pre, float* img, cudaStream_t st, int shift) {
+  launch_pdl(image_finish_kernel, dim3((pixels + 255) / 256), dim3(256), 0, st, conv_out, ld, pixels, pre, img, shift);
 }
-void image_finish_backward(const float* g_img, const float* pre, int pixels, int ld, act_t* g_out, cudaStream_t st) {
-  launch_pdl(image_finish_bwd_kernel, dim3((pixels + 255) / 256), dim3(256), 0, st, g_img, pre, pixels, ld, g_out);
+void image_finish_backward(const float* g_img, const float* pre, int pixels, int ld, act_t* g_out, cudaStream_t st,
+                           int shift) {
+  launch_pdl(image_finish_bwd_kernel, dim3((pixels + 255) / 256), dim3(256), 0, st, g_img, pre, pixels, ld, g_out, shift);
 }
 
 void pixel_synth(const float* z, int rows, int cols, int H, int W, float* pre, float* img, cudaStream_t st) {

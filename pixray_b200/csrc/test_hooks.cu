@@ -38,6 +38,7 @@ static void fill_epilogue(GemmEpilogue& e, const pxr_test_gemm_desc* d) {
   e.bs0 = d->c_bs0;
   e.bs1 = d->c_bs1;
   e.tma_epi = d->tma_epi;
+  e.act_col0 = d->act_col0;
 }
 
 extern "C" int pxr_test_gemm(const pxr_test_gemm_desc* d, char* err, int errlen) {

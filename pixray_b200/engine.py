@@ -10,13 +10,15 @@ import torch
 
 from . import _lib
 
-DRAWER_VQGAN, DRAWER_PIXEL, DRAWER_FFT, DRAWER_VDIFF, DRAWER_POLYGON = 0, 1, 2, 3, 4
+DRAWER_VQGAN, DRAWER_PIXEL, DRAWER_FFT, DRAWER_VDIFF, DRAWER_POLYGON, DRAWER_SUPERRES = 0, 1, 2, 3, 4, 5
 LOSS_SYMMETRY, LOSS_SATURATION, LOSS_PALETTE, LOSS_SMOOTHNESS, LOSS_EDGE, LOSS_GAUSSIAN, LOSS_AESTHETIC = range(7)
 ANCHOR_SPHERICAL, ANCHOR_MSE, ANCHOR_COS, ANCHOR_PIX = 0, 1, 2, 3
 FILTER_TILER, FILTER_WALLPAPER, FILTER_LOOKUP = range(3)
 PAD_REFLECTION, PAD_BORDER = 0, 1
 MOD_VQGAN, MOD_CLIP0, MOD_CLIP1 = 0, 1, 2
 
+# RRDBNet of RealESRGAN_x4plus (super_resolution.py:53): RRDBNet(3, 3, num_feat=64, num_block=23, num_grow_ch=32, scale=4)
+RRDBNET_X4PLUS = dict(num_feat=64, num_block=23, num_grow_ch=32)
 VQGAN_F16_16384 = dict(z_channels=256, n_embed=16384, ch=128, ch_mult=(1, 1, 2, 2, 4), num_res_blocks=2,
                        attn_resolution=16, resolution=256)
 CLIP_ARCH = {
@@ -33,7 +35,8 @@ class EngineError(RuntimeError):
 class B200Engine:
     def __init__(self, *, drawer=DRAWER_VQGAN, image_hw=(256, 256), vqgan=None, grid=None, cutn=64, cut_size=224,
                  clip=(), noise_fac=0.1, seed=0, device=0, rank=0, world=1, grad_scale=0.0, lr_betas=(0.9, 0.999),
-                 adam_eps=1e-8, fft_decay=0.0, fft_colors=0.0, fft_contrast=0.0, cut_aspect=1.0, polygons=None):
+                 adam_eps=1e-8, fft_decay=0.0, fft_colors=0.0, fft_contrast=0.0, cut_aspect=1.0, polygons=None,
+                 superres=None):
         if not torch.cuda.is_available():
             raise EngineError("pixray_b200 needs a CUDA device (H100); there is no CPU fallback")
         self.lib = _lib.load()
@@ -53,6 +56,13 @@ class B200Engine:
         elif drawer == DRAWER_VDIFF:
             # VdiffDrawer's x (vdiff.py:118): [1, 3, gen_height, gen_width]
             self.z_shape = (1, 3, image_hw[0], image_hw[1])
+        elif drawer == DRAWER_SUPERRES:
+            # SuperResolutionDrawer's z (super_resolution.py:75-76): [1, 3, H/4, W/4]; the canvas is 4x the latent
+            if image_hw[0] % 4 or image_hw[1] % 4:
+                raise EngineError("drawer=DRAWER_SUPERRES needs canvas sides that are multiples of 4")
+            r = dict(RRDBNET_X4PLUS) if superres is None else dict(superres)
+            cfg.ch, cfg.num_block, cfg.num_grow_ch = r["num_feat"], r["num_block"], r["num_grow_ch"]
+            self.z_shape = (1, 3, image_hw[0] // 4, image_hw[1] // 4)
         elif drawer == DRAWER_FFT:
             # FftDrawer params (fftdrawer.py:57-61): rfft2 spectrum [1, 3, H, W/2+1, 2]
             self.z_shape = (1, 3, image_hw[0], image_hw[1] // 2 + 1, 2)

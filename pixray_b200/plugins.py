@@ -359,6 +359,81 @@ class VdiffDrawer(DrawingInterface):
         return self.x.clone()
 
 
+class SuperResolutionDrawer(DrawingInterface):
+    """super_resolution.py:34-107 (with real_esrganer.py at tile 0 / pre_pad 0 / scale 4): z = a quarter-size image in
+    [0, 1], synth = clamp_with_grad(RRDBNet(z), 0, 1) on the engine (PXR_DRAWER_SUPERRES), Adam at the global learning
+    rate, clip_z clamps z to [0, 1]."""
+
+    models = ("RealESRGAN_x4plus",)  # superresolution_checkpoint_table (super_resolution.py:12-14)
+
+    @staticmethod
+    def add_settings(parser):
+        parser.add_argument("--super_resolution_model", type=str, help="Super resolution model", default="RealESRGAN_x4plus", dest="super_resolution_model")
+        return parser
+
+    def __init__(self, settings, session: Session):
+        super().__init__(settings)
+        self.session = session
+        self.super_resolution_model = SuperResolutionDrawer.check_model(settings.super_resolution_model)
+        self.z = None
+
+    @staticmethod
+    def check_model(name):
+        """The reference looks the name up in its checkpoint table: any other name raises (KeyError there)."""
+        if name not in SuperResolutionDrawer.models:
+            raise ValueError(f"super_resolution_model '{name}' is not in the checkpoint table {list(SuperResolutionDrawer.models)}")
+        return name
+
+    def load_model(self, settings, device):
+        self.device = device
+
+    def get_opts(self, decay_divisor):
+        return None
+
+    def get_num_resolutions(self):
+        return None
+
+    def get_z_from_tensor(self, ref_tensor):
+        """F.interpolate((t + 1) / 2, size=shape // 4, bilinear, align_corners=False) (super_resolution.py:75-76)."""
+        return F.interpolate((ref_tensor + 1) / 2, size=(torch.tensor(ref_tensor.shape[-2:]) // 4).tolist(),
+                             mode="bilinear", align_corners=False)
+
+    def init_from_tensor(self, init_tensor):
+        """A start image is required: the reference fails on None, here init_tensor None raises ValueError."""
+        if init_tensor is None:
+            raise ValueError("the super_resolution drawer starts from an image: init_from_tensor needs a tensor")
+        z = self.get_z_from_tensor(init_tensor)
+        if tuple(z.shape) != tuple(self.session.engine.z_shape):
+            raise ValueError(f"the start image gives a latent of shape {tuple(z.shape)}; the engine was built for "
+                             f"{tuple(self.session.engine.z_shape)}")
+        self.z = z.to(self.session.engine.device, torch.float32).contiguous()
+
+    def reapply_from_tensor(self, new_tensor):
+        new_z = self.get_z_from_tensor(new_tensor)
+        with torch.no_grad():
+            self.z.copy_(new_z)
+
+    def synth(self, cur_iteration):
+        return self.session.engine.synth(self.z)
+
+    def clip_z(self):
+        with torch.no_grad():
+            self.z.copy_(self.z.clip(0, 1))
+
+    def get_z(self):
+        return self.z
+
+    def set_z(self, new_z):
+        if self.z is None:
+            self.z = new_z.detach().to(self.session.engine.device, torch.float32).contiguous().clone()
+            return self.z
+        with torch.no_grad():
+            return self.z.copy_(new_z)
+
+    def get_z_copy(self):
+        return self.z.clone()
+
+
 class FftDrawer(DrawingInterface):
     """fftdrawer.py:13-109, `fft_use="fft"`: params = the rfft2 spectrum [1, 3, H, W/2+1, 2] ~ N(0, 0.01^2)
     (aphantasia fft_image), synth = to_valid_rgb(fft_image)(contrast=0.9); the drawer owns its Adam (lr fft_lrate /

@@ -258,3 +258,43 @@ def vdiff_state_dict(seed=0, c=128):
     block("net.7", cs[0], cs[0], cs[0])
     block("net.8", cs[0], cs[0], 3, last=True)
     return sd
+
+
+def rrdbnet_state_dict(seed=0, num_feat=64, num_block=23, num_grow_ch=32, last_bias=0.5):
+    """Real-ESRGAN's RRDBNet tensors under the checkpoint's own keys (basicsr rrdbnet_arch), seeded random with basicsr's
+    initialisation: the dense-block convolutions kaiming-normal (fan_in, gain sqrt(2)) times 0.1 with zero bias
+    (default_init_weights(..., 0.1)), every other convolution PyTorch's default (uniform(+-1/sqrt(fan_in)) for weight and
+    bias).  conv_last's bias is centred on `last_bias`, so that most pixels of the image land inside (0, 1) rather than
+    on ClampWithGrad's edges."""
+    g = torch.Generator().manual_seed(seed)
+    sd = {}
+
+    def default(key, cin, cout):
+        b = (1.0 / (cin * 9)) ** 0.5
+        sd[key + ".weight"] = (torch.rand(cout, cin, 3, 3, generator=g) * 2 - 1) * b
+        sd[key + ".bias"] = (torch.rand(cout, generator=g) * 2 - 1) * b
+
+    def dense(key, cin, cout):
+        sd[key + ".weight"] = torch.randn(cout, cin, 3, 3, generator=g) * (2.0 / (cin * 9)) ** 0.5 * 0.1
+        sd[key + ".bias"] = torch.zeros(cout)
+
+    nf, gc = num_feat, num_grow_ch
+    default("conv_first", 3, nf)
+    for i in range(num_block):
+        for j in (1, 2, 3):
+            for k in range(1, 6):
+                dense(f"body.{i}.rdb{j}.conv{k}", nf + gc * (k - 1), gc if k < 5 else nf)
+    for key in ("conv_body", "conv_up1", "conv_up2", "conv_hr"):
+        default(key, nf, nf)
+    default("conv_last", nf, 3)
+    sd["conv_last.bias"] = sd["conv_last.bias"] + last_bias
+    return sd
+
+
+def superres_fwd_flops(h, w, num_feat=64, num_block=23, num_grow_ch=32):
+    """Multiply-add FLOPs (2 per MAC) of one RRDBNet forward on an h x w latent (image 4h x 4w); the dgrad costs the same."""
+    nf, gc, px = num_feat, num_grow_ch, h * w
+    per_px = lambda cin, cout: 2.0 * 9 * cin * cout  # noqa: E731
+    dense = sum(per_px(nf + gc * k, gc) for k in range(4)) + per_px(nf + 4 * gc, nf)
+    low = per_px(3, nf) + 3 * num_block * dense + per_px(nf, nf)
+    return px * low + 4 * px * per_px(nf, nf) + 16 * px * (2 * per_px(nf, nf) + per_px(nf, 3))
