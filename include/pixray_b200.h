@@ -312,12 +312,21 @@ typedef struct {
   /* act 5: out = (alpha acc + bias + residual) * (aux_in > 0 ? 1 : 0.2) in the columns >= act_col0, aux_in = the saved
    * post-activation (same layout as the output); the columns below act_col0 are stored unmasked */
   int act_col0;
+  /* > 1: split-K.  The plan runs ceil(nkb / ceil(nkb / k_splits)) splits of ceil(nkb / k_splits) 64-deep k-blocks each and
+   * writes split s's fp32 partial sums to slab s of out_f32 (slab pitch M * ldc for a GEMM, H * W * ldc for a conv);
+   * needs one unbatched image, out_f32 only, no bias, residual or activation.  0 or 1: one split. */
+  int k_splits;
 } pxr_test_gemm_desc;
 
 int pxr_test_gemm(const pxr_test_gemm_desc* d, char* err, int errlen);
 /* implicit-GEMM conv over NHWC fp16: d->a = input (pixel stride lda), d->b = weights [taps*cout_pad, c_in] */
 int pxr_test_conv(const pxr_test_gemm_desc* d, int batch, int H, int W, int c_in, int cout_pad, int ksize, char* err,
                   int errlen);
+/* the split-K reduce: out[p, c] = fp16(bias[c] + ws[0][p, c] + ... + ws[splits-1][p, c] + res[p, c]) for c < N, in that
+ * order.  ws DEVICE fp32 [splits][pixels][ld_ws]; bias (nullable) fp32 [N]; res (nullable) / out fp16 [pixels][ld_out];
+ * N, ld_ws, ld_out multiples of 8.  Synchronous; -1 on unsupported arguments. */
+int pxr_test_splitk_reduce(const float* ws, int splits, long long pixels, int N, int ld_ws, const float* bias, const void* res,
+                           void* out, int ld_out);
 
 /* host-side evaluation of the ColorJitter pixel body and its vector-Jacobian product (no GPU needed) */
 int pxr_test_color_jitter_host(const float* rgb, int n, int code, float saturation, float hue, const float* g_out,
@@ -341,11 +350,40 @@ int pxr_test_attention(const void* qkv, void* o, float* lse, const void* d_o, vo
 /* GroupNorm(32, C, eps 1e-6)(+ swish) of the VQGAN decoder (taming Normalize + nonlinearity), forward and -- when dy or
  * ws_dy is given -- backward, on DEVICE NHWC fp16 tensors [pixels, C].  variant 0: single-kernel grid-barrier version,
  * 1: one thread-block cluster per group; with ws / ws_dy (variant 1) the kernel is also the epilogue of a split-K
- * convolution (fp32 partial sums [splits][pixels][C]).  scratch: 64 * (num_sms + 2) floats + 8 zeroed bytes. */
+ * convolution (fp32 partial sums [splits][pixels][C]); 2: the three-kernel version (statistics, final, apply), which the
+ * engine takes when neither of the others fits.  scratch: variants 0 and 1: 64 * (num_sms + 2) floats + 8 zeroed bytes
+ * (the grid barrier's counter, at float offset 64 * (num_sms + 2)); variant 2: 128 * gn_partials + 64 floats with
+ * gn_partials = ceil(pixels / r), r = ceil(pixels / 592) rounded up to a multiple of 32 (at least 32). */
 int pxr_test_groupnorm(int variant, const void* x, const float* ws, int splits, const float* bias, const void* res,
                        void* x_out, const float* gamma, const float* beta, int pixels, int C, int swish, void* y,
                        float* stats, const void* dy, const float* ws_dy, int splits_dy, const void* dres, void* dx,
                        float* scratch, int repeat);
+
+/* the vdiff U-Net's norm (GroupNorm(1, C) + modulation, as vd_norm / vd_norm_bwd run it on the grid-barrier kernel):
+ * y = act(norm(x) * (gamma + gamma_add) + beta) (+ res), act 0 none, 1 swish, 2 ReLU; gamma / beta / res nullable;
+ * backward when dy is given: dx = norm'(x) applied to dy through the activation (+ dres).  DEVICE NHWC fp16 [pixels, C],
+ * stats [32][2]; scratch as variant 0 of pxr_test_groupnorm (its counter zeroed before every call).  -1 when the
+ * single-kernel path does not cover the shape. */
+int pxr_test_groupnorm_unet(const void* x, const float* gamma, const float* beta, float gamma_add, int act, const void* res,
+                            float eps, int pixels, int C, void* y, float* stats, const void* dy, const void* dres, void* dx,
+                            float* scratch);
+
+/* one resampling / copy kernel on DEVICE NHWC fp16 tensors, by op:
+ *   0 upsample2x              in [H, W] (pixel stride ld_in) -> out [2H, 2W]             nearest
+ *   1 downsum2x               in [2H, 2W] -> out [H, W]                                  sum of each 2 x 2 block
+ *   2 avgpool2x               in [H, W] (pixel stride ld_in) -> out [H/2, W/2]           mean of each 2 x 2 block
+ *   3 avgpool2x_backward      in [H/2, W/2] -> out [H, W] (accumulate: adds to out)      its adjoint
+ *   4 bilinear_up2x           in [H, W] -> out [2H, 2W] (pixel stride ld_out)            bilinear, align_corners=False
+ *   5 bilinear_up2x_backward  in [2H, 2W] (pixel stride ld_in) -> out [H, W]             its adjoint
+ *   6 im2col3x3               in [H, W] -> out [H W, 9 C], tap-major, zero outside
+ *   7 copy_channels           in [H W] (pixel stride ld_in) -> out (pixel stride ld_out), C channels (accumulate: adds)
+ * Sides without a stride above are dense (ld 0 or C); ld 0 means C.  Synchronous.  -1: C % 8 != 0, H or W < 1, or an
+ * ld below C or not a multiple of 8; -2: unknown op; -3: a stride or accumulate the op does not take. */
+int pxr_test_resample(int op, const void* in, int ld_in, void* out, int ld_out, int H, int W, int C, int accumulate);
+
+/* the U-Net's fp16-weight GEMV: y[r] = act(sum_k w[r, k] x[k] + bias[r]) (+ res[r]), act = ReLU when relu != 0.
+ * w DEVICE fp16 [R, K] (K % 8 == 0), x / bias / res / y DEVICE fp32; bias and res nullable.  Synchronous. */
+int pxr_test_gemv(const void* w, int K, int R, const float* x, const float* bias, int relu, const float* res, float* y);
 
 /* the row softmax of the unfused attention on DEVICE fp16 [rows, ld] (ld % 8 == 0, cols <= ld; pad columns come back
  * 0): backward == 0 turns the scores in p_or_s into probabilities in place; backward != 0 overwrites dp (dP) with

@@ -60,7 +60,7 @@ class TestGemmDesc(C.Structure):
         ("out_f32", C.c_void_p), ("out_f16", C.c_void_p),
         ("ldc", C.c_longlong), ("c_bs0", C.c_longlong), ("c_bs1", C.c_longlong),
         ("stream", C.c_void_p), ("repeat", C.c_int), ("cta_group", C.c_int), ("tma_epi", C.c_int),
-        ("act_col0", C.c_int),
+        ("act_col0", C.c_int), ("k_splits", C.c_int),
     ]
 
 
@@ -73,6 +73,7 @@ EXPORTS = [
     "pxr_test_attention", "pxr_test_color_jitter_host", "pxr_test_color_jitter_device", "pxr_set_color_jitter", "pxr_set_image_prompts", "pxr_set_image_prompts_sized", "pxr_add_aux_loss", "pxr_add_filter", "pxr_clear_filters", "pxr_set_filter_shifts", "pxr_clear_aux_losses", "pxr_add_anchor", "pxr_clear_anchors", "pxr_num_losses", "pxr_read_losses",
     "pxr_test_pool_bounds", "pxr_test_groupnorm", "pxr_test_softmax", "pxr_test_layernorm", "pxr_set_spot_prompts", "pxr_set_spot_mask", "pxr_state_size", "pxr_save_state", "pxr_load_state", "pxr_set_schedule", "pxr_poll_status", "pxr_set_batches", "pxr_set_z_grad", "pxr_vdiff_set_schedule", "pxr_vdiff_set_clip_embed", "pxr_vdiff_set_iteration", "pxr_vdiff_renoise",
     "pxr_set_polygons", "pxr_set_synth_iteration", "pxr_test_raster_samples",
+    "pxr_test_splitk_reduce", "pxr_test_groupnorm_unet", "pxr_test_resample", "pxr_test_gemv",
 ]
 
 _lib = None

@@ -1087,8 +1087,8 @@ void Engine::build_vqgan() {
   const int h = cfg.image_h / f, w = cfg.image_w / f, hw = h * w;
   z_numel = (int64_t)zc * hw;
   // GN scratch sized for the largest activation
-  // (the cooperative kernels use up to one block per SM, the three-kernel path gn_num_partials blocks)
-  gn_part = dalloc<float>((size_t)std::max(gn_num_partials(cfg.image_h * cfg.image_w, 64), num_sms + 1) * 64 + 64);
+  // (the cooperative kernels use up to one block per SM, the three-kernel path two sets of gn_num_partials blocks)
+  gn_part = dalloc<float>((size_t)std::max(2 * gn_num_partials(cfg.image_h * cfg.image_w, 64), num_sms + 1) * 64 + 64);
   gn_bar.counter = dalloc<unsigned long long>(1);
   splitk_ws_elems = (size_t)8 << 20;  // 32 MiB of fp32 partial sums: covers every conv the split-K rule selects
   splitk_ws = dalloc<float>(splitk_ws_elems, false);

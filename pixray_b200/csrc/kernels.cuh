@@ -56,6 +56,13 @@ struct GnOpts {
   float gamma_add = 0.f;
   const act_t* res = nullptr;  // forward only: y = act(norm(x)) + res
 };
+#ifdef __CUDACC__
+// The GroupNorm kernels take the variance as E[x^2] - mean^2 from fp32 partial sums, whose rounding error grows with
+// mean^2 / var (the sums of x^2 carry mean^2 where the variance is var): at a mean of 64 standard deviations rstd is off by
+// up to 6e-4 relative.  A group whose mean exceeds sqrt(32) standard deviations (error below 5e-6) gets its statistics
+// again from sums of x - mean, a second pass; every other group keeps the one-pass result.
+__device__ __forceinline__ bool gn_refine_variance(double mean, double var) { return mean * mean > 32.0 * var; }
+#endif
 bool gn_coop_supported(int pixels, int C, int num_sms);
 void gn_forward_coop(const act_t* x, const float* gamma, const float* beta, int pixels, int C, int swish, float eps,
                      float* part, float* stats, act_t* y, int num_sms, GridBarrier* gb, cudaStream_t st,

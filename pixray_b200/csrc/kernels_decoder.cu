@@ -170,64 +170,15 @@ __device__ __forceinline__ void store8(act_t* p, const float (&f)[8]) {
   *reinterpret_cast<uint4*>(p) = u;
 }
 
-// Accumulates, per group, sum(a) and sum(b) where (a, b) = F(element).  MODE 0: (x, x^2); MODE 1: backward sums
-// (dxh, dxh * xh).  Block: 256 threads = (256 / (C/8)) pixel lanes x (C/8) channel vectors.
-template <int MODE>
-__global__ void __launch_bounds__(256) gn_partial_kernel(const act_t* __restrict__ x, const act_t* __restrict__ dy,
-                                                         const float* __restrict__ stats,
-                                                         const float* __restrict__ gamma,
-                                                         const float* __restrict__ beta, int pixels, int C, int swish,
-                                                         float* __restrict__ part) {
-  pdl_prologue();
-  __shared__ float acc[GN_G][2];
-  const int vecs = C / 8, cpg = C / GN_G;
+// The shift gn_partial_kernel subtracts for its pivoted sums: x at pixel 0 in group g's first channel, one value per group
+// that every block reads alike.
+__device__ __forceinline__ float gn_pivot(const act_t* x, int C, int g) { return __half2float(x[g * (C / GN_G)]); }
+
+// Fixed-order block reduction of the thread sums s[half][a/b] to out[32 groups][2] (no atomics: every rank of the
+// cutout-sharded mode must produce the same bits, and so must every run): pixel lanes -> channel vector -> group.
+__device__ __forceinline__ void gn_block_reduce(const float (&s)[2][2], float (*red)[256], float (*acc)[2], int vecs, int cpg,
+                                                float* __restrict__ out) {
   const int vc = threadIdx.x % vecs, pl = threadIdx.x / vecs, plane = 256 / vecs;
-  const int c0 = vc * 8;
-  const int rpb = gn_rows_per_block(pixels);
-  const int p_begin = blockIdx.x * rpb;
-  const int p_end = min(pixels, p_begin + rpb);
-  float s[2][2] = {{0.f, 0.f}, {0.f, 0.f}};  // [half][a/b] : halves of the 8-vector (cpg == 4 splits groups)
-  float g8[8], b8[8], mean8[8], rstd8[8];
-  if (MODE == 1) {
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      g8[i] = gamma[c0 + i];
-      b8[i] = beta[c0 + i];
-      int g = (c0 + i) / cpg;
-      mean8[i] = stats[2 * g];
-      rstd8[i] = stats[2 * g + 1];
-    }
-  }
-  for (int p = p_begin + pl; p < p_end; p += plane) {
-    float xv[8];
-    load8(x + (size_t)p * C + c0, xv);
-    if (MODE == 0) {
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        s[i >> 2][0] += xv[i];
-        s[i >> 2][1] += xv[i] * xv[i];
-      }
-    } else {
-      float dv[8];
-      load8(dy + (size_t)p * C + c0, dv);
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        float xh = (xv[i] - mean8[i]) * rstd8[i];
-        float d = dv[i];
-        if (swish) {
-          float a = g8[i] * xh + b8[i];
-          float sg = 1.f / (1.f + __expf(-a));
-          d *= sg * (1.f + a * (1.f - sg));
-        }
-        float dxh = d * g8[i];
-        s[i >> 2][0] += dxh;
-        s[i >> 2][1] += dxh * xh;
-      }
-    }
-  }
-  // Fixed-order block reduction (no atomics: every rank of the cutout-sharded mode must produce the same bits, and so
-  // must every run): pixel lanes -> channel vector -> group.
-  __shared__ float red[4][256];
   red[0][threadIdx.x] = s[0][0];
   red[1][threadIdx.x] = s[0][1];
   red[2][threadIdx.x] = s[1][0];
@@ -254,29 +205,112 @@ __global__ void __launch_bounds__(256) gn_partial_kernel(const act_t* __restrict
     acc[g][which] = t;
   }
   __syncthreads();
-  if (threadIdx.x < GN_G * 2) part[(size_t)blockIdx.x * GN_G * 2 + threadIdx.x] = (&acc[0][0])[threadIdx.x];
+  if (threadIdx.x < GN_G * 2) out[threadIdx.x] = (&acc[0][0])[threadIdx.x];
 }
 
-// MODE 0: stats[g] = (mean, rstd).  MODE 1: gstats[g] = (mean dxh, mean dxh*xh).   One block of 64 threads.
+// Accumulates, per group, sum(a) and sum(b) where (a, b) = F(element).  MODE 0: (x, x^2) into part[block], and
+// (d, d^2) with d = x - pivot into part[gridDim.x + block], the pivot of a group being x at pixel 0 in the group's first
+// channel (gn_pivot): gn_final_kernel takes the statistics from the second set where the first loses its precision
+// (gn_refine_variance).  MODE 1: backward sums (dxh, dxh * xh).  Block: 256 threads = (256 / (C/8)) pixel lanes x (C/8)
+// channel vectors.
 template <int MODE>
-__global__ void gn_final_kernel(const float* __restrict__ part, int nblk, double count, float eps,
+__global__ void __launch_bounds__(256) gn_partial_kernel(const act_t* __restrict__ x, const act_t* __restrict__ dy,
+                                                         const float* __restrict__ stats,
+                                                         const float* __restrict__ gamma,
+                                                         const float* __restrict__ beta, int pixels, int C, int swish,
+                                                         float* __restrict__ part) {
+  pdl_prologue();
+  __shared__ float acc[GN_G][2];
+  const int vecs = C / 8, cpg = C / GN_G;
+  const int vc = threadIdx.x % vecs, pl = threadIdx.x / vecs, plane = 256 / vecs;
+  const int c0 = vc * 8;
+  const int rpb = gn_rows_per_block(pixels);
+  const int p_begin = blockIdx.x * rpb;
+  const int p_end = min(pixels, p_begin + rpb);
+  float s[2][2] = {{0.f, 0.f}, {0.f, 0.f}};  // [half][a/b] : halves of the 8-vector (cpg == 4 splits groups)
+  float sp[2][2] = {{0.f, 0.f}, {0.f, 0.f}};  // MODE 0: the pivoted sums
+  float g8[8], b8[8], mean8[8], rstd8[8], pv[2];
+  if (MODE == 0) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) pv[h] = gn_pivot(x, C, (c0 + 4 * h) / cpg);
+  }
+  if (MODE == 1) {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      g8[i] = gamma[c0 + i];
+      b8[i] = beta[c0 + i];
+      int g = (c0 + i) / cpg;
+      mean8[i] = stats[2 * g];
+      rstd8[i] = stats[2 * g + 1];
+    }
+  }
+  for (int p = p_begin + pl; p < p_end; p += plane) {
+    float xv[8];
+    load8(x + (size_t)p * C + c0, xv);
+    if (MODE == 0) {
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        s[i >> 2][0] += xv[i];
+        s[i >> 2][1] += xv[i] * xv[i];
+        const float d = xv[i] - pv[i >> 2];
+        sp[i >> 2][0] += d;
+        sp[i >> 2][1] += d * d;
+      }
+    } else {
+      float dv[8];
+      load8(dy + (size_t)p * C + c0, dv);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        float xh = (xv[i] - mean8[i]) * rstd8[i];
+        float d = dv[i];
+        if (swish) {
+          float a = g8[i] * xh + b8[i];
+          float sg = 1.f / (1.f + __expf(-a));
+          d *= sg * (1.f + a * (1.f - sg));
+        }
+        float dxh = d * g8[i];
+        s[i >> 2][0] += dxh;
+        s[i >> 2][1] += dxh * xh;
+      }
+    }
+  }
+  __shared__ float red[4][256];
+  gn_block_reduce(s, red, acc, vecs, cpg, part + (size_t)blockIdx.x * GN_G * 2);
+  if (MODE == 0) gn_block_reduce(sp, red, acc, vecs, cpg, part + (size_t)(gridDim.x + blockIdx.x) * GN_G * 2);
+}
+
+// MODE 0: stats[g] = (mean, rstd), from the plain sums or, where those lose their precision, from the pivoted ones
+// (x: the tensor, for the pivots).  MODE 1: gstats[g] = (mean dxh, mean dxh*xh).  One block of 256 threads.
+template <int MODE>
+__global__ void gn_final_kernel(const float* __restrict__ part, int nblk, double count, float eps, const act_t* x, int C,
                                 float* __restrict__ out) {
   pdl_prologue();
   const int t = threadIdx.x & 63, q = threadIdx.x >> 6;  // 256 threads: slot (group, which) x quarter of the partials
-  double s = 0.0;
+  double s = 0.0, sp = 0.0;
   for (int b = q; b < nblk; b += 4) s += (double)part[(size_t)b * GN_G * 2 + t];
-  __shared__ double acc4[4][GN_G * 2];
-  __shared__ double sh[GN_G * 2];
+  if (MODE == 0)
+    for (int b = q; b < nblk; b += 4) sp += (double)part[(size_t)(nblk + b) * GN_G * 2 + t];
+  __shared__ double acc4[4][GN_G * 2], acc4p[4][GN_G * 2];
+  __shared__ double sh[GN_G * 2], shp[GN_G * 2];
   acc4[q][t] = s;
+  acc4p[q][t] = sp;
   __syncthreads();
-  if (q == 0) sh[t] = (acc4[0][t] + acc4[1][t] + acc4[2][t] + acc4[3][t]) / count;
+  if (q == 0) {
+    sh[t] = (acc4[0][t] + acc4[1][t] + acc4[2][t] + acc4[3][t]) / count;
+    shp[t] = (acc4p[0][t] + acc4p[1][t] + acc4p[2][t] + acc4p[3][t]) / count;
+  }
   __syncthreads();
   if (q != 0) return;
   if (MODE == 0) {
     if ((t & 1) == 0) {
-      double mean = sh[t], ex2 = sh[t + 1];
-      double var = ex2 - mean * mean;
+      double mean = sh[t], var = sh[t + 1] - mean * mean;
       if (var < 0) var = 0;
+      if (gn_refine_variance(mean, var)) {
+        const double md = shp[t];
+        mean = gn_pivot(x, C, t >> 1) + md;
+        var = shp[t + 1] - md * md;
+        if (var < 0) var = 0;
+      }
       out[t] = (float)mean;
       out[t + 1] = (float)(1.0 / sqrt(var + (double)eps));
     }
@@ -519,19 +553,59 @@ __global__ void __launch_bounds__(GNC_THREADS, 1)
     gnc_fold(part, gridDim.x, (double)pixels * cpg, acc4, sh);
   }
   if (o.one_group) gnc_merge_groups(sh);  // GroupNorm(1, C): every group takes the statistics of the whole tensor
+  __shared__ int refine;
+  if (threadIdx.x == 0) refine = 0;
+  __syncthreads();
   if (threadIdx.x < GN_G) {
     const double mean = sh[2 * threadIdx.x], ex2 = sh[2 * threadIdx.x + 1];
     double var = ex2 - mean * mean;
     if (var < 0) var = 0;
-    const float m = (float)mean, r = (float)(1.0 / sqrt(var + (double)eps));
-    st[2 * threadIdx.x] = m;
-    st[2 * threadIdx.x + 1] = r;
-    if (blockIdx.x == 0) {
-      stats_out[2 * threadIdx.x] = m;
-      stats_out[2 * threadIdx.x + 1] = r;
-    }
+    if (gn_refine_variance(mean, var)) refine = 1;
+    st[2 * threadIdx.x] = (float)mean;
+    st[2 * threadIdx.x + 1] = (float)(1.0 / sqrt(var + (double)eps));
   }
   __syncthreads();
+  // Every block folded the same partials, so `refine` is the same in the whole grid.  The second pass sums x - mean (the
+  // first pass's fp32 mean) over the slab in shared memory; its partials replace the first ones in `part` once every block
+  // has read those (second barrier), and are read after the third.  Without it a block adds its two arrivals at once.
+  if (refine) {
+    float m2[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) m2[h] = st[2 * ((c0 + 4 * h) / cpg)];
+    float s2[2][2] = {{0.f, 0.f}, {0.f, 0.f}};
+    for (int p = p_begin + pl; p < p_end; p += plane) {
+      float xv[8];
+      load8(cx + (size_t)(p - p_begin) * C + c0, xv);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const float d = xv[i] - m2[i >> 2];
+        s2[i >> 2][0] += d;
+        s2[i >> 2][1] += d * d;
+      }
+    }
+    __shared__ float cpart2[GN_G * 2];
+    gnc_block_partials(s2, red, vecs, cpg, cpart2);
+    if (CLUSTER) {
+      gnc_cluster_fold(cpart2, gridDim.x, (double)pixels * cpg, acc4, sh);
+    } else {
+      gnc_grid_barrier(bar, bar_target + gridDim.x);
+      if (threadIdx.x < GN_G * 2) part[(size_t)blockIdx.x * GN_G * 2 + threadIdx.x] = cpart2[threadIdx.x];
+      gnc_grid_barrier(bar, bar_target + 2 * gridDim.x);
+      gnc_fold(part, gridDim.x, (double)pixels * cpg, acc4, sh);
+    }
+    if (o.one_group) gnc_merge_groups(sh);
+    if (threadIdx.x < GN_G) {
+      const double md = sh[2 * threadIdx.x];
+      double var = sh[2 * threadIdx.x + 1] - md * md;
+      if (var < 0) var = 0;
+      st[2 * threadIdx.x] = (float)((double)st[2 * threadIdx.x] + md);
+      st[2 * threadIdx.x + 1] = (float)(1.0 / sqrt(var + (double)eps));
+    }
+    __syncthreads();
+  } else if (!CLUSTER && threadIdx.x == 0) {
+    atomicAdd(bar, 2ULL);
+  }
+  if (blockIdx.x == 0 && threadIdx.x < GN_G * 2) stats_out[threadIdx.x] = st[threadIdx.x];
   float sc8[8], sh8[8];  // y = x * sc + sh
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
@@ -832,7 +906,7 @@ int gn_num_partials(int pixels, int C) {
 void gn_stats(const act_t* x, int pixels, int C, float eps, float* part, float* stats, cudaStream_t st) {
   const int nblk = gn_num_partials(pixels, C);
   launch_pdl(gn_partial_kernel<0>, dim3(nblk), dim3(256), 0, st, x, nullptr, nullptr, nullptr, nullptr, pixels, C, 0, part);
-  launch_pdl(gn_final_kernel<0>, dim3(1), dim3(256), 0, st, part, nblk, (double)pixels * (C / GN_G), eps, stats);
+  launch_pdl(gn_final_kernel<0>, dim3(1), dim3(256), 0, st, part, nblk, (double)pixels * (C / GN_G), eps, x, C, stats);
 }
 
 void gn_apply(const act_t* x, const float* stats, const float* gamma, const float* beta, int pixels, int C, int swish,
@@ -846,7 +920,8 @@ void gn_backward(const act_t* dy, const act_t* x, const float* stats, const floa
                  cudaStream_t st) {
   const int nblk = gn_num_partials(pixels, C);
   launch_pdl(gn_partial_kernel<1>, dim3(nblk), dim3(256), 0, st, x, dy, stats, gamma, beta, pixels, C, swish, part);
-  launch_pdl(gn_final_kernel<1>, dim3(1), dim3(256), 0, st, part, nblk, (double)pixels * (C / GN_G), 0.f, gstats);
+  launch_pdl(gn_final_kernel<1>, dim3(1), dim3(256), 0, st, part, nblk, (double)pixels * (C / GN_G), 0.f,
+             (const act_t*)nullptr, C, gstats);
   const long long nvec = (long long)pixels * C / 8;
   launch_pdl(gn_bwd_apply_kernel, dim3(grid_for(nvec, 256)), dim3(256), 0, st, dy, x, stats, gstats, gamma, beta, nvec, C, swish, dres,
                                                            dx);
@@ -919,7 +994,8 @@ void gn_forward_coop(const act_t* x, const float* gamma, const float* beta, int 
   const size_t smem = 4 * GNC_THREADS * 4 + (size_t)rpb * C * 2;
   launch_pdl(gn_coop_fwd_kernel<false>, dim3(grid), dim3(GNC_THREADS), smem, st, x, gamma, beta, pixels, C, swish, eps, rpb, part, stats, y,
                                                              gb->counter, gb->issued + grid, o);
-  if (cudaPeekAtLastError() == cudaSuccess) gb->issued += grid;  // a rejected launch must not move the target
+  // three barriers' worth of arrivals per block (the second pass's two are added at once when it is not needed)
+  if (cudaPeekAtLastError() == cudaSuccess) gb->issued += 3 * grid;  // a rejected launch must not move the target
 }
 
 void gn_backward_coop(const act_t* dy, const act_t* x, const float* stats, const float* gamma, const float* beta,

@@ -143,7 +143,7 @@ __global__ void __launch_bounds__(GG_MAX_THREADS)
                         float eps, float* __restrict__ stats_out, act_t* __restrict__ y) {
   pdl_launch_dependents();
   __shared__ double red[32];
-  __shared__ double cpart[2];
+  __shared__ double cpart[2], cpart2[2];
   const GgGeom q = gg_geometry(px, C);
   float ga[8], be[8], bi[8];
 #pragma unroll
@@ -190,9 +190,30 @@ __global__ void __launch_bounds__(GG_MAX_THREADS)
   double ta, tb;
   gg_cluster_sum((double)s0, (double)s1, red, cpart, ta, tb);
   const double n = (double)px * (C / GG_G);
-  const double mean = ta / n;
+  double mean = ta / n;
   double var = tb / n - mean * mean;
   if (var < 0) var = 0;
+  if (gn_refine_variance(mean, var)) {  // every CTA of the cluster holds the same sums: a cluster-uniform branch
+    const float m0 = (float)mean;
+    float d0 = 0.f, d1 = 0.f;
+#pragma unroll
+    for (int k = 0; k < UPT; ++k) {
+      if (q.u_begin + threadIdx.x + k * blockDim.x < q.u_end) {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const float d = xv[k][i] - m0;
+          d0 += d;
+          d1 += d * d;
+        }
+      }
+    }
+    double ua, ub;
+    gg_cluster_sum((double)d0, (double)d1, red, cpart2, ua, ub);
+    const double md = ua / n;
+    mean = (double)m0 + md;
+    var = ub / n - md * md;
+    if (var < 0) var = 0;
+  }
   const float m = (float)mean, rs = (float)(1.0 / sqrt(var + (double)eps));
   if (cg::this_cluster().block_rank() == 0 && threadIdx.x == 0) {
     stats_out[2 * q.g] = m;

@@ -71,17 +71,17 @@ __global__ void avgpool2x_kernel(const act_t* __restrict__ x, int H, int W, int 
     st8(y + (size_t)p * C + vc * 8, s);
   }
 }
-// adjoint: gx[2oy+dy, 2ox+dx] (+)= 0.25 gy[oy, ox]
+// adjoint: gx[2oy+dy, 2ox+dx] (+)= 0.25 gy[oy, ox]; an odd last row / column (floored away by the forward) gets 0
 __global__ void avgpool2x_bwd_kernel(const act_t* __restrict__ gy, int H, int W, int C, int accumulate,
                                      act_t* __restrict__ gx) {
-  const int vecs = C / 8, Wo = W / 2;
+  const int vecs = C / 8, Ho = H / 2, Wo = W / 2;
   const long long n = (long long)H * W * vecs;
   for (long long v = blockIdx.x * 256LL + threadIdx.x; v < n; v += (long long)gridDim.x * 256) {
     const int vc = (int)(v % vecs);
     const long long p = v / vecs;
     const int ix = (int)(p % W), iy = (int)(p / W);
-    float g[8], a[8];
-    ld8(gy + ((size_t)(iy >> 1) * Wo + (ix >> 1)) * C + vc * 8, g);
+    float g[8] = {0, 0, 0, 0, 0, 0, 0, 0}, a[8];
+    if ((iy >> 1) < Ho && (ix >> 1) < Wo) ld8(gy + ((size_t)(iy >> 1) * Wo + (ix >> 1)) * C + vc * 8, g);
     if (accumulate) ld8(gx + (size_t)p * C + vc * 8, a);
 #pragma unroll
     for (int i = 0; i < 8; ++i) g[i] = 0.25f * g[i] + (accumulate ? a[i] : 0.f);

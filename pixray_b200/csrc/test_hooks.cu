@@ -39,6 +39,7 @@ static void fill_epilogue(GemmEpilogue& e, const pxr_test_gemm_desc* d) {
   e.bs1 = d->c_bs1;
   e.tma_epi = d->tma_epi;
   e.act_col0 = d->act_col0;
+  e.k_splits = d->k_splits;
 }
 
 extern "C" int pxr_test_gemm(const pxr_test_gemm_desc* d, char* err, int errlen) {
@@ -90,6 +91,22 @@ extern "C" int pxr_test_conv(const pxr_test_gemm_desc* d, int batch, int H, int 
     return -100;
   }
   return 0;
+}
+
+static int sync_status() {
+  cudaError_t ce = cudaDeviceSynchronize();
+  if (ce == cudaSuccess) ce = cudaGetLastError();
+  return ce == cudaSuccess ? 0 : -100;
+}
+
+// splitk_reduce on caller DEVICE tensors: ws [splits][pixels][ld_ws] fp32 -> out [pixels][ld_out] fp16 (+ bias, + res)
+extern "C" int pxr_test_splitk_reduce(const float* ws, int splits, long long pixels, int N, int ld_ws, const float* bias,
+                                      const void* res, void* out, int ld_out) {
+  if (!ws || !out || splits < 1 || pixels < 1 || N < 8 || N % 8 || ld_ws < N || ld_ws % 8 || ld_out < N || ld_out % 8)
+    return -1;
+  splitk_reduce(ws, splits, pixels, N, ld_ws, bias, static_cast<const __half*>(res), static_cast<__half*>(out), ld_out,
+                nullptr);
+  return sync_status();
 }
 
 // Fused attention forward (+ backward when d_o != NULL) on caller tensors: qkv [B*T, 3W] fp16, o [B*T, W] fp16,
@@ -224,9 +241,11 @@ extern "C" int pxr_test_raster_samples(uint64_t seed, int iter, int H, int W, fl
 
 // GroupNorm(32, C, eps 1e-6)(+ swish) forward, and backward when dy (or ws_dy) is given, on caller DEVICE tensors
 // (NHWC fp16 [pixels, C]).  variant 0: the single-kernel grid-barrier GroupNorm; 1: one cluster per group
-// (kernels_gn_group.cu).  variant 1 only: ws != NULL makes the forward the epilogue of a split-K convolution
-// (x_out = fp16(sum_s ws[s] + bias + res), then normalised); ws_dy != NULL feeds the backward from split-K partials.
-// scratch: >= 64 * (num_sms + 2) floats + one zero-initialised u64 at its END (variant 0's grid barrier).
+// (kernels_gn_group.cu); 2: the three-kernel GroupNorm (gn_stats + gn_apply, gn_backward).  variant 1 only: ws != NULL
+// makes the forward the epilogue of a split-K convolution (x_out = fp16(sum_s ws[s] + bias + res), then normalised);
+// ws_dy != NULL feeds the backward from split-K partials.
+// scratch: variants 0 / 1: >= 64 * (num_sms + 2) floats + one zero-initialised u64 at its END (variant 0's grid barrier);
+// variant 2: 2 * 64 * gn_num_partials(pixels, C) partials, then the 64 floats of the backward's gstats (no barrier word).
 extern "C" int pxr_test_groupnorm(int variant, const void* x, const float* ws, int splits, const float* bias, const void* res,
                                   void* x_out, const float* gamma, const float* beta, int pixels, int C, int swish, void* y,
                                   float* stats, const void* dy, const float* ws_dy, int splits_dy, const void* dres, void* dx,
@@ -237,11 +256,21 @@ extern "C" int pxr_test_groupnorm(int variant, const void* x, const float* ws, i
   gb.counter = reinterpret_cast<unsigned long long*>(scratch + 64 * (nsm + 2));
   if (variant == 0) {
     if (ws || ws_dy || !gn_coop_supported(pixels, C, nsm)) return -1;
+  } else if (variant == 2) {
+    // gn_partial_kernel: 256 threads = whole pixel lanes x C/8 vectors; a group is 4 channels or whole vectors
+    if (ws || ws_dy || !x || pixels < 1 || C < 32 || C % 32 || 256 % (C / 8) || (C / 32 != 4 && (C / 32) % 8)) return -1;
   } else {
     if (!gn_group_possible(pixels, C)) return -2;
   }
   for (int it = 0; it < (repeat > 0 ? repeat : 1); ++it) {
-    if (variant == 0) {
+    if (variant == 2) {
+      float* gstats = scratch + 2 * 64 * gn_num_partials(pixels, C);
+      gn_stats(xin, pixels, C, 1e-6f, scratch, stats, nullptr);
+      gn_apply(xin, stats, gamma, beta, pixels, C, swish, static_cast<act_t*>(y), nullptr);
+      if (dy)
+        gn_backward(static_cast<const act_t*>(dy), xin, stats, gamma, beta, pixels, C, swish, static_cast<const act_t*>(dres),
+                    scratch, gstats, static_cast<act_t*>(dx), nullptr);
+    } else if (variant == 0) {
       gn_forward_coop(xin, gamma, beta, pixels, C, swish, 1e-6f, scratch, stats, static_cast<act_t*>(y), nsm, &gb, nullptr);
       if (dy)
         gn_backward_coop(static_cast<const act_t*>(dy), xin, stats, gamma, beta, pixels, C, swish,
@@ -264,7 +293,62 @@ extern "C" int pxr_test_groupnorm(int variant, const void* x, const float* ws, i
                           static_cast<const act_t*>(dres), static_cast<act_t*>(dx), nullptr);
     }
   }
-  cudaError_t ce = cudaDeviceSynchronize();
-  if (ce == cudaSuccess) ce = cudaGetLastError();
-  return ce == cudaSuccess ? 0 : -100;
+  return sync_status();
+}
+
+// The U-Net's GroupNorm(1, C) + modulation (+ activation, + residual) exactly as Engine::vd_norm / vd_norm_bwd call the
+// grid-barrier kernels; scratch as variant 0 above.
+extern "C" int pxr_test_groupnorm_unet(const void* x, const float* gamma, const float* beta, float gamma_add, int act,
+                                       const void* res, float eps, int pixels, int C, void* y, float* stats, const void* dy,
+                                       const void* dres, void* dx, float* scratch) {
+  const int nsm = num_sms();
+  if (!x || !y || !stats || !scratch || act < 0 || act > 2 || (dy && !dx) || !gn_coop_supported(pixels, C, nsm)) return -1;
+  GridBarrier gb;
+  gb.counter = reinterpret_cast<unsigned long long*>(scratch + 64 * (nsm + 2));
+  GnOpts o;
+  o.one_group = 1;
+  o.gamma_add = gamma_add;
+  o.res = static_cast<const act_t*>(res);
+  const act_t* xin = static_cast<const act_t*>(x);
+  gn_forward_coop(xin, gamma, beta, pixels, C, act, eps, scratch, stats, static_cast<act_t*>(y), nsm, &gb, nullptr, o);
+  if (dy) {
+    o.res = nullptr;  // the residual is a forward-only term: its gradient is dy itself, added by the caller
+    gn_backward_coop(static_cast<const act_t*>(dy), xin, stats, gamma, beta, pixels, C, act, static_cast<const act_t*>(dres),
+                     scratch, static_cast<act_t*>(dx), nsm, &gb, nullptr, o);
+  }
+  return sync_status();
+}
+
+// One resampling / copy launcher chosen by `op` (include/pixray_b200.h lists the ops and their layouts).
+extern "C" int pxr_test_resample(int op, const void* in, int ld_in, void* out, int ld_out, int H, int W, int C, int accumulate) {
+  if (!in || !out || C < 8 || C % 8 || H < 1 || W < 1) return -1;
+  if (ld_in == 0) ld_in = C;
+  if (ld_out == 0) ld_out = C;
+  if (ld_in < C || ld_in % 8 || ld_out < C || ld_out % 8) return -1;
+  // which side of each op takes a pixel stride, and whether it accumulates
+  static const struct { bool ld_in, ld_out, acc; } caps[8] = {
+      {true, false, false}, {false, false, false}, {true, false, false}, {false, false, true},
+      {false, true, false}, {true, false, false},  {false, false, false}, {true, true, true}};
+  if (op < 0 || op > 7) return -2;
+  if ((!caps[op].ld_in && ld_in != C) || (!caps[op].ld_out && ld_out != C) || (!caps[op].acc && accumulate)) return -3;
+  const act_t* x = static_cast<const act_t*>(in);
+  act_t* y = static_cast<act_t*>(out);
+  switch (op) {
+    case 0: upsample2x(x, H, W, C, y, nullptr, ld_in); break;
+    case 1: downsum2x(x, H, W, C, y, nullptr); break;
+    case 2: avgpool2x(x, H, W, C, ld_in, y, nullptr); break;
+    case 3: avgpool2x_backward(x, H, W, C, accumulate, y, nullptr); break;
+    case 4: bilinear_up2x(x, H, W, C, y, ld_out, nullptr); break;
+    case 5: bilinear_up2x_backward(x, H, W, C, ld_in, y, nullptr); break;
+    case 6: im2col3x3(x, H, W, C, y, nullptr); break;
+    default: copy_channels(x, ld_in, y, ld_out, C, (long long)H * W, accumulate, nullptr); break;
+  }
+  return sync_status();
+}
+
+extern "C" int pxr_test_gemv(const void* w, int K, int R, const float* x, const float* bias, int relu, const float* res,
+                             float* y) {
+  if (!w || !x || !y || K < 8 || K % 8 || R < 1) return -1;
+  gemv_f16(static_cast<const act_t*>(w), K, R, x, bias, relu, res, y, nullptr);
+  return sync_status();
 }

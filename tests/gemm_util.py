@@ -13,9 +13,10 @@ def _ptr(t):
 def run_gemm(A, B, M, N, K, *, a_mode=0, b_mode=0, lda=None, ldb=None, a_mn=None, a_k=None, b_mn=None, b_k=None,
              nb0=1, nb1=1, a_bs=(0, 0), b_bs=(0, 0), b_batched=0, block_n=128, fmt=0, alpha=1.0, bias=None,
              bias_per_row=0, act=0, aux_in=None, aux_out=None, res_f32=None, res_f16=None, out_f32=None, out_f16=None,
-             ldc=None, c_bs=(0, 0), repeat=1, cta_group=0, tma_epi=0):
+             ldc=None, c_bs=(0, 0), repeat=1, cta_group=0, tma_epi=0, k_splits=0):
     lib = _lib.load()
     d = _lib.TestGemmDesc()
+    d.k_splits = k_splits
     d.cta_group = cta_group
     d.tma_epi = tma_epi
     d.a, d.a_mode = _ptr(A), a_mode
@@ -47,10 +48,11 @@ def run_gemm(A, B, M, N, K, *, a_mode=0, b_mode=0, lda=None, ldb=None, a_mn=None
 
 
 def run_conv(x_nhwc, wt, n_out, cout_pad, ksize, *, block_n=128, fmt=0, bias=None, out_f32=None, out_f16=None,
-             res_f16=None, res_f32=None, ldc=None, alpha=1.0, repeat=1, cta_group=0, tma_epi=0):
+             res_f16=None, res_f32=None, ldc=None, alpha=1.0, repeat=1, cta_group=0, tma_epi=0, k_splits=0):
     lib = _lib.load()
     Bn, H, W, Cin = x_nhwc.shape
     d = _lib.TestGemmDesc()
+    d.k_splits = k_splits
     d.a, d.lda = _ptr(x_nhwc), x_nhwc.stride(2)
     d.b = _ptr(wt)
     d.N, d.block_n, d.fmt = n_out, block_n, fmt

@@ -35,6 +35,18 @@ def test_struct_sizes_match_header_layout():
     assert C.sizeof(_lib.CutParams) == 8 + 4 + 4 + 8 + 8 + 8  # + color_jitter
 
 
+def test_test_gemm_desc_fields_follow_the_header():
+    """ctypes lays TestGemmDesc out by its field list: it must name the header's fields in the header's order."""
+    src = re.sub(r"/\*.*?\*/", "", open(HEADER).read(), flags=re.S)
+    body = re.search(r"typedef struct \{([^}]*)\} pxr_test_gemm_desc;", src).group(1)
+    names = []
+    for decl in filter(None, (d.strip() for d in body.split(";"))):
+        first, *rest = decl.split(",")
+        names += [re.sub(r"^.*[\s*]", "", first.strip())] + [r.strip() for r in rest]
+    assert [f[0] for f in _lib.TestGemmDesc._fields_] == names
+    assert names[-1] == "k_splits"
+
+
 def test_version_string():
     lib = _lib.load()
     assert b"sm_90a" in lib.pxr_version()
