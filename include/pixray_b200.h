@@ -111,6 +111,16 @@ int pxr_load_weight(pxr_handle h, int module_id, const char* name, const float* 
 /* After all weights: builds every kernel plan / workspace.  Fails listing the first missing weight. */
 int pxr_finalize(pxr_handle h);
 
+/* Image tower of perceptor clip_idx, before pxr_finalize (default PXR_TOWER_OPENAI_CLIP):
+ *   OPENAI_CLIP  openai-CLIP VisionTransformer (clip.load, slip.py:173-186): CLIP mean / std, conv1 without bias,
+ *                class_embedding + positional_embedding, ln_pre, QuickGELU, LayerNorm eps 1e-5, ln_post, proj
+ *   TIMM_VIT     timm VisionTransformer of SLIP_Base (slip.py:84-157, SLIP/models.py:130-134): ImageNet mean / std,
+ *                patch_embed.proj with bias, cls_token + pos_embed without a LayerNorm before the blocks, exact GELU,
+ *                LayerNorm eps 1e-6, final norm, image_projection; keys visual.* and image_projection after the
+ *                checkpoint's `module.` prefix is stripped */
+enum { PXR_TOWER_OPENAI_CLIP = 0, PXR_TOWER_TIMM_VIT = 1 };
+int pxr_set_clip_tower(pxr_handle h, int clip_idx, int kind);
+
 /* Prompt(embed, weight, stop) list of one perceptor (pixray.py:859-915).  embeds host [n, D]. */
 int pxr_set_prompts(pxr_handle h, int clip_idx, const float* embeds, int n, int D, const float* weights,
                     const float* stops);
@@ -297,7 +307,9 @@ typedef struct {
   float alpha;
   const float* bias;
   int bias_per_row, act; /* act: 0 none, 1 QuickGELU (+ pre-activation to aux_out), 2 QuickGELU backward, 4 LeakyReLU(0.2),
-                          * 5 LeakyReLU backward (see act_col0); others are refused */
+                          * 5 LeakyReLU backward (see act_col0), 6 exact GELU 0.5 u (1 + erf(u / sqrt 2)) of the fp16
+                          * pre-activation u (+ u to aux_out), 7 GELU backward: times Phi(u) + u phi(u) of the saved fp16 u
+                          * (aux_in); others are refused */
   const void* aux_in;
   void* aux_out;
   const float* res_f32;

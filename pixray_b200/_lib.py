@@ -66,7 +66,7 @@ class TestGemmDesc(C.Structure):
 
 # every symbol include/pixray_b200.h declares (tests check the library exports all of them)
 EXPORTS = [
-    "pxr_last_error", "pxr_version", "pxr_create", "pxr_destroy", "pxr_load_weight", "pxr_finalize",
+    "pxr_last_error", "pxr_version", "pxr_create", "pxr_destroy", "pxr_load_weight", "pxr_finalize", "pxr_set_clip_tower",
     "pxr_set_prompts", "pxr_set_comm", "pxr_get_unique_id", "pxr_synth", "pxr_vqgan_encode", "pxr_make_cutouts", "pxr_encode_image",
     "pxr_prompt_loss", "pxr_backward", "pxr_step", "pxr_iterate", "pxr_reset_optimizer", "pxr_sync",
     "pxr_num_kernel_launches", "pxr_get_stream", "pxr_z_numel", "pxr_z_bounds", "pxr_test_gemm", "pxr_test_conv", "pxr_debug_read", "pxr_profile_iteration", "pxr_profile_iteration2",

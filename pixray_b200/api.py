@@ -5,12 +5,18 @@ front-ends use (run.py, cogrun.py) plus the notebook one-liner.
 Scope (SURVEY.md 8): the per-iteration hot path.  Every option of the reference's parser is KNOWN here (same dest,
 same default: the "requested setting not found" check of pixray.py:2088-2093 behaves identically), but options that
 switch on something outside the hot path (spot prompts, overlays, animation, init images through the VQGAN encoder,
-filters, transparency, non-Adam optimisers, SLIP perceptors, video) raise NotImplementedError when they are set to a
-non-default value instead of being silently ignored.  What the reference fetches from the network at init time comes in
-through three extra settings instead:
+filters, transparency, non-Adam optimisers, the `perceptors` preset, video) raise NotImplementedError when they are set
+to a non-default value instead of being silently ignored.
 
-    b200_weights        {"vqgan": state_dict | path, "ViT-B/16": state_dict | path, ...} with the reference's own keys
-                        (taming `state_dict`, openai-CLIP `visual.*`); None = seeded synthetic weights (benchmarks)
+Perceptors are named in `clip_models`, as get_clip_perceptor keys on them (slip.py:173-186): the openai-CLIP ViTs
+(engine.CLIP_ARCH) and the SLIP_Base ViTs (engine.SLIP_ARCH: SLIP_VITB16, SLIP_CC3M, SLIP_CC12M, CLIP_VITB16,
+SLIP_VITL16, CLIP_VITL16), alone or two of them mixed.  The reference's `perceptors` option only picks a default
+`clip_models` from its quality table (pixray.py:1832-1845); naming the models in `clip_models` runs the same towers.
+What the reference fetches from the network at init time comes in through three extra settings instead:
+
+    b200_weights        {"vqgan": state_dict | path, "ViT-B/16": state_dict | path, "SLIP_VITB16": ...} with the
+                        reference's own keys (taming `state_dict`, openai-CLIP `visual.*`, the SLIP checkpoint's
+                        {'state_dict', 'args'} with its `module.` prefix); None = seeded synthetic weights (benchmarks)
     b200_text_encoder   callable(clip_model_name, text) -> [1, D] tensor (e.g. the reference's perceptor.encode_text);
                         the text towers are init-time and stay in PyTorch
     b200_allow_synthetic  accept seeded pseudo-embeddings for text prompts when no encoder is given (default False)
@@ -278,10 +284,12 @@ def _load_state_dict(spec):
             obj = torch.jit.load(str(spec), map_location="cpu").state_dict()  # openai-CLIP ships TorchScript archives
         except Exception:
             obj = torch.load(str(spec), map_location="cpu", weights_only=False)
-        if isinstance(obj, dict) and "state_dict" in obj:  # taming checkpoints (vqgan.py:128-133)
+        if isinstance(obj, dict) and "state_dict" in obj:  # taming checkpoints (vqgan.py:128-133), SLIP {state_dict, args}
             obj = obj["state_dict"]
     else:
         obj = spec
+    if isinstance(obj, dict) and any(isinstance(k, str) and k.startswith("module.") for k in obj):
+        obj = {k.replace("module.", ""): v for k, v in obj.items()}  # SLIP's DDP checkpoints (slip.py:126-128)
     if isinstance(obj, dict) and ("params_ema" in obj or "params" in obj):  # Real-ESRGAN (real_esrganer.py:42-48)
         obj = obj["params_ema"] if "params_ema" in obj else obj["params"]
     return obj
@@ -324,8 +332,11 @@ def do_init(args):
     """pixray.py:569-1020 for the hot path: engine + drawer + perceptors + cutouts + prompts + losses + optimiser."""
     st = _state
     for m in args.clip_models:
-        if m not in E.CLIP_ARCH:
-            raise NotImplementedError(f"perceptor '{m}': only the ViT image towers {sorted(E.CLIP_ARCH)} are built")
+        if m in E.SLIP_UNSUPPORTED:
+            raise NotImplementedError(f"perceptor '{m}': {E.SLIP_UNSUPPORTED[m]}")
+        if m not in E.CLIP_ARCH and m not in E.SLIP_ARCH:
+            raise NotImplementedError(f"perceptor '{m}': only the ViT image towers {sorted(E.CLIP_ARCH)} (openai-CLIP) "
+                                      f"and {sorted(E.SLIP_ARCH)} (SLIP) are built")
     if len(args.clip_models) > 2:
         raise NotImplementedError("at most two perceptors per session")
     st.seed = _seed_everything(args)
@@ -349,7 +360,7 @@ def do_init(args):
     # != 1 stretches the pooled image before the warps and changes the wide augmentation stack (pixray.py:420-432, 468-472)
     aspect = float(args.size[0]) / float(args.size[1])
     device = int(str(args.cuda_device).split(":")[1]) if ":" in str(args.cuda_device) else 0
-    clip_cfgs = [E.CLIP_ARCH[m] for m in args.clip_models]
+    clip_cfgs = [E.CLIP_ARCH[m] if m in E.CLIP_ARCH else E.SLIP_ARCH[m] for m in args.clip_models]
     kw = dict(drawer=kind, image_hw=engine_hw, cutn=args.num_cuts, clip=clip_cfgs, seed=st.seed, device=device)
     if aspect != 1.0:
         kw["cut_aspect"] = aspect
@@ -382,7 +393,12 @@ def do_init(args):
             vq_sd = S.rrdbnet_state_dict(0)
         eng.load_module(E.MOD_VQGAN, vq_sd)
     for i, m in enumerate(args.clip_models):
-        sd = _load_state_dict(weights[m]) if m in weights else S.clip_state_dict(E.CLIP_ARCH[m], 1 + i)
+        if m in weights:
+            sd = _load_state_dict(weights[m])
+        elif m in E.SLIP_ARCH:
+            sd = S.slip_state_dict(E.SLIP_ARCH[m], 1 + i)
+        else:
+            sd = S.clip_state_dict(E.CLIP_ARCH[m], 1 + i)
         eng.load_module(E.MOD_CLIP0 + i, sd)
     eng.finalize()
     if world > 1:

@@ -140,10 +140,12 @@ class Engine {
   // ---- perceptors
   struct Clip {
     pxr_clip_cfg c;
+    int tower = PXR_TOWER_OPENAI_CLIP;  // pxr_set_clip_tower
+    ChannelNorm norm = kClipNorm;       // the tower's preprocess mean / std
     int T, np, Kp, ldT, M, B;
     // weights
     act_t* conv1 = nullptr;
-    float *cls = nullptr, *pos = nullptr, *proj = nullptr;
+    float *cls = nullptr, *pos = nullptr, *proj = nullptr, *conv1_b = nullptr;
     NormW ln_pre, ln_post;
     struct Layer {
       act_t *wqkv, *wo, *wfc, *wproj;
@@ -1622,27 +1624,37 @@ void Engine::build_clip(int i) {
   C.M = M;
   C.B = B;
   cudaStream_t cs = st;
+  // The two towers differ only at the edges of the same pre-norm ViT (pxr_set_clip_tower): the timm one has a patch-embed
+  // bias, no ln_pre (tokens + pos_embed enter the blocks directly), exact GELU, LayerNorm eps 1e-6, and its own key names.
+  const bool timm = C.tower == PXR_TOWER_TIMM_VIT;
+  const float eps = timm ? 1e-6f : 1e-5f;
+  C.norm = timm ? kImageNetNorm : kClipNorm;
+  const std::string k_patch = timm ? "visual.patch_embed.proj.weight" : "visual.conv1.weight";
+  const std::string k_proj = timm ? "image_projection" : "visual.proj";
+  const HostWeight& w_cls = timm ? W(mod, "visual.cls_token", {1, 1, Wd}) : W(mod, "visual.class_embedding", {Wd});
+  const HostWeight& w_pos = timm ? W(mod, "visual.pos_embed", {1, T, Wd}) : W(mod, "visual.positional_embedding", {T, Wd});
   // ---- weights
   {
-    const HostWeight& w = W(mod, "visual.conv1.weight", {Wd, 3, P, P});
+    const HostWeight& w = W(mod, k_patch, {Wd, 3, P, P});
     std::vector<float> f((size_t)Wd * Kp, 0.f);
     for (int o = 0; o < Wd; ++o)
       for (int k = 0; k < 3 * P * P; ++k) f[(size_t)o * Kp + k] = w.data[(size_t)o * 3 * P * P + k];
     C.conv1 = upload_f16(f);
   }
-  C.cls = upload(W(mod, "visual.class_embedding", {Wd}).data);
-  C.pos = upload(W(mod, "visual.positional_embedding", {T, Wd}).data);
-  C.proj = upload(W(mod, "visual.proj", {Wd, D}).data);
-  C.proj16 = upload_f16(W(mod, "visual.proj", {Wd, D}).data);
-  C.ln_pre = load_norm(mod, "visual.ln_pre", Wd);
-  C.ln_post = load_norm(mod, "visual.ln_post", Wd);
+  if (timm) C.conv1_b = upload(W(mod, "visual.patch_embed.proj.bias", {Wd}).data);
+  C.cls = upload(w_cls.data);
+  C.pos = upload(w_pos.data);
+  C.proj = upload(W(mod, k_proj, {Wd, D}).data);
+  C.proj16 = upload_f16(W(mod, k_proj, {Wd, D}).data);
+  if (!timm) C.ln_pre = load_norm(mod, "visual.ln_pre", Wd);
+  C.ln_post = load_norm(mod, timm ? "visual.norm" : "visual.ln_post", Wd);
   // ---- buffers
   C.patches = dalloc<act_t>((size_t)B * np * Kp);
   C.g_patches = dalloc<act_t>((size_t)B * np * Kp);
   C.t = dalloc<float>((size_t)M * Wd);
-  {  // class-token rows are constant: t[b*T + 0] = class_embedding
+  {  // class-token rows are constant: t[b*T + 0] = class_embedding (cls_token)
     std::vector<float> t0((size_t)M * Wd, 0.f);
-    const auto& cls = W(mod, "visual.class_embedding").data;
+    const auto& cls = w_cls.data;
     for (int b = 0; b < B; ++b)
       for (int k = 0; k < Wd; ++k) t0[(size_t)b * T * Wd + k] = cls[k];
     PXR_CUDA(cudaMemcpyAsync(C.t, t0.data(), t0.size() * sizeof(float), cudaMemcpyHostToDevice, st));
@@ -1674,10 +1686,10 @@ void Engine::build_clip(int i) {
   void* x_cur = xalloc();
   void* x0 = x_cur;
   // LayerNorm on either stream type
-  auto ln_fwd = [s16, cs](const void* x, long long stride, const float* pos, int T_, const NormW& nw, int rows, int W_,
-                          act_t* y16, float* y32, float* stats) {
-    if (s16) layernorm_forward(static_cast<const act_t*>(x), stride, pos, T_, nw.gamma, nw.beta, rows, W_, 1e-5f, y16, y32, stats, cs);
-    else layernorm_forward(static_cast<const float*>(x), stride, pos, T_, nw.gamma, nw.beta, rows, W_, 1e-5f, y16, y32, stats, cs);
+  auto ln_fwd = [s16, cs, eps](const void* x, long long stride, const float* pos, int T_, const NormW& nw, int rows,
+                               int W_, act_t* y16, float* y32, float* stats) {
+    if (s16) layernorm_forward(static_cast<const act_t*>(x), stride, pos, T_, nw.gamma, nw.beta, rows, W_, eps, y16, y32, stats, cs);
+    else layernorm_forward(static_cast<const float*>(x), stride, pos, T_, nw.gamma, nw.beta, rows, W_, eps, y16, y32, stats, cs);
   };
   auto ln_bwd = [s16, cs](const act_t* dy, const void* x, long long stride, const float* stats, const NormW& nw, int rows,
                           int W_, int accumulate, float* gx, act_t* gx16) {
@@ -1701,32 +1713,39 @@ void Engine::build_clip(int i) {
   // ---- forward: patch embed (conv1 as GEMM over im2col'd patches, written straight into the token rows 1..np)
   {
     GemmEpilogue e;
+    e.bias = C.conv1_b;
     e.out_f32 = C.t + Wd;
     e.ldc = Wd;
     e.bs0 = (long long)T * Wd;
     add_gemm(C.fwd, opK(C.patches, Kp, np, Kp, B, (long long)np * Kp), opK(C.conv1, Kp, Wd, Kp), np, Wd, Kp, e);
   }
-  {
+  {  // x0 = ln_pre(t + pos) (openai-CLIP), or t + pos_embed (timm)
     Clip* c = &C;
     void* xo = x0;
-    C.fwd.add(1, [=] {
-      layernorm_forward(c->t, Wd, c->pos, T, c->ln_pre.gamma, c->ln_pre.beta, M, Wd, 1e-5f, s16 ? static_cast<act_t*>(xo) : nullptr,
-                        s16 ? nullptr : static_cast<float*>(xo), c->stats_pre, cs);
-    }, 0.0, "layernorm_forward");
+    act_t* xo16 = s16 ? static_cast<act_t*>(xo) : nullptr;
+    float* xo32 = s16 ? nullptr : static_cast<float*>(xo);
+    if (timm)
+      C.fwd.add(1, [=] { add_pos_embed(c->t, c->pos, T, M, Wd, xo16, xo32, cs); }, 0.0, "add_pos_embed");
+    else
+      C.fwd.add(1, [=] {
+        layernorm_forward(c->t, Wd, c->pos, T, c->ln_pre.gamma, c->ln_pre.beta, M, Wd, eps, xo16, xo32, c->stats_pre, cs);
+      }, 0.0, "layernorm_forward");
   }
   for (int l = 0; l < L; ++l) {
     Clip::Layer& Ly = C.layers[l];
-    std::string p = "visual.transformer.resblocks." + std::to_string(l);
-    Ly.wqkv = upload_f16(W(mod, p + ".attn.in_proj_weight", {3 * Wd, Wd}).data);
-    Ly.bqkv = upload(W(mod, p + ".attn.in_proj_bias", {3 * Wd}).data);
-    Ly.wo = upload_f16(W(mod, p + ".attn.out_proj.weight", {Wd, Wd}).data);
-    Ly.bo = upload(W(mod, p + ".attn.out_proj.bias", {Wd}).data);
-    Ly.wfc = upload_f16(W(mod, p + ".mlp.c_fc.weight", {4 * Wd, Wd}).data);
-    Ly.bfc = upload(W(mod, p + ".mlp.c_fc.bias", {4 * Wd}).data);
-    Ly.wproj = upload_f16(W(mod, p + ".mlp.c_proj.weight", {Wd, 4 * Wd}).data);
-    Ly.bproj = upload(W(mod, p + ".mlp.c_proj.bias", {Wd}).data);
-    Ly.ln1 = load_norm(mod, p + ".ln_1", Wd);
-    Ly.ln2 = load_norm(mod, p + ".ln_2", Wd);
+    // the same tensors under each tower's names: in_proj = attn.qkv (q | k | v, heads contiguous), out_proj = attn.proj,
+    // c_fc / c_proj = mlp.fc1 / mlp.fc2, ln_1 / ln_2 = norm1 / norm2
+    std::string p = (timm ? "visual.blocks." : "visual.transformer.resblocks.") + std::to_string(l);
+    Ly.wqkv = upload_f16(W(mod, p + (timm ? ".attn.qkv.weight" : ".attn.in_proj_weight"), {3 * Wd, Wd}).data);
+    Ly.bqkv = upload(W(mod, p + (timm ? ".attn.qkv.bias" : ".attn.in_proj_bias"), {3 * Wd}).data);
+    Ly.wo = upload_f16(W(mod, p + (timm ? ".attn.proj.weight" : ".attn.out_proj.weight"), {Wd, Wd}).data);
+    Ly.bo = upload(W(mod, p + (timm ? ".attn.proj.bias" : ".attn.out_proj.bias"), {Wd}).data);
+    Ly.wfc = upload_f16(W(mod, p + (timm ? ".mlp.fc1.weight" : ".mlp.c_fc.weight"), {4 * Wd, Wd}).data);
+    Ly.bfc = upload(W(mod, p + (timm ? ".mlp.fc1.bias" : ".mlp.c_fc.bias"), {4 * Wd}).data);
+    Ly.wproj = upload_f16(W(mod, p + (timm ? ".mlp.fc2.weight" : ".mlp.c_proj.weight"), {Wd, 4 * Wd}).data);
+    Ly.bproj = upload(W(mod, p + (timm ? ".mlp.fc2.bias" : ".mlp.c_proj.bias"), {Wd}).data);
+    Ly.ln1 = load_norm(mod, p + (timm ? ".norm1" : ".ln_1"), Wd);
+    Ly.ln2 = load_norm(mod, p + (timm ? ".norm2" : ".ln_2"), Wd);
     Ly.x_in = x_cur;
     Ly.x_mid = xalloc();
     void* x_next = xalloc();
@@ -1762,10 +1781,10 @@ void Engine::build_clip(int i) {
       add_gemm(C.fwd, opK(fuse_attn ? ly.o : C.o16, xld, Mr, Wd), opK(ly.wo, Wd, Wd, Wd), Mr, Wd, Wd, e);
     }
     C.fwd.add(1, [=] { ln_fwd(ly.x_mid, xld, nullptr, T, ly.ln2, Mr, Wd, c->h16, nullptr, ly.stats2); }, 0.0, "layernorm_forward");
-    {  // gact = quickgelu(h Wfc^T + bfc), keep pre-activation u   (h16 / gact / u hold the Mr rows compactly)
+    {  // gact = quickgelu / gelu(h Wfc^T + bfc), keep pre-activation u   (h16 / gact / u hold the Mr rows compactly)
       GemmEpilogue e;
       e.bias = ly.bfc;
-      e.act = ACT_QUICKGELU;
+      e.act = timm ? ACT_GELU : ACT_QUICKGELU;
       e.aux_out = ly.u;
       e.out_f16 = C.gact;
       e.ldc = 4 * Wd;
@@ -1810,9 +1829,9 @@ void Engine::build_clip(int i) {
     const bool cls_only = clip_last_cls && l == L - 1;  // see the forward: the row-wise tail of the last layer, class rows only
     const int Mr = cls_only ? B : M;
     const long long xld = cls_only ? (long long)T * Wd : (long long)Wd;
-    {  // g4 = (gx Wproj) * quickgelu'(u)
+    {  // g4 = (gx Wproj) * quickgelu'(u) / gelu'(u)
       GemmEpilogue e;
-      e.act = ACT_QUICKGELU_BWD;
+      e.act = timm ? ACT_GELU_BWD : ACT_QUICKGELU_BWD;
       e.aux_in = ly.u;
       e.out_f16 = C.g4;
       e.ldc = 4 * Wd;
@@ -1844,9 +1863,11 @@ void Engine::build_clip(int i) {
     }
     C.bwd.add(1, [=] { ln_bwd(c->gh, ly.x_in, Wd, ly.stats1, ly.ln1, M, Wd, 1, c->gx, c->gx16); }, 0.0, "layernorm_backward");
   }
-  {  // ln_pre backward (x = t + pos), then patch-embed dgrad on token rows 1..np of every image
+  {  // ln_pre backward (x = t + pos), then patch-embed dgrad on token rows 1..np of every image.  timm: x0 = t + pos_embed,
+     // so the stream gradient in gx16 already is d/dt
     Clip* c = &C;
-    C.bwd.add(1, [=] { layernorm_backward(c->gx16, c->t, Wd, c->pos, T, c->stats_pre, c->ln_pre.gamma, M, Wd, 0, c->gx, c->gx16, cs); }, 0.0, "layernorm_backward");
+    if (!timm)
+      C.bwd.add(1, [=] { layernorm_backward(c->gx16, c->t, Wd, c->pos, T, c->stats_pre, c->ln_pre.gamma, M, Wd, 0, c->gx, c->gx16, cs); }, 0.0, "layernorm_backward");
     GemmEpilogue e;
     e.out_f16 = C.g_patches;
     e.ldc = Kp;
@@ -1857,7 +1878,7 @@ void Engine::build_clip(int i) {
 
 void Engine::forward_clip(int i) {
   Clip& C = clip[i];
-  patchify_forward(batch, range, n_local, cfg.cut_size, C.c.patch, C.Kp, C.patches, st);
+  patchify_forward(batch, range, n_local, cfg.cut_size, C.c.patch, C.Kp, C.patches, C.norm, st);
   launches += 1;
   run(C.fwd);
   check_launch("clip forward");
@@ -1954,7 +1975,7 @@ void Engine::encode_image_prompts() {
     for (int i = 0; i < cfg.n_clip; ++i) {
       Clip& C = clip[i];
       const int D = C.c.out_dim;
-      patchify_forward(batch, range, n_local, cfg.cut_size, C.c.patch, C.Kp, C.patches, st);
+      patchify_forward(batch, range, n_local, cfg.cut_size, C.c.patch, C.Kp, C.patches, C.norm, st);
       run(C.fwd);
       float* rows = C.prompts + (size_t)(C.n_text + k * cfg.cutn) * D;
       if (comm) PXR_CUDA(cudaMemsetAsync(rows, 0, sizeof(float) * cfg.cutn * D, st));
@@ -2053,7 +2074,8 @@ void Engine::backward_to_image(const CutoutArgs& a, int mask_which, bool accumul
     Clip& C = clip[i];
     if (mask_which >= 0 && C.spot[mask_which].n == 0) continue;
     run(C.bwd);
-    patchify_backward(C.g_patches, batch, range, n_local, cfg.cut_size, C.c.patch, C.Kp, !first, g_batch, sums_fx, fx_sums, st);
+    patchify_backward(C.g_patches, batch, range, n_local, cfg.cut_size, C.c.patch, C.Kp, !first, g_batch, sums_fx, fx_sums,
+                      C.norm, st);
     first = false;
     launches += 1;
   }
@@ -2506,6 +2528,17 @@ int pxr_load_weight(pxr_handle h, int module_id, const char* name, const float* 
 }
 
 int pxr_finalize(pxr_handle h) { PXR_TRY(h, h->e->finalize()); }
+
+int pxr_set_clip_tower(pxr_handle h, int clip_idx, int kind) {
+  PXR_TRY(h, {
+    Engine* e = h->e;
+    if (e->finalized) throw EngineError(-12, "pxr_set_clip_tower: the tower cannot change after pxr_finalize");
+    if (clip_idx < 0 || clip_idx >= e->cfg.n_clip) throw EngineError(-14, "bad clip index");
+    if (kind != PXR_TOWER_OPENAI_CLIP && kind != PXR_TOWER_TIMM_VIT)
+      throw EngineError(-10, "unknown tower kind (0 openai-CLIP, 1 timm ViT)");
+    e->clip[clip_idx].tower = kind;
+  });
+}
 
 int pxr_set_prompts(pxr_handle h, int clip_idx, const float* embeds, int n, int D, const float* weights,
                     const float* stops) {

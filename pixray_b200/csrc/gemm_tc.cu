@@ -61,6 +61,14 @@ __device__ __forceinline__ float quickgelu_grad(float u) {
   float s = fast_sigmoid(1.702f * u);
   return s * (1.f + 1.702f * u * (1.f - s));
 }
+// exact GELU (nn.GELU(): u Phi(u) = 0.5 u (1 + erf(u / sqrt 2))) and its derivative Phi(u) + u phi(u), in fp32 -- no
+// tanh form.  Phi(u) = 0.5 erfc(-u / sqrt 2): 1 + erff cancels for u < -4 (erf -> -1), where gelu(u) is an fp16 subnormal
+// and the fp32 cancellation error exceeds its ulp; erfcf keeps the relative accuracy there.
+__device__ __forceinline__ float gelu_phi(float u) { return 0.5f * erfcf(u * -0.70710678118654752f); }
+__device__ __forceinline__ float gelu_erf(float u) { return u * gelu_phi(u); }
+__device__ __forceinline__ float gelu_erf_grad(float u) {
+  return gelu_phi(u) + u * 0.39894228040143268f * expf(-0.5f * u * u);
+}
 
 constexpr int TB_LD = 33;                       // transposer row pitch (floats): conflict-free both ways
 constexpr int TB_FLOATS = 32 * TB_LD;           // one 32 x 32 block per epilogue warp
@@ -192,7 +200,9 @@ struct BlockMap {
 
 // Which input tensor (if any) is prefetched for the block: residual fp32, residual fp16 or the saved pre-activation.
 __device__ __forceinline__ int prefetch_kind(const GemmParams& p) {
-  return p.res_f32 ? 1 : (p.res_f16 ? 2 : ((p.act == ACT_QUICKGELU_BWD || p.act == ACT_LRELU_BWD) ? 3 : 0));
+  return p.res_f32 ? 1
+                   : (p.res_f16 ? 2
+                                : ((p.act == ACT_QUICKGELU_BWD || p.act == ACT_GELU_BWD || p.act == ACT_LRELU_BWD) ? 3 : 0));
 }
 
 // Issue the global loads of the block's input tensor BEFORE the accumulator block is read, so their DRAM latency
@@ -244,7 +254,8 @@ __device__ __forceinline__ void unpack_pf(const uint4& u, int kind, float (&x)[E
 
 // Generic epilogue of one staged 32 x 32 block.  E elements per lane: 8 when every tensor is fp16 (16-byte accesses,
 // 8 rows per warp instruction), 4 when an fp32 tensor takes part (16-byte accesses on the fp32 side, 4 rows).
-template <int E>
+// ERF: the kernels that take the exact-GELU codes; the others compile without them (erfcf costs registers and stack).
+template <int E, bool ERF>
 __device__ __forceinline__ void epilogue_block(const GemmParams& p, const float* tb, int ld, const long long* s_off,
                                                const int* s_row, int lane, int col_base, int col_limit, int kind,
                                                const uint4 (&pf)[BlockMap<E>::NIT]) {
@@ -293,6 +304,16 @@ __device__ __forceinline__ void epilogue_block(const GemmParams& p, const float*
       else ld_f16<E>(p.aux_in + o, vec, nv, u);
 #pragma unroll
       for (int j = 0; j < E; ++j) x[j] *= quickgelu_grad(u[j]);
+    } else if (ERF && p.act == ACT_GELU) {
+      if (p.aux_out) st_f16<E>(p.aux_out + o, vec, nv, x);
+#pragma unroll
+      for (int j = 0; j < E; ++j) x[j] = gelu_erf(__half2float(__float2half_rn(x[j])));  // of the saved fp16 u
+    } else if (ERF && p.act == ACT_GELU_BWD) {
+      float u[E];
+      if (vec && kind == 3) unpack_pf<E>(pf[it], 3, u);
+      else ld_f16<E>(p.aux_in + o, vec, nv, u);
+#pragma unroll
+      for (int j = 0; j < E; ++j) x[j] *= gelu_erf_grad(u[j]);
     }
     if (p.res_f32) {
       float t[E];
@@ -544,7 +565,10 @@ __device__ __forceinline__ void tma_epilogue_tile(const GemmParams& p, const Til
                                                   uint64_t* in_bar, const float* arow, int warp, int lane,
                                                   uint32_t& cnt) {
   constexpr bool F32 = (MODE == TE_RES32);
-  constexpr bool IN = (MODE == TE_GELU_BWD || MODE == TE_RES32 || MODE == TE_RES16);
+  constexpr bool ERF = (MODE == TE_ERF_GELU || MODE == TE_ERF_GELU_BWD);  // exact GELU, else QuickGELU
+  constexpr bool ACT_FWD = (MODE == TE_GELU || MODE == TE_ERF_GELU);
+  constexpr bool ACT_BWD = (MODE == TE_GELU_BWD || MODE == TE_ERF_GELU_BWD);
+  constexpr bool IN = (ACT_BWD || MODE == TE_RES32 || MODE == TE_RES16);
   constexpr int BW = F32 ? 16 : 32;  // columns per 64-byte box row
   const int q = warp & 3;            // row quarter of the tile
   const int half = warp >> 2;        // the two warps of a quarter alternate over the column blocks
@@ -576,7 +600,7 @@ __device__ __forceinline__ void tma_epilogue_tile(const GemmParams& p, const Til
       const int s = half + 2 * j;
       const int col = t.n0 + s * BW;
       const uint32_t k = cnt + j;
-      uint8_t* buf = wbuf + ((MODE == TE_GELU) ? (k & 1) * 2 : (k & 3)) * TE_BUF_BYTES;
+      uint8_t* buf = wbuf + (ACT_FWD ? (k & 1) * 2 : (k & 3)) * TE_BUF_BYTES;
       if (lane == 0) {
         if (IN) {
           if (j + 2 < my) {
@@ -585,7 +609,7 @@ __device__ __forceinline__ void tma_epilogue_tile(const GemmParams& p, const Til
             mbar_arrive_expect_tx(&in_bar[b], TE_BUF_BYTES);
             tma_load_4d(&p.tma_d, &in_bar[b], wbuf + b * TE_BUF_BYTES, t.n0 + (s + 4) * BW, c1, c2, c3);
           }
-        } else if (MODE == TE_GELU) {
+        } else if (ACT_FWD) {
           bulk_wait_group_read<1>();
         } else {
           bulk_wait_group_read<3>();
@@ -615,27 +639,43 @@ __device__ __forceinline__ void tma_epilogue_tile(const GemmParams& p, const Til
       if (MODE == TE_F16) {
 #pragma unroll
         for (int c = 0; c < 4; ++c) *reinterpret_cast<uint4*>(buf + te_off(lane, c)) = pack8(x + 8 * c);
-      } else if (MODE == TE_GELU) {
+      } else if (ACT_FWD) {
 #pragma unroll
         for (int c = 0; c < 4; ++c) {
           uint4 u = pack8(x + 8 * c);  // the saved pre-activation (fp16), and the activation of exactly that value
           *reinterpret_cast<uint4*>(buf + te_off(lane, c)) = u;
-          __half2* h = reinterpret_cast<__half2*>(&u);
+          if (ERF) {
+            float v[8];
+            unpack8(u, v);
 #pragma unroll
-          for (int j = 0; j < 4; ++j) h[j] = quickgelu_h2(h[j]);
+            for (int i = 0; i < 8; ++i) v[i] = gelu_erf(v[i]);
+            u = pack8(v);
+          } else {
+            __half2* h = reinterpret_cast<__half2*>(&u);
+#pragma unroll
+            for (int j = 0; j < 4; ++j) h[j] = quickgelu_h2(h[j]);
+          }
           *reinterpret_cast<uint4*>(buf + TE_BUF_BYTES + te_off(lane, c)) = u;
         }
-      } else if (MODE == TE_GELU_BWD) {
+      } else if (ACT_BWD) {
 #pragma unroll
         for (int c = 0; c < 4; ++c) {
           uint4* ptr = reinterpret_cast<uint4*>(buf + te_off(lane, c));
           uint4 u = *ptr;
-          uint4 g = pack8(x + 8 * c);
-          const __half2* uh = reinterpret_cast<const __half2*>(&u);
-          __half2* gh = reinterpret_cast<__half2*>(&g);
+          if (ERF) {  // fp32 product, as the generic epilogue forms it
+            float v[8];
+            unpack8(u, v);
 #pragma unroll
-          for (int j = 0; j < 4; ++j) gh[j] = __hmul2(gh[j], quickgelu_grad_h2(uh[j]));
-          *ptr = g;
+            for (int i = 0; i < 8; ++i) x[8 * c + i] *= gelu_erf_grad(v[i]);
+            *ptr = pack8(x + 8 * c);
+          } else {
+            uint4 g = pack8(x + 8 * c);
+            const __half2* uh = reinterpret_cast<const __half2*>(&u);
+            __half2* gh = reinterpret_cast<__half2*>(&g);
+#pragma unroll
+            for (int j = 0; j < 4; ++j) gh[j] = __hmul2(gh[j], quickgelu_grad_h2(uh[j]));
+            *ptr = g;
+          }
         }
       } else if (MODE == TE_RES16) {
 #pragma unroll
@@ -661,7 +701,7 @@ __device__ __forceinline__ void tma_epilogue_tile(const GemmParams& p, const Til
       fence_proxy_async_smem();
       __syncwarp();
       if (lane == 0) {
-        if (MODE == TE_GELU) {
+        if (ACT_FWD) {
           tma_store_4d(&p.tma_d, buf, col, c1, c2, c3);
           tma_store_4d(&p.tma_c, buf + TE_BUF_BYTES, col, c1, c2, c3);
         } else {
@@ -685,7 +725,7 @@ __host__ __device__ __forceinline__ int acc_ld(int block_n) { return (block_n + 
 // ahead through the stage ring, so the next tile's operands stream in while the epilogue of this one runs.
 // TE: the tensor-map epilogue's mode, or TE_NONE for the generic epilogue.  HAS_IN: the generic epilogue reads an input
 // tensor (residual / saved pre-activation) that is prefetched; kept out of the input-free kernel so that one stays lean.
-template <bool HAS_IN, int TE, int NF>
+template <bool HAS_IN, int TE, int NF, bool ERF = false>
 __device__ __forceinline__ void gemm_body(const GemmParams& p) {
   pdl_launch_dependents();
   extern __shared__ uint8_t smem_raw[];
@@ -763,11 +803,11 @@ __device__ __forceinline__ void gemm_body(const GemmParams& p) {
         if (wide) {
           uint4 pf[BlockMap<4>::NIT];
           if (HAS_IN) prefetch_block<4>(p, s_off, lane, t.n0 + s * 32, col_limit, kind, pf);
-          epilogue_block<4>(p, blk + s * 32, ald, s_off, s_row, lane, t.n0 + s * 32, col_limit, kind, pf);
+          epilogue_block<4, ERF>(p, blk + s * 32, ald, s_off, s_row, lane, t.n0 + s * 32, col_limit, kind, pf);
         } else {
           uint4 pf[BlockMap<8>::NIT];
           if (HAS_IN) prefetch_block<8>(p, s_off, lane, t.n0 + s * 32, col_limit, kind, pf);
-          epilogue_block<8>(p, blk + s * 32, ald, s_off, s_row, lane, t.n0 + s * 32, col_limit, kind, pf);
+          epilogue_block<8, ERF>(p, blk + s * 32, ald, s_off, s_row, lane, t.n0 + s * 32, col_limit, kind, pf);
         }
       }
     }
@@ -776,13 +816,13 @@ __device__ __forceinline__ void gemm_body(const GemmParams& p) {
   if (TE != TE_NONE && lane == 0) bulk_wait_group<0>();
 }
 
-template <int NF>
+template <int NF, bool ERF = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_constant__ GemmParams p) {
-  gemm_body<false, TE_NONE, NF>(p);
+  gemm_body<false, TE_NONE, NF, ERF>(p);
 }
-template <int NF>
+template <int NF, bool ERF = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_in_kernel(const __grid_constant__ GemmParams p) {
-  gemm_body<true, TE_NONE, NF>(p);
+  gemm_body<true, TE_NONE, NF, ERF>(p);
 }
 template <int MODE, int NF>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tce_kernel(const __grid_constant__ GemmParams p) {
@@ -798,10 +838,14 @@ void (*plain_kernel(const GemmParams& p))(GemmParams) {
     case TE_GELU_BWD: return gemm_tce_kernel<TE_GELU_BWD, NF>;
     case TE_RES32: return gemm_tce_kernel<TE_RES32, NF>;
     case TE_RES16: return gemm_tce_kernel<TE_RES16, NF>;
+    case TE_ERF_GELU: return gemm_tce_kernel<TE_ERF_GELU, NF>;
+    case TE_ERF_GELU_BWD: return gemm_tce_kernel<TE_ERF_GELU_BWD, NF>;
     default: break;
   }
-  if (p.res_f32 || p.res_f16 || p.act == ACT_QUICKGELU_BWD || p.act == ACT_LRELU_BWD) return gemm_tc_in_kernel<NF>;
-  return gemm_tc_kernel<NF>;
+  const bool erf = p.act == ACT_GELU || p.act == ACT_GELU_BWD;
+  if (p.res_f32 || p.res_f16 || p.act == ACT_QUICKGELU_BWD || p.act == ACT_GELU_BWD || p.act == ACT_LRELU_BWD)
+    return erf ? gemm_tc_in_kernel<NF, true> : gemm_tc_in_kernel<NF>;
+  return erf ? gemm_tc_kernel<NF, true> : gemm_tc_kernel<NF>;
 }
 void (*kernel_for(const GemmParams& p))(GemmParams) {
   if (p.fmt == 0 && p.block_n == 128) return plain_kernel<2>(p);
@@ -926,8 +970,10 @@ int decide_tma_epi(const GemmParams& p, const GemmEpilogue& e, int block_n) {
   int mode = TE_NONE;
   const bool no_res = !e.res_f32 && !e.res_f16;
   if (e.act == ACT_NONE && e.out_f16 && !e.out_f32 && !e.res_f32 && !e.aux_out) mode = e.res_f16 ? TE_RES16 : TE_F16;
-  else if (e.act == ACT_QUICKGELU && e.aux_out && e.out_f16 && !e.out_f32 && no_res) mode = TE_GELU;
-  else if (e.act == ACT_QUICKGELU_BWD && e.aux_in && e.out_f16 && !e.out_f32 && no_res) mode = TE_GELU_BWD;
+  else if ((e.act == ACT_QUICKGELU || e.act == ACT_GELU) && e.aux_out && e.out_f16 && !e.out_f32 && no_res)
+    mode = e.act == ACT_GELU ? TE_ERF_GELU : TE_GELU;
+  else if ((e.act == ACT_QUICKGELU_BWD || e.act == ACT_GELU_BWD) && e.aux_in && e.out_f16 && !e.out_f32 && no_res)
+    mode = e.act == ACT_GELU_BWD ? TE_ERF_GELU_BWD : TE_GELU_BWD;
   else if (e.act == ACT_NONE && e.out_f32 && !e.out_f16 && e.res_f32 && !e.res_f16 && !e.aux_out) mode = TE_RES32;
   if (mode == TE_NONE) return TE_NONE;
   const int bw = mode == TE_RES32 ? 16 : 32;
@@ -996,13 +1042,17 @@ int finish_plan(GemmPlan* plan, const GemmEpilogue& epi, int block_n, int num_sm
     return -10;
   }
   if (epi.act != ACT_NONE && epi.act != ACT_QUICKGELU && epi.act != ACT_QUICKGELU_BWD && epi.act != ACT_LRELU &&
-      epi.act != ACT_LRELU_BWD) {
-    set_err(err, errlen, "unknown epilogue activation (act must be 0 none, 1 QuickGELU, 2 QuickGELU backward, 4 LeakyReLU "
-                         "or 5 LeakyReLU backward)");
+      epi.act != ACT_LRELU_BWD && epi.act != ACT_GELU && epi.act != ACT_GELU_BWD) {
+    set_err(err, errlen, "unknown epilogue activation (act must be 0 none, 1 QuickGELU, 2 QuickGELU backward, 4 LeakyReLU, "
+                         "5 LeakyReLU backward, 6 GELU or 7 GELU backward)");
     return -12;
   }
   if (epi.act == ACT_LRELU_BWD && !epi.aux_in) {
     set_err(err, errlen, "the LeakyReLU backward needs the saved post-activation (aux_in)");
+    return -14;
+  }
+  if (epi.act == ACT_GELU_BWD && !epi.aux_in) {
+    set_err(err, errlen, "the GELU backward needs the saved pre-activation (aux_in)");
     return -14;
   }
   if (p.b_mode == OP_MNMAJOR && block_n % 64) {
@@ -1015,11 +1065,11 @@ int finish_plan(GemmPlan* plan, const GemmEpilogue& epi, int block_n, int num_sm
     const bool f32 = p.tma_epi == TE_RES32;
     int rc = encode_epilogue_map(&p.tma_c, f32 ? static_cast<const void*>(epi.out_f32) : epi.out_f16, f32, p, epi, err,
                                  errlen);
-    const void* second = p.tma_epi == TE_GELU       ? static_cast<const void*>(epi.aux_out)
-                         : p.tma_epi == TE_GELU_BWD ? static_cast<const void*>(epi.aux_in)
-                         : p.tma_epi == TE_RES32    ? static_cast<const void*>(epi.res_f32)
-                         : p.tma_epi == TE_RES16    ? static_cast<const void*>(epi.res_f16)
-                                                    : nullptr;
+    const void* second = (p.tma_epi == TE_GELU || p.tma_epi == TE_ERF_GELU)  ? static_cast<const void*>(epi.aux_out)
+                         : (p.tma_epi == TE_GELU_BWD || p.tma_epi == TE_ERF_GELU_BWD) ? static_cast<const void*>(epi.aux_in)
+                         : p.tma_epi == TE_RES32                                 ? static_cast<const void*>(epi.res_f32)
+                         : p.tma_epi == TE_RES16                                 ? static_cast<const void*>(epi.res_f16)
+                                                                                 : nullptr;
     if (!rc && second) rc = encode_epilogue_map(&p.tma_d, second, f32, p, epi, err, errlen);
     if (rc) p.tma_epi = TE_NONE;  // a stride the tensor map cannot express: generic epilogue
   }
@@ -1055,13 +1105,13 @@ int finish_plan(GemmPlan* plan, const GemmEpilogue& epi, int block_n, int num_sm
   static std::once_flag once;
   std::call_once(once, [] {
     for (int nf = 0; nf < 3; ++nf)
-      for (int te = TE_NONE; te <= TE_RES16; ++te)
-        for (int in = 0; in < 2; ++in) {
+      for (int te = TE_NONE; te <= TE_ERF_GELU_BWD; ++te)
+        for (int act : {ACT_NONE, ACT_QUICKGELU_BWD, ACT_GELU, ACT_GELU_BWD}) {  // every generic kernel
           GemmParams q{};
           q.fmt = 0;
           q.block_n = nf == 2 ? 128 : (nf == 1 ? 64 : 16);
           q.tma_epi = te;
-          q.act = in ? ACT_QUICKGELU_BWD : ACT_NONE;
+          q.act = act;
           cudaFuncSetAttribute(kernel_for(q), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
         }
   });

@@ -26,7 +26,12 @@ enum OperandMode : int { OP_KMAJOR = 0, OP_MNMAJOR = 1, OP_CONV = 2 };
 // ACT_LRELU: LeakyReLU(0.2) after the bias.  ACT_LRELU_BWD: the sum (accumulator + bias + residual) times 1 where the saved
 // post-activation aux_in is > 0, else 0.2, in the columns >= act_col0 (the others pass unmasked): the dense blocks of the
 // super-resolution net mask one channel slice of a wider gradient (engine_superres.inc).
-enum EpiAct : int { ACT_NONE = 0, ACT_QUICKGELU = 1, ACT_QUICKGELU_BWD = 2, ACT_LRELU = 4, ACT_LRELU_BWD = 5 };
+// ACT_GELU / ACT_GELU_BWD: exact (erf) GELU of timm's ViT MLP (nn.GELU()), the counterparts of the QuickGELU pair:
+// forward stores the pre-activation u to aux_out as fp16 and returns gelu of exactly that fp16 value; backward multiplies
+// the sum by Phi(u) + u phi(u) of the saved fp16 u.  Both are evaluated in fp32 (erfcf / expf).
+enum EpiAct : int {
+  ACT_NONE = 0, ACT_QUICKGELU = 1, ACT_QUICKGELU_BWD = 2, ACT_LRELU = 4, ACT_LRELU_BWD = 5, ACT_GELU = 6, ACT_GELU_BWD = 7
+};
 
 constexpr int GEMM_BLOCK_M = 128;
 constexpr int GEMM_BLOCK_K = 64;
@@ -74,7 +79,11 @@ struct GemmParams {
   CUtensorMap tma_d;   // second tensor: aux_out (TE_GELU), aux_in (TE_GELU_BWD), res_f32 (TE_RES32), res_f16 (TE_RES16)
 };
 
-enum TmaEpi : int { TE_NONE = 0, TE_F16 = 1, TE_GELU = 2, TE_GELU_BWD = 3, TE_RES32 = 4, TE_RES16 = 5 };
+// TE_GELU / TE_GELU_BWD: the activation pair with the saved pre-activation; QuickGELU (ACT_QUICKGELU*) as TE_GELU /
+// TE_GELU_BWD, exact GELU (ACT_GELU*) as TE_ERF_GELU / TE_ERF_GELU_BWD -- one code path, specialised on the activation.
+enum TmaEpi : int {
+  TE_NONE = 0, TE_F16 = 1, TE_GELU = 2, TE_GELU_BWD = 3, TE_RES32 = 4, TE_RES16 = 5, TE_ERF_GELU = 6, TE_ERF_GELU_BWD = 7
+};
 
 // Host-side description of one operand.
 struct GemmOperand {

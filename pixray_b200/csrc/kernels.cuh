@@ -206,13 +206,20 @@ void minmax_partials(const float* x, long long n, int nparts, float* part_min, f
 // range[0]=min, range[1]=R (max of x-min, 1 if zero), range[2]=max, range[3]=R!=0; irange = argmin / argmax element
 void minmax_reduce(const float* batch_or_null, const float* part_min, const float* part_max, const int* part_imin,
                    const int* part_imax, int nparts, float* range, int* irange, cudaStream_t st);
+// The perceptor's input normalisation (transforms.Normalize of its preprocess)
+struct ChannelNorm {
+  float mean[3], std[3];
+};
+constexpr ChannelNorm kClipNorm = {{0.48145466f, 0.4578275f, 0.40821073f}, {0.26862954f, 0.26130258f, 0.27577711f}};  // slip.py:55
+constexpr ChannelNorm kImageNetNorm = {{0.485f, 0.456f, 0.406f}, {0.229f, 0.224f, 0.225f}};  // SLIP_Base, slip.py:117-121
 // patches[(n*gp + py)*gp + px, (c*P + iy)*P + ix] = ((x - min)/R - mean_c)/std_c   (slip.py:52-60 + conv1 im2col)
 void patchify_forward(const float* batch, const float* range, int n, int cs, int P, int ld, act_t* patches,
-                      cudaStream_t st);
+                      const ChannelNorm& nrm, cudaStream_t st);
 // g_batch (=|+=) d/d(batch) of the direct term; sums_fx[0] += sum g_a, sums_fx[1] += sum g_a * a / R in 64-bit fixed point
 // (order-independent: identical bits on every run); range_sums_finish converts to fp32 and clears the accumulator
 void patchify_backward(const act_t* g_patches, const float* batch, const float* range, int n, int cs, int P, int ld,
-                       int accumulate, float* g_batch, long long* sums_fx, FxPass fx, cudaStream_t st);
+                       int accumulate, float* g_batch, long long* sums_fx, FxPass fx, const ChannelNorm& nrm,
+                       cudaStream_t st);
 void range_sums_finish(long long* sums_fx, FxPass fx, float* sums, cudaStream_t st);
 // adds the argmin / argmax terms of the global range normalise, then scatters through the bilinear taps
 // g_pooled: [3, src_h, src_w] (overwritten); acc: zeroed fixed-point accumulator of the same extent (cleared again on return)
@@ -249,6 +256,9 @@ int layernorm_forward_variant(int variant, const void* x, long long x_stride, co
 int layernorm_backward_variant(int variant, const act_t* dy, const void* x, long long x_stride, const float* pos, int T,
                                const float* stats, const float* gamma, int rows, int W, int accumulate, float* gx,
                                act_t* gx16, cudaStream_t st);
+// timm ViT tokens (no LayerNorm before the blocks): y[r] = t[r] + pos[r % T] into the residual stream, y16 (fp16) when
+// non-null, else y32; t [rows, W], pos [T, W] fp32, W % 4 == 0
+void add_pos_embed(const float* t, const float* pos, int T, int rows, int W, act_t* y16, float* y32, cudaStream_t st);
 // in-place row softmax over the first `cols` of each row of length ld (pad columns zeroed); rows total; any ld % 8 == 0
 void softmax_forward(act_t* s, int rows, int cols, int ld, cudaStream_t st);
 void softmax_backward(const act_t* p, act_t* dp_to_ds, int rows, int cols, int ld, cudaStream_t st);

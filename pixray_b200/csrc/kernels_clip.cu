@@ -655,8 +655,30 @@ __global__ void cast_kernel(const float* x, act_t* y, long long n, float scale) 
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
     y[i] = __float2half_rn(x[i] * scale);
 }
+// timm ViT token embedding: y[r, :] = t[r, :] + pos[r % T, :], four columns per thread
+template <typename YT>
+__global__ void add_pos_kernel(const float* __restrict__ t, const float* __restrict__ pos, int T, long long n4, int W4,
+                               YT* __restrict__ y) {
+  pdl_prologue();
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
+    const long long r = i / W4;
+    const float4 a = reinterpret_cast<const float4*>(t)[i];
+    const float4 b = reinterpret_cast<const float4*>(pos)[(r % T) * W4 + i % W4];
+    const float4 s = make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);
+    if constexpr (sizeof(YT) == 4) reinterpret_cast<float4*>(y)[i] = s;
+    else st_half4(reinterpret_cast<act_t*>(y) + 4 * i, s.x, s.y, s.z, s.w);
+  }
+}
 
 }  // namespace
+
+void add_pos_embed(const float* t, const float* pos, int T, int rows, int W, act_t* y16, float* y32, cudaStream_t st) {
+  const long long n4 = (long long)rows * W / 4;
+  const long long blocks = (n4 + 255) / 256;
+  const int grid = (int)(blocks < 148 * 8 ? blocks : 148 * 8);
+  if (y16) launch_pdl(add_pos_kernel<act_t>, dim3(grid), dim3(256), 0, st, t, pos, T, n4, W / 4, y16);
+  else launch_pdl(add_pos_kernel<float>, dim3(grid), dim3(256), 0, st, t, pos, T, n4, W / 4, y32);
+}
 
 // PXR_LN16_WIDE=0 keeps the 8-byte-vector LayerNorm kernels on the fp16 stream (A/B switch)
 static bool ln16_wide_ok() {

@@ -15,8 +15,6 @@
 namespace pxr {
 namespace {
 
-__constant__ float c_clip_mean[3] = {0.48145466f, 0.4578275f, 0.40821073f};
-__constant__ float c_clip_std[3] = {0.26862954f, 0.26130258f, 0.27577711f};
 
 // ATen adaptive pooling window [floor(i*in/out), ceil((i+1)*in/out)): pool_start / pool_end of pool_bounds.cuh
 
@@ -502,10 +500,13 @@ __global__ void range_unpack_kernel(const float* __restrict__ xbuf, float* __res
   range[3] = (R != 0.f) ? 1.f : 0.f;
 }
 
+// channel c's entry of a per-channel kernel argument, by selects: a dynamic index would copy the argument to local memory
+__device__ __forceinline__ float by_channel(const float (&v)[3], int c) { return c == 0 ? v[0] : (c == 1 ? v[1] : v[2]); }
+
 // thread: 8 consecutive k of one patch row (ix..ix+7), requires P % 8 == 0
 __global__ void __launch_bounds__(256) patchify_fwd_kernel(const float* __restrict__ batch,
                                                            const float* __restrict__ range, int n, int cs, int P,
-                                                           int ld, act_t* __restrict__ patches) {
+                                                           int ld, act_t* __restrict__ patches, ChannelNorm nrm) {
   pdl_prologue();
   const int gp = cs / P;
   const int vec_per_row = 3 * P * P / 8;
@@ -523,7 +524,7 @@ __global__ void __launch_bounds__(256) patchify_fwd_kernel(const float* __restri
     float v[8] = {a.x, a.y, a.z, a.w, b4.x, b4.y, b4.z, b4.w};
     uint4 u;
     __half2* h = reinterpret_cast<__half2*>(&u);
-    const float mean = c_clip_mean[c], stdv = c_clip_std[c];
+    const float mean = by_channel(nrm.mean, c), stdv = by_channel(nrm.std, c);
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       float y0 = (((v[2 * i] - mn) / R) - mean) / stdv;
@@ -539,7 +540,7 @@ __global__ void __launch_bounds__(256) patchify_bwd_kernel(const act_t* __restri
                                                            const float* __restrict__ range, int n, int cs, int P,
                                                            int ld, int accumulate, float* __restrict__ g_batch,
                                                            long long* __restrict__ sums, unsigned int* poison,
-                                                           unsigned int pass) {
+                                                           unsigned int pass, ChannelNorm nrm) {
   pdl_prologue();
   const int gp = cs / P;
   const int vec_per_row = 3 * P * P / 8;
@@ -559,7 +560,7 @@ __global__ void __launch_bounds__(256) patchify_bwd_kernel(const act_t* __restri
     float4 xa = reinterpret_cast<const float4*>(batch + o)[0], xb = reinterpret_cast<const float4*>(batch + o)[1];
     float xv[8] = {xa.x, xa.y, xa.z, xa.w, xb.x, xb.y, xb.z, xb.w};
     float g[8];
-    const float k = 1.f / (c_clip_std[c] * R);
+    const float k = 1.f / (by_channel(nrm.std, c) * R);
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       float2 f = __half22float2(h[i]);
@@ -606,7 +607,8 @@ __global__ void __launch_bounds__(256) patchify_bwd_kernel(const act_t* __restri
 // Any patch size (e.g. ViT-L/14: P = 14): one thread per patch element, coalesced over k.
 __global__ void __launch_bounds__(256) patchify_fwd_generic_kernel(const float* __restrict__ batch,
                                                                    const float* __restrict__ range, int n, int cs,
-                                                                   int P, int ld, act_t* __restrict__ patches) {
+                                                                   int P, int ld, act_t* __restrict__ patches,
+                                                                   ChannelNorm nrm) {
   pdl_prologue();
   const int gp = cs / P, K = 3 * P * P;
   const long long total = (long long)n * gp * gp * K;
@@ -618,7 +620,7 @@ __global__ void __launch_bounds__(256) patchify_fwd_generic_kernel(const float* 
     const int px = (int)(row % gp), py = (int)((row / gp) % gp), b = (int)(row / (gp * gp));
     const int ix = k % P, iy = (k / P) % P, c = k / (P * P);
     const float v = batch[(((size_t)b * 3 + c) * cs + py * P + iy) * cs + px * P + ix];
-    patches[(size_t)row * ld + k] = __float2half_rn((((v - mn) / R) - c_clip_mean[c]) / c_clip_std[c]);
+    patches[(size_t)row * ld + k] = __float2half_rn((((v - mn) / R) - by_channel(nrm.mean, c)) / by_channel(nrm.std, c));
   }
 }
 
@@ -629,7 +631,7 @@ __global__ void __launch_bounds__(256) patchify_bwd_generic_kernel(const act_t* 
                                                                    int P, int ld, int accumulate,
                                                                    float* __restrict__ g_batch,
                                                                    long long* __restrict__ sums, unsigned int* poison,
-                                                           unsigned int pass) {
+                                                           unsigned int pass, ChannelNorm nrm) {
   pdl_prologue();
   const int gp = cs / P;
   const long long total = (long long)n * 3 * cs * cs;
@@ -643,7 +645,7 @@ __global__ void __launch_bounds__(256) patchify_bwd_generic_kernel(const act_t* 
     if (y < gp * P && x < gp * P) {
       const long long row = ((long long)b * gp + y / P) * gp + x / P;
       const int k = (c * P + y % P) * P + x % P;
-      g = __half2float(g_patches[(size_t)row * ld + k]) / (c_clip_std[c] * R);
+      g = __half2float(g_patches[(size_t)row * ld + k]) / (by_channel(nrm.std, c) * R);
     }
     s1 += g;
     s2 += g * (batch[t] - mn) / R;
@@ -800,26 +802,26 @@ static int patch_grid(long long total) {
 }
 
 void patchify_forward(const float* batch, const float* range, int n, int cs, int P, int ld, act_t* patches,
-                      cudaStream_t st) {
+                      const ChannelNorm& nrm, cudaStream_t st) {
   if (P % 8) {
     const long long tot = (long long)n * (cs / P) * (cs / P) * 3 * P * P;
-    launch_pdl(patchify_fwd_generic_kernel, dim3(patch_grid(tot)), dim3(256), 0, st, batch, range, n, cs, P, ld, patches);
+    launch_pdl(patchify_fwd_generic_kernel, dim3(patch_grid(tot)), dim3(256), 0, st, batch, range, n, cs, P, ld, patches, nrm);
     return;
   }
   const long long total = (long long)n * (cs / P) * (cs / P) * (3 * P * P / 8);
-  launch_pdl(patchify_fwd_kernel, dim3(patch_grid(total)), dim3(256), 0, st, batch, range, n, cs, P, ld, patches);
+  launch_pdl(patchify_fwd_kernel, dim3(patch_grid(total)), dim3(256), 0, st, batch, range, n, cs, P, ld, patches, nrm);
 }
 void patchify_backward(const act_t* g_patches, const float* batch, const float* range, int n, int cs, int P, int ld,
-                       int accumulate, float* g_batch, long long* sums, FxPass fx, cudaStream_t st) {
+                       int accumulate, float* g_batch, long long* sums, FxPass fx, const ChannelNorm& nrm, cudaStream_t st) {
   if (P % 8) {
     const long long tot = (long long)n * 3 * cs * cs;
     launch_pdl(patchify_bwd_generic_kernel, dim3(patch_grid(tot)), dim3(256), 0, st, g_patches, batch, range, n, cs, P, ld, accumulate,
-                                                                 g_batch, sums, fx.poison, fx.pass);
+                                                                 g_batch, sums, fx.poison, fx.pass, nrm);
     return;
   }
   const long long total = (long long)n * (cs / P) * (cs / P) * (3 * P * P / 8);
   launch_pdl(patchify_bwd_kernel, dim3(patch_grid(total)), dim3(256), 0, st, g_patches, batch, range, n, cs, P, ld, accumulate, g_batch,
-                                                         sums, fx.poison, fx.pass);
+                                                         sums, fx.poison, fx.pass, nrm);
 }
 void cutout_backward(const CutoutArgs& a, const float* g_batch, const float* range, const int* irange,
                      const float* sums, long long* acc, FxPass fx, float* g_pooled, cudaStream_t st) {

@@ -26,6 +26,23 @@ CLIP_ARCH = {
     "ViT-B/16": dict(width=768, layers=12, heads=12, patch=16, image_res=224, out_dim=512),
     "ViT-L/14": dict(width=1024, layers=24, heads=16, patch=14, image_res=224, out_dim=768),
 }
+# Image towers (pxr_set_clip_tower): openai-CLIP's VisionTransformer, or the timm VisionTransformer of SLIP_Base
+TOWER_OPENAI_CLIP, TOWER_TIMM_VIT = 0, 1
+# SLIP_Base models (slip.py:84-157, SLIP/models.py:288-331) whose image tower the engine builds: timm ViTs with 64-wide
+# heads.  SLIP_CC3M / SLIP_CC12M are the B/16 architecture on other data (slip.py:134-135).  `tower` is not a ClipCfg
+# field: B200Engine hands it to pxr_set_clip_tower.
+_VIT_B16 = dict(width=768, layers=12, heads=12, patch=16, image_res=224, out_dim=512, tower=TOWER_TIMM_VIT)
+_VIT_L16 = dict(width=1024, layers=24, heads=16, patch=16, image_res=224, out_dim=512, tower=TOWER_TIMM_VIT)
+SLIP_ARCH = {"SLIP_VITB16": _VIT_B16, "SLIP_CC3M": _VIT_B16, "SLIP_CC12M": _VIT_B16, "CLIP_VITB16": _VIT_B16,
+             "SLIP_VITL16": _VIT_L16, "CLIP_VITL16": _VIT_L16}
+# SLIP models the engine refuses, with the reason
+SLIP_UNSUPPORTED = {
+    "SLIP_VITS16": "its vit_small_mocov3 tower has 12 heads over width 384 (32-wide heads); the fused attention and the "
+                   "ViT builder cover 64-wide heads only",
+    "CLIP_VITS16": "its vit_small_mocov3 tower has 12 heads over width 384 (32-wide heads); the fused attention and the "
+                   "ViT builder cover 64-wide heads only",
+    "SIMCLR_VITS16": "SIMCLR has no image_projection and no text tower, so it cannot score text prompts",
+}
 
 
 class EngineError(RuntimeError):
@@ -81,7 +98,8 @@ class B200Engine:
         cfg.n_clip = len(clip)
         for i, c in enumerate(clip):
             for k, val in c.items():
-                setattr(cfg.clip[i], k, val)
+                if k != "tower":
+                    setattr(cfg.clip[i], k, val)
         cfg.noise_fac, cfg.seed = noise_fac, seed
         cfg.op_dtype, cfg.grad_scale = 0, grad_scale
         cfg.beta1, cfg.beta2, cfg.adam_eps = lr_betas[0], lr_betas[1], adam_eps
@@ -107,6 +125,9 @@ class B200Engine:
             raise EngineError(f"pxr_create failed ({rc}): {self.lib.pxr_last_error(None).decode()}")
         self.h = h
         self._keep = []
+        for i, c in enumerate(clip):
+            if c.get("tower", TOWER_OPENAI_CLIP) != TOWER_OPENAI_CLIP:
+                self._check(self.lib.pxr_set_clip_tower(self.h, i, int(c["tower"])), "pxr_set_clip_tower")
         if drawer == DRAWER_POLYGON:
             rc = self.lib.pxr_set_polygons(self.h, xy.ctypes.data_as(C.c_void_p), off.ctypes.data_as(C.c_void_p),
                                            int(off.size) - 1)

@@ -43,6 +43,37 @@ def clip_state_dict(arch, seed=0):
     return sd
 
 
+def slip_state_dict(arch, seed=0):
+    """The image-tower tensors of a SLIP_Base checkpoint (after `module.` is stripped, slip.py:126-128): timm's
+    VisionTransformer under 'visual.*' and 'image_projection' (SLIP/models.py:130-134), at the scales of clip_state_dict."""
+    g = torch.Generator().manual_seed(seed)
+    W, L, P, D = arch["width"], arch["layers"], arch["patch"], arch["out_dim"]
+    T = (arch["image_res"] // P) ** 2 + 1
+    sd = {}
+    sd["visual.cls_token"] = _randn(g, 1, 1, W, std=W ** -0.5)
+    sd["visual.pos_embed"] = _randn(g, 1, T, W, std=0.01)
+    sd["visual.patch_embed.proj.weight"] = _randn(g, W, 3, P, P, std=(3 * P * P) ** -0.5)
+    sd["visual.patch_embed.proj.bias"] = _randn(g, W, std=0.02)
+    proj_std, attn_std, fc_std = (W ** -0.5) * ((2 * L) ** -0.5), W ** -0.5, (2 * W) ** -0.5
+    for i in range(L):
+        p = f"visual.blocks.{i}."
+        for nm in ("norm1", "norm2"):
+            sd[p + nm + ".weight"] = 1 + 0.1 * _randn(g, W)
+            sd[p + nm + ".bias"] = 0.05 * _randn(g, W)
+        sd[p + "attn.qkv.weight"] = _randn(g, 3 * W, W, std=attn_std)
+        sd[p + "attn.qkv.bias"] = _randn(g, 3 * W, std=0.02)
+        sd[p + "attn.proj.weight"] = _randn(g, W, W, std=proj_std)
+        sd[p + "attn.proj.bias"] = _randn(g, W, std=0.02)
+        sd[p + "mlp.fc1.weight"] = _randn(g, 4 * W, W, std=fc_std)
+        sd[p + "mlp.fc1.bias"] = _randn(g, 4 * W, std=0.02)
+        sd[p + "mlp.fc2.weight"] = _randn(g, W, 4 * W, std=proj_std)
+        sd[p + "mlp.fc2.bias"] = _randn(g, W, std=0.02)
+    sd["visual.norm.weight"] = 1 + 0.1 * _randn(g, W)
+    sd["visual.norm.bias"] = 0.05 * _randn(g, W)
+    sd["image_projection"] = _randn(g, W, D, std=W ** -0.5)
+    return sd
+
+
 def vqgan_state_dict(v, seed=0, with_encoder=False):
     """taming VQModel tensors pixray uses: quantize.embedding, post_quant_conv, decoder.* (vqgan.py:122-142) and, with
     with_encoder, encoder.* + quant_conv (model.encode: VqganDrawer.init_from_tensor, vqgan.py:174-185)."""
