@@ -31,7 +31,7 @@ extern "C" {
 typedef struct pxr_engine* pxr_handle;
 
 enum { PXR_DRAWER_VQGAN = 0, PXR_DRAWER_PIXEL = 1, PXR_DRAWER_FFT = 2, PXR_DRAWER_VDIFF = 3, PXR_DRAWER_POLYGON = 4,
-       PXR_DRAWER_SUPERRES = 5 };
+       PXR_DRAWER_SUPERRES = 5, PXR_DRAWER_STROKES = 6 };
 enum { PXR_PAD_REFLECTION = 0, PXR_PAD_BORDER = 1, PXR_PAD_ZEROS = 2 };
 enum { PXR_DTYPE_F16 = 0, PXR_DTYPE_BF16 = 1 };
 /* module ids for pxr_load_weight */
@@ -161,6 +161,14 @@ int pxr_synth(pxr_handle h, const float* z, float* out_img /* [3,H,W] */);
  * and iteration), even-odd fill, topmost polygon wins, pixel = mean of its samples, no clamp; clip_z keeps RGB in [0, 1]
  * and alpha at 1. */
 int pxr_set_polygons(pxr_handle h, const float* xy, const int* offsets, int n);
+/* Line-sketch drawer (PXR_DRAWER_STROKES; LineDrawer, linedrawer.py): n_paths open paths of n_segments cubic Béziers,
+ * stroked in opaque black over an opaque paper rectangle.  z = [points n_paths x (3 n_segments + 1) x 2 canvas
+ * coordinates | stroke widths n_paths (half widths) | paper RGBA 4].  The fused Adam steps the three ranges at lr,
+ * lr / 10 and lr / 100 (the paper only when paper_trainable, else it stays fixed) and clamps the widths to
+ * [1, max_width]; the managed step keeps no best-z copy.  The render takes the polygon drawer's 2 x 2 jittered samples
+ * (pxr_test_raster_samples); a sample is covered when it lies within a path's width of one of its chords (each cubic
+ * flattened into 16 chords).  Before pxr_finalize; max_width finite and positive. */
+int pxr_set_strokes(pxr_handle h, int n_paths, int n_segments, float max_width, int paper_trainable);
 /* The iteration the per-op pxr_synth renders (drawer.synth(cur_iteration)): keys the polygon drawer's sample positions,
  * ignored by the other drawers.  pxr_iterate uses its own `iter` (and leaves it set). */
 int pxr_set_synth_iteration(pxr_handle h, int iter);

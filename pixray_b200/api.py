@@ -45,9 +45,9 @@ from .util import apply_overlay, get_learning_rate_drops, parse_unit, split_pipe
 # PixelDrawer's five options; its default rect grid runs as fast_pixel (the square cells diffvg renders, SURVEY.md 2,
 # row 6), every other pixel_type on the polygon rasteriser (do_init)
 class_table = {"vqgan": P.VqganDrawer, "fast_pixel": P.FastPixelDrawer, "pixel": P.PixelDrawer, "fft": P.FftDrawer,
-               "vdiff": P.VdiffDrawer, "super_resolution": P.SuperResolutionDrawer}
+               "vdiff": P.VdiffDrawer, "super_resolution": P.SuperResolutionDrawer, "line_sketch": P.LineDrawer}
 _DRAWER_KIND = {"vqgan": E.DRAWER_VQGAN, "fast_pixel": E.DRAWER_PIXEL, "pixel": E.DRAWER_PIXEL, "fft": E.DRAWER_FFT,
-                "vdiff": E.DRAWER_VDIFF, "super_resolution": E.DRAWER_SUPERRES}
+                "vdiff": E.DRAWER_VDIFF, "super_resolution": E.DRAWER_SUPERRES, "line_sketch": E.DRAWER_STROKES}
 loss_class_table = L.loss_class_table
 filters_class_table = FL.filters_class_table
 
@@ -375,6 +375,12 @@ def do_init(args):
         kw["polygons"] = PS.polygons((sideX, sideY), rows, cols, args.pixel_type)
     if kind == E.DRAWER_FFT:
         kw.update(fft_decay=args.fft_decay, fft_colors=args.fft_colors)
+    if kind == E.DRAWER_STROKES:
+        # the reference's z_orig would be get_z_copy() = None and its anchors would fail on it (linedrawer.py:186-193)
+        for dest in ("init_weight", "init_weight_dist", "init_weight_cos", "init_weight_pix", "image_labels"):
+            if getattr(args, dest):
+                raise ValueError(f"{dest}: the line_sketch drawer has no latent to anchor to (get_z_copy is None)")
+        kw["strokes"] = (args.strokes, args.stroke_length, P.LineDrawer.max_width(args, sideY), bool(args.allow_paper_color))
     eng = _engine_factory(**kw)
     weights = args.b200_weights or {}
     if kind in (E.DRAWER_VQGAN, E.DRAWER_VDIFF, E.DRAWER_SUPERRES):

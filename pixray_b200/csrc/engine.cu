@@ -565,6 +565,12 @@ class Engine {
   RasterScene scene{};
   int* poly_winner = nullptr;
   int synth_iter = 0;
+  void build_strokes();
+  // line-sketch drawer: the shape from pxr_set_strokes and the per-render scene (kernels.cuh StrokeScene)
+  int stroke_paths = 0, stroke_segments = 0, stroke_paper = 0;
+  float stroke_max_width = 0.f;
+  StrokeScene sscene{};
+  ZRanges zr = zranges_single();  // per-range Adam rates and clamp (the line drawer's three optimisers)
   void build_fft();
   FftPlans* fft = nullptr;
   void build_cutouts();
@@ -1413,6 +1419,58 @@ void Engine::build_polygon() {
   drawer_bwd.add(1, [=] { raster_backward(sc, win, gi, H, Wd, inv, zg, cs); }, 0.0, "raster_backward");
 }
 
+// LineDrawer (linedrawer.py:44-166): z = [points | widths | paper RGBA]; the capsules are flattened and binned afresh on
+// every render because the geometry is what the optimiser moves.  The three Adams of get_opts (linedrawer.py:128-136)
+// become one fused Adam with rates x1 / x0.1 / x0.01 over the three ranges; the paper range has rate 0 unless it is
+// trainable.  clip_z clamps the widths to [1, max_width].
+void Engine::build_strokes() {
+  const int N = stroke_paths, L = stroke_segments, H = cfg.image_h, Wd = cfg.image_w;
+  if (N < 1) throw EngineError(-78, "line drawer: call pxr_set_strokes before pxr_finalize");
+  const int n_pts = N * (3 * L + 1) * 2;
+  z_numel = (int64_t)n_pts + N + 4;
+  z_buf = dalloc<float>(z_numel);
+  z_grad = dalloc<float>(z_numel);
+  img = dalloc<float>((size_t)3 * H * Wd);
+  img_pre = img;  // synth has no clamp (linedrawer.py:156-166)
+  g_img = dalloc<float>((size_t)3 * H * Wd);
+  StrokeScene& s = sscene;
+  s.n_paths = N;
+  s.n_segments = L;
+  s.n_caps = N * L * STROKE_CHORDS;
+  s.W = Wd;
+  s.H = H;
+  s.tiles_x = (Wd + RASTER_TILE - 1) / RASTER_TILE;
+  s.tiles_y = (H + RASTER_TILE - 1) / RASTER_TILE;
+  s.width_offset = n_pts;
+  s.paper_trainable = stroke_paper;
+  const size_t tiles = (size_t)s.tiles_x * s.tiles_y;
+  s.caps = dalloc<float4>(s.n_caps);
+  s.cap_tiles = dalloc<int4>(s.n_caps);
+  s.tile_start = dalloc<int>(tiles + 1);
+  s.tile_list = dalloc<int>((size_t)s.n_caps * tiles);  // every capsule in every tile: the geometry is unbounded
+  s.winner = dalloc<int>((size_t)4 * H * Wd);
+  s.pix_g = dalloc<float>((size_t)H * Wd);
+  s.paper_part = dalloc<float>((size_t)stroke_paper_blocks(H, Wd) * 4);
+  s.cap_grad = dalloc<float>((size_t)s.n_caps * 5);
+  zr.end0 = n_pts;
+  zr.end1 = n_pts + N;
+  zr.scale[0] = 1.f;
+  zr.scale[1] = 0.1f;
+  zr.scale[2] = stroke_paper ? 0.01f : 0.f;
+  zr.lo1 = 1.f;
+  zr.hi1 = stroke_max_width;
+  cudaStream_t cs = st;
+  float *zb = z_buf, *im = img, *gi = g_img, *zg = z_grad;
+  const StrokeScene sc = s;
+  const uint64_t seed = cfg.seed;
+  const float inv = 1.f / S;
+  const int* iter = &synth_iter;
+  drawer_fwd.add(1, [=] { stroke_flatten(sc, zb, cs); }, 0.0, "stroke_flatten");
+  drawer_fwd.add(3, [=] { stroke_bin(sc, cs); }, 0.0, "stroke_bin");
+  drawer_fwd.add(1, [=] { stroke_raster_forward(sc, zb, seed, *iter, im, cs); }, 0.0, "stroke_raster_fwd");
+  drawer_bwd.add(3, [=] { stroke_raster_backward(sc, zb, gi, inv, zg, cs); }, 0.0, "stroke_raster_bwd");
+}
+
 // FftDrawer.synth (fftdrawer.py:78-84): params = rfft2 spectrum [1,3,H,W/2+1,2]; see kernels_fft.cu
 void Engine::build_fft() {
   const int H = cfg.image_h, Wd = cfg.image_w, W2 = Wd / 2 + 1;
@@ -2198,6 +2256,7 @@ bool Engine::spot_pass(int which, bool accumulate_img) {
 int Engine::clip_mode() const {
   if (cfg.drawer == PXR_DRAWER_PIXEL || cfg.drawer == PXR_DRAWER_SUPERRES) return CLIP_01;
   if (cfg.drawer == PXR_DRAWER_POLYGON) return CLIP_RGBA;
+  if (cfg.drawer == PXR_DRAWER_STROKES) return CLIP_STROKES;
   return CLIP_NONE;
 }
 
@@ -2205,7 +2264,7 @@ void Engine::step(float lr) {
   ++adam_t;
   const int per_channel = (cfg.drawer == PXR_DRAWER_VQGAN) ? (int)(z_numel / cfg.z_channels) : 1;
   adam_clip_step(z_buf, adam_m, adam_v, batches > 1 ? z_grad_acc : z_grad, 1.f, (int)z_numel, per_channel, zmin, zmax,
-                 clip_mode(), lr, cfg.beta1, cfg.beta2, cfg.adam_eps, adam_t, st);
+                 clip_mode(), zr, lr, cfg.beta1, cfg.beta2, cfg.adam_eps, adam_t, st);
   launches += 1;
 }
 
@@ -2368,8 +2427,10 @@ void Engine::write_initial_drop_state() {
 void Engine::step_managed(int iter) {
   const int per_channel = (cfg.drawer == PXR_DRAWER_VQGAN) ? (int)(z_numel / cfg.z_channels) : 1;
   const float* g = batches > 1 ? z_grad_acc : z_grad;
-  adam_clip_managed(z_buf, adam_m, adam_v, g, best_z, 1.f, (int)z_numel, per_channel, zmin, zmax,
-                    clip_mode(), cfg.beta1, cfg.beta2, cfg.adam_eps, losses_dev, num_losses(), iter,
+  // the line drawer's get_z_copy is None (linedrawer.py:189-190): no best-z snapshot for it
+  float* best = cfg.drawer == PXR_DRAWER_STROKES ? nullptr : best_z;
+  adam_clip_managed(z_buf, adam_m, adam_v, g, best, 1.f, (int)z_numel, per_channel, zmin, zmax,
+                    clip_mode(), zr, cfg.beta1, cfg.beta2, cfg.adam_eps, losses_dev, num_losses(), iter,
                     drop_cfg, drop_state + drop_parity, drop_state + (drop_parity ^ 1), drop_status_dev, st);
   drop_parity ^= 1;
   launches += 1;
@@ -2383,6 +2444,7 @@ void Engine::finalize() {
   else if (cfg.drawer == PXR_DRAWER_VDIFF) build_vdiff();
   else if (cfg.drawer == PXR_DRAWER_POLYGON) build_polygon();
   else if (cfg.drawer == PXR_DRAWER_SUPERRES) build_superres();
+  else if (cfg.drawer == PXR_DRAWER_STROKES) build_strokes();
   else throw EngineError(-47, "unknown drawer kind");
   adam_m = dalloc<float>(z_numel);
   adam_v = dalloc<float>(z_numel);
@@ -2431,6 +2493,10 @@ void Engine::finalize() {
     reg("z", z_buf, z_numel * 4);
     reg("losses", losses_dev, 64 * 4);
     if (poly_winner) reg("poly_winner", poly_winner, npx / 3 * 4 * sizeof(int));
+    if (sscene.winner) {
+      reg("stroke_winner", sscene.winner, npx / 3 * 4 * sizeof(int));
+      reg("stroke_caps", sscene.caps, (size_t)sscene.n_caps * sizeof(float4));
+    }
     if (vd_pred) {
       reg("vd_pred", vd_pred, npx * 4);
       reg("vd_v", vd_v, npx * 4);
@@ -2675,6 +2741,25 @@ int pxr_set_polygons(pxr_handle h, const float* xy, const int* offsets, int n) {
         throw EngineError(-77, "pxr_set_polygons: vertex " + std::to_string(i / 2) + " has a non-finite coordinate");
     e->poly_xy.assign(xy, xy + 2 * nv);
     e->poly_off.assign(offsets, offsets + n + 1);
+  });
+}
+
+// The line drawer's shape (LineDrawer.load_model, linedrawer.py:44-126): n_paths open paths of n_segments cubics, widths
+// clamped to [1, max_width] by clip_z, the paper colour optimised only when paper_trainable.  Before pxr_finalize.
+int pxr_set_strokes(pxr_handle h, int n_paths, int n_segments, float max_width, int paper_trainable) {
+  PXR_TRY(h, {
+    Engine* e = h->e;
+    if (e->cfg.drawer != PXR_DRAWER_STROKES) throw EngineError(-79, "pxr_set_strokes: not a line-drawer engine");
+    if (e->finalized) throw EngineError(-12, "pxr_set_strokes: the strokes cannot change after pxr_finalize");
+    if (n_paths < 1 || n_segments < 1)
+      throw EngineError(-80, "pxr_set_strokes: n_paths = " + std::to_string(n_paths) + ", n_segments = " +
+                                 std::to_string(n_segments) + "; at least one of each is needed");
+    if (!std::isfinite(max_width) || !(max_width > 0.f))
+      throw EngineError(-80, "pxr_set_strokes: max_width must be finite and positive");
+    e->stroke_paths = n_paths;
+    e->stroke_segments = n_segments;
+    e->stroke_max_width = max_width;
+    e->stroke_paper = paper_trainable ? 1 : 0;
   });
 }
 

@@ -146,6 +146,41 @@ void raster_forward(const RasterScene& s, const float* z, int H, int W, uint64_t
 void raster_backward(const RasterScene& s, const int* winner, const float* g_img, int H, int W, float inv_scale,
                      float* z_grad, cudaStream_t st);
 
+// ------------------------------------------------------------------ line-sketch drawer (kernels_strokes.cu; LineDrawer,
+// linedrawer.py:44-166).  n_paths open paths of n_segments cubic Béziers over an opaque paper rectangle; every stroke is
+// opaque black.  z = [points n_paths * (3 n_segments + 1) * 2 | widths n_paths | paper RGBA 4].
+//   Geometry: each cubic is flattened into STROKE_CHORDS chords at t = i / STROKE_CHORDS; a path covers the points within
+//   its width w (the half width) of one of its chords, i.e. a union of round-capped capsules.
+//   Forward: 2 x 2 jittered samples per pixel (raster_samples.cuh); a sample's winner is the topmost path covering it.
+//   The pixel's RGBA is the mean of its samples' (black, or the paper's RGBA), composited as synth does:
+//   out = rgb a + (1 - a).
+//   Backward: the exact derivative of the box-filtered coverage with respect to the outline, integral over the visible
+//   capsule boundary of G(pixel) v_n ds, where G = sum_ch g_ch d out_ch / d coverage at the forward's coverage.  Straight
+//   sides are walked across the pixel grid and their visible parts (no other capsule strictly covers them) integrate
+//   exactly; each vertex circle uses STROKE_ARC_NODES midpoint nodes.  The paper colour gets the interior term.
+//   Capsules are re-binned into RASTER_TILE tiles every render (the geometry moves every step).
+constexpr int STROKE_CHORDS = 16;
+constexpr int STROKE_ARC_NODES = 64;
+struct StrokeScene {
+  int n_paths, n_segments, n_caps, W, H, tiles_x, tiles_y, width_offset, paper_trainable;
+  float4* caps;      // [n_caps] chord endpoints (ax, ay, bx, by); capsule c = chord c % S of segment c / S (path-major)
+  int4* cap_tiles;   // [n_caps] tile range (tx0, ty0, tx1, ty1) of the box grown by the width; empty when tx1 < tx0
+  int* tile_start;   // [tiles + 1]
+  int* tile_list;    // [n_caps * tiles] capsule indices per tile, highest index (topmost) first
+  int* winner;       // [4, H, W] path index per sample, -1 = paper
+  float* pix_g;      // [H, W] d loss / d coverage
+  float* paper_part; // [stroke_paper_blocks(H, W), 4]
+  float* cap_grad;   // [n_caps, 5] d loss / d (a, b, w) of each capsule
+};
+int stroke_paper_blocks(int H, int W);
+void stroke_flatten(const StrokeScene& s, const float* z, cudaStream_t st);
+void stroke_bin(const StrokeScene& s, cudaStream_t st);  // count, scan, fill
+void stroke_raster_forward(const StrokeScene& s, const float* z, uint64_t seed, int iter, float* img, cudaStream_t st);
+// z_grad = inv_scale * d loss / dz (overwritten; the paper part is 0 unless paper_trainable).  No atomics: bit-identical
+// on repeats.
+void stroke_raster_backward(const StrokeScene& s, const float* z, const float* g_img, float inv_scale, float* z_grad,
+                            cudaStream_t st);
+
 // ------------------------------------------------------------------ FFT drawer (fftdrawer.py:78-84)
 struct FftPlans;  // cuFFT C2R / R2C plans (3 planes of H x W), resolved through dlopen
 FftPlans* fft_plans_create(int H, int W, cudaStream_t st, const char** err);
@@ -275,17 +310,28 @@ void prompt_loss(const float* e, int B, int D, const float* prompts, const float
 //   CLIP_NONE  no clamp
 //   CLIP_01    [0, 1] (fast_pixeldrawer.py:98-100)
 //   CLIP_RGBA  z is [n, 4] RGBA fill colours: RGB to [0, 1], alpha to [1, 1] (pixeldrawer.py:378-382)
-enum { CLIP_NONE = 0, CLIP_01 = 1, CLIP_RGBA = 2 };
+//   CLIP_STROKES  the line drawer's z: range 1 (the widths) to [lo1, hi1] (linedrawer.py:179-184)
+// ZRanges splits z into [0, end0) [end0, end1) [end1, n), each with its own multiple of the learning rate: the line
+// drawer's three Adams (linedrawer.py:128-136).  Every other drawer uses one range at scale 1 (zranges_single).
+enum { CLIP_NONE = 0, CLIP_01 = 1, CLIP_RGBA = 2, CLIP_STROKES = 3 };
+struct ZRanges {
+  int end0, end1;
+  float scale[3];
+  float lo1, hi1;
+};
+inline ZRanges zranges_single() { return ZRanges{0x7fffffff, 0x7fffffff, {1.f, 1.f, 1.f}, 0.f, 0.f}; }
 #ifdef __CUDACC__
-__device__ __forceinline__ float clip_mode_apply(int clip_mode, int i, float zi) {
+__device__ __forceinline__ int zrange_of(const ZRanges& r, int i) { return i < r.end0 ? 0 : i < r.end1 ? 1 : 2; }
+__device__ __forceinline__ float clip_mode_apply(int clip_mode, int i, float zi, const ZRanges& r) {
   if (clip_mode == CLIP_01) return fminf(fmaxf(zi, 0.f), 1.f);
   if (clip_mode == CLIP_RGBA) return (i & 3) == 3 ? 1.f : fminf(fmaxf(zi, 0.f), 1.f);
+  if (clip_mode == CLIP_STROKES && zrange_of(r, i) == 1) return fminf(fmaxf(zi, r.lo1), r.hi1);
   return zi;
 }
 #endif
 void adam_clip_step(float* z, float* m, float* v, const float* g, float inv_scale, int n, int per_channel,
-                    const float* zmin, const float* zmax, int clip_mode, float lr, float b1, float b2, float eps, int t,
-                    cudaStream_t st);
+                    const float* zmin, const float* zmax, int clip_mode, const ZRanges& zr, float lr, float b1, float b2,
+                    float eps, int t, cudaStream_t st);
 
 // ------------------------------------------------------------------ device-side checkdrop + Adam (pixray.py:1090-1109, 1464-1512)
 // train()'s per-iteration control decisions without a host round trip.  The optimiser step of iteration `it` reads the
@@ -324,8 +370,8 @@ struct DropStatus {
   volatile int seq_end;
 };
 void adam_clip_managed(float* z, float* m, float* v, const float* g, float* best_z, float inv_scale, int n,
-                       int per_channel, const float* zmin, const float* zmax, int clip_mode, float b1, float b2,
-                       float eps, const float* losses, int n_losses, int iter, const DropConfig& cfg,
+                       int per_channel, const float* zmin, const float* zmax, int clip_mode, const ZRanges& zr, float b1,
+                       float b2, float eps, const float* losses, int n_losses, int iter, const DropConfig& cfg,
                        const DropState* cur, DropState* next, DropStatus* status_mapped, cudaStream_t st);
 // acc (=|+=) g: gradient accumulation over the `batches` passes of one iteration (pixray.py:1464-1482)
 void accumulate_f32(const float* g, float* acc, long long n, int accumulate, cudaStream_t st);

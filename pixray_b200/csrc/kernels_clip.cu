@@ -532,7 +532,7 @@ __global__ void __launch_bounds__(128) prompt_loss_kernel(const float* __restric
 __global__ void adam_clip_kernel(float* __restrict__ z, float* __restrict__ m, float* __restrict__ v,
                                  const float* __restrict__ g, float inv_scale, int n, int per_channel,
                                  const float* __restrict__ zmin, const float* __restrict__ zmax, int clip_mode,
-                                 float step_size, float b1, float b2, float eps, float inv_sqrt_bc2) {
+                                 ZRanges zr, float step_size, float b1, float b2, float eps, float inv_sqrt_bc2) {
   pdl_prologue();
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
@@ -542,12 +542,12 @@ __global__ void adam_clip_kernel(float* __restrict__ z, float* __restrict__ m, f
   m[i] = mi;
   v[i] = vi;
   float denom = sqrtf(vi) * inv_sqrt_bc2 + eps;
-  float zi = z[i] - step_size * mi / denom;
+  float zi = z[i] - step_size * zr.scale[zrange_of(zr, i)] * mi / denom;
   if (zmin) {
     int c = i / per_channel;
     zi = fminf(fmaxf(zi, zmin[c]), zmax[c]);  // vqgan.py:202-204
   } else {
-    zi = clip_mode_apply(clip_mode, i, zi);
+    zi = clip_mode_apply(clip_mode, i, zi, zr);
   }
   z[i] = zi;
 }
@@ -556,7 +556,8 @@ __global__ void adam_clip_kernel(float* __restrict__ z, float* __restrict__ m, f
 __global__ void adam_clip_managed_kernel(float* __restrict__ z, float* __restrict__ m, float* __restrict__ v,
                                          const float* __restrict__ g, float* __restrict__ best_z, float inv_scale, int n,
                                          int per_channel, const float* __restrict__ zmin, const float* __restrict__ zmax,
-                                         int clip_mode, float b1, float b2, float eps, const float* __restrict__ losses,
+                                         int clip_mode, ZRanges zr, float b1, float b2, float eps,
+                                         const float* __restrict__ losses,
                                          int n_losses, int iter, DropConfig cfg, const DropState* __restrict__ cur,
                                          DropState* __restrict__ next, DropStatus* status) {
   pdl_prologue();
@@ -586,7 +587,10 @@ __global__ void adam_clip_managed_kernel(float* __restrict__ z, float* __restric
     nx.adam_t = t;
     // torch.optim.Adam: step_size = lr / (1 - b1^t); denom = sqrt(v) / sqrt(1 - b2^t) + eps
     const double bc1 = 1.0 - pow((double)b1, (double)t), bc2 = 1.0 - pow((double)b2, (double)t);
-    const float step_size = (float)((double)s.lr / bc1), inv_sqrt_bc2 = (float)(1.0 / sqrt(bc2));
+    // one step size per z range (scale 1 everywhere except the line drawer's widths and paper colour)
+    float step_r[3];
+    for (int r = 0; r < 3; ++r) step_r[r] = (float)((double)s.lr * (double)zr.scale[r] / bc1);
+    const float inv_sqrt_bc2 = (float)(1.0 / sqrt(bc2));
     if (rebuild) {
       nx.num_loss_drop = s.num_loss_drop + 1;
       if (nx.num_loss_drop > cfg.max_loss_drops) {
@@ -608,12 +612,12 @@ __global__ void adam_clip_managed_kernel(float* __restrict__ z, float* __restric
       m[i] = fresh ? 0.f : mi;
       v[i] = fresh ? 0.f : vi;
       const float denom = sqrtf(vi) * inv_sqrt_bc2 + eps;
-      float zi = z0 - step_size * mi / denom;
+      float zi = z0 - step_r[zrange_of(zr, i)] * mi / denom;
       if (zmin) {
         const int c = i / per_channel;
         zi = fminf(fmaxf(zi, zmin[c]), zmax[c]);
       } else {
-        zi = clip_mode_apply(clip_mode, i, zi);
+        zi = clip_mode_apply(clip_mode, i, zi, zr);
       }
       z[i] = zi;
     }
@@ -816,22 +820,22 @@ void prompt_loss(const float* e, int B, int D, const float* prompts, const float
 }
 
 void adam_clip_step(float* z, float* m, float* v, const float* g, float inv_scale, int n, int per_channel,
-                    const float* zmin, const float* zmax, int clip_mode, float lr, float b1, float b2, float eps, int t,
-                    cudaStream_t st) {
+                    const float* zmin, const float* zmax, int clip_mode, const ZRanges& zr, float lr, float b1, float b2,
+                    float eps, int t, cudaStream_t st) {
   // torch.optim.Adam: step_size = lr / (1 - b1^t); denom = sqrt(v) / sqrt(1 - b2^t) + eps
   const double bc1 = 1.0 - pow((double)b1, t), bc2 = 1.0 - pow((double)b2, t);
-  launch_pdl(adam_clip_kernel, dim3((n + 255) / 256), dim3(256), 0, st, z, m, v, g, inv_scale, n, per_channel, zmin, zmax, clip_mode,
+  launch_pdl(adam_clip_kernel, dim3((n + 255) / 256), dim3(256), 0, st, z, m, v, g, inv_scale, n, per_channel, zmin, zmax, clip_mode, zr,
                                                     (float)(lr / bc1), b1, b2, eps, (float)(1.0 / sqrt(bc2)));
 }
 
 void adam_clip_managed(float* z, float* m, float* v, const float* g, float* best_z, float inv_scale, int n,
-                       int per_channel, const float* zmin, const float* zmax, int clip_mode, float b1, float b2,
-                       float eps, const float* losses, int n_losses, int iter, const DropConfig& cfg,
+                       int per_channel, const float* zmin, const float* zmax, int clip_mode, const ZRanges& zr, float b1,
+                       float b2, float eps, const float* losses, int n_losses, int iter, const DropConfig& cfg,
                        const DropState* cur, DropState* next, DropStatus* status_mapped, cudaStream_t st) {
   int grid = (n + 255) / 256;
   if (grid > 148 * 4) grid = 148 * 4;
   launch_pdl(adam_clip_managed_kernel, dim3(grid), dim3(256), 0, st, z, m, v, g, best_z, inv_scale, n, per_channel, zmin,
-             zmax, clip_mode, b1, b2, eps, losses, n_losses, iter, cfg, cur, next, status_mapped);
+             zmax, clip_mode, zr, b1, b2, eps, losses, n_losses, iter, cfg, cur, next, status_mapped);
 }
 
 void accumulate_f32(const float* g, float* acc, long long n, int accumulate, cudaStream_t st) {

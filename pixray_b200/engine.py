@@ -10,7 +10,7 @@ import torch
 
 from . import _lib
 
-DRAWER_VQGAN, DRAWER_PIXEL, DRAWER_FFT, DRAWER_VDIFF, DRAWER_POLYGON, DRAWER_SUPERRES = 0, 1, 2, 3, 4, 5
+DRAWER_VQGAN, DRAWER_PIXEL, DRAWER_FFT, DRAWER_VDIFF, DRAWER_POLYGON, DRAWER_SUPERRES, DRAWER_STROKES = 0, 1, 2, 3, 4, 5, 6
 LOSS_SYMMETRY, LOSS_SATURATION, LOSS_PALETTE, LOSS_SMOOTHNESS, LOSS_EDGE, LOSS_GAUSSIAN, LOSS_AESTHETIC = range(7)
 ANCHOR_SPHERICAL, ANCHOR_MSE, ANCHOR_COS, ANCHOR_PIX = 0, 1, 2, 3
 FILTER_TILER, FILTER_WALLPAPER, FILTER_LOOKUP = range(3)
@@ -49,11 +49,16 @@ class EngineError(RuntimeError):
     pass
 
 
+def stroke_z_layout(n_paths, n_segments):
+    """Sizes of the line drawer's z ranges: (points, widths, paper RGBA)."""
+    return n_paths * (3 * n_segments + 1) * 2, n_paths, 4
+
+
 class B200Engine:
     def __init__(self, *, drawer=DRAWER_VQGAN, image_hw=(256, 256), vqgan=None, grid=None, cutn=64, cut_size=224,
                  clip=(), noise_fac=0.1, seed=0, device=0, rank=0, world=1, grad_scale=0.0, lr_betas=(0.9, 0.999),
                  adam_eps=1e-8, fft_decay=0.0, fft_colors=0.0, fft_contrast=0.0, cut_aspect=1.0, polygons=None,
-                 superres=None):
+                 superres=None, strokes=None):
         if not torch.cuda.is_available():
             raise EngineError("pixray_b200 needs a CUDA device (H100); there is no CPU fallback")
         self.lib = _lib.load()
@@ -91,6 +96,13 @@ class B200Engine:
             xy = np.ascontiguousarray(np.asarray(polygons[0], dtype=np.float32).reshape(-1, 2))
             off = np.ascontiguousarray(np.asarray(polygons[1], dtype=np.int32).reshape(-1))
             self.z_shape = (int(off.size) - 1, 4)
+        elif drawer == DRAWER_STROKES:
+            # LineDrawer (linedrawer.py:44-126): strokes = (n_paths, n_segments, max_width, paper_trainable); z = the packed
+            # [points n_paths * (3 n_segments + 1) * 2 | widths n_paths | paper RGBA 4] (stroke_z_layout)
+            if strokes is None:
+                raise EngineError("drawer=DRAWER_STROKES needs strokes=(n_paths, n_segments, max_width, paper_trainable)")
+            n_paths, n_segments = int(strokes[0]), int(strokes[1])
+            self.z_shape = (sum(stroke_z_layout(n_paths, n_segments)),)
         else:
             cfg.grid_rows, cfg.grid_cols = grid
             self.z_shape = (1, 3, grid[0], grid[1])
@@ -132,6 +144,9 @@ class B200Engine:
             rc = self.lib.pxr_set_polygons(self.h, xy.ctypes.data_as(C.c_void_p), off.ctypes.data_as(C.c_void_p),
                                            int(off.size) - 1)
             self._check(rc, "pxr_set_polygons")
+        if drawer == DRAWER_STROKES:
+            rc = self.lib.pxr_set_strokes(self.h, n_paths, n_segments, C.c_float(float(strokes[2])), int(bool(strokes[3])))
+            self._check(rc, "pxr_set_strokes")
         self._ext = None  # torch view of the engine's stream (ordering against torch-side producers of z / noise)
 
     # ------------------------------------------------------------------ plumbing

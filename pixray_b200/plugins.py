@@ -292,6 +292,145 @@ class PixelDrawer(DrawingInterface):
         return self.z.clone()
 
 
+PAPER_RGBA = (242 / 255.0, 238 / 255.0, 203 / 255.0, 1.0)  # linedrawer.py:65
+
+
+def line_start_points(canvas_width, canvas_height, num_paths, num_segments, rng=None):
+    """The start control points of LineDrawer.load_model (linedrawer.py:73-99), [num_paths, 3 num_segments + 1, 2] float32
+    canvas coordinates, drawn from `rng` (default: the `random` module, which the session seeds right before) in the
+    reference's order and with its arithmetic."""
+    import random
+    rng = random if rng is None else rng
+    bound = lambda value, low, high: max(low, min(high, value))  # noqa: E731 (linedrawer.py:23-24)
+    out = []
+    for _ in range(num_paths):
+        points = []
+        radius = 0.5
+        radius_x = 0.5
+        p0 = (0.5 + radius_x * (rng.random() - 0.5), 0.5 + radius * (rng.random() - 0.5))
+        points.append(p0)
+        for _ in range(num_segments):
+            radius = 1.0 / (num_segments + 2)
+            radius_x = radius * canvas_height / canvas_width
+            p1 = (p0[0] + radius_x * (rng.random() - 0.5), p0[1] + radius * (rng.random() - 0.5))
+            p2 = (p1[0] + radius_x * (rng.random() - 0.5), p1[1] + radius * (rng.random() - 0.5))
+            p3 = (p2[0] + radius_x * (rng.random() - 0.5), p2[1] + radius * (rng.random() - 0.5))
+            points += [p1, p2, p3]
+            p0 = (bound(p3[0], 0, 1), bound(p3[1], 0, 1))
+        points = torch.tensor(points)
+        points[:, 0] *= canvas_width
+        points[:, 1] *= canvas_height
+        out.append(points)
+    return torch.stack(out)
+
+
+class LineDrawer(DrawingInterface):
+    """linedrawer.py (`line_sketch`): num_paths open paths of stroke_length cubic Béziers stroked in black over paper,
+    rendered and differentiated by the engine's stroke rasteriser (PXR_DRAWER_STROKES).  z is the packed
+    [points | widths | paper RGBA] vector; its three Adams (get_opts) run as one fused Adam with per-range rates."""
+
+    @staticmethod
+    def add_settings(parser):
+        from .api import str2bool
+        parser.add_argument("--strokes", type=int, help="number strokes", default=24, dest="strokes")
+        parser.add_argument("--stroke_length", type=int, help="stroke length", default=8, dest="stroke_length")
+        parser.add_argument("--min_stroke_width", type=float, help="min width (percent of height)", default=0.5, dest="min_stroke_width")
+        parser.add_argument("--max_stroke_width", type=float, help="max width (percent of height)", default=2, dest="max_stroke_width")
+        parser.add_argument("--allow_paper_color", type=str2bool, help="allow paper color to change", default=False, dest="allow_paper_color")
+        return parser
+
+    @staticmethod
+    def max_width(settings, canvas_height):
+        return settings.max_stroke_width * canvas_height / 100  # linedrawer.py:52
+
+    def __init__(self, settings, session: Session):
+        super().__init__(settings)
+        self.session = session
+        self.canvas_height, self.canvas_width = session.engine.image_hw
+        self.num_paths, self.stroke_length = settings.strokes, settings.stroke_length
+        self.allow_paper_color = bool(settings.allow_paper_color)
+        self.z = None
+        self.img = None
+
+    def load_model(self, settings, device):
+        """The start geometry (linedrawer.py:44-126): points from `random`, every width max_width / 10, the paper colour."""
+        self.device = device
+        self.max_width = LineDrawer.max_width(settings, self.canvas_height)
+        points = line_start_points(self.canvas_width, self.canvas_height, self.num_paths, self.stroke_length)
+        widths = torch.full((self.num_paths,), float(torch.tensor(self.max_width / 10)))
+        paper = torch.tensor(PAPER_RGBA)
+        z = torch.cat([points.reshape(-1), widths, paper])
+        self.z = z.to(self.session.engine.device, torch.float32).contiguous()
+
+    def get_opts(self, decay_divisor=1):
+        """The rates of the points, widths and (with allow_paper_color) paper Adams (linedrawer.py:128-136)."""
+        opts = [{"lr": 1.0 / decay_divisor}, {"lr": 0.1 / decay_divisor}]
+        if self.allow_paper_color:
+            opts.append({"lr": 0.01 / decay_divisor})
+        return opts
+
+    def get_num_resolutions(self):
+        return None
+
+    def rand_init(self, toksX, toksY):
+        pass
+
+    def init_from_tensor(self, init_tensor):
+        pass  # the reference leaves it a TODO (linedrawer.py:142-144)
+
+    def reapply_from_tensor(self, new_tensor):
+        pass
+
+    def get_z_from_tensor(self, ref_tensor):
+        return None
+
+    def _ranges(self):
+        n_pts, n_w, _ = E.stroke_z_layout(self.num_paths, self.stroke_length)
+        return n_pts, n_pts + n_w
+
+    def points(self):
+        """[num_paths, 3 stroke_length + 1, 2] view of z."""
+        return self.z[:self._ranges()[0]].view(self.num_paths, 3 * self.stroke_length + 1, 2)
+
+    def widths(self):
+        a, b = self._ranges()
+        return self.z[a:b]
+
+    def paper(self):
+        return self.z[self._ranges()[1]:]
+
+    def synth(self, cur_iteration):
+        """The render of cur_iteration's sample positions composited over white, [1, 3, H, W]."""
+        eng = self.session.engine
+        eng.set_synth_iteration(cur_iteration)
+        self.img = eng.synth(self.z)
+        return self.img
+
+    @torch.no_grad()
+    def to_image(self):
+        """The current geometry rendered with the session's iteration, as linedrawer.py:168-177 converts it (x 254)."""
+        from PIL import Image
+        img = self.synth(self.session.cur_iteration)
+        arr = np.uint8(np.clip(img[0].detach().cpu().numpy().transpose(1, 2, 0), 0, 1) * 254)
+        return Image.fromarray(arr, mode="RGB")
+
+    def clip_z(self):
+        with torch.no_grad():
+            self.widths().clamp_(1.0, self.max_width)  # the stroke colours are fixed black, not part of z
+
+    def get_z(self):
+        """The packed parameters.  The reference returns None and optimises its tensors through get_opts; the engine
+        needs one vector, as for FftDrawer."""
+        return self.z
+
+    def set_z(self, new_z):
+        with torch.no_grad():
+            return self.z.copy_(new_z.reshape(self.z.shape))
+
+    def get_z_copy(self):
+        return None  # as the reference (linedrawer.py:189-190): no best state is ever restored
+
+
 class VdiffDrawer(DrawingInterface):
     """vdiff.py:58-190 (cc12m_1): z = the noisy image x; synth = one v-prediction step + ClampWithGrad; after every
     optimiser step the loop re-noises x (`makenoise`, pixray.py:1489-1495) and builds a fresh Adam."""
