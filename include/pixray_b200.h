@@ -250,7 +250,17 @@ int pxr_vdiff_set_clip_embed(pxr_handle h, const float* embed, int D);
 int pxr_vdiff_set_iteration(pxr_handle h, int i);
 int pxr_vdiff_renoise(pxr_handle h, float* z, int i, const float* noise);
 
-int pxr_reset_optimizer(pxr_handle h); /* rebuild_optimisers: fresh Adam state (pixray.py:520-555, 1511) */
+int pxr_reset_optimizer(pxr_handle h); /* rebuild_optimisers: a fresh instance of the current rule (pixray.py:520-555, 1511) */
+
+/* args.optimiser (pixray.py:536-551): the update rule of pxr_step / pxr_iterate, each with the constructor defaults pixray
+ * builds it with (only lr is passed).  AdamW, Adamax and DiffGrad take beta1 / beta2 / adam_eps from pxr_config; AdamW's
+ * weight decay is 0.01 and Adagrad's eps 1e-10.  Valid after pxr_finalize; has pxr_reset_optimizer's effects (fresh state,
+ * t = 0, and in managed mode fresh drop bookkeeping) and refuses an unknown kind.  The default is PXR_OPT_ADAM.
+ * Checkpoints of an Adam session are version 1 {header, z, m, v}; the other rules write version 2 {header, kind, z,
+ * state arrays} (Adagrad: m, unused, and s; Adamax: m, u; DiffGrad: m, v, previous gradient).  A blob loads only into a session of
+ * its own rule. */
+enum { PXR_OPT_ADAM = 0, PXR_OPT_ADAMW, PXR_OPT_ADAGRAD, PXR_OPT_ADAMAX, PXR_OPT_DIFFGRAD };
+int pxr_set_optimizer(pxr_handle h, int kind);
 
 /* train()'s control decisions on the device (checkdrop pixray.py:1090-1109; scheduled learning-rate drops, auto-stop and
  * rebuild_optimisers 1464-1512): the optimiser step of every pxr_iterate reads the iteration's loss vector, tracks the best

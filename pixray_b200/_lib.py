@@ -72,7 +72,7 @@ EXPORTS = [
     "pxr_num_kernel_launches", "pxr_get_stream", "pxr_z_numel", "pxr_z_bounds", "pxr_test_gemm", "pxr_test_conv", "pxr_debug_read", "pxr_profile_iteration", "pxr_profile_iteration2",
     "pxr_test_attention", "pxr_test_color_jitter_host", "pxr_test_color_jitter_device", "pxr_set_color_jitter", "pxr_set_image_prompts", "pxr_set_image_prompts_sized", "pxr_add_aux_loss", "pxr_add_filter", "pxr_clear_filters", "pxr_set_filter_shifts", "pxr_clear_aux_losses", "pxr_add_anchor", "pxr_clear_anchors", "pxr_num_losses", "pxr_read_losses",
     "pxr_test_pool_bounds", "pxr_test_groupnorm", "pxr_test_softmax", "pxr_test_layernorm", "pxr_set_spot_prompts", "pxr_set_spot_mask", "pxr_state_size", "pxr_save_state", "pxr_load_state", "pxr_set_schedule", "pxr_poll_status", "pxr_set_batches", "pxr_set_z_grad", "pxr_vdiff_set_schedule", "pxr_vdiff_set_clip_embed", "pxr_vdiff_set_iteration", "pxr_vdiff_renoise",
-    "pxr_set_polygons", "pxr_set_synth_iteration", "pxr_test_raster_samples", "pxr_set_strokes",
+    "pxr_set_polygons", "pxr_set_synth_iteration", "pxr_test_raster_samples", "pxr_set_strokes", "pxr_set_optimizer",
     "pxr_test_splitk_reduce", "pxr_test_groupnorm_unet", "pxr_test_resample", "pxr_test_gemv",
 ]
 

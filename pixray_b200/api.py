@@ -5,8 +5,13 @@ front-ends use (run.py, cogrun.py) plus the notebook one-liner.
 Scope (SURVEY.md 8): the per-iteration hot path.  Every option of the reference's parser is KNOWN here (same dest,
 same default: the "requested setting not found" check of pixray.py:2088-2093 behaves identically), but options that
 switch on something outside the hot path (spot prompts, overlays, animation, init images through the VQGAN encoder,
-filters, transparency, non-Adam optimisers, the `perceptors` preset, video) raise NotImplementedError when they are set
+filters, transparency, the AdamP optimiser, the `perceptors` preset, video) raise NotImplementedError when they are set
 to a non-default value instead of being silently ignored.
+
+`optimiser` takes Adam, AdamW, Adagrad, Adamax or DiffGrad (pixray.py:536-551), each with the constructor defaults the
+reference builds it with.  Like the reference, only the drawers whose get_opts() is None (vqgan, fast_pixel,
+super_resolution, vdiff) consult it; fft, pixel and line_sketch keep their own Adams.  An Adam session issues the same
+engine calls whether or not the option is given; another rule adds one set_optimizer per switch of the engine's rule.
 
 Perceptors are named in `clip_models`, as get_clip_perceptor keys on them (slip.py:173-186): the openai-CLIP ViTs
 (engine.CLIP_ARCH) and the SLIP_Base ViTs (engine.SLIP_ARCH: SLIP_VITB16, SLIP_CC3M, SLIP_CC12M, CLIP_VITB16,
@@ -115,7 +120,7 @@ _ENGINE_OPTIONS = [(("--b200_weights",), "b200_weights", None, None), (("--b200_
 _OFF_PATH = {
     "labels": ([],),
     "target_images": (None, []), "animation_dir": (None,),
-    "perceptors": ("clip",), "optimiser": ("Adam",), "make_video": (False,), "transparent": (False,),
+    "perceptors": ("clip",), "optimiser": tuple(E.OPTIMISERS), "make_video": (False,), "transparent": (False,),
     "image_prompt_shuffle": (False,),
 }
 
@@ -211,6 +216,9 @@ def _parse_palette(p):
 def process_args(vq_parser, namespace):
     """pixray.py:1824-1997 for the hot-path options: quality presets, size, unit strings, prompt splitting."""
     args = vq_parser.parse_args(args=[], namespace=namespace)
+    if args.optimiser == "AdamP":
+        raise NotImplementedError("optimiser 'AdamP' needs a per-slice projection of the update (AdamP's projection onto "
+                                  "the weight's tangent space), which is not built")
     for dest, off in _OFF_PATH.items():
         if getattr(args, dest, off[0]) not in off:
             raise NotImplementedError(f"setting '{dest}' leaves the per-iteration hot path this engine covers (SURVEY.md 8)")
@@ -639,12 +647,16 @@ def re_average_z(args):
 
 
 def rebuild_optimisers(args):
-    """pixray.py:520-555: a FRESH Adam at learning_rate / 10^drops (or the drawer's own rate, fftdrawer.py:63-67)."""
+    """pixray.py:520-555: a FRESH optimiser at learning_rate / 10^drops -- args.optimiser's rule -- or the drawer's own
+    Adam and rate (fftdrawer.py:63-67)."""
     st = _state
     drop_divisor = 10 ** st.num_loss_drop
     own = st.drawer.get_opts(drop_divisor)
     st.lr = own[0]["lr"] if own else args.learning_rate / drop_divisor
-    st.engine.reset_optimizer()
+    # the reference's PixelDrawer always builds its own Adam (pixeldrawer.py:311-317), also for the rect grid that runs
+    # as FastPixelDrawer here
+    consults = not own and args.drawer != "pixel"
+    st.session.use_optimizer(E.OPTIMISERS[args.optimiser] if consults else E.OPT_ADAM)
     return st.lr
 
 
@@ -689,7 +701,7 @@ def train(args, cur_it):
         lr = float(st.drawer.sigmas[cur_it] / st.drawer.alphas[cur_it])
         st.drawer.makenoise(cur_it)
         st.lr = min(lr * 0.001, 0.01)
-        st.engine.reset_optimizer()
+        st.session.use_optimizer(E.OPT_ADAM)  # optim.Adam whatever args.optimiser chose
     if cur_it == args.iterations:
         checkin(args, cur_it, st.losses)
         return False

@@ -51,6 +51,11 @@ class Engine {
   float* z_grad = nullptr;
   float *adam_m = nullptr, *adam_v = nullptr;
   int adam_t = 0;
+  // the optimiser's update rule (PXR_OPT_*); Adagrad keeps its sum in adam_v, Adamax its norm; DiffGrad's previous
+  // gradient lives in opt_p, allocated when DiffGrad is first chosen
+  int opt_kind = PXR_OPT_ADAM;
+  float* opt_p = nullptr;
+  void reset_opt_state();
   // device-side checkdrop / learning-rate drops / auto-stop (kernels.cuh): off until pxr_set_schedule
   bool managed = false;
   DropConfig drop_cfg{};
@@ -2263,8 +2268,8 @@ int Engine::clip_mode() const {
 void Engine::step(float lr) {
   ++adam_t;
   const int per_channel = (cfg.drawer == PXR_DRAWER_VQGAN) ? (int)(z_numel / cfg.z_channels) : 1;
-  adam_clip_step(z_buf, adam_m, adam_v, batches > 1 ? z_grad_acc : z_grad, 1.f, (int)z_numel, per_channel, zmin, zmax,
-                 clip_mode(), zr, lr, cfg.beta1, cfg.beta2, cfg.adam_eps, adam_t, st);
+  adam_clip_step(opt_kind, z_buf, adam_m, adam_v, opt_p, batches > 1 ? z_grad_acc : z_grad, 1.f, (int)z_numel, per_channel,
+                 zmin, zmax, clip_mode(), zr, lr, cfg.beta1, cfg.beta2, cfg.adam_eps, adam_t, st);
   launches += 1;
 }
 
@@ -2429,7 +2434,7 @@ void Engine::step_managed(int iter) {
   const float* g = batches > 1 ? z_grad_acc : z_grad;
   // the line drawer's get_z_copy is None (linedrawer.py:189-190): no best-z snapshot for it
   float* best = cfg.drawer == PXR_DRAWER_STROKES ? nullptr : best_z;
-  adam_clip_managed(z_buf, adam_m, adam_v, g, best, 1.f, (int)z_numel, per_channel, zmin, zmax,
+  adam_clip_managed(opt_kind, z_buf, adam_m, adam_v, opt_p, g, best, 1.f, (int)z_numel, per_channel, zmin, zmax,
                     clip_mode(), zr, cfg.beta1, cfg.beta2, cfg.adam_eps, losses_dev, num_losses(), iter,
                     drop_cfg, drop_state + drop_parity, drop_state + (drop_parity ^ 1), drop_status_dev, st);
   drop_parity ^= 1;
@@ -2979,6 +2984,7 @@ int pxr_set_schedule(pxr_handle h, float base_lr, int iter_drop_delay, int max_l
     e->managed = true;
     PXR_CUDA(cudaMemsetAsync(e->adam_m, 0, e->z_numel * sizeof(float), e->st));
     PXR_CUDA(cudaMemsetAsync(e->adam_v, 0, e->z_numel * sizeof(float), e->st));
+    if (e->opt_p) PXR_CUDA(cudaMemsetAsync(e->opt_p, 0, e->z_numel * sizeof(float), e->st));
     e->write_initial_drop_state();
   });
 }
@@ -3283,13 +3289,38 @@ int pxr_read_losses(pxr_handle h, float* out_host) {
   });
 }
 
-int pxr_reset_optimizer(pxr_handle h) {
+// a fresh instance of the current rule: state 0, t = 0; in managed mode the drop bookkeeping restarts too
+void Engine::reset_opt_state() {
+  PXR_CUDA(cudaMemsetAsync(adam_m, 0, z_numel * sizeof(float), st));
+  PXR_CUDA(cudaMemsetAsync(adam_v, 0, z_numel * sizeof(float), st));
+  if (opt_p) PXR_CUDA(cudaMemsetAsync(opt_p, 0, z_numel * sizeof(float), st));
+  adam_t = 0;
+  if (managed) write_initial_drop_state();  // a fresh session: best-loss tracking and the drop count restart too
+}
+
+int pxr_reset_optimizer(pxr_handle h) { PXR_TRY(h, h->e->reset_opt_state()); }
+
+namespace {
+const char* opt_name(int kind) {
+  static const char* names[] = {"Adam", "AdamW", "Adagrad", "Adamax", "DiffGrad"};
+  return kind >= 0 && kind < pxr::OPT_KINDS ? names[kind] : "unknown";
+}
+}  // namespace
+
+static_assert(PXR_OPT_ADAM == pxr::OPT_ADAM && PXR_OPT_ADAMW == pxr::OPT_ADAMW && PXR_OPT_ADAGRAD == pxr::OPT_ADAGRAD &&
+                  PXR_OPT_ADAMAX == pxr::OPT_ADAMAX && PXR_OPT_DIFFGRAD == pxr::OPT_DIFFGRAD,
+              "the kernels' rule codes are the ABI's");
+
+int pxr_set_optimizer(pxr_handle h, int kind) {
   PXR_TRY(h, {
     Engine* e = h->e;
-    PXR_CUDA(cudaMemsetAsync(e->adam_m, 0, e->z_numel * sizeof(float), e->st));
-    PXR_CUDA(cudaMemsetAsync(e->adam_v, 0, e->z_numel * sizeof(float), e->st));
-    e->adam_t = 0;
-    if (e->managed) e->write_initial_drop_state();  // a fresh session: best-loss tracking and the drop count restart too
+    if (!e->finalized) throw EngineError(-13, "call pxr_finalize first");
+    if (kind < 0 || kind >= pxr::OPT_KINDS)
+      throw EngineError(-93, "pxr_set_optimizer: unknown optimiser kind " + std::to_string(kind) +
+                                 " (PXR_OPT_ADAM .. PXR_OPT_DIFFGRAD)");
+    if (kind == PXR_OPT_DIFFGRAD && !e->opt_p) e->opt_p = e->dalloc<float>(e->z_numel);
+    e->opt_kind = kind;
+    e->reset_opt_state();
   });
 }
 
@@ -3302,21 +3333,32 @@ struct StateHeader {
   pxr::DropState drop;
 };
 constexpr uint32_t kStateMagic = 0x50585253u;  // "PXRS"
+// Version 1 (Adam): {header, z, m, v}.  Version 2 (every other rule): {header, kind, z, its two or three state arrays}.
+struct StateKind {
+  int32_t kind, pad;
+};
+int64_t state_payload_offset(int kind) { return (int64_t)sizeof(StateHeader) + (kind == PXR_OPT_ADAM ? 0 : (int64_t)sizeof(StateKind)); }
+std::vector<float*> state_arrays(Engine* e, int kind) {
+  std::vector<float*> a{e->z_buf, e->adam_m, e->adam_v};
+  if (kind == PXR_OPT_DIFFGRAD) a.push_back(e->opt_p);
+  return a;
+}
 }  // namespace
 
 int pxr_state_size(pxr_handle h, int64_t* nbytes) {
-  *nbytes = (int64_t)sizeof(StateHeader) + 3 * h->e->z_numel * (int64_t)sizeof(float);
+  const int kind = h->e->opt_kind;
+  *nbytes = state_payload_offset(kind) + (1 + pxr::opt_state_arrays(kind)) * h->e->z_numel * (int64_t)sizeof(float);
   return 0;
 }
 
-// host buffer of pxr_state_size bytes <- {header, z, m, v}.  Blocking.
+// host buffer of pxr_state_size bytes <- {header, [kind,] z, state arrays}.  Blocking.
 int pxr_save_state(pxr_handle h, void* host_buf) {
   PXR_TRY(h, {
     Engine* e = h->e;
     if (!host_buf) throw EngineError(-10, "pxr_save_state: null buffer");
     StateHeader hd{};
     hd.magic = kStateMagic;
-    hd.version = 1;
+    hd.version = e->opt_kind == PXR_OPT_ADAM ? 1 : 2;
     hd.z_numel = e->z_numel;
     hd.adam_t = e->adam_t;
     hd.managed = e->managed ? 1 : 0;
@@ -3325,11 +3367,16 @@ int pxr_save_state(pxr_handle h, void* host_buf) {
       PXR_CUDA(cudaMemcpyAsync(&hd.drop, e->drop_state + e->drop_parity, sizeof(pxr::DropState), cudaMemcpyDeviceToHost, e->st));
     char* out = static_cast<char*>(host_buf);
     const size_t zb = (size_t)e->z_numel * sizeof(float);
-    PXR_CUDA(cudaMemcpyAsync(out + sizeof hd, e->z_buf, zb, cudaMemcpyDeviceToHost, e->st));
-    PXR_CUDA(cudaMemcpyAsync(out + sizeof hd + zb, e->adam_m, zb, cudaMemcpyDeviceToHost, e->st));
-    PXR_CUDA(cudaMemcpyAsync(out + sizeof hd + 2 * zb, e->adam_v, zb, cudaMemcpyDeviceToHost, e->st));
+    char* payload = out + state_payload_offset(e->opt_kind);
+    const std::vector<float*> arrays = state_arrays(e, e->opt_kind);
+    for (size_t k = 0; k < arrays.size(); ++k)
+      PXR_CUDA(cudaMemcpyAsync(payload + k * zb, arrays[k], zb, cudaMemcpyDeviceToHost, e->st));
     PXR_CUDA(cudaStreamSynchronize(e->st));
     memcpy(out, &hd, sizeof hd);
+    if (hd.version == 2) {
+      const StateKind sk{e->opt_kind, 0};
+      memcpy(out + sizeof hd, &sk, sizeof sk);
+    }
   });
 }
 
@@ -3341,13 +3388,21 @@ int pxr_load_state(pxr_handle h, const void* host_buf) {
     if (!host_buf) throw EngineError(-10, "pxr_load_state: null buffer");
     StateHeader hd;
     memcpy(&hd, host_buf, sizeof hd);
-    if (hd.magic != kStateMagic || hd.version != 1) throw EngineError(-68, "pxr_load_state: not a pixray_b200 state blob");
+    if (hd.magic != kStateMagic || (hd.version != 1 && hd.version != 2))
+      throw EngineError(-68, "pxr_load_state: not a pixray_b200 state blob");
     if (hd.z_numel != e->z_numel) throw EngineError(-68, "pxr_load_state: the blob belongs to a different latent shape");
     const char* in = static_cast<const char*>(host_buf);
+    StateKind sk{PXR_OPT_ADAM, 0};
+    if (hd.version == 2) memcpy(&sk, in + sizeof hd, sizeof sk);
+    if (sk.kind == PXR_OPT_ADAM && hd.version == 2) throw EngineError(-68, "pxr_load_state: not a pixray_b200 state blob");
+    if (sk.kind != e->opt_kind)
+      throw EngineError(-68, std::string("pxr_load_state: the blob holds ") + opt_name(sk.kind) + " state, this session runs " +
+                                 opt_name(e->opt_kind) + " (pxr_set_optimizer)");
     const size_t zb = (size_t)e->z_numel * sizeof(float);
-    PXR_CUDA(cudaMemcpyAsync(e->z_buf, in + sizeof hd, zb, cudaMemcpyHostToDevice, e->st));
-    PXR_CUDA(cudaMemcpyAsync(e->adam_m, in + sizeof hd + zb, zb, cudaMemcpyHostToDevice, e->st));
-    PXR_CUDA(cudaMemcpyAsync(e->adam_v, in + sizeof hd + 2 * zb, zb, cudaMemcpyHostToDevice, e->st));
+    const char* payload = in + state_payload_offset(sk.kind);
+    const std::vector<float*> arrays = state_arrays(e, sk.kind);
+    for (size_t k = 0; k < arrays.size(); ++k)
+      PXR_CUDA(cudaMemcpyAsync(arrays[k], payload + k * zb, zb, cudaMemcpyHostToDevice, e->st));
     e->adam_t = hd.adam_t;
     if (hd.managed && e->managed) {
       PXR_CUDA(cudaMemcpyAsync(e->drop_state + e->drop_parity, &hd.drop, sizeof(pxr::DropState), cudaMemcpyHostToDevice, e->st));

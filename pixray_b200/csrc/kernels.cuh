@@ -329,15 +329,35 @@ __device__ __forceinline__ float clip_mode_apply(int clip_mode, int i, float zi,
   return zi;
 }
 #endif
-void adam_clip_step(float* z, float* m, float* v, const float* g, float inv_scale, int n, int per_channel,
-                    const float* zmin, const float* zmax, int clip_mode, const ZRanges& zr, float lr, float b1, float b2,
-                    float eps, int t, cudaStream_t st);
+// The update rule (PXR_OPT_* in include/pixray_b200.h, pixray.py:536-551), every one with pixray's constructor defaults
+// and the engine's betas / eps:
+//   ADAM      m, v            torch.optim.Adam
+//   ADAMW     m, v            torch.optim.AdamW, weight decay kAdamWDecay applied to z before the Adam step
+//   ADAGRAD   s (in v)        torch.optim.Adagrad, eps kAdagradEps, no lr decay, accumulator starts at 0
+//   ADAMAX    m, u (in v)     torch.optim.Adamax
+//   DIFFGRAD  m, v, p         torch_optimizer 0.1.0 DiffGrad: Adam moments times the friction 1 / (1 + exp(-|p - g|)),
+//                             p = the previous gradient; eps outside the bias correction
+// The step count t belongs to the current instance of the rule; a fresh instance has t = 0 and all state at 0.
+enum { OPT_ADAM = 0, OPT_ADAMW = 1, OPT_ADAGRAD = 2, OPT_ADAMAX = 3, OPT_DIFFGRAD = 4, OPT_KINDS = 5 };
+constexpr double kAdamWDecay = 0.01, kAdagradEps = 1e-10;
+// the learning-rate multiplier of step t: 1 / bc1 (Adam, AdamW, Adamax), sqrt(bc2) / bc1 (DiffGrad), 1 (Adagrad), as
+// step = lr * num / den in double
+__host__ __device__ inline double opt_step_size(int kind, double lr, double bc1, double bc2) {
+  if (kind == OPT_ADAGRAD) return lr;
+  if (kind == OPT_DIFFGRAD) return lr * sqrt(bc2) / bc1;
+  return lr / bc1;
+}
+inline int opt_state_arrays(int kind) { return kind == OPT_DIFFGRAD ? 3 : 2; }  // z-sized arrays besides z (Adagrad's m idle)
+// p: DiffGrad's previous gradient (nullptr for the other kinds)
+void adam_clip_step(int kind, float* z, float* m, float* v, float* p, const float* g, float inv_scale, int n,
+                    int per_channel, const float* zmin, const float* zmax, int clip_mode, const ZRanges& zr, float lr,
+                    float b1, float b2, float eps, int t, cudaStream_t st);
 
 // ------------------------------------------------------------------ device-side checkdrop + Adam (pixray.py:1090-1109, 1464-1512)
 // train()'s per-iteration control decisions without a host round trip.  The optimiser step of iteration `it` reads the
-// iteration's loss vector, decides like checkdrop / the scheduled learning-rate drops / auto_stop do, applies Adam + clip_z
-// with the CURRENT learning rate and Adam state, and -- when the decision is "rebuild the optimisers" -- leaves a fresh
-// Adam (m = v = 0, t = 0) at learning_rate / 10^num_loss_drop behind for the next iteration, or raises `stopped` when
+// iteration's loss vector, decides like checkdrop / the scheduled learning-rate drops / auto_stop do, applies the update
+// rule + clip_z with the CURRENT learning rate and optimiser state, and -- when the decision is "rebuild the optimisers" --
+// leaves a fresh instance of the rule (state 0, t = 0) at learning_rate / 10^num_loss_drop behind for the next iteration, or raises `stopped` when
 // the drops are used up (after which further iterations leave z untouched).  State is double-buffered (read cur, write
 // next) so every block of the kernel sees the same decision inputs.
 struct DropState {
@@ -346,7 +366,7 @@ struct DropState {
   int num_loss_drop;
   int stopped;
   float lr;
-  int adam_t;          // steps taken by the current Adam instance
+  int adam_t;          // steps taken by the current optimiser instance, whichever rule it runs
   int pad[2];
 };
 struct DropConfig {
@@ -369,7 +389,7 @@ struct DropStatus {
   float losses[64];
   volatile int seq_end;
 };
-void adam_clip_managed(float* z, float* m, float* v, const float* g, float* best_z, float inv_scale, int n,
+void adam_clip_managed(int kind, float* z, float* m, float* v, float* p, const float* g, float* best_z, float inv_scale, int n,
                        int per_channel, const float* zmin, const float* zmax, int clip_mode, const ZRanges& zr, float b1,
                        float b2, float eps, const float* losses, int n_losses, int iter, const DropConfig& cfg,
                        const DropState* cur, DropState* next, DropStatus* status_mapped, cudaStream_t st);

@@ -529,20 +529,80 @@ __global__ void __launch_bounds__(128) prompt_loss_kernel(const float* __restric
   }
 }
 
+// ---- the update rules (kernels.cuh OPT_*).  apply() reads element i's state, writes it back (0 when `fresh`: the managed
+// step's rebuild leaves a fresh instance behind) and returns z before clip_z.  `step` is the range's step size from
+// opt_step_size, `decay` AdamW's factor 1 - lr * kAdamWDecay.  The moment updates and Adam's denominator are written as
+// the fmaf contractions the Adam kernels have always evaluated, so Adam's bits do not depend on how the compiler contracts
+// them in each instance.
+struct OptHyper {
+  float b1, b2, eps, inv_sqrt_bc2;
+};
+struct OptAdam {
+  static constexpr int kind = OPT_ADAM;
+  static __device__ __forceinline__ float apply(const OptHyper& h, float step, float, int i, float z0, float gi, float* m,
+                                                float* v, float*, bool fresh) {
+    const float mi = fmaf(h.b1, m[i], (1.f - h.b1) * gi);
+    const float vi = fmaf(h.b2, v[i], (1.f - h.b2) * gi * gi);
+    m[i] = fresh ? 0.f : mi;
+    v[i] = fresh ? 0.f : vi;
+    const float denom = fmaf(sqrtf(vi), h.inv_sqrt_bc2, h.eps);
+    return z0 - step * mi / denom;
+  }
+};
+struct OptAdamW {
+  static constexpr int kind = OPT_ADAMW;
+  static __device__ __forceinline__ float apply(const OptHyper& h, float step, float decay, int i, float z0, float gi,
+                                                float* m, float* v, float* p, bool fresh) {
+    return OptAdam::apply(h, step, 0.f, i, z0 * decay, gi, m, v, p, fresh);
+  }
+};
+struct OptAdagrad {
+  static constexpr int kind = OPT_ADAGRAD;
+  static __device__ __forceinline__ float apply(const OptHyper&, float step, float, int i, float z0, float gi, float*,
+                                                float* s, float*, bool fresh) {
+    const float si = s[i] + gi * gi;
+    s[i] = fresh ? 0.f : si;
+    return z0 - step * gi / (sqrtf(si) + (float)kAdagradEps);
+  }
+};
+struct OptAdamax {
+  static constexpr int kind = OPT_ADAMAX;
+  static __device__ __forceinline__ float apply(const OptHyper& h, float step, float, int i, float z0, float gi, float* m,
+                                                float* u, float*, bool fresh) {
+    const float mi = fmaf(h.b1, m[i], (1.f - h.b1) * gi);
+    const float ui = fmaxf(h.b2 * u[i], fabsf(gi) + h.eps);
+    m[i] = fresh ? 0.f : mi;
+    u[i] = fresh ? 0.f : ui;
+    return z0 - step * mi / ui;
+  }
+};
+struct OptDiffGrad {
+  static constexpr int kind = OPT_DIFFGRAD;
+  static __device__ __forceinline__ float apply(const OptHyper& h, float step, float, int i, float z0, float gi, float* m,
+                                                float* v, float* p, bool fresh) {
+    const float mi = fmaf(h.b1, m[i], (1.f - h.b1) * gi);
+    const float vi = fmaf(h.b2, v[i], (1.f - h.b2) * gi * gi);
+    const float xi = 1.f / (1.f + expf(-fabsf(p[i] - gi)));
+    m[i] = fresh ? 0.f : mi;
+    v[i] = fresh ? 0.f : vi;
+    p[i] = fresh ? 0.f : gi;
+    return z0 - step * (mi * xi) / (sqrtf(vi) + h.eps);
+  }
+};
+
+template <class Rule>
 __global__ void adam_clip_kernel(float* __restrict__ z, float* __restrict__ m, float* __restrict__ v,
-                                 const float* __restrict__ g, float inv_scale, int n, int per_channel,
-                                 const float* __restrict__ zmin, const float* __restrict__ zmax, int clip_mode,
-                                 ZRanges zr, float step_size, float b1, float b2, float eps, float inv_sqrt_bc2) {
+                                 float* __restrict__ p, const float* __restrict__ g, float inv_scale, int n,
+                                 int per_channel, const float* __restrict__ zmin, const float* __restrict__ zmax,
+                                 int clip_mode, ZRanges zr, OptHyper h, float3 step_r, float3 decay_r) {
   pdl_prologue();
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   float gi = g[i] * inv_scale;
-  float mi = b1 * m[i] + (1.f - b1) * gi;
-  float vi = b2 * v[i] + (1.f - b2) * gi * gi;
-  m[i] = mi;
-  v[i] = vi;
-  float denom = sqrtf(vi) * inv_sqrt_bc2 + eps;
-  float zi = z[i] - step_size * zr.scale[zrange_of(zr, i)] * mi / denom;
+  const int r = zrange_of(zr, i);
+  const float step = r == 0 ? step_r.x : r == 1 ? step_r.y : step_r.z;
+  const float decay = r == 0 ? decay_r.x : r == 1 ? decay_r.y : decay_r.z;
+  float zi = Rule::apply(h, step, decay, i, z[i], gi, m, v, p, false);
   if (zmin) {
     int c = i / per_channel;
     zi = fminf(fmaxf(zi, zmin[c]), zmax[c]);  // vqgan.py:202-204
@@ -553,11 +613,12 @@ __global__ void adam_clip_kernel(float* __restrict__ z, float* __restrict__ m, f
 }
 
 // see kernels.cuh "device-side checkdrop + Adam"
+template <class Rule>
 __global__ void adam_clip_managed_kernel(float* __restrict__ z, float* __restrict__ m, float* __restrict__ v,
-                                         const float* __restrict__ g, float* __restrict__ best_z, float inv_scale, int n,
-                                         int per_channel, const float* __restrict__ zmin, const float* __restrict__ zmax,
-                                         int clip_mode, ZRanges zr, float b1, float b2, float eps,
-                                         const float* __restrict__ losses,
+                                         float* __restrict__ p, const float* __restrict__ g, float* __restrict__ best_z,
+                                         float inv_scale, int n, int per_channel, const float* __restrict__ zmin,
+                                         const float* __restrict__ zmax, int clip_mode, ZRanges zr, float b1,
+                                         float b2, float eps, const float* __restrict__ losses,
                                          int n_losses, int iter, DropConfig cfg, const DropState* __restrict__ cur,
                                          DropState* __restrict__ next, DropStatus* status) {
   pdl_prologue();
@@ -588,9 +649,13 @@ __global__ void adam_clip_managed_kernel(float* __restrict__ z, float* __restric
     // torch.optim.Adam: step_size = lr / (1 - b1^t); denom = sqrt(v) / sqrt(1 - b2^t) + eps
     const double bc1 = 1.0 - pow((double)b1, (double)t), bc2 = 1.0 - pow((double)b2, (double)t);
     // one step size per z range (scale 1 everywhere except the line drawer's widths and paper colour)
-    float step_r[3];
-    for (int r = 0; r < 3; ++r) step_r[r] = (float)((double)s.lr * (double)zr.scale[r] / bc1);
-    const float inv_sqrt_bc2 = (float)(1.0 / sqrt(bc2));
+    float step_r[3], decay_r[3];
+    for (int r = 0; r < 3; ++r) {
+      const double lr_r = (double)s.lr * (double)zr.scale[r];
+      step_r[r] = (float)opt_step_size(Rule::kind, lr_r, bc1, bc2);
+      decay_r[r] = (float)(1.0 - lr_r * kAdamWDecay);
+    }
+    const OptHyper h{b1, b2, eps, (float)(1.0 / sqrt(bc2))};
     if (rebuild) {
       nx.num_loss_drop = s.num_loss_drop + 1;
       if (nx.num_loss_drop > cfg.max_loss_drops) {
@@ -607,12 +672,8 @@ __global__ void adam_clip_managed_kernel(float* __restrict__ z, float* __restric
       const float z0 = z[i];
       if (new_best && best_z) best_z[i] = z0;  // best_z = drawer.get_z_copy() (pixray.py:1104): z BEFORE this step
       const float gi = g[i] * inv_scale;
-      const float mi = b1 * m[i] + (1.f - b1) * gi;
-      const float vi = b2 * v[i] + (1.f - b2) * gi * gi;
-      m[i] = fresh ? 0.f : mi;
-      v[i] = fresh ? 0.f : vi;
-      const float denom = sqrtf(vi) * inv_sqrt_bc2 + eps;
-      float zi = z0 - step_r[zrange_of(zr, i)] * mi / denom;
+      const int r = zrange_of(zr, i);
+      float zi = Rule::apply(h, step_r[r], decay_r[r], i, z0, gi, m, v, p, fresh);
       if (zmin) {
         const int c = i / per_channel;
         zi = fminf(fmaxf(zi, zmin[c]), zmax[c]);
@@ -819,23 +880,45 @@ void prompt_loss(const float* e, int B, int D, const float* prompts, const float
                                                            1.f / cutn_global, grad_scale, e_unit, losses, de, de16);
 }
 
-void adam_clip_step(float* z, float* m, float* v, const float* g, float inv_scale, int n, int per_channel,
-                    const float* zmin, const float* zmax, int clip_mode, const ZRanges& zr, float lr, float b1, float b2,
-                    float eps, int t, cudaStream_t st) {
-  // torch.optim.Adam: step_size = lr / (1 - b1^t); denom = sqrt(v) / sqrt(1 - b2^t) + eps
-  const double bc1 = 1.0 - pow((double)b1, t), bc2 = 1.0 - pow((double)b2, t);
-  launch_pdl(adam_clip_kernel, dim3((n + 255) / 256), dim3(256), 0, st, z, m, v, g, inv_scale, n, per_channel, zmin, zmax, clip_mode, zr,
-                                                    (float)(lr / bc1), b1, b2, eps, (float)(1.0 / sqrt(bc2)));
+// calls f(Rule{}) with the functor of `kind`
+template <class F>
+void with_opt_rule(int kind, F&& f) {
+  switch (kind) {
+    case OPT_ADAM: f(OptAdam{}); break;
+    case OPT_ADAMW: f(OptAdamW{}); break;
+    case OPT_ADAGRAD: f(OptAdagrad{}); break;
+    case OPT_ADAMAX: f(OptAdamax{}); break;
+    case OPT_DIFFGRAD: f(OptDiffGrad{}); break;
+  }
 }
 
-void adam_clip_managed(float* z, float* m, float* v, const float* g, float* best_z, float inv_scale, int n,
+void adam_clip_step(int kind, float* z, float* m, float* v, float* p, const float* g, float inv_scale, int n,
+                    int per_channel, const float* zmin, const float* zmax, int clip_mode, const ZRanges& zr, float lr,
+                    float b1, float b2, float eps, int t, cudaStream_t st) {
+  // torch.optim.Adam: step_size = lr / (1 - b1^t); denom = sqrt(v) / sqrt(1 - b2^t) + eps
+  const double bc1 = 1.0 - pow((double)b1, t), bc2 = 1.0 - pow((double)b2, t);
+  // the step size converts to float once; its per-range multiple is a float product (scale 1 for all but the line drawer)
+  const float step = (float)opt_step_size(kind, lr, bc1, bc2);
+  const float3 step_r = make_float3(step * zr.scale[0], step * zr.scale[1], step * zr.scale[2]);
+  float decay[3];
+  for (int r = 0; r < 3; ++r) decay[r] = (float)(1.0 - (double)lr * (double)zr.scale[r] * kAdamWDecay);
+  const OptHyper h{b1, b2, eps, (float)(1.0 / sqrt(bc2))};
+  with_opt_rule(kind, [&](auto rule) {
+    launch_pdl(adam_clip_kernel<decltype(rule)>, dim3((n + 255) / 256), dim3(256), 0, st, z, m, v, p, g, inv_scale, n,
+               per_channel, zmin, zmax, clip_mode, zr, h, step_r, make_float3(decay[0], decay[1], decay[2]));
+  });
+}
+
+void adam_clip_managed(int kind, float* z, float* m, float* v, float* p, const float* g, float* best_z, float inv_scale, int n,
                        int per_channel, const float* zmin, const float* zmax, int clip_mode, const ZRanges& zr, float b1,
                        float b2, float eps, const float* losses, int n_losses, int iter, const DropConfig& cfg,
                        const DropState* cur, DropState* next, DropStatus* status_mapped, cudaStream_t st) {
   int grid = (n + 255) / 256;
   if (grid > 148 * 4) grid = 148 * 4;
-  launch_pdl(adam_clip_managed_kernel, dim3(grid), dim3(256), 0, st, z, m, v, g, best_z, inv_scale, n, per_channel, zmin,
-             zmax, clip_mode, zr, b1, b2, eps, losses, n_losses, iter, cfg, cur, next, status_mapped);
+  with_opt_rule(kind, [&](auto rule) {
+    launch_pdl(adam_clip_managed_kernel<decltype(rule)>, dim3(grid), dim3(256), 0, st, z, m, v, p, g, best_z, inv_scale, n,
+               per_channel, zmin, zmax, clip_mode, zr, b1, b2, eps, losses, n_losses, iter, cfg, cur, next, status_mapped);
+  });
 }
 
 void accumulate_f32(const float* g, float* acc, long long n, int accumulate, cudaStream_t st) {

@@ -16,6 +16,9 @@ ANCHOR_SPHERICAL, ANCHOR_MSE, ANCHOR_COS, ANCHOR_PIX = 0, 1, 2, 3
 FILTER_TILER, FILTER_WALLPAPER, FILTER_LOOKUP = range(3)
 PAD_REFLECTION, PAD_BORDER = 0, 1
 MOD_VQGAN, MOD_CLIP0, MOD_CLIP1 = 0, 1, 2
+# optimiser update rules (pxr_set_optimizer), by the reference's args.optimiser names (pixray.py:536-551)
+OPT_ADAM, OPT_ADAMW, OPT_ADAGRAD, OPT_ADAMAX, OPT_DIFFGRAD = range(5)
+OPTIMISERS = {"Adam": OPT_ADAM, "AdamW": OPT_ADAMW, "Adagrad": OPT_ADAGRAD, "Adamax": OPT_ADAMAX, "DiffGrad": OPT_DIFFGRAD}
 
 # RRDBNet of RealESRGAN_x4plus (super_resolution.py:53): RRDBNet(3, 3, num_feat=64, num_block=23, num_grow_ch=32, scale=4)
 RRDBNET_X4PLUS = dict(num_feat=64, num_block=23, num_grow_ch=32)
@@ -467,8 +470,12 @@ class B200Engine:
     def reset_optimizer(self):
         self._check(self.lib.pxr_reset_optimizer(self.h), "pxr_reset_optimizer")
 
+    def set_optimizer(self, kind):
+        """Switch the update rule to `kind` (OPT_*) with fresh state, as reset_optimizer leaves it (pxr_set_optimizer)."""
+        self._check(self.lib.pxr_set_optimizer(self.h, int(kind)), "pxr_set_optimizer")
+
     def save_state(self):
-        """bytes: z, Adam m / v / step and the drop bookkeeping (pxr_save_state)."""
+        """bytes: z, the optimiser's state and step count, and the drop bookkeeping (pxr_save_state)."""
         n = C.c_int64()
         self.lib.pxr_state_size(self.h, C.byref(n))
         buf = (C.c_ubyte * n.value)()

@@ -49,6 +49,16 @@ class Session:
         self.global_padding_mode = "reflection"
         self.global_fill_color = 0.0
         self.last_embeds = {}  # clip_idx -> the tensor Perceptor.encode_image handed out this iteration
+        self.opt_kind = E.OPT_ADAM  # the engine's optimiser update rule
+
+    def use_optimizer(self, kind):
+        """A fresh optimiser of update rule `kind` (E.OPT_*) on z, as rebuild_optimisers builds one: reset_optimizer when
+        the engine already runs that rule (an Adam-only session never issues anything else), set_optimizer otherwise."""
+        if kind == self.opt_kind:
+            self.engine.reset_optimizer()
+        else:
+            self.engine.set_optimizer(kind)
+            self.opt_kind = kind
 
     def begin_iteration(self, cur_iteration, fill=None, rng=None):
         self.cur_iteration = cur_iteration
@@ -754,11 +764,15 @@ from .util import get_learning_rate_drops  # noqa: E402,F401  (pixray.py:1999-20
 
 
 class Optimizer:
-    """optim.Adam([drawer.get_z()], lr) as rebuild_optimisers builds it (pixray.py:520-555): zero_grad / step."""
+    """optim.<name>([drawer.get_z()], lr) as rebuild_optimisers builds it (pixray.py:520-555): zero_grad / step.  name is
+    one of the reference's args.optimiser values the engine runs (E.OPTIMISERS: Adam, AdamW, Adagrad, Adamax,
+    DiffGrad), each with its constructor defaults."""
 
-    def __init__(self, session: Session, drawer, lr):
+    def __init__(self, session: Session, drawer, lr, name="Adam"):
+        if name not in E.OPTIMISERS:
+            raise NotImplementedError(f"optimiser {name!r} is not built; available: {sorted(E.OPTIMISERS)}")
         self.session, self.drawer, self.lr = session, drawer, lr
-        session.engine.reset_optimizer()
+        session.use_optimizer(E.OPTIMISERS[name])
 
     def zero_grad(self):
         z = self.drawer.get_z()
@@ -787,10 +801,11 @@ def train_iteration(session: Session, drawer, make_cutouts, perceptors, prompt_t
     opt.step()
     drawer.clip_z()
     if isinstance(drawer, VdiffDrawer) and session.cur_iteration >= 1:
-        # pixray.py:1489-1495: re-noise x for the next timestep and start a fresh Adam with the schedule's step size
+        # pixray.py:1489-1495: re-noise x for the next timestep and start a fresh Adam (whatever args.optimiser chose)
+        # with the schedule's step size
         it = session.cur_iteration
         lr = float(drawer.sigmas[it] / drawer.alphas[it])
         drawer.makenoise(it)
         opt.lr = min(lr * 0.001, 0.01)
-        session.engine.reset_optimizer()
+        session.use_optimizer(E.OPT_ADAM)
     return result
