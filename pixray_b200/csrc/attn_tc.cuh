@@ -1,14 +1,16 @@
 // Fused multi-head self-attention of the CLIP ViT (nn.MultiheadAttention inside SLIP/models.py:18-64 residual blocks;
-// openai-CLIP VisionTransformer) and of the v-diffusion U-Net for sm_90a: one kernel for the forward, two for the
-// backward, all on the tensor cores (warp-level mma.sync m16n8k16, fp16 operands, fp32 accumulators in registers).
+// openai-CLIP VisionTransformer) and of the v-diffusion U-Net for sm_90a: one kernel for the forward, one for the
+// backward, both on the tensor cores (warp-level mma.sync m16n8k16, fp16 operands, fp32 accumulators in registers).
 // Replaces, per layer, {QK^T GEMM, softmax, PV GEMM} and {dP GEMM, softmax backward, dQ / dK / dV GEMMs} of the unfused
 // path (which stays for sequences longer than 240 tokens).
 //
-// Flash-attention style: a CTA owns 64 query rows (forward, dQ) or 64 key rows (dK / dV) of one (image, head) pair and
-// stages that pair's K, V (or Q, dO) in shared memory; the scores of a warp's 16 rows live in registers and are never
-// written to memory.  Forward keeps only the row log-sum-exp; backward recomputes P = exp(S - lse) from Q, K and uses
-// D_i = dO_i . O_i for the softmax backward.  Every output element is written by exactly one thread (no atomics), so
-// results are deterministic.
+// Flash-attention style: a CTA owns one (image, head) pair -- or, with fewer pairs than SMs, a share of the pair's
+// 16-row tiles -- and stages the pair's Q, K, V (backward: and dO) once in shared memory with cp.async; ldmatrix feeds
+// the MMAs, .trans where an operand is needed transposed.  The scores of a warp's 16 rows live in registers and are never
+// written to memory.  T is rounded up to 16, not further: key chunks and query tiles past T do no MMA work.  Forward
+// keeps only the row log-sum-exp; backward recomputes P = exp(S - lse) from Q, K, takes D_i = dO_i . O_i once per row,
+// and accumulates dK / dV over key tiles, then dQ over query tiles, in the same kernel.  Every output element is written
+// by exactly one thread (no atomics), so results are deterministic.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -29,7 +31,8 @@ struct AttnParams {
 
 struct AttnPlan {
   AttnParams p;
-  int smem_fwd = 0, smem_dq = 0, smem_dkv = 0;
+  int splits = 1;  // CTAs per (image, head) pair
+  int smem_fwd = 0, smem_bwd = 0;
   double flops_fwd = 0, flops_bwd = 0;
   double bytes_fwd = 0, bytes_bwd = 0;  // compulsory traffic: qkv in, o out (+ lse) / qkv, o, dO in, dqkv out
 };

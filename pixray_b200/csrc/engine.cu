@@ -1004,7 +1004,7 @@ act_t* Engine::add_attention(OpList& fwd, OpList* bwd, const act_t* qkv, act_t* 
     fwd.add(1, [ap, cs] { attn_forward_launch(*ap, cs); }, ap->flops_fwd, lab, ap->bytes_fwd);
     if (bwd) {  // dQ, dK, dV in one kernel (recomputes P from Q, K and the saved log-sum-exp)
       snprintf(lab, sizeof lab, "attn_bwd B=%d T=%d heads=%d", images, T, heads);
-      bwd->add(2, [ap, cs] { attn_backward_launch(*ap, cs); }, ap->flops_bwd, lab, ap->bytes_bwd);
+      bwd->add(1, [ap, cs] { attn_backward_launch(*ap, cs); }, ap->flops_bwd, lab, ap->bytes_bwd);
     }
     return nullptr;
   }
