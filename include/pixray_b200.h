@@ -194,8 +194,12 @@ int pxr_iterate(pxr_handle h, float* z, float lr, int iter, const pxr_cut_params
  *   SYMMETRY   {symmetry_weight}                                            Losses/SymmetryLoss.py:14-17   (image)
  *   SATURATION {saturation_weight}                                          Losses/SaturationLoss.py:15-30 (cutouts)
  *   PALETTE    {palette_weight, r0,g0,b0, r1,g1,b1, ...}  colours in [0,1]  Losses/PaletteLoss.py:25-35    (cutouts)
- *   SMOOTHNESS {smoothness_weight, type (0 default, 1 clipped, 2 log), spacing}   Losses/SmoothnessLoss.py:89-108
- *   EDGE       {edge_color_weight, global_color_weight, left,right,upper,lower (pixels), r,g,b}  Losses/EdgeLoss.py:60-108
+ *   SMOOTHNESS {smoothness_weight, type (0 default, 1 clipped, 2 log), spacing[, edge_order (1|2)[, n, taps[n*n]]]}
+ *              Losses/SmoothnessLoss.py:9-108 (cutouts).  n > 0: GaussianSmoothing's normalised 2-D kernel (row-major,
+ *              separable), a valid blur before torch.gradient; cut_size - n + 1 must be >= edge_order + 1.
+ *   EDGE       {edge_color_weight, global_color_weight, left,right,upper,lower (pixels), r,g,b[, mode,
+ *              target[3*H*W] if mode & 1, mask[H*W] if mode & 2]}  Losses/EdgeLoss.py:60-108 (image).  The target
+ *              replaces the colour; the mask (> 0: masked) replaces the margins.  H, W: the canvas.
  *   GAUSSIAN   {gaussian_weight, std_y, std_x, R,G,B (0..255)}              Losses/GaussianLoss.py:31-44   (image)
  *   AESTHETIC  {aesthetic_target, bias, w[D]}  linear head on the last perceptor's embeddings  Losses/AestheticLoss.py:30-33 */
 enum { PXR_LOSS_SYMMETRY = 0, PXR_LOSS_SATURATION = 1, PXR_LOSS_PALETTE = 2, PXR_LOSS_SMOOTHNESS = 3, PXR_LOSS_EDGE = 4,

@@ -217,7 +217,7 @@ class Engine {
     int kind;
     float weight;
     std::vector<float> prm;
-    float* dev = nullptr;  // palette colours / aesthetic head weights
+    float* dev = nullptr;  // palette colours / aesthetic head weights / smoothness blur taps / edge target, then mask
     int n_dev = 0;
   };
   std::vector<AuxLoss> aux;
@@ -226,6 +226,9 @@ class Engine {
   float* aux_A = nullptr;       // smoothness per-pixel factor
   float* aux_halo = nullptr;    // smoothness rows of the neighbouring ranks
   float* aux_xbuf = nullptr;    // smoothness halo exchange buffer
+  float* aux_blur = nullptr;    // smoothness_gaussian_kernel: blurred batch, its gradient, the one-axis scratch
+  float* aux_g_blur = nullptr;  //   (allocated when the first blurred smoothness loss is added, [n_local, 3, cs, cs] each)
+  float* aux_blur_tmp = nullptr;
   int* aux_best = nullptr;      // palette argmin per pixel (bookkeeping, also a debug buffer)
   // ---- anchors to a stored copy (pixray.py:1344-1375): loss-vector entries between the prompts and the auxiliary losses
   struct Anchor {
@@ -2092,16 +2095,30 @@ void Engine::aux_on_cutouts() {
       aux_palette(batch, n_local, cs_, cfg.cutn, a.dev, a.n_dev / 3, a.weight * a.prm[0], S, g_batch, aux_best, aux_part, slot, st);
       launches += 2;
     } else if (a.kind == PXR_LOSS_SMOOTHNESS) {
+      // {w, type, spacing[, edge_order[, n, taps]]}: a.dev holds the n 1-D taps of the blur when n > 0
+      const int order = a.prm.size() > 3 ? (int)a.prm[3] : 1, nt = a.dev ? a.n_dev : 0;
+      const float* src = batch;
+      int cs2 = cs_;
+      if (nt) {  // the gradient runs on the blurred cutouts (SmoothnessLoss.py:92-94)
+        cs2 = cs_ - nt + 1;
+        aux_smooth_blur(batch, n_local, cs_, a.dev, nt, aux_blur_tmp, aux_blur, st);
+        src = aux_blur;
+        launches += 2;
+      }
       if (comm) {  // torch.gradient runs over the stacked rows of ALL cutouts: two halo rows from each neighbour
-        PXR_CUDA(cudaMemsetAsync(aux_xbuf, 0, sizeof(float) * 12 * cs_ * cfg.world, st));
-        aux_smooth_pack_halo(batch, n_local, cs_, cfg.rank, aux_xbuf, st);
-        nccl_check(Comm::api().all_reduce(aux_xbuf, aux_xbuf, (size_t)12 * cs_ * cfg.world, Comm::kFloat32, Comm::kSum, comm, st), "allreduce(smoothness halo)");
-        aux_smooth_unpack_halo(aux_xbuf, cs_, cfg.rank, cfg.world, aux_halo, st);
+        PXR_CUDA(cudaMemsetAsync(aux_xbuf, 0, sizeof(float) * 12 * cs2 * cfg.world, st));
+        aux_smooth_pack_halo(src, n_local, cs2, cfg.rank, aux_xbuf, st);
+        nccl_check(Comm::api().all_reduce(aux_xbuf, aux_xbuf, (size_t)12 * cs2 * cfg.world, Comm::kFloat32, Comm::kSum, comm, st), "allreduce(smoothness halo)");
+        aux_smooth_unpack_halo(aux_xbuf, cs2, cfg.rank, cfg.world, aux_halo, st);
         launches += 3;
       }
-      aux_smoothness(batch, n_local, cs_, first_global, cfg.cutn, aux_halo, a.prm[2], (int)a.prm[1], a.weight * a.prm[0], S,
-                     aux_A, g_batch, aux_part, slot, st);
+      aux_smoothness(src, n_local, cs2, first_global, cfg.cutn, aux_halo, a.prm[2], (int)a.prm[1], order,
+                     a.weight * a.prm[0], S, aux_A, nt ? aux_g_blur : g_batch, nt ? 0 : 1, aux_part, slot, st);
       launches += 3;
+      if (nt) {
+        aux_smooth_blur_adjoint(aux_g_blur, n_local, cs_, a.dev, nt, aux_blur_tmp, g_batch, st);
+        launches += 2;
+      }
     }
   }
 }
@@ -2118,7 +2135,12 @@ void Engine::aux_on_image() {
       launches += 2;
     } else if (a.kind == PXR_LOSS_EDGE) {
       const int m[4] = {(int)a.prm[2], (int)a.prm[3], (int)a.prm[4], (int)a.prm[5]};
-      aux_edge(img, H, Wd, m, &a.prm[6], a.prm[0], a.prm[1], a.weight, S, g_img, aux_part, slot, st);
+      const int mode = a.prm.size() > 9 ? (int)a.prm[9] : 0;
+      if (mode && (H != cfg.image_h || Wd != cfg.image_w))
+        throw EngineError(-81, "edge loss target / mask were sized for the canvas, the image the loss reads differs");
+      const float* target = (mode & 1) ? a.dev : nullptr;
+      const float* mask = (mode & 2) ? a.dev + ((mode & 1) ? 3 * (size_t)H * Wd : 0) : nullptr;
+      aux_edge(img, H, Wd, m, &a.prm[6], target, mask, a.prm[0], a.prm[1], a.weight, S, g_img, aux_part, slot, st);
       launches += 2;
     } else if (a.kind == PXR_LOSS_GAUSSIAN) {
       aux_gaussian(img, H, Wd, a.prm[1], a.prm[2], &a.prm[3], a.weight * a.prm[0], S, g_img, aux_part, slot, st);
@@ -3167,11 +3189,69 @@ int pxr_add_aux_loss(pxr_handle h, int kind, float weight, const float* params, 
         a.dev = e->upload(std::vector<float>(params + 1, params + n_params));
         a.n_dev = n_params - 1;
         break;
-      case PXR_LOSS_SMOOTHNESS:
-        need(3, "smoothness needs {smoothness_weight, type, spacing}");
+      case PXR_LOSS_SMOOTHNESS: {
+        need(3, "smoothness needs {smoothness_weight, type, spacing[, edge_order[, n, taps[n * n]]]}");
         if (params[1] < 0 || params[1] > 2 || params[2] <= 0) throw EngineError(-80, "pxr_add_aux_loss: smoothness type in {0,1,2}, spacing > 0");
+        const int order = n_params > 3 ? (int)params[3] : 1;
+        if (n_params > 3 && params[3] != 1.f && params[3] != 2.f)
+          throw EngineError(-80, "pxr_add_aux_loss: smoothness edge_order must be 1 or 2 (torch.gradient)");
+        const float nf = n_params > 4 ? params[4] : 0.f;
+        if (nf < 0 || nf != std::floor(nf) || nf > 1024)
+          throw EngineError(-80, "pxr_add_aux_loss: smoothness blur tap count must be an integer in [0, 1024] (kernel size >= 0)");
+        const int n = (int)nf;
+        if (n_params != (n_params > 4 ? 5 + n * n : n_params))
+          throw EngineError(-80, "pxr_add_aux_loss: smoothness blur needs n * n taps after n");
+        const int cs2 = e->cfg.cut_size - (n ? n - 1 : 0);
+        if (cs2 < order + 1)
+          throw EngineError(-80, "pxr_add_aux_loss: smoothness blur leaves " + std::to_string(cs2) + " pixels per cutout side; "
+                                 "torch.gradient with edge_order " + std::to_string(order) + " needs at least " +
+                                 std::to_string(order + 1));
+        if (n) {
+          // GaussianSmoothing's kernel is u (x) u with sum(u) = 1: apply it as two 1-D passes of the row sums
+          const float* K = params + 5;
+          std::vector<double> u(n, 0.0);
+          double kmax = 0.0, total = 0.0;
+          for (int i = 0; i < n * n; ++i) {
+            if (!std::isfinite(K[i]) || K[i] < 0.f)
+              throw EngineError(-80, "pxr_add_aux_loss: smoothness blur taps must be finite and >= 0 (std > 0)");
+            u[i / n] += K[i];
+            kmax = std::max(kmax, (double)K[i]);
+            total += K[i];
+          }
+          if (!(std::fabs(total - 1.0) <= 1e-4))
+            throw EngineError(-80, "pxr_add_aux_loss: smoothness blur taps must sum to 1");
+          for (int i = 0; i < n * n; ++i)
+            if (std::fabs(K[i] - u[i / n] * u[i % n]) > 1e-5 * kmax)
+              throw EngineError(-80, "pxr_add_aux_loss: smoothness blur taps must be separable (an outer product u u^T)");
+          a.dev = e->upload(std::vector<float>(u.begin(), u.end()));
+          a.n_dev = n;
+          if (!e->aux_blur) {
+            const size_t sz = (size_t)e->n_local * 3 * e->cfg.cut_size * e->cfg.cut_size;
+            e->aux_blur = e->dalloc<float>(sz);
+            e->aux_g_blur = e->dalloc<float>(sz);
+            e->aux_blur_tmp = e->dalloc<float>(sz);
+          }
+        }
         break;
-      case PXR_LOSS_EDGE: need(9, "edge needs {edge_color_weight, global_color_weight, left,right,upper,lower, r,g,b}"); break;
+      }
+      case PXR_LOSS_EDGE: {
+        need(9, "edge needs {edge_color_weight, global_color_weight, left,right,upper,lower, r,g,b[, mode, target, mask]}");
+        const int mode = n_params > 9 ? (int)params[9] : 0;
+        if (n_params > 9 && (params[9] != (float)mode || mode < 0 || mode > 3))
+          throw EngineError(-80, "pxr_add_aux_loss: edge mode is 0 (colour), 1 (target image), 2 (mask) or 3 (both)");
+        const size_t hw = (size_t)e->cfg.image_h * e->cfg.image_w;
+        const size_t extra = ((mode & 1) ? 3 * hw : 0) + ((mode & 2) ? hw : 0);
+        if (n_params > 9 && (size_t)n_params != 10 + extra)
+          throw EngineError(-80, "pxr_add_aux_loss: edge target must be [3, " + std::to_string(e->cfg.image_h) + ", " +
+                                 std::to_string(e->cfg.image_w) + "] and mask [" + std::to_string(e->cfg.image_h) + ", " +
+                                 std::to_string(e->cfg.image_w) + "] floats (the image the loss reads)");
+        if (extra) {
+          a.dev = e->upload(std::vector<float>(params + 10, params + n_params));
+          a.n_dev = (int)extra;
+          a.prm.resize(10);  // the arrays live on the device
+        }
+        break;
+      }
       case PXR_LOSS_GAUSSIAN:
         need(6, "gaussian needs {gaussian_weight, std_y, std_x, R,G,B}");
         if (params[1] <= 0 || params[2] <= 0) throw EngineError(-80, "pxr_add_aux_loss: gaussian std must be positive");

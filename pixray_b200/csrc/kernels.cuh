@@ -410,10 +410,11 @@ void anchor_pix(const float* img, const float* ref, long long n, float weight, f
                 float* loss_out, cudaStream_t st);
 void aux_symmetry(const float* img, int H, int W, float weight, float grad_scale, float* g_img, double* part,
                   float* loss_out, cudaStream_t st);
-// margins = (left, right, upper, lower) in pixels (EdgeLoss.py:82-88), colour in [0,1]
-void aux_edge(const float* img, int H, int W, const int margins[4], const float color[3], float edge_color_weight,
-              float global_color_weight, float weight, float grad_scale, float* g_img, double* part, float* loss_out,
-              cudaStream_t st);
+// margins = (left, right, upper, lower) in pixels (EdgeLoss.py:82-88), colour in [0,1]; target [3, H, W] replaces the
+// colour and mask [H, W] (> 0: masked) replaces the margins when not null
+void aux_edge(const float* img, int H, int W, const int margins[4], const float color[3], const float* target,
+              const float* mask, float edge_color_weight, float global_color_weight, float weight, float grad_scale,
+              float* g_img, double* part, float* loss_out, cudaStream_t st);
 void aux_gaussian(const float* img, int H, int W, float stdy, float stdx, const float color255[3], float weight,
                   float grad_scale, float* g_img, double* part, float* loss_out, cudaStream_t st);
 // best_out (optional): nearest-palette index per pixel [n_img * cs * cs] (the loss's integer bookkeeping)
@@ -424,10 +425,17 @@ void aux_palette(const float* batch, int n_img, int cs, int cutn_global, const f
 void aux_saturation_moments(const float* batch, int n_img, int cs, double* part, double* sums, cudaStream_t st);
 void aux_saturation_grad(const float* batch, int n_img, int cs, int cutn_global, const double* sums, float weight,
                          float grad_scale, int write_loss, float* g_batch, float* loss_out, cudaStream_t st);
-// A: scratch [(n_img * cs + 2) * cs] floats; halo: [2][2][3][cs] rows around this rank's slab (unused when world == 1)
+// A: scratch [(n_img * cs + 2) * cs] floats; halo: [2][2][3][cs] rows around this rank's slab (unused when world == 1).
+// accumulate = 0 stores the gradient instead of adding it (the blurred path's scratch).
 void aux_smoothness(const float* batch, int n_img, int cs, int first_global, int cutn_global, const float* halo,
-                    float spacing, int kind, float weight, float grad_scale, float* A, float* g_batch, double* part,
-                    float* loss_out, cudaStream_t st);
+                    float spacing, int kind, int edge_order, float weight, float grad_scale, float* A, float* g_batch,
+                    int accumulate, double* part, float* loss_out, cudaStream_t st);
+// smoothness_gaussian_kernel: the valid blur of [n_img, 3, cs, cs] by the separable taps u (x) u (n each) into
+// out [n_img, 3, cs', cs'], cs' = cs - n + 1, and its adjoint added into g_batch.  tmp: [n_img, 3, cs, cs'] scratch.
+void aux_smooth_blur(const float* batch, int n_img, int cs, const float* taps, int n, float* tmp, float* out,
+                     cudaStream_t st);
+void aux_smooth_blur_adjoint(const float* g_out, int n_img, int cs, const float* taps, int n, float* tmp, float* g_batch,
+                             cudaStream_t st);
 void aux_smooth_pack_halo(const float* batch, int n_img, int cs, int rank, float* xbuf, cudaStream_t st);
 void aux_smooth_unpack_halo(const float* xbuf, int cs, int rank, int world, float* halo, cudaStream_t st);
 void aux_aesthetic(const float* e, int n_local, int D, int cutn_global, const float* w_dev, float bias, float target,

@@ -71,6 +71,9 @@ struct EdgeArgs {
   int left, right, upper, lower;
   float color[3];
   float inv_l, inv_r, inv_u, inv_d, gw;  // 1 / element count of each strip (0 when the margin is 0), global weight / N
+  const float* target;  // [3, H, W] edge_input_image resized to the image, or null: the flat colour
+  const float* mask;    // [H, W] edge_mask_image resized to the image, or null: the margins
+  float inv_n;          // 1 / (3 H W): the masked term is a mean over every element, masked ones included
 };
 
 __global__ void __launch_bounds__(AUX_THREADS) edge_kernel(const float* __restrict__ img, int H, int W, EdgeArgs a,
@@ -80,13 +83,18 @@ __global__ void __launch_bounds__(AUX_THREADS) edge_kernel(const float* __restri
   double acc = 0.0;
   for (long long i = blockIdx.x * (long long)AUX_THREADS + threadIdx.x; i < n; i += (long long)gridDim.x * AUX_THREADS) {
     const int x = (int)(i % W), y = (int)((i / W) % H), c = (int)(i / ((long long)W * H));
-    const bool mid = x >= a.left && x < W - a.right;  // the upper / lower strips exclude the corner columns (EdgeLoss.py:91-92)
     float w = a.gw;
-    if (x < a.left) w += a.inv_l;
-    if (x >= W - a.right) w += a.inv_r;
-    if (mid && y < a.upper) w += a.inv_u;
-    if (mid && y >= H - a.lower) w += a.inv_d;
-    const float d = img[i] - a.color[c];
+    if (a.mask) {
+      // mse(where(mask > 0, target, out), target): only the unmasked elements differ from the target (EdgeLoss.py:100-103)
+      if (!(a.mask[(size_t)y * W + x] > 0.f)) w += a.inv_n;
+    } else {
+      const bool mid = x >= a.left && x < W - a.right;  // the upper / lower strips exclude the corner columns (EdgeLoss.py:91-92)
+      if (x < a.left) w += a.inv_l;
+      if (x >= W - a.right) w += a.inv_r;
+      if (mid && y < a.upper) w += a.inv_u;
+      if (mid && y >= H - a.lower) w += a.inv_d;
+    }
+    const float d = img[i] - (a.target ? a.target[i] : a.color[c]);
     acc += (double)(w * d) * d;
     g_img[i] += gcoef * w * d;
   }
@@ -203,7 +211,8 @@ __global__ void __launch_bounds__(AUX_THREADS) saturation_grad_kernel(const floa
 
 // ---- smoothness.  The reference reshapes the batch to [cutn * cs, cs, 3] and takes torch.gradient over that 2-D
 // grid, so the row difference runs across cutout boundaries (and, when the cutouts are sharded, across ranks: the
-// two rows either side of this rank's slab come in through `halo`).
+// two rows either side of this rank's slab come in through `halo`).  With smoothness_gaussian_kernel the grid is the
+// blurred batch (side cs' = cs - taps + 1, see blur_axis_kernel), and `cs` below is that side.
 struct SmoothArgs {
   const float* batch;  // [n_img, 3, cs, cs]
   const float* halo;   // [2 sides][2 rows][3][cs]: rows (-2, -1) and (rows, rows + 1) of the global stack, or unused
@@ -211,6 +220,7 @@ struct SmoothArgs {
   long long g0, gt;    // global index of local row 0, total rows of the global stack (cutn * cs)
   float inv_sp;        // 1 / spacing
   int kind;            // 0 default, 1 clipped (max 0.5), 2 log(1 + s)
+  int order;           // torch.gradient edge_order: 1 or 2 (only the first / last point of each axis differ)
 };
 
 __device__ __forceinline__ float sm_x(const SmoothArgs& a, int c, long long r, int x) {
@@ -223,17 +233,43 @@ __device__ __forceinline__ float sm_x(const SmoothArgs& a, int c, long long r, i
   const int k = r < 0 ? (int)(r + 2) : (int)(r - rows);
   return a.halo[(((size_t)side * 2 + k) * 3 + c) * a.cs + x];
 }
-// d/drow at local row r (global row g0 + r must exist), torch.gradient edge_order = 1
+// d/drow at local row r (global row g0 + r must exist), torch.gradient
 __device__ __forceinline__ float sm_gy(const SmoothArgs& a, int c, long long r, int x) {
   const long long G = a.g0 + r;
-  if (G == 0) return (sm_x(a, c, r + 1, x) - sm_x(a, c, r, x)) * a.inv_sp;
-  if (G == a.gt - 1) return (sm_x(a, c, r, x) - sm_x(a, c, r - 1, x)) * a.inv_sp;
+  if (G == 0) {
+    if (a.order == 2)  // (-3 f0 + 4 f1 - f2) / 2h
+      return (-1.5f * sm_x(a, c, r, x) + 2.f * sm_x(a, c, r + 1, x) - 0.5f * sm_x(a, c, r + 2, x)) * a.inv_sp;
+    return (sm_x(a, c, r + 1, x) - sm_x(a, c, r, x)) * a.inv_sp;
+  }
+  if (G == a.gt - 1) {
+    if (a.order == 2)  // (3 fn - 4 fn-1 + fn-2) / 2h
+      return (1.5f * sm_x(a, c, r, x) - 2.f * sm_x(a, c, r - 1, x) + 0.5f * sm_x(a, c, r - 2, x)) * a.inv_sp;
+    return (sm_x(a, c, r, x) - sm_x(a, c, r - 1, x)) * a.inv_sp;
+  }
   return (sm_x(a, c, r + 1, x) - sm_x(a, c, r - 1, x)) * (0.5f * a.inv_sp);
 }
 __device__ __forceinline__ float sm_gx(const SmoothArgs& a, int c, long long r, int x) {
-  if (x == 0) return (sm_x(a, c, r, 1) - sm_x(a, c, r, 0)) * a.inv_sp;
-  if (x == a.cs - 1) return (sm_x(a, c, r, x) - sm_x(a, c, r, x - 1)) * a.inv_sp;
+  if (x == 0) {
+    if (a.order == 2) return (-1.5f * sm_x(a, c, r, 0) + 2.f * sm_x(a, c, r, 1) - 0.5f * sm_x(a, c, r, 2)) * a.inv_sp;
+    return (sm_x(a, c, r, 1) - sm_x(a, c, r, 0)) * a.inv_sp;
+  }
+  if (x == a.cs - 1) {
+    if (a.order == 2) return (1.5f * sm_x(a, c, r, x) - 2.f * sm_x(a, c, r, x - 1) + 0.5f * sm_x(a, c, r, x - 2)) * a.inv_sp;
+    return (sm_x(a, c, r, x) - sm_x(a, c, r, x - 1)) * a.inv_sp;
+  }
   return (sm_x(a, c, r, x + 1) - sm_x(a, c, r, x - 1)) * (0.5f * a.inv_sp);
+}
+// weight of f(o + d) in torch.gradient's derivative at point o (global index Go of n points along the axis)
+__device__ __forceinline__ float sm_w(long long Go, long long n, int d, int order, float inv_sp) {
+  if (Go == 0) {
+    if (order == 2) return d == 0 ? -1.5f * inv_sp : (d == 1 ? 2.f * inv_sp : (d == 2 ? -0.5f * inv_sp : 0.f));
+    return d == 0 ? -inv_sp : (d == 1 ? inv_sp : 0.f);
+  }
+  if (Go == n - 1) {
+    if (order == 2) return d == 0 ? 1.5f * inv_sp : (d == -1 ? -2.f * inv_sp : (d == -2 ? 0.5f * inv_sp : 0.f));
+    return d == 0 ? inv_sp : (d == -1 ? -inv_sp : 0.f);
+  }
+  return d == 1 ? 0.5f * inv_sp : (d == -1 ? -0.5f * inv_sp : 0.f);
 }
 
 // phase 1: per pixel of rows [-1, rows]: A = coef * f'(s) / s (0 where the global row does not exist); loss partials
@@ -273,12 +309,14 @@ __global__ void __launch_bounds__(AUX_THREADS) smooth_sharp_kernel(SmoothArgs a,
   if (threadIdx.x == 0) part[blockIdx.x] = t;
 }
 
-// phase 2 (gather form of the stencil's adjoint): d loss / d X(c, r, x) for every local element
+// phase 2 (gather form of the stencil's adjoint): d loss / d X(c, r, x) for every local element, added into g_out
+// (accumulate) or stored (the blurred path's scratch).  An edge_order 2 end point reads two rows / columns inward; the
+// global first / last rows are always local (every rank holds >= 3 rows then), so A is only read inside [-1, rows].
 __global__ void __launch_bounds__(AUX_THREADS) smooth_grad_kernel(SmoothArgs a, const float* __restrict__ A,
-                                                                  float* __restrict__ g_batch) {
+                                                                  float* __restrict__ g_out, int accumulate) {
   const long long rows = (long long)a.n_img * a.cs;
   const long long n = rows * a.cs * 3;
-  const int cs = a.cs;
+  const int cs = a.cs, R = a.order;
   for (long long i = blockIdx.x * (long long)AUX_THREADS + threadIdx.x; i < n; i += (long long)gridDim.x * AUX_THREADS) {
     const int x = (int)(i % cs);
     const long long q = i / cs;
@@ -287,27 +325,65 @@ __global__ void __launch_bounds__(AUX_THREADS) smooth_grad_kernel(SmoothArgs a, 
     const long long img = q / ((long long)cs * 3);
     const long long r = img * cs + y;
     float g = 0.f;
-    // rows whose d/drow reads X(r): r - 1, r, r + 1
-    for (int dr = -1; dr <= 1; ++dr) {
+    // rows whose d/drow reads X(r): r - R .. r + R
+    for (int dr = -R; dr <= R; ++dr) {
       const long long ro = r + dr, G = a.g0 + ro;
       if (G < 0 || G >= a.gt) continue;
-      float w;
-      if (G == 0) w = dr == 0 ? -a.inv_sp : (dr == -1 ? a.inv_sp : 0.f);                  // (X(ro+1) - X(ro)) / sp
-      else if (G == a.gt - 1) w = dr == 0 ? a.inv_sp : (dr == 1 ? -a.inv_sp : 0.f);        // (X(ro) - X(ro-1)) / sp
-      else w = dr == -1 ? 0.5f * a.inv_sp : (dr == 1 ? -0.5f * a.inv_sp : 0.f);            // (X(ro+1) - X(ro-1)) / 2sp
+      const float w = sm_w(G, a.gt, -dr, a.order, a.inv_sp);
       if (w != 0.f) g += w * A[(ro + 1) * cs + x] * sm_gy(a, c, ro, x);
     }
-    // columns whose d/dcol reads X(x): x - 1, x, x + 1 (same row)
-    for (int dx = -1; dx <= 1; ++dx) {
+    // columns whose d/dcol reads X(x) (same row)
+    for (int dx = -R; dx <= R; ++dx) {
       const int xo = x + dx;
       if (xo < 0 || xo >= cs) continue;
-      float w;
-      if (xo == 0) w = dx == 0 ? -a.inv_sp : (dx == -1 ? a.inv_sp : 0.f);
-      else if (xo == cs - 1) w = dx == 0 ? a.inv_sp : (dx == 1 ? -a.inv_sp : 0.f);
-      else w = dx == -1 ? 0.5f * a.inv_sp : (dx == 1 ? -0.5f * a.inv_sp : 0.f);
+      const float w = sm_w(xo, cs, -dx, a.order, a.inv_sp);
       if (w != 0.f) g += w * A[(r + 1) * cs + xo] * sm_gx(a, c, r, xo);
     }
-    g_batch[i] += g;
+    g_out[i] = accumulate ? g_out[i] + g : g;
+  }
+}
+
+// GaussianSmoothing (SmoothnessLoss.py:9-72) as two 1-D passes: its 2-D kernel is the outer product of one vector with
+// itself normalised to sum 1, i.e. u (x) u with u = v / sum(v).  Valid correlation of planes [P, Hs, Ws] along one axis
+// (0: rows, 1: columns) with the n taps u; the output loses n - 1 lines along that axis.
+__global__ void __launch_bounds__(AUX_THREADS) blur_axis_kernel(const float* __restrict__ src, int P, int Hs, int Ws,
+                                                                int axis, const float* __restrict__ u, int n,
+                                                                float* __restrict__ dst) {
+  const int Ho = axis == 0 ? Hs - n + 1 : Hs, Wo = axis == 1 ? Ws - n + 1 : Ws;
+  const long long total = (long long)P * Ho * Wo;
+  const int step = axis == 0 ? Ws : 1;
+  for (long long i = blockIdx.x * (long long)AUX_THREADS + threadIdx.x; i < total; i += (long long)gridDim.x * AUX_THREADS) {
+    const int x = (int)(i % Wo);
+    const long long q = i / Wo;
+    const int y = (int)(q % Ho);
+    const long long p = q / Ho;
+    const float* s = src + ((size_t)p * Hs + y) * Ws + x;
+    float acc = 0.f;
+    for (int t = 0; t < n; ++t) acc = fmaf(__ldg(u + t), s[(size_t)t * step], acc);
+    dst[i] = acc;
+  }
+}
+// its adjoint (full correlation with the flipped taps) as a gather: dst [P, Hd, Wd] (+)= sum_t u[t] src[j - t], one
+// writer per element
+__global__ void __launch_bounds__(AUX_THREADS) blur_axis_adjoint_kernel(const float* __restrict__ src, int P, int Hd,
+                                                                        int Wd, int axis, const float* __restrict__ u,
+                                                                        int n, float* __restrict__ dst, int accumulate) {
+  const int Hs = axis == 0 ? Hd - n + 1 : Hd, Ws = axis == 1 ? Wd - n + 1 : Wd;
+  const int L = axis == 0 ? Hs : Ws;
+  const int step = axis == 0 ? Ws : 1;
+  const long long total = (long long)P * Hd * Wd;
+  for (long long i = blockIdx.x * (long long)AUX_THREADS + threadIdx.x; i < total; i += (long long)gridDim.x * AUX_THREADS) {
+    const int x = (int)(i % Wd);
+    const long long q = i / Wd;
+    const int y = (int)(q % Hd);
+    const long long p = q / Hd;
+    const int j = axis == 0 ? y : x;
+    const int t0 = j - (L - 1) > 0 ? j - (L - 1) : 0, t1 = j < n - 1 ? j : n - 1;
+    // src element at line j - t of the blurred axis, same position on the other axis
+    const float* s = src + (size_t)p * Hs * Ws + (axis == 0 ? (size_t)x : (size_t)y * Ws) + (size_t)j * step;
+    float acc = 0.f;
+    for (int t = t0; t <= t1; ++t) acc = fmaf(__ldg(u + t), s[-(long long)t * step], acc);
+    dst[i] = accumulate ? dst[i] + acc : acc;
   }
 }
 
@@ -481,9 +557,9 @@ void aux_symmetry(const float* img, int H, int W, float weight, float grad_scale
   aux_final_kernel<<<1, AUX_THREADS, 0, st>>>(part, grid, 1, 1, (double)weight / (double)n, loss_out, nullptr, 0);
 }
 
-void aux_edge(const float* img, int H, int W, const int margins[4], const float color[3], float edge_color_weight,
-              float global_color_weight, float weight, float grad_scale, float* g_img, double* part, float* loss_out,
-              cudaStream_t st) {
+void aux_edge(const float* img, int H, int W, const int margins[4], const float color[3], const float* target,
+              const float* mask, float edge_color_weight, float global_color_weight, float weight, float grad_scale,
+              float* g_img, double* part, float* loss_out, cudaStream_t st) {
   EdgeArgs a;
   a.left = margins[0];
   a.right = margins[1];
@@ -497,6 +573,9 @@ void aux_edge(const float* img, int H, int W, const int margins[4], const float 
   a.inv_d = (a.lower > 0 && mid > 0) ? 1.f / (3.f * a.lower * mid) : 0.f;
   const long long n = 3LL * H * W;
   a.gw = global_color_weight / (float)n;
+  a.target = target;
+  a.mask = mask;
+  a.inv_n = 1.f / (float)n;
   const int grid = aux_grid(n);
   const float k = edge_color_weight * weight;
   edge_kernel<<<grid, AUX_THREADS, 0, st>>>(img, H, W, a, 2.f * k * grad_scale, g_img, part);
@@ -542,8 +621,8 @@ void aux_saturation_grad(const float* batch, int n_img, int cs, int cutn_global,
 }
 
 void aux_smoothness(const float* batch, int n_img, int cs, int first_global, int cutn_global, const float* halo,
-                    float spacing, int kind, float weight, float grad_scale, float* A, float* g_batch, double* part,
-                    float* loss_out, cudaStream_t st) {
+                    float spacing, int kind, int edge_order, float weight, float grad_scale, float* A, float* g_batch,
+                    int accumulate, double* part, float* loss_out, cudaStream_t st) {
   SmoothArgs a;
   a.batch = batch;
   a.halo = halo;
@@ -553,12 +632,26 @@ void aux_smoothness(const float* batch, int n_img, int cs, int first_global, int
   a.gt = (long long)cutn_global * cs;
   a.inv_sp = 1.f / spacing;
   a.kind = kind;
+  a.order = edge_order;
   const double n_glob = (double)cutn_global * cs * cs;
   const long long rows = (long long)n_img * cs;
   const int grid1 = aux_grid((rows + 2) * cs);
   smooth_sharp_kernel<<<grid1, AUX_THREADS, 0, st>>>(a, (float)(weight * grad_scale / n_glob), A, part);
   aux_final_kernel<<<1, AUX_THREADS, 0, st>>>(part, grid1, 1, 1, (double)weight / n_glob, loss_out, nullptr, 1);
-  smooth_grad_kernel<<<aux_grid(rows * cs * 3), AUX_THREADS, 0, st>>>(a, A, g_batch);
+  smooth_grad_kernel<<<aux_grid(rows * cs * 3), AUX_THREADS, 0, st>>>(a, A, g_batch, accumulate);
+}
+
+void aux_smooth_blur(const float* batch, int n_img, int cs, const float* taps, int n, float* tmp, float* out,
+                     cudaStream_t st) {
+  const int P = 3 * n_img, cs2 = cs - n + 1;
+  blur_axis_kernel<<<aux_grid((long long)P * cs * cs2), AUX_THREADS, 0, st>>>(batch, P, cs, cs, 1, taps, n, tmp);
+  blur_axis_kernel<<<aux_grid((long long)P * cs2 * cs2), AUX_THREADS, 0, st>>>(tmp, P, cs, cs2, 0, taps, n, out);
+}
+void aux_smooth_blur_adjoint(const float* g_out, int n_img, int cs, const float* taps, int n, float* tmp, float* g_batch,
+                             cudaStream_t st) {
+  const int P = 3 * n_img, cs2 = cs - n + 1;
+  blur_axis_adjoint_kernel<<<aux_grid((long long)P * cs * cs2), AUX_THREADS, 0, st>>>(g_out, P, cs, cs2, 0, taps, n, tmp, 0);
+  blur_axis_adjoint_kernel<<<aux_grid((long long)P * cs * cs), AUX_THREADS, 0, st>>>(tmp, P, cs, cs, 1, taps, n, g_batch, 1);
 }
 
 void aux_smooth_pack_halo(const float* batch, int n_img, int cs, int rank, float* xbuf, cudaStream_t st) {

@@ -7,9 +7,13 @@ returns the value the engine computed for the current iteration -- gradients nev
     loss = SmoothnessLoss(device=dev); args = loss.parse_settings(args); loss.attach(session, args, weight)
 """
 import argparse
+import glob
+import math
+import re
 
 import numpy as np
 import torch
+import torch.nn.functional as F
 
 from . import engine as E
 
@@ -105,8 +109,21 @@ class PaletteLoss(LossInterface):
         return [args.palette_weight] + pal.reshape(-1).tolist()
 
 
+def gaussian_smoothing_kernel(kernel_size, sigma):
+    """GaussianSmoothing's 2-D weight (SmoothnessLoss.py:29-44), built with the reference's own expression: `kernel_size`
+    is a float, so there are ceil(k) taps centred at (k - 1) / 2 (off-centre for a non-integer k), and the exponent
+    divides by 2 sigma, not 2 sigma^2."""
+    kernel = 1
+    meshgrids = torch.meshgrid([torch.arange(size, dtype=torch.float32) for size in (kernel_size, kernel_size)],
+                               indexing="ij")
+    for size, std, mgrid in zip((kernel_size, kernel_size), (sigma, sigma), meshgrids):
+        mean = (size - 1) / 2
+        kernel = kernel * (1 / (std * math.sqrt(2 * math.pi)) * torch.exp(-((mgrid - mean) / (2 * std)) ** 2))
+    return kernel / torch.sum(kernel)
+
+
 class SmoothnessLoss(LossInterface):
-    """Losses/SmoothnessLoss.py."""
+    """Losses/SmoothnessLoss.py, with the pre-blur (smoothness_gaussian_kernel) and edge_order 1 or 2."""
     kind = E.LOSS_SMOOTHNESS
     _types = {"default": 0, "clipped": 1, "log": 2}
 
@@ -121,17 +138,80 @@ class SmoothnessLoss(LossInterface):
         return parser
 
     def engine_params(self, args, session):
-        if getattr(args, "smoothness_gaussian_kernel", 0):
-            raise NotImplementedError("smoothness_gaussian_kernel != 0 (pre-blur) is not implemented in the engine")
-        if getattr(args, "smoothness_edge_order", 1) != 1:
-            raise NotImplementedError("only smoothness_edge_order = 1 is implemented in the engine")
+        k = float(getattr(args, "smoothness_gaussian_kernel", 0) or 0)
+        order = getattr(args, "smoothness_edge_order", 1)
+        if order not in (1, 2):
+            raise ValueError("torch.gradient only supports edge_order=1 and edge_order=2.")
+        if k < 0:
+            raise ValueError(f"smoothness_gaussian_kernel must be >= 0 (got {k})")
         # any other string falls through to the un-clipped branch in the reference (SmoothnessLoss.py:101-104)
-        return [args.smoothness_weight, self._types.get(args.smoothness_type, 0), getattr(args, "smoothness_spacing", 1)]
+        params = [args.smoothness_weight, self._types.get(args.smoothness_type, 0), getattr(args, "smoothness_spacing", 1)]
+        if not k and order == 1:
+            return params
+        taps = [0]
+        if k:
+            std = float(getattr(args, "smoothness_gaussian_std", 1))
+            if not std > 0:
+                raise ValueError(f"smoothness_gaussian_std must be > 0 (got {std})")
+            K = gaussian_smoothing_kernel(k, std)
+            taps = [K.shape[0]] + K.reshape(-1).tolist()
+        return params + [order] + taps
+
+
+def _braceexpand(pattern):
+    """braceexpand's alternatives {a,b} and integer ranges {1..3}, nested, no escapes."""
+    m = re.search(r"\{([^{}]*)\}", pattern)
+    if not m:
+        return [pattern]
+    body = m.group(1)
+    r = re.fullmatch(r"(-?\d+)\.\.(-?\d+)", body)
+    if r:
+        a, b = int(r.group(1)), int(r.group(2))
+        items = [str(i) for i in (range(a, b + 1) if a <= b else range(a, b - 1, -1))]
+    elif "," in body:
+        items = body.split(",")
+    else:  # a literal {x}: keep it, expand what follows
+        return [pattern[:m.end()] + e for e in _braceexpand(pattern[m.end():])]
+    out = []
+    for it in items:
+        out += _braceexpand(pattern[:m.start()] + it + pattern[m.end():])
+    return out
+
+
+def real_glob(rglob):
+    """util.real_glob: brace expansion, then each glob, then sorted."""
+    files = []
+    for g in _braceexpand(rglob):
+        files = files + glob.glob(g)
+    return sorted(files)
+
+
+def _open_first(path, mode, what):
+    from PIL import Image
+    if "http" in path:  # EdgeLoss.parse_settings downloads these
+        raise ValueError(f"edge loss: {what} '{path}' is a URL; download it and pass a local file")
+    files = real_glob(path)
+    if not files:
+        raise FileNotFoundError(f"edge loss: {what} '{path}' matches no file")
+    return Image.open(files[0]).convert(mode)
+
+
+def resize_bicubic(pil_img, hw):
+    """TF.resize(TF.to_tensor(img)[None], hw, BICUBIC) of EdgeLoss.get_loss (EdgeLoss.py:61-68) for a float tensor:
+    torchvision 0.26 calls F.interpolate(bicubic, align_corners=False, antialias=True) and does not clamp."""
+    x = torch.from_numpy(np.array(pil_img, dtype=np.uint8, copy=True))
+    x = (x[None] if x.ndim == 2 else x.permute(2, 0, 1)).contiguous().to(torch.float32).div(255)
+    return F.interpolate(x[None], size=tuple(hw), mode="bicubic", align_corners=False, antialias=True)
 
 
 class EdgeLoss(LossInterface):
-    """Losses/EdgeLoss.py with a colour target (edge_input_image / edge_mask_image are file-based variants, not built)."""
+    """Losses/EdgeLoss.py: a flat colour or an image (edge_input_image) as the target, in the margins or wherever a mask
+    image (edge_mask_image, > 0 after the bicubic resize) is not set."""
     kind = E.LOSS_EDGE
+
+    def __init__(self, device=None):
+        super().__init__(device)
+        self.image, self.mask = None, None
 
     @staticmethod
     def add_settings(parser):
@@ -159,16 +239,29 @@ class EdgeLoss(LossInterface):
         if args.edge_margins is None:
             t = args.edge_thickness
             args.edge_margins = (t, t, t, t)
-        if getattr(args, "edge_input_image", "") or getattr(args, "edge_mask_image", ""):
-            raise NotImplementedError("edge_input_image / edge_mask_image are not implemented in the engine")
+        if getattr(args, "edge_input_image", ""):
+            self.image = _open_first(args.edge_input_image, "RGB", "edge_input_image")
+        self.mask = _open_first(args.edge_mask_image, "L", "edge_mask_image") if getattr(args, "edge_mask_image", "") else None
         return args
 
+    def resized(self, hw):
+        """(target [1, 3, H, W] or None, mask [1, 1, H, W] or None): the reference's resized images for an image of size hw."""
+        return (None if self.image is None else resize_bicubic(self.image, hw),
+                None if self.mask is None else resize_bicubic(self.mask, hw))
+
     def engine_params(self, args, session):
+        # the canvas: the filtered image the loss reads has its size (super_resolution canvases are multiples of 4)
         H, W = session.engine.image_hw
         left, right, upper, lower = args.edge_margins
         # util.map_number(n, 0, 100, 0, size) then int() (EdgeLoss.py:85-88)
         px = [int(left / 100.0 * W), int(right / 100.0 * W), int(upper / 100.0 * H), int(lower / 100.0 * H)]
-        return [args.edge_color_weight, args.global_color_weight] + px + list(args.edge_color)
+        params = [args.edge_color_weight, args.global_color_weight] + px + list(args.edge_color)
+        if self.image is None and self.mask is None:
+            return params
+        target, mask = self.resized((H, W))
+        mode = (1 if target is not None else 0) | (2 if mask is not None else 0)
+        arrays = [t.reshape(-1).numpy() for t in (target, mask) if t is not None]
+        return np.concatenate([np.asarray(params + [mode], dtype=np.float32)] + arrays)
 
 
 class GaussianLoss(LossInterface):
