@@ -424,6 +424,16 @@ int pxr_test_gemv(const void* w, int K, int R, const float* x, const float* bias
  * dS = P * (dP - <P, dP>), P in p_or_s.  Synchronous on the default stream. */
 int pxr_test_softmax(int backward, void* p_or_s, void* dp, int rows, int cols, int ld);
 
+/* the Prompt loss (pixray.py:275-280) of B embeddings against n prompt rows, as the engine runs it: e [B, D] ->
+ * e_unit [B, D] (nullable) = e / max(|e|, 1e-12); losses[slots[j]] += |w_j| dist_bj inv_rows[j] / cutn_global summed over
+ * the rows b (the caller zeroes losses; slots / inv_rows nullable: j / 1); de [B, D] = grad_scale * d(sum of losses) / de
+ * with the gradient of row (b, j) kept only where dist_bj > stops[j] (replace_grad(dists, maximum(dists, stop))),
+ * de16 (nullable) its fp16 copy.  dist_bj = 2 asin(min(|e_unit_b - p_j| / 2, 1))^2 sign(w_j).  All DEVICE; D * 8 bytes of
+ * shared memory per block.  Synchronous on the default stream; -1 on bad arguments. */
+int pxr_test_prompt_loss(const float* e, int B, int D, const float* prompts, const float* weights, const float* stops,
+                         const int* slots, const float* inv_rows, int n, int cutn_global, float grad_scale, float* e_unit,
+                         float* losses, float* de, void* de16);
+
 /* one CLIP LayerNorm kernel chosen explicitly -- variant 0: fp32 residual stream, 1: fp16 stream with 8-byte vectors,
  * 2: fp16 stream with 16-byte vectors (W % 256 == 0, no pos, fp16 output only) -- forward, or backward (accumulate
  * adds into gx / gx16).  Arguments as the engine's layernorm_forward / layernorm_backward; x is fp32 for variant 0 and

@@ -177,6 +177,8 @@ class Engine {
     int* pslot = nullptr;
     float* pinv = nullptr;
     float* scratch = nullptr;  // pxr_prompt_loss on caller-provided embeddings
+    float* ploss_part = nullptr;          // the prompt loss's per-row terms, [B, most rows of one call]
+    unsigned int* ploss_count = nullptr;  // its last-block ticket
     // spot prompts (pixray.py:1283-1293): text Prompts scored on the embeddings of the masked cutouts.
     // [1] = args.spot_prompts (make_cutouts(out, spot=1)), [0] = args.spot_prompts_off (spot=0)
     struct Spot {
@@ -1977,6 +1979,10 @@ void Engine::rebuild_prompt_rows() {
       }
     }
     const int D = C.c.out_dim, rows = C.n_text + n_img * cfg.cutn;
+    const int most = std::max(rows, std::max(C.spot[0].n, C.spot[1].n));
+    dfree(C.ploss_part);
+    if (most > 0) C.ploss_part = dalloc<float>((size_t)C.B * most, false);
+    if (!C.ploss_count) C.ploss_count = dalloc<unsigned int>(1);
     std::vector<float> pr((size_t)rows * D, 0.f), w(rows), stp(rows), inv(rows);
     std::vector<int> slot(rows);
     std::copy(C.text_rows.begin(), C.text_rows.end(), pr.begin());
@@ -2047,7 +2053,7 @@ void Engine::encode_image_prompts() {
       if (comm) PXR_CUDA(cudaMemsetAsync(rows, 0, sizeof(float) * cfg.cutn * D, st));
       // zero prompt rows: the kernel only normalises (slip.py:66) into `rows`; de is overwritten by the main pass
       prompt_loss(C.e, C.B, D, C.prompts, C.pweights, C.pstops, C.pslot, C.pinv, 0, cfg.cutn, S,
-                  rows + (size_t)first_global * D, losses_dev + C.loss_offset, C.de, C.de16, st);
+                  rows + (size_t)first_global * D, losses_dev + C.loss_offset, C.de, C.de16, nullptr, nullptr, st);
       launches += 2;
       if (comm)  // every rank needs all cutn rows; each rank filled its own, the others are zero: the sum is exact
         nccl_check(Comm::api().all_reduce(rows, rows, (size_t)cfg.cutn * D, Comm::kFloat32, Comm::kSum, comm, st),
@@ -2061,7 +2067,7 @@ void Engine::loss_clip(int i) {
   Clip& C = clip[i];
   if (C.n_prompts == 0) throw EngineError(-70, "no prompts set for perceptor " + std::to_string(i));
   prompt_loss(C.e, C.B, C.c.out_dim, C.prompts, C.pweights, C.pstops, C.pslot, C.pinv, C.n_rows, cfg.cutn, S, C.e_unit,
-              losses_dev + C.loss_offset, C.de, C.de16, st);
+              losses_dev + C.loss_offset, C.de, C.de16, C.ploss_part, C.ploss_count, st);
   launches += 1;
   if (i == cfg.n_clip - 1 && !aux.empty()) aux_after_embed();
 }
@@ -2271,7 +2277,7 @@ bool Engine::spot_pass(int which, bool accumulate_img) {
     if (sp.n == 0) continue;
     forward_clip(i);
     prompt_loss(C.e, C.B, C.c.out_dim, sp.d_rows, sp.d_w, sp.d_stop, sp.d_slot, sp.d_inv, sp.n, cfg.cutn, S, C.e_unit,
-                losses_dev + sp.loss_offset, C.de, C.de16, st);
+                losses_dev + sp.loss_offset, C.de, C.de16, C.ploss_part, C.ploss_count, st);
     launches += 1;
   }
   backward_to_image(a, which, accumulate_img, false);
@@ -2896,7 +2902,7 @@ int pxr_prompt_loss(pxr_handle h, int clip_idx, const float* embeds, float* out_
       PXR_CUDA(cudaMemcpyAsync(se, embeds, sizeof(float) * n, cudaMemcpyDeviceToDevice, e->st));
       PXR_CUDA(cudaMemsetAsync(sl, 0, 64 * sizeof(float), e->st));
       pxr::prompt_loss(se, C.B, C.c.out_dim, C.prompts, C.pweights, C.pstops, C.pslot, C.pinv, C.n_rows, e->cfg.cutn, e->S, su,
-                       sl, sd, sd16, e->st);
+                       sl, sd, sd16, C.ploss_part, C.ploss_count, e->st);
       e->launches += 1;
       if (out_losses)
         PXR_CUDA(cudaMemcpyAsync(out_losses, sl, sizeof(float) * C.n_prompts, cudaMemcpyDeviceToDevice, e->st));

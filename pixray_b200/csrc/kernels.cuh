@@ -299,10 +299,12 @@ void softmax_forward(act_t* s, int rows, int cols, int ld, cudaStream_t st);
 void softmax_backward(const act_t* p, act_t* dp_to_ds, int rows, int cols, int ld, cudaStream_t st);
 // Prompt.forward for all prompts of one perceptor + its gradient w.r.t. the un-normalised embeds.
 //   e [B, D]; prompts [n, D] (unit rows), weights/stops [n]; de [B, D].  slots / inv_rows (nullable): row j adds into
-//   losses[slots[j]] with 1 / (rows of its Prompt) -- multi-row embeds (image prompts).  losses += partial, caller zeroes.
+//   losses[slots[j]] with 1 / (rows of its Prompt) -- multi-row embeds (image prompts).  losses += partial, caller zeroes;
+//   the partials are summed in a fixed order (the same bits on every run) through part [B, n] floats of scratch and
+//   `count`, one zero-initialised counter the call leaves at zero.  Both may be null when n == 0.
 void prompt_loss(const float* e, int B, int D, const float* prompts, const float* weights, const float* stops,
                  const int* slots, const float* inv_rows, int n, int cutn_global, float grad_scale, float* e_unit,
-                 float* losses, float* de, act_t* de16, cudaStream_t st);
+                 float* losses, float* de, act_t* de16, float* part, unsigned int* count, cudaStream_t st);
 
 // ------------------------------------------------------------------ optimiser (pixray.py:538-539, 1484-1487)
 // Adam (bias-corrected, torch.optim.Adam semantics) on z with gradient g * inv_scale, then clip_z to per-channel

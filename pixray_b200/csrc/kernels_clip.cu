@@ -454,7 +454,10 @@ __global__ void __launch_bounds__(256) softmax_bwd_long_kernel(const act_t* __re
   }
 }
 
-// one block (128 threads) per cutout row.  Accumulates losses with atomics (n prompts).
+// one block (128 threads) per cutout row.  The loss terms of the rows are summed in a fixed order: every block stores
+// its row's n terms in part [B, n], and the last block to finish (a ticket drawn on `count`, which it resets) adds the
+// columns of part to `losses`.  Float atomics would make the last bit of every loss depend on the order the blocks
+// arrive in, and so differ between identical runs.
 __global__ void __launch_bounds__(128) prompt_loss_kernel(const float* __restrict__ e, int D,
                                                           const float* __restrict__ prompts,
                                                           const float* __restrict__ weights,
@@ -463,7 +466,8 @@ __global__ void __launch_bounds__(128) prompt_loss_kernel(const float* __restric
                                                           const float* __restrict__ inv_rows, int n, float inv_count,
                                                           float grad_scale, float* __restrict__ e_unit,
                                                           float* __restrict__ losses, float* __restrict__ de,
-                                                          act_t* __restrict__ de16) {
+                                                          act_t* __restrict__ de16, float* __restrict__ part,
+                                                          unsigned int* __restrict__ count) {
   pdl_prologue();
   extern __shared__ float sh[];  // en [D], gen [D]
   float* en = sh;
@@ -508,7 +512,7 @@ __global__ void __launch_bounds__(128) prompt_loss_kernel(const float* __restric
     // row j of a Prompt whose embed has 1/inv_rows[j] rows (image prompts: [cutn, D], pixray.py:1327-1333); the mean
     // of Prompt.forward runs over [cutn, rows]
     const float inv_n = inv_count * (inv_rows ? inv_rows[j] : 1.f);
-    if (threadIdx.x == 0) atomicAdd(&losses[slots ? slots[j] : j], fabsf(w) * dist * inv_n);
+    if (threadIdx.x == 0) part[(size_t)b * n + j] = fabsf(w) * dist * inv_n;
     // replace_grad(dists, maximum(dists, stop)): gradient only where dists > stop (pixray.py:280)
     if (dist > stop && r > 0.f) {
       // d dist / d r = sgn * 2 asin(r/2) / sqrt(1 - r^2/4)
@@ -527,6 +531,22 @@ __global__ void __launch_bounds__(128) prompt_loss_kernel(const float* __restric
     de[(size_t)b * D + d] = v;
     if (de16) de16[(size_t)b * D + d] = __float2half_rn(v);
   }
+  if (n == 0) return;
+  __shared__ bool s_last;
+  if (threadIdx.x == 0) {
+    __threadfence();  // this block's terms are visible before its ticket
+    s_last = atomicAdd(count, 1u) == gridDim.x - 1;
+  }
+  __syncthreads();
+  if (!s_last) return;
+  __threadfence();
+  for (int j = 0; j < n; ++j) {
+    float s = 0.f;
+    for (int r = threadIdx.x; r < (int)gridDim.x; r += 128) s += __ldcg(part + (size_t)r * n + j);
+    s = block_sum(s);
+    if (threadIdx.x == 0) losses[slots ? slots[j] : j] += s;
+  }
+  if (threadIdx.x == 0) *count = 0;
 }
 
 // ---- the update rules (kernels.cuh OPT_*).  apply() reads element i's state, writes it back (0 when `fresh`: the managed
@@ -874,10 +894,10 @@ void softmax_backward(const act_t* p, act_t* dp_to_ds, int rows, int cols, int l
 }
 void prompt_loss(const float* e, int B, int D, const float* prompts, const float* weights, const float* stops,
                  const int* slots, const float* inv_rows, int n, int cutn_global, float grad_scale, float* e_unit,
-                 float* losses, float* de, act_t* de16, cudaStream_t st) {
+                 float* losses, float* de, act_t* de16, float* part, unsigned int* count, cudaStream_t st) {
   // Prompt.forward means over [cutn, n_embed] per prompt (pixray.py:280)
   launch_pdl(prompt_loss_kernel, dim3(B), dim3(128), 2 * D * sizeof(float), st, e, D, prompts, weights, stops, slots, inv_rows, n,
-                                                           1.f / cutn_global, grad_scale, e_unit, losses, de, de16);
+                                                           1.f / cutn_global, grad_scale, e_unit, losses, de, de16, part, count);
 }
 
 // calls f(Rule{}) with the functor of `kind`

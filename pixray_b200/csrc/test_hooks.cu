@@ -109,6 +109,28 @@ extern "C" int pxr_test_splitk_reduce(const float* ws, int splits, long long pix
   return sync_status();
 }
 
+// The Prompt loss kernel (prompt_loss, kernels_clip.cu) on caller DEVICE tensors: e [B, D] -> e_unit [B, D], losses
+// [max slot + 1] (summed into: the caller zeroes them), de [B, D] fp32 and de16 [B, D] fp16 (nullable).
+extern "C" int pxr_test_prompt_loss(const float* e, int B, int D, const float* prompts, const float* weights,
+                                    const float* stops, const int* slots, const float* inv_rows, int n, int cutn_global,
+                                    float grad_scale, float* e_unit, float* losses, float* de, void* de16) {
+  if (!e || !de || B < 1 || D < 1 || n < 0 || cutn_global < 1 || (n > 0 && (!prompts || !weights || !stops || !losses)))
+    return -1;
+  float* part = nullptr;
+  unsigned int* count = nullptr;
+  if (n > 0 && (cudaMalloc(&part, sizeof(float) * B * n) != cudaSuccess || cudaMalloc(&count, sizeof(unsigned int)) != cudaSuccess ||
+                cudaMemset(count, 0, sizeof(unsigned int)) != cudaSuccess)) {
+    cudaFree(part);
+    return -100;
+  }
+  prompt_loss(e, B, D, prompts, weights, stops, slots, inv_rows, n, cutn_global, grad_scale, e_unit, losses, de,
+              static_cast<act_t*>(de16), part, count, nullptr);
+  const int rc = sync_status();
+  cudaFree(part);
+  cudaFree(count);
+  return rc;
+}
+
 // Fused attention forward (+ backward when d_o != NULL) on caller tensors: qkv [B*T, 3W] fp16, o [B*T, W] fp16,
 // lse [B*H*T] fp32, d_o [B*T, W] fp16, gqkv [B*T, 3W] fp16.
 extern "C" int pxr_test_attention(const void* qkv, void* o, float* lse, const void* d_o, void* gqkv, int B, int T, int H,

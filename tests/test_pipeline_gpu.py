@@ -420,9 +420,8 @@ def test_every_attention_path_matches_the_oracle(path, monkeypatch):
 
 def test_last_layer_on_all_rows_is_bit_identical(monkeypatch):
     """The last ViT layer restricted to the class rows (default) and run on all rows (PXR_CLIP_LAST_CLS=0) compute the
-    class rows with the same operations: embeddings and z.grad are bit-identical.  (The loss values are not compared
-    bit for bit: the prompt-loss kernel sums them over the cutouts with atomics, so their last bits vary from call to
-    call in either session.)"""
+    class rows with the same operations: embeddings, loss values and z.grad are bit-identical (the prompt-loss kernel
+    sums the losses over the cutouts in a fixed order)."""
     outs = {}
     for last_cls in ("1", "0"):
         for k in ("PXR_FUSED_ATTN", "PXR_CLIP_STREAM"):
@@ -432,9 +431,10 @@ def test_last_layer_on_all_rows_is_bit_identical(monkeypatch):
         outs[last_cls], err = _stagewise(vq, clip, eng, prompts, z, 32, 23)
         eng.close()
         _assert_pipeline_tolerances(err)
-    (img1, emb1, _, g1), (img0, emb0, _, g0) = outs["1"], outs["0"]
+    (img1, emb1, l1, g1), (img0, emb0, l0, g0) = outs["1"], outs["0"]
     assert torch.equal(img1, img0)
     assert torch.equal(emb1, emb0)
+    assert torch.equal(l1, l0)
     assert torch.equal(g1, g0)
 
 

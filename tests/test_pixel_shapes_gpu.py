@@ -329,6 +329,6 @@ def test_latent_anchor_gradient_on_the_rgba_colours():
     g1, l1 = grad(2)
     want = w * (z - ref) / z.numel()
     assert (g1 - g0 - want).abs().max().item() <= 1e-6 * want.abs().max().item() + 1e-9
-    # the prompt loss is unchanged (its value is summed with atomics, so only to its last bits: DESIGN §3)
+    # the prompt loss is unchanged
     assert abs(float(l1[0]) - float(l0[0])) <= 1e-6 * abs(float(l0[0]))
     assert abs(float(l1[1]) - w / 2 * float(((z.double() - ref.double()) ** 2).mean())) <= 1e-6
