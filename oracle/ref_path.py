@@ -323,10 +323,11 @@ COLORLOOKUP_DEFAULT_TABLE = [[0, 0, 0], [255, 255, 255], [63, 40, 50], [38, 43, 
 
 
 def filter_colorlookup(img, color_table=None, beta=10.0):
-    """filters/colorlookup.py:51-86 (3-channel path): nearest table colour, straight-through value, VQ-style loss."""
+    """filters/colorlookup.py:51-86 (3-channel path): nearest table colour, straight-through value, VQ-style loss.  The
+    table takes the image's dtype (float32 in the reference)."""
     if color_table is None:
         color_table = [[c / 255.0 for c in rgb] for rgb in COLORLOOKUP_DEFAULT_TABLE]
-    table = torch.as_tensor(color_table, dtype=torch.float32)
+    table = torch.as_tensor(color_table, dtype=img.dtype)
     z3 = img.permute(0, 2, 3, 1).contiguous()
     ind = torch.cdist(z3, table).argmin(dim=-1)
     z_q = torch.index_select(table, 0, ind.flatten()).view(z3.shape)
@@ -708,35 +709,39 @@ def pixel_synth(z, out_hw):
 _COLOR_SVD_SQRT = ((0.26, 0.09, 0.02), (0.27, 0.00, -0.05), (0.27, -0.09, 0.03))
 
 
-def fft_freq_scale(h, w, decay_power=1.5):
+def fft_freq_scale(h, w, decay_power=1.5, dtype=torch.float32):
     """aphantasia fft_image's per-frequency scale [UPSTREAM]: 1 / max(|f|, 4/max(h,w))**decay * sqrt(w*h) on the
-    rfft2 grid (SURVEY.md 8c).  Returns [h, w//2+1] float32."""
+    rfft2 grid (SURVEY.md 8c).  Returns [h, w//2+1] (computed in float64, returned in `dtype`)."""
     import numpy as np
     fy = np.fft.fftfreq(h)[:, None]
     fx = np.fft.fftfreq(w)[: w // 2 + 1]
     freqs = np.sqrt(fx * fx + fy * fy)
     scale = 1.0 / np.maximum(freqs, 4.0 / max(h, w)) ** decay_power
     scale *= np.sqrt(w * h)
-    return torch.tensor(scale, dtype=torch.float32)
+    return torch.tensor(scale, dtype=dtype)
 
 
-def color_matrix(colors=1.5):
+def color_matrix(colors=1.5, dtype=torch.float32):
+    """to_valid_rgb's colour matrix, first column / colors, over the largest column norm, evaluated in `dtype`."""
     import numpy as np
-    m = np.asarray(_COLOR_SVD_SQRT, dtype=np.float32)
-    m = m / np.asarray([colors, 1.0, 1.0], dtype=np.float32)
+    nt = np.float64 if dtype == torch.float64 else np.float32
+    m = np.asarray(_COLOR_SVD_SQRT, dtype=nt)
+    m = m / np.asarray([colors, 1.0, 1.0], dtype=nt)
     m = m / np.max(np.linalg.norm(m, axis=0))
-    return torch.tensor(m, dtype=torch.float32)
+    return torch.tensor(m, dtype=dtype)
 
 
 def fft_synth(spectrum, decay_power=1.5, colors=1.5, contrast=0.9):
     """FftDrawer.synth, fftdrawer.py:78-84: to_valid_rgb(fft_image(...))(contrast=0.9).
-    spectrum [1, 3, H, W//2+1, 2] (real, imag); returns [1, 3, H, W] in (0, 1)."""
+    spectrum [1, 3, H, W//2+1, 2] (real, imag); returns [1, 3, H, W] in (0, 1), in the spectrum's dtype (float32 or
+    float64) and on its device: the scale grid and the colour matrix follow it."""
     _, _, h, w2, _ = spectrum.shape
     w = (w2 - 1) * 2
-    scaled = fft_freq_scale(h, w, decay_power)[None, None, :, :, None] * spectrum
+    scale = fft_freq_scale(h, w, decay_power, spectrum.dtype).to(spectrum.device)
+    scaled = scale[None, None, :, :, None] * spectrum
     image = torch.fft.irfftn(torch.view_as_complex(scaled.contiguous()), s=(h, w), norm="ortho")
     image = image * contrast / image.std()
-    m = color_matrix(colors)
+    m = color_matrix(colors, spectrum.dtype).to(spectrum.device)
     image = torch.matmul(image.permute(0, 2, 3, 1), m.T).permute(0, 3, 1, 2)
     return torch.sigmoid(image)
 

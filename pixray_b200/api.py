@@ -382,7 +382,9 @@ def do_init(args):
         rows, cols = P.PixelDrawer.grid_for(args, (sideX, sideY))
         kw["polygons"] = PS.polygons((sideX, sideY), rows, cols, args.pixel_type)
     if kind == E.DRAWER_FFT:
-        kw.update(fft_decay=args.fft_decay, fft_colors=args.fft_colors)
+        # fft_colors is not passed: FftDrawer builds to_valid_rgb(image_f, colors=1.5) with the value written into the call
+        # (fftdrawer.py:61), and self.colors only reaches dwt_image; the engine's default is that 1.5
+        kw.update(fft_decay=args.fft_decay)
     if kind == E.DRAWER_STROKES:
         # the reference's z_orig would be get_z_copy() = None and its anchors would fail on it (linedrawer.py:186-193)
         for dest in ("init_weight", "init_weight_dist", "init_weight_cos", "init_weight_pix", "image_labels"):

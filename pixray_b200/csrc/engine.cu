@@ -104,8 +104,8 @@ class Engine {
   float *cut_img = nullptr, *g_cut_img = nullptr;
   int cut_h = 0, cut_w = 0;
   bool filtered_valid = false;  // cut_img holds the filtered image of the current z (fused path); else use img
-  float* filter_dummy = nullptr;
-  int* lookup_best = nullptr;
+  int* lookup_best = nullptr;  // nearest-colour index per pixel of a lookup's input (the largest of the program's lookups)
+  size_t lookup_best_n = 0;
   void rebuild_filters();
   void filters_forward(int iter);
   void filters_backward();
@@ -2389,8 +2389,16 @@ void Engine::rebuild_filters() {
   g_cut_img = cur_g;
   cut_h = H;
   cut_w = Wd;
-  if (!filter_dummy) filter_dummy = dalloc<float>(4);
-  if (!lookup_best) lookup_best = dalloc<int>((size_t)4 * cfg.image_h * cfg.image_w);
+  // every "shift" wallpaper doubles the height, so a lookup late in the chain can see many times the canvas
+  size_t lookup_px = 0;
+  for (const FilterPrim& pr : fprims)
+    if (pr.kind == FP_LOOKUP) lookup_px = std::max(lookup_px, (size_t)pr.Hin * pr.Win);
+  if (lookup_px > lookup_best_n) {
+    lookup_best = dalloc<int>(lookup_px);
+    lookup_best_n = lookup_px;
+  }
+  reg("filtered", cut_img, (size_t)3 * cut_h * cut_w * 4);
+  reg("g_filtered", g_cut_img, (size_t)3 * cut_h * cut_w * 4);
   rebuild_prompt_rows();
 }
 
@@ -2435,7 +2443,7 @@ void Engine::filters_backward() {
       case FP_WSHIFT: filter_wallpaper_shift_backward(pr.g_out, pr.Hin, pr.Win, F.sh, F.sw, 0, pr.g_in, st); break;
       case FP_CROP: filter_crop_backward(pr.g_out, pr.Hin, pr.Win, pr.top, pr.left, pr.Hout, pr.Wout, pr.g_in, st); break;
       case FP_EDGE:  // a tap: adds its loss gradient to the gradient of the tensor it looks at
-        filter_edge_match(pr.in, pr.Hin, pr.Win, pr.em, pr.axis, F.weight, S, 0, pr.g_in, filter_dummy, st);
+        filter_edge_match(pr.in, pr.Hin, pr.Win, pr.em, pr.axis, F.weight, S, 0, pr.g_in, nullptr, st);
         break;
       case FP_LOOKUP:
         filter_colorlookup_backward(pr.g_out, pr.in, pr.out, pr.Hin * pr.Win, pr.beta, F.weight, S, 0, pr.g_in, st);
@@ -2511,6 +2519,8 @@ void Engine::finalize() {
     reg("img", img, npx * 4);
     reg("img_pre", img_pre, npx * 4);
     reg("g_img", g_img, npx * 4);
+    reg("filtered", img, npx * 4);  // the filter chain's output and its gradient; rebuild_filters moves them
+    reg("g_filtered", g_img, npx * 4);
     reg("pooled", pooled, ncs * 4);
     reg("cut_src", cut_src, (size_t)3 * src_h * src_w * 4);
     reg("pool_argmax", pool_argmax, ncs * 4);

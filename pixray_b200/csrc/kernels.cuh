@@ -453,7 +453,8 @@ void filter_wallpaper_shift(const float* x, int H, int W, int sh, int sw, float*
 void filter_wallpaper_shift_backward(const float* gy, int H, int W, int sh, int sw, int accumulate, float* gx, cudaStream_t st);
 void filter_crop(const float* x, int H, int W, int top, int left, int Hc, int Wc, float* y, cudaStream_t st);
 void filter_crop_backward(const float* gy, int H, int W, int top, int left, int Hc, int Wc, float* gx, cudaStream_t st);
-// loss = weight * mse(first em, last em) / em along axis (0: columns, 1: rows); g (nullable) += grad_scale * dloss/dx
+// loss_out (nullable) (=|+=) weight * mse(first em, last em) / em along axis (0: columns, 1: rows);
+// g (nullable) += grad_scale * weight * dloss/dx, one writer per element
 void filter_edge_match(const float* x, int H, int W, int em, int axis, float weight, float grad_scale, int accumulate_loss,
                        float* g, float* loss_out, cudaStream_t st);
 // nearest palette colour (first minimum), loss = weight * (beta + 1) * mean((z_q - z)^2); part: AUX_MAX_BLOCKS doubles

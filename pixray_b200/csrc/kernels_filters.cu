@@ -71,10 +71,9 @@ __global__ void crop_bwd_kernel(const float* __restrict__ gy, int H, int W, int 
 }
 
 // edge match (wallpaper.py:47-53, 58-66): loss = mse(x[first em], x[last em]) / em along one axis; single block reduces in
-// a fixed order (the strips are small).  axis 0: columns (horizontal wrap), axis 1: rows.  loss_out += weight * loss;
-// g (+=) grad_scale * weight * dloss/dx.
-__global__ void edge_match_kernel(const float* __restrict__ x, int H, int W, int em, int axis, float weight, float grad_scale,
-                                  int accumulate_loss, float* __restrict__ g, float* __restrict__ loss_out) {
+// a fixed order (the strips are small).  axis 0: columns (horizontal wrap), axis 1: rows.  loss_out (=|+=) weight * loss.
+__global__ void edge_match_loss_kernel(const float* __restrict__ x, int H, int W, int em, int axis, float weight,
+                                       int accumulate_loss, float* __restrict__ loss_out) {
   pdl_prologue();
   const int n = axis == 0 ? 3 * H * em : 3 * em * W;
   const float k = 1.f / ((float)n * (float)em);
@@ -93,12 +92,6 @@ __global__ void edge_match_kernel(const float* __restrict__ x, int H, int W, int
     }
     const float d = x[ia] - x[ib];
     s += (double)d * d;
-    if (g) {
-      const float gd = grad_scale * weight * 2.f * d * k;
-      // the two strips can overlap when 2 em > size: serialise through atomics (tiny)
-      atomicAdd(g + ia, gd);
-      atomicAdd(g + ib, -gd);
-    }
   }
   red[threadIdx.x] = s;
   __syncthreads();
@@ -108,6 +101,31 @@ __global__ void edge_match_kernel(const float* __restrict__ x, int H, int W, int
     const float l = weight * (float)(t * (double)k);
     *loss_out = accumulate_loss ? *loss_out + l : l;
   }
+}
+// its gradient, g += grad_scale * weight * dloss/dx, in gather form: one thread per element of the union of the two strips
+// (the first em and the last em positions along the axis; the whole axis when 2 em > size, where the strips overlap and an
+// element takes both terms), so every element has one writer and its value does not depend on scheduling.
+__global__ void edge_match_grad_kernel(const float* __restrict__ x, int H, int W, int em, int axis, float weight,
+                                       float grad_scale, float* __restrict__ g) {
+  pdl_prologue();
+  const int L = axis == 0 ? W : H, other = axis == 0 ? H : W;
+  const int nu = 2 * em < L ? 2 * em : L;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= 3 * other * nu) return;
+  int j, r, c;
+  if (axis == 0) {
+    j = i % nu, r = (i / nu) % H, c = i / (nu * H);
+  } else {
+    r = i % W, j = (i / W) % nu, c = i / (W * nu);
+  }
+  const int n = 3 * other * em, lo = L - em;
+  const float k = 1.f / ((float)n * (float)em), coef = grad_scale * weight * 2.f * k;
+  auto at = [&](int p) -> size_t { return axis == 0 ? ((size_t)c * H + r) * W + p : ((size_t)c * H + p) * W + r; };
+  const int p = j < em ? j : L - nu + j;  // position along the axis
+  float v = g[at(p)];
+  if (p < em) v += coef * (x[at(p)] - x[at(lo + p)]);            // p in the first strip: + d(p)
+  if (p >= lo) v -= coef * (x[at(p - lo)] - x[at(p)]);           // p in the last strip: - d(p - (L - em))
+  g[at(p)] = v;
 }
 
 // ColorLookup (colorlookup.py:51-86): z_q = nearest palette colour (torch.cdist + argmin: first minimum), value out = z_q,
@@ -186,7 +204,11 @@ void filter_crop_backward(const float* gy, int H, int W, int top, int left, int 
 }
 void filter_edge_match(const float* x, int H, int W, int em, int axis, float weight, float grad_scale, int accumulate_loss,
                        float* g, float* loss_out, cudaStream_t st) {
-  launch_pdl(edge_match_kernel, dim3(1), dim3(256), 0, st, x, H, W, em, axis, weight, grad_scale, accumulate_loss, g, loss_out);
+  if (loss_out) launch_pdl(edge_match_loss_kernel, dim3(1), dim3(256), 0, st, x, H, W, em, axis, weight, accumulate_loss, loss_out);
+  if (g) {
+    const int L = axis == 0 ? W : H, n = 3 * (axis == 0 ? H : W) * (2 * em < L ? 2 * em : L);
+    launch_pdl(edge_match_grad_kernel, dim3((n + 255) / 256), dim3(256), 0, st, x, H, W, em, axis, weight, grad_scale, g);
+  }
 }
 void filter_colorlookup(const float* x, int pixels, const float* pal, int n_col, float beta, float weight, float* y,
                         int* best_out, double* part, float* loss_out, cudaStream_t st) {

@@ -279,6 +279,16 @@ def test_pixel_drawer_grid_follows_the_reference_defaults(fake, tmp_path):
     assert api._state.engine.kw["grid"] == (80, 80)
 
 
+def test_fft_colors_leaves_the_fft_image_alone(fake, tmp_path):
+    """FftDrawer builds to_valid_rgb(image_f, colors=1.5) with the value written into the call (fftdrawer.py:61); its
+    fft_colors only reaches dwt_image.  So fft_colors=3.0 still builds the engine's colour matrix from 1.5 (the engine's
+    0 means 1.5), while fft_decay does reach it."""
+    _init(tmp_path, prompts="x", drawer="fft", clip_models="ViT-B/32", fft_colors=3.0, fft_decay=2.0)
+    kw = api._state.engine.kw
+    assert kw["drawer"] == E.DRAWER_FFT and kw["fft_decay"] == 2.0
+    assert (kw.get("fft_colors") or 1.5) == 1.5
+
+
 def test_aesthetic_loss_is_usable_through_the_settings(fake, tmp_path):
     """custom_loss='aesthetic' (pixray.py:131-140, Losses/AestheticLoss.py): the linear AVA head the reference downloads comes
     in through `aesthetic_head` (dict or .pth path); without it the error names the missing file."""

@@ -33,7 +33,7 @@ Out of scope: exact ties of the batch extremes (torch's full-reduction min() / m
 tied elements, the engine gives it to the first index; pixray always adds noise, pixray.py:508-510, so such ties do not
 occur in the reference -- each case plants two unmistakable extremes); spot-prompt passes (only the last pass's
 g_patches can be read back; tests/test_spot_prompts_gpu.py covers them); colour jitter (tests/test_color_jitter.py, at a
-bound derived from its HSV discontinuities); the FFT drawer's backward.
+bound derived from its HSV discontinuities).
 """
 import numpy as np
 import pytest
