@@ -2554,14 +2554,27 @@ void Engine::finalize() {
       reg(p + "g_patches", C.g_patches, (size_t)C.B * C.np * C.Kp * 2);
       reg(p + "t", C.t, mw * 4);
       const size_t xb = stream16 ? 2 : 4;  // bytes per residual-stream element
-      reg(p + "x0", C.layers[0].x_in, mw * xb);
-      reg(p + "x_mid0", C.layers[0].x_mid, mw * xb);
-      reg(p + "qkv0", C.layers[0].qkv, mw * 3 * 2);
-      if (C.layers[0].P) reg(p + "P0", C.layers[0].P, (size_t)C.B * C.c.heads * C.T * C.ldT * 2);
+      // every layer's saved activations: x{l} its input (x{L} is x_out), x_mid{l}, qkv{l}, u{l} the MLP pre-activation
+      // (B rows, compact, in a class-rows-only last layer), and o{l} (fused attention) or P{l} (row softmax, pitch ldT)
+      const int L = (int)C.layers.size();
+      for (int l = 0; l < L; ++l) {
+        const Clip::Layer& Ly = C.layers[l];
+        const std::string s = std::to_string(l);
+        reg(p + "x" + s, Ly.x_in, mw * xb);
+        reg(p + "x_mid" + s, Ly.x_mid, mw * xb);
+        reg(p + "qkv" + s, Ly.qkv, mw * 3 * 2);
+        reg(p + "u" + s, Ly.u, mw * 4 * 2);
+        if (Ly.o) reg(p + "o" + s, Ly.o, mw * 2);
+        if (Ly.P) reg(p + "P" + s, Ly.P, (size_t)C.B * C.c.heads * C.T * C.ldT * 2);
+      }
+      reg(p + "x" + std::to_string(L), C.x_out, mw * xb);
       reg(p + "x_out", C.x_out, mw * xb);
+      reg(p + "hcls", C.hcls, (size_t)C.B * C.c.width * 2);
       reg(p + "e", C.e, (size_t)C.B * C.c.out_dim * 4);
       reg(p + "de", C.de, (size_t)C.B * C.c.out_dim * 4);
+      reg(p + "de16", C.de16, (size_t)C.B * C.c.out_dim * 2);
       if (C.gx) reg(p + "gx", C.gx, mw * 4);
+      reg(p + "gx16", C.gx16, mw * 2);
     }
   }
   for (auto& m : weights) m.clear();  // host copies no longer needed
