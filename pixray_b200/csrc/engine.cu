@@ -375,8 +375,9 @@ class Engine {
   }
   // Tile width by a wave-quantisation cost model: a persistent grid of num_sms CTAs runs ceil(tiles / num_sms) waves
   // of tiles whose cost grows with bn (plus a fixed per-tile overhead); e.g. M = 12608, N = 768 is 297 tiles of 256
-  // (3 waves for 2.007 waves of work) but 396 tiles of 192 (3 cheaper waves).
-  int pick_bn(int N, bool b_mn, long long m_tiles) const {
+  // (3 waves for 2.007 waves of work) but 396 tiles of 192 (3 cheaper waves).  wide: the GEMM may use 192- and 256-wide
+  // tiles (gemm_wide_ok); every other GEMM and convolution has tiles of at most 128 columns.
+  int pick_bn(int N, bool b_mn, long long m_tiles, bool wide = false) const {
     const int step = b_mn ? 64 : 16;
     {  // PXR_GEMM_BN="3072:256,768:192": tile width by output width, for A/B measurements of the cost model's choices
       static const std::map<int, int> forced = [] {
@@ -400,8 +401,8 @@ class Engine {
     if (N <= 128 && m_tiles * 1 >= num_sms / 2) return narrow(N);
     int best = 0;
     double best_cost = 1e30;
-    for (int bn = 128; bn >= 64; bn -= 64) {  // gemm_tc.cu: tiles are at most 128 wide
-      if (bn % step) continue;
+    for (int bn : {256, 192, 128, 64}) {
+      if (bn % step || (bn > 128 && !wide)) continue;
       const long long tiles = m_tiles * ((N + bn - 1) / bn);
       const long long waves = (tiles + num_sms - 1) / num_sms;
       // narrower tiles re-read A more often and sit closer to the smem-bandwidth limit: mild penalty
@@ -416,7 +417,7 @@ class Engine {
   }
   void add_gemm(OpList& l, const GemmOperand& A, const GemmOperand& B, int M, int N, int K, const GemmEpilogue& e,
                 int bn = 0) {
-    if (!bn) bn = pick_bn(N, B.mode == OP_MNMAJOR, (long long)((M + 127) / 128) * A.nb0 * A.nb1);
+    if (!bn) bn = pick_bn(N, B.mode == OP_MNMAJOR, (long long)((M + 127) / 128) * A.nb0 * A.nb1, gemm_wide_ok(A, N, e, fmt));
     auto plan = std::make_shared<GemmPlan>();
     char buf[256] = {0};
     int rc = gemm_plan_make(plan.get(), A, B, M, N, K, e, bn, fmt, num_sms, buf, sizeof buf);

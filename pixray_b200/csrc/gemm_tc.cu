@@ -420,7 +420,7 @@ __device__ __forceinline__ void producer_loop(const GemmParams& p, uint8_t* smem
 }
 
 // Accumulator of one warpgroup: 64 rows x NCH 64-column wgmma fragments, sized per kernel: NF for the 64- / 128-wide
-// fp16 kernels, two for the generic-width kernel (tiles are at most 128 wide, so a 16-column tail always lands in the
+// fp16 kernels, two for the generic-width kernel (this kernel's tiles are at most 128 wide, so a 16-column tail always lands in the
 // first two fragments).
 template <int NCH>
 struct WgAcc {
@@ -558,6 +558,34 @@ __device__ __forceinline__ __half2 quickgelu_grad_h2(__half2 u) {
   return __hfma2(s, b, s);                       // s (1 + 1.702 u (1 - s))
 }
 
+// Per-element arithmetic of both tensor-map epilogues (this kernel's and gemm_wide_kernel's), so the two compute the
+// same bits: x = acc * alpha, then + bias, each rounded on its own (__fmul_rn / __fadd_rn: FMUL then FADD, never a
+// contracted FFMA), then the mode's tail on one column pair.  `in` is the pair of the input tensor (residual or saved
+// pre-activation); the forward activations also return the saved fp16 pre-activation in `aux`.
+__device__ __forceinline__ float te_scale(float acc, float alpha) { return __fmul_rn(acc, alpha); }
+__device__ __forceinline__ float te_add(float x, float b) { return __fadd_rn(x, b); }
+__device__ __forceinline__ uint32_t h2_bits(__half2 h) { return *reinterpret_cast<uint32_t*>(&h); }
+__device__ __forceinline__ __half2 bits_h2(uint32_t u) { return *reinterpret_cast<__half2*>(&u); }
+template <int MODE>
+__device__ __forceinline__ uint32_t te_pair(float x0, float x1, uint32_t in, uint32_t& aux) {
+  if (MODE == TE_F16) return h2_bits(__floats2half2_rn(x0, x1));
+  if (MODE == TE_RES16) {
+    const float2 u = __half22float2(bits_h2(in));
+    return h2_bits(__floats2half2_rn(te_add(x0, u.x), te_add(x1, u.y)));
+  }
+  if (MODE == TE_GELU || MODE == TE_ERF_GELU) {  // the saved pre-activation (fp16), and the activation of exactly that value
+    const __half2 u = __floats2half2_rn(x0, x1);
+    aux = h2_bits(u);
+    if (MODE == TE_GELU) return h2_bits(quickgelu_h2(u));
+    const float2 v = __half22float2(u);
+    return h2_bits(__floats2half2_rn(gelu_erf(v.x), gelu_erf(v.y)));
+  }
+  if (MODE == TE_GELU_BWD) return h2_bits(__hmul2(__floats2half2_rn(x0, x1), quickgelu_grad_h2(bits_h2(in))));
+  // TE_ERF_GELU_BWD: fp32 product, as the generic epilogue forms it
+  const float2 v = __half22float2(bits_h2(in));
+  return h2_bits(__floats2half2_rn(__fmul_rn(x0, gelu_erf_grad(v.x)), __fmul_rn(x1, gelu_erf_grad(v.y))));
+}
+
 // One tile of the tensor-map epilogue for warp `warp` (rows [32 q, 32 q + 32) of the tile, column blocks half, half + 2,
 // ...).  `cnt` counts the blocks this warp has processed: box rotation and input-barrier parity.
 template <int MODE>
@@ -565,7 +593,6 @@ __device__ __forceinline__ void tma_epilogue_tile(const GemmParams& p, const Til
                                                   uint64_t* in_bar, const float* arow, int warp, int lane,
                                                   uint32_t& cnt) {
   constexpr bool F32 = (MODE == TE_RES32);
-  constexpr bool ERF = (MODE == TE_ERF_GELU || MODE == TE_ERF_GELU_BWD);  // exact GELU, else QuickGELU
   constexpr bool ACT_FWD = (MODE == TE_GELU || MODE == TE_ERF_GELU);
   constexpr bool ACT_BWD = (MODE == TE_GELU_BWD || MODE == TE_ERF_GELU_BWD);
   constexpr bool IN = (ACT_BWD || MODE == TE_RES32 || MODE == TE_RES16);
@@ -622,80 +649,45 @@ __device__ __forceinline__ void tma_epilogue_tile(const GemmParams& p, const Til
         float a[32];
         load_acc(arow + s * BW, (!F32 && p.block_n - s * BW > 16) ? 32 : 16, a);  // block_n % 32 == 16: last block half wide
 #pragma unroll
-        for (int i = 0; i < BW; ++i) x[i] = a[i] * p.alpha;
+        for (int i = 0; i < BW; ++i) x[i] = te_scale(a[i], p.alpha);
       }
       if (p.bias) {
         const float4* bp = reinterpret_cast<const float4*>(p.bias + col);
 #pragma unroll
         for (int i = 0; i < BW / 4; ++i) {
           const float4 b = __ldg(bp + i);
-          x[4 * i] += b.x;
-          x[4 * i + 1] += b.y;
-          x[4 * i + 2] += b.z;
-          x[4 * i + 3] += b.w;
+          x[4 * i] = te_add(x[4 * i], b.x);
+          x[4 * i + 1] = te_add(x[4 * i + 1], b.y);
+          x[4 * i + 2] = te_add(x[4 * i + 2], b.z);
+          x[4 * i + 3] = te_add(x[4 * i + 3], b.w);
         }
       }
       if (IN) mbar_wait(&in_bar[k & 3], (k >> 2) & 1);
-      if (MODE == TE_F16) {
-#pragma unroll
-        for (int c = 0; c < 4; ++c) *reinterpret_cast<uint4*>(buf + te_off(lane, c)) = pack8(x + 8 * c);
-      } else if (ACT_FWD) {
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          uint4 u = pack8(x + 8 * c);  // the saved pre-activation (fp16), and the activation of exactly that value
-          *reinterpret_cast<uint4*>(buf + te_off(lane, c)) = u;
-          if (ERF) {
-            float v[8];
-            unpack8(u, v);
-#pragma unroll
-            for (int i = 0; i < 8; ++i) v[i] = gelu_erf(v[i]);
-            u = pack8(v);
-          } else {
-            __half2* h = reinterpret_cast<__half2*>(&u);
-#pragma unroll
-            for (int j = 0; j < 4; ++j) h[j] = quickgelu_h2(h[j]);
-          }
-          *reinterpret_cast<uint4*>(buf + TE_BUF_BYTES + te_off(lane, c)) = u;
-        }
-      } else if (ACT_BWD) {
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          uint4* ptr = reinterpret_cast<uint4*>(buf + te_off(lane, c));
-          uint4 u = *ptr;
-          if (ERF) {  // fp32 product, as the generic epilogue forms it
-            float v[8];
-            unpack8(u, v);
-#pragma unroll
-            for (int i = 0; i < 8; ++i) x[8 * c + i] *= gelu_erf_grad(v[i]);
-            *ptr = pack8(x + 8 * c);
-          } else {
-            uint4 g = pack8(x + 8 * c);
-            const __half2* uh = reinterpret_cast<const __half2*>(&u);
-            __half2* gh = reinterpret_cast<__half2*>(&g);
-#pragma unroll
-            for (int j = 0; j < 4; ++j) gh[j] = __hmul2(gh[j], quickgelu_grad_h2(uh[j]));
-            *ptr = g;
-          }
-        }
-      } else if (MODE == TE_RES16) {
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          uint4* ptr = reinterpret_cast<uint4*>(buf + te_off(lane, c));
-          float u[8];
-          unpack8(*ptr, u);
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            if (MODE == TE_GELU_BWD) x[8 * c + i] *= quickgelu_grad(u[i]);
-            else x[8 * c + i] += u[i];
-          }
-          *ptr = pack8(x + 8 * c);
-        }
-      } else {  // TE_RES32
+      if constexpr (MODE == TE_RES32) {
 #pragma unroll
         for (int c = 0; c < 4; ++c) {
           float4* ptr = reinterpret_cast<float4*>(buf + te_off(lane, c));
           const float4 r = *ptr;
-          *ptr = make_float4(x[4 * c] + r.x, x[4 * c + 1] + r.y, x[4 * c + 2] + r.z, x[4 * c + 3] + r.w);
+          *ptr = make_float4(te_add(x[4 * c], r.x), te_add(x[4 * c + 1], r.y), te_add(x[4 * c + 2], r.z),
+                             te_add(x[4 * c + 3], r.w));
+        }
+      } else {
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+          uint4* ptr = reinterpret_cast<uint4*>(buf + te_off(lane, c));
+          const uint4 in = IN ? *ptr : make_uint4(0, 0, 0, 0);
+          uint4 o, aux = make_uint4(0, 0, 0, 0);
+          const float* xc = x + 8 * c;
+          o.x = te_pair<MODE>(xc[0], xc[1], in.x, aux.x);
+          o.y = te_pair<MODE>(xc[2], xc[3], in.y, aux.y);
+          o.z = te_pair<MODE>(xc[4], xc[5], in.z, aux.z);
+          o.w = te_pair<MODE>(xc[6], xc[7], in.w, aux.w);
+          if (ACT_FWD) {  // box: the pre-activation (tma_d); box + 1: the activation (tma_c)
+            *ptr = aux;
+            *reinterpret_cast<uint4*>(buf + TE_BUF_BYTES + te_off(lane, c)) = o;
+          } else {
+            *ptr = o;
+          }
         }
       }
       fence_proxy_async_smem();
@@ -829,6 +821,233 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tce_kernel(const __grid_
   gemm_body<false, MODE, NF>(p);
 }
 
+// -------------------------------------------------------------------------------- wide kernel: 128 x 192 / 128 x 256
+// For fp16 GEMMs with a K-major, unbatched A, no split-K and a tensor-map epilogue other than TE_RES32 (the ViT linear
+// layers and their dgrads), a requested block_n of 192 or 256 runs here instead of in gemm_body.
+//   * 384 threads.  Warpgroup 0 is the producer: one lane walks producer_tiles, the warpgroup drops to 40 registers.
+//     Warpgroups 1 and 2 own tile rows [0, 64) and [64, 128) and rise to 232 registers: 40 * 128 + 232 * 256 = 64,512
+//     = 168 * 384, what one CTA holds at __launch_bounds__(384, 1).  A 64 x 256 fp32 accumulator is 128 of them.
+//   * One m64nBNk16 wgmma per consumer warpgroup and k16 step (a single static instruction, no runtime-guarded chain),
+//     each stage released as soon as its wgmma group has retired, as in mma_tile.
+//   * Epilogue straight from the accumulator registers, 64 columns at a time: each warp converts its 16 rows to fp16
+//     (te_pair, the arithmetic of tma_epilogue_tile), writes them with stmatrix into a 16 x 128-byte box (128-byte
+//     swizzle) and hands the box to a TMA store, which clips ragged M and N.  TE_ERF_GELU_BWD stays on gemm_body: its
+//     32 erfc / exp evaluations per chunk beside the 128-register accumulator spill at 232 registers.  An input tensor (fp16 residual, saved
+//     pre-activation) arrives by TMA in the same box up to two chunks ahead and is read into the fragment layout with
+//     ldmatrix.  No staged fp32 tile and no barrier between the consumer warpgroups; the producer refills the ring for
+//     the next tile while they run it.
+// Shared memory (227 KiB = 232,448 bytes): 1 KiB alignment slack, the stage ring, GEMM_BAR_BYTES of barriers and two
+// 2 KiB boxes per consumer warp (32 KiB); the ring gets the remaining 197,632 bytes: 4 stages of 48 KiB at BN = 256,
+// 4 of 40 KiB at BN = 192.
+constexpr int WB_BYTES = 2048;  // one box: 16 rows x 64 fp16 columns
+constexpr int WB_BOXES = 2;     // per consumer warp
+constexpr int WIDE_CONSUMER_WARPS = 8;
+constexpr int WIDE_EPI_BYTES = WIDE_CONSUMER_WARPS * WB_BOXES * WB_BYTES;
+
+// byte offset of 16-byte chunk c (0..7) of row r (0..15) in a CU_TENSOR_MAP_SWIZZLE_128B box (chunk ^= address bits 7..9)
+__device__ __forceinline__ uint32_t wb_off(int r, int c) {
+  return static_cast<uint32_t>(r * 128 + ((c ^ (r & 7)) << 4));
+}
+
+// Consumer warpgroup `wg` (0 or 1): wgmma over the n_kb k-blocks of one tile, as mma_tile with one instruction per k16
+// step.  `first` runs once the first k-block has been issued (the epilogue's input prefetch).
+template <int BN, int TB, typename First>
+__device__ __forceinline__ void mma_tile_wide(float (&acc)[BN / 2], int wg, int n_kb, int stages, uint32_t smem0,
+                                              uint32_t full0, uint64_t* empty_bar, int& stage, uint32_t& phase,
+                                              First&& first) {
+  constexpr uint32_t stage_bytes = A_TILE_BYTES + BN * GEMM_BLOCK_K * 2;
+  const uint64_t b_kstep = (TB ? 2048 : 32) >> 4;
+  const uint64_t a_desc0 = make_smem_desc_sw128(smem0 + wg * 8192, 0, 1024);
+  const uint64_t b_desc0 = make_smem_desc_sw128(smem0 + A_TILE_BYTES, TB ? MN_ATOM_BYTES : 0, 1024);
+  const bool elected = (threadIdx.x & 127) == 0;
+  int prev = -1;
+  for (int kb = 0; kb < n_kb; ++kb) {
+    mbar_wait_s(full0 + stage * 8, phase);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const uint64_t ad = a_desc0 + stage * (stage_bytes >> 4) + k * (32 >> 4);
+      const uint64_t bd = b_desc0 + stage * (stage_bytes >> 4) + k * b_kstep;
+      const uint32_t scale_d = (kb | k) ? 1u : 0u;
+      if constexpr (BN == 256) wgmma_m64n256<0, TB>(acc, ad, bd, scale_d);
+      else wgmma_m64n192<0, TB>(acc, ad, bd, scale_d);
+    }
+    wgmma_commit();
+    if (kb == 0) first();
+    wgmma_wait<1>();
+    if (prev >= 0 && elected) mbar_arrive(&empty_bar[prev]);
+    prev = stage;
+    if (++stage == stages) {
+      stage = 0;
+      phase ^= 1;
+    }
+  }
+  wgmma_wait<0>();
+  if (prev >= 0 && elected) mbar_arrive(&empty_bar[prev]);
+}
+
+// TMA load of the input tensor's 64-column chunk at `col` into one box of this warp (lane 0)
+__device__ __forceinline__ void wide_in_load(const GemmParams& p, uint64_t* bar, uint8_t* box, int col, int row0,
+                                             const TileCoord& t) {
+  mbar_arrive_expect_tx(bar, WB_BYTES);
+  tma_load_4d(&p.tma_d, bar, box, col, row0, t.b0, t.b1);
+}
+
+// One tile's epilogue for one consumer warp: rows [row0, row0 + 16) of the output, the 64-column chunks with at least one
+// column inside N.  `cnt` counts the chunks this warp has processed: chunk j of the tile goes to box (cnt + j) % 2 (the
+// forward activations use both boxes for every chunk).  in_ph: the parity of each box's input barrier.
+template <int MODE, int BN>
+__device__ __forceinline__ void wide_epilogue_tile(const GemmParams& p, const TileCoord& t, const float (&acc)[BN / 2],
+                                                   uint8_t* wbuf, uint64_t* in_bar, int row0, int lane, uint32_t& cnt,
+                                                   uint32_t& in_ph) {
+  constexpr bool ACT_FWD = (MODE == TE_GELU || MODE == TE_ERF_GELU);
+  constexpr bool IN = (MODE == TE_RES16 || MODE == TE_GELU_BWD || MODE == TE_ERF_GELU_BWD);
+  const int nch = (min(p.N - t.n0, BN) + 63) / 64;
+  const uint32_t wb0 = smem_u32(wbuf);
+  // stmatrix / ldmatrix x4 over column groups (2 q, 2 q + 1): matrix m = lane / 8 is rows 8 (m % 2) .. + 7 of group
+  // 2 q + m / 2, and its register is the fragment's pair 4 q + m, i.e. accumulator registers 8 q + 2 m, + 1 of the chunk
+  const int mrow = (lane & 7) + 8 * ((lane >> 3) & 1), mgrp = lane >> 4;
+#pragma unroll
+  for (int j = 0; j < BN / 64; ++j) {
+    if (j < nch) {
+      const int col = t.n0 + 64 * j;
+      const int b = ACT_FWD ? 0 : ((cnt + j) & 1);
+      const uint32_t box = wb0 + b * WB_BYTES;
+      if (lane == 0) {
+        if (ACT_FWD) bulk_wait_group_read<0>();  // both boxes' stores of the previous chunk have read them
+        else if (!IN) bulk_wait_group_read<1>();  // this box's store, two chunks back (possibly in the previous tile)
+      }
+      __syncwarp();
+      uint32_t in[16];
+      if (IN) {
+        mbar_wait(&in_bar[b], (in_ph >> b) & 1);
+        in_ph ^= 1u << b;
+#pragma unroll
+        for (int q = 0; q < 4; ++q) ldmatrix_x4(box + wb_off(mrow, 2 * q + mgrp), in[4 * q], in[4 * q + 1], in[4 * q + 2], in[4 * q + 3]);
+      } else {
+#pragma unroll
+        for (int i = 0; i < 16; ++i) in[i] = 0;
+      }
+      uint32_t out[16], aux[16];
+#pragma unroll
+      for (int g = 0; g < 8; ++g) {  // column group g: columns col + 8 g + 2 (lane % 4), + 1; rows lo / hi
+        const int c = col + 8 * g + 2 * (lane & 3);
+        float2 bb = make_float2(0.f, 0.f);
+        if (p.bias && c < p.N) bb = __ldg(reinterpret_cast<const float2*>(p.bias + c));
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int r = 32 * j + 4 * g + 2 * h;
+          float x0 = te_scale(acc[r], p.alpha), x1 = te_scale(acc[r + 1], p.alpha);
+          if (p.bias) {
+            x0 = te_add(x0, bb.x);
+            x1 = te_add(x1, bb.y);
+          }
+          aux[2 * g + h] = 0;
+          out[2 * g + h] = te_pair<MODE>(x0, x1, in[2 * g + h], aux[2 * g + h]);
+        }
+      }
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const uint32_t o = wb_off(mrow, 2 * q + mgrp);
+        if (ACT_FWD) {  // box 0: the pre-activation (tma_d), box 1: the activation (tma_c)
+          stmatrix_x4(wb0 + o, aux[4 * q], aux[4 * q + 1], aux[4 * q + 2], aux[4 * q + 3]);
+          stmatrix_x4(wb0 + WB_BYTES + o, out[4 * q], out[4 * q + 1], out[4 * q + 2], out[4 * q + 3]);
+        } else {
+          stmatrix_x4(box + o, out[4 * q], out[4 * q + 1], out[4 * q + 2], out[4 * q + 3]);
+        }
+      }
+      fence_proxy_async_smem();
+      __syncwarp();
+      if (lane == 0) {
+        if (ACT_FWD) {
+          tma_store_4d(&p.tma_d, wbuf, col, row0, t.b0, t.b1);
+          tma_store_4d(&p.tma_c, wbuf + WB_BYTES, col, row0, t.b0, t.b1);
+        } else {
+          tma_store_4d(&p.tma_c, wbuf + b * WB_BYTES, col, row0, t.b0, t.b1);
+        }
+        bulk_commit_group();
+        if (IN && j + 2 < nch) {
+          bulk_wait_group_read<0>();  // the store just issued has read the box
+          wide_in_load(p, &in_bar[b], wbuf + b * WB_BYTES, col + 128, row0, t);
+        }
+      }
+    }
+  }
+  cnt += nch;
+}
+
+template <int MODE, int BN, int TB>
+__global__ void __launch_bounds__(GEMM_WIDE_THREADS, 1) gemm_wide_kernel(const __grid_constant__ GemmParams p) {
+  pdl_launch_dependents();
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t smem_base_u32 = smem_u32(smem_raw);
+  uint8_t* smem = smem_raw + (((smem_base_u32 + 1023u) & ~1023u) - smem_base_u32);
+  constexpr uint32_t stage_bytes = A_TILE_BYTES + BN * GEMM_BLOCK_K * 2;
+  constexpr bool IN = (MODE == TE_RES16 || MODE == TE_GELU_BWD || MODE == TE_ERF_GELU_BWD);
+  uint8_t* bar_block = smem + static_cast<size_t>(p.stages) * stage_bytes;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(bar_block);
+  uint64_t* empty_bar = full_bar + GEMM_MAX_STAGES;
+  uint64_t* in_bars = reinterpret_cast<uint64_t*>(bar_block + 256);  // [WIDE_CONSUMER_WARPS][WB_BOXES]
+  uint8_t* boxes = bar_block + GEMM_BAR_BYTES;                        // 1024-byte aligned (128-byte swizzle)
+
+  if (threadIdx.x == 0) {
+    prefetch_tmap(&p.tma_a);
+    prefetch_tmap(&p.tma_b);
+    prefetch_tmap(&p.tma_c);
+    if (MODE != TE_F16) prefetch_tmap(&p.tma_d);
+    for (int i = 0; i < p.stages; ++i) {
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], 2);  // one arrive per consumer warpgroup
+    }
+    for (int i = 0; i < WIDE_CONSUMER_WARPS * WB_BOXES; ++i) mbar_init(&in_bars[i], 1);
+    fence_barrier_init();
+  }
+  __syncthreads();
+  pdl_wait();  // everything above touched only parameters and shared memory
+
+  if (threadIdx.x < 128) {
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) producer_tiles<OP_KMAJOR, TB ? OP_MNMAJOR : OP_KMAJOR>(p, smem, full_bar, empty_bar, stage_bytes);
+    return;
+  }
+  setmaxnreg_inc<232>();
+  const int wg = (threadIdx.x >> 7) - 1;  // consumer warpgroup: tile rows [64 wg, 64 wg + 64)
+  const int cw = (threadIdx.x >> 5) - 4;  // consumer warp 0..7
+  const int lane = threadIdx.x & 31;
+  uint8_t* wbuf = boxes + cw * (WB_BOXES * WB_BYTES);
+  uint64_t* in_bar = in_bars + cw * WB_BOXES;
+  const uint32_t smem0 = smem_u32(smem), full0 = smem_u32(full_bar);
+  int stage = 0;
+  uint32_t phase = 0, cnt = 0, in_ph = 0;
+  float acc[BN / 2];
+  for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+    const TileCoord t = decode_tile(p, tile);
+    const int row0 = t.m0 + 64 * wg + 16 * (cw & 3);
+    mma_tile_wide<BN, TB>(acc, wg, p.num_k_blocks, p.stages, smem0, full0, empty_bar, stage, phase, [&] {
+      if (IN && lane == 0) {  // the first two input chunks, while the rest of the tile's k-blocks run
+        const int nch = (min(p.N - t.n0, BN) + 63) / 64;
+        bulk_wait_group_read<0>();  // the previous tile's stores have read the boxes
+        for (int j = 0; j < WB_BOXES && j < nch; ++j)
+          wide_in_load(p, &in_bar[(cnt + j) & 1], wbuf + ((cnt + j) & 1) * WB_BYTES, t.n0 + 64 * j, row0, t);
+      }
+    });
+    wide_epilogue_tile<MODE, BN>(p, t, acc, wbuf, in_bar, row0, lane, cnt, in_ph);
+  }
+  if (lane == 0) bulk_wait_group<0>();
+}
+
+template <int BN, int TB>
+void (*wide_kernel(const GemmParams& p))(GemmParams) {
+  switch (p.tma_epi) {
+    case TE_F16: return gemm_wide_kernel<TE_F16, BN, TB>;
+    case TE_RES16: return gemm_wide_kernel<TE_RES16, BN, TB>;
+    case TE_GELU: return gemm_wide_kernel<TE_GELU, BN, TB>;
+    case TE_GELU_BWD: return gemm_wide_kernel<TE_GELU_BWD, BN, TB>;
+    case TE_ERF_GELU: return gemm_wide_kernel<TE_ERF_GELU, BN, TB>;
+    default: return nullptr;
+  }
+}
+
 // The kernel for a plan: fragment width NF (see mma_tile) and epilogue.
 template <int NF>
 void (*plain_kernel(const GemmParams& p))(GemmParams) {
@@ -848,6 +1067,8 @@ void (*plain_kernel(const GemmParams& p))(GemmParams) {
   return erf ? gemm_tc_kernel<NF, true> : gemm_tc_kernel<NF>;
 }
 void (*kernel_for(const GemmParams& p))(GemmParams) {
+  if (p.block_n == 256) return p.b_mode == OP_MNMAJOR ? wide_kernel<256, 1>(p) : wide_kernel<256, 0>(p);
+  if (p.block_n == 192) return p.b_mode == OP_MNMAJOR ? wide_kernel<192, 1>(p) : wide_kernel<192, 0>(p);
   if (p.fmt == 0 && p.block_n == 128) return plain_kernel<2>(p);
   if (p.fmt == 0 && p.block_n == 64) return plain_kernel<1>(p);
   return plain_kernel<0>(p);
@@ -952,12 +1173,14 @@ int tmap_encode_4d(CUtensorMap* out, const void* ptr, int fmt, const uint64_t di
 }
 
 namespace {
-// Widest tile: the staged fp32 accumulator tile (128 x block_n) shares the 227 KiB of shared memory with the stage ring
-// and the epilogue buffers; at 128 columns two stages still fit beside the tensor-map epilogue's boxes, three beside the
-// generic epilogue's.  A wider request runs as 128.
+// Widest tile of gemm_body: the staged fp32 accumulator tile (128 x block_n) shares the 227 KiB of shared memory with the
+// stage ring and the epilogue buffers; at 128 columns two stages still fit beside the tensor-map epilogue's boxes, three
+// beside the generic epilogue's.  192 and 256 run in gemm_wide_kernel when the plan allows it (gemm_wide_ok); any other
+// wider request runs as 128.
 constexpr int GEMM_MAX_BN_PLAIN = 128;
 
 int effective_block_n(int block_n) { return block_n > GEMM_MAX_BN_PLAIN ? GEMM_MAX_BN_PLAIN : block_n; }
+bool wide_block_n(int block_n) { return block_n == 192 || block_n == 256; }
 
 // Tensor-map epilogue (see tma_epilogue_tile) when the epilogue is one of its shapes and every tensor can be described
 // by a tensor map; anything else keeps the generic epilogue.  PXR_GEMM_TMA_EPI=0 disables it globally.
@@ -992,13 +1215,16 @@ int decide_tma_epi(const GemmParams& p, const GemmEpilogue& e, int block_n) {
   return mode;
 }
 
+// Boxes of 32 rows x 64 bytes, 64-byte swizzle (tma_epilogue_tile) or, for the wide kernel, 16 rows x 64 fp16 columns,
+// 128-byte swizzle (wide_epilogue_tile).
 int encode_epilogue_map(CUtensorMap* out, const void* ptr, bool f32, const GemmParams& p, const GemmEpilogue& e,
                         char* err, int errlen) {
+  const bool wide = p.block_n > GEMM_MAX_BN_PLAIN;
   uint64_t dims[4], strides[3];
   uint32_t box[4];
   const uint64_t ldc = static_cast<uint64_t>(e.ldc);
   dims[0] = p.N;
-  box[0] = f32 ? 16 : 32;
+  box[0] = wide ? 64 : (f32 ? 16 : 32);
   if (p.a_mode == OP_CONV) {
     dims[1] = p.conv_W;
     dims[2] = p.conv_H;
@@ -1017,10 +1243,10 @@ int encode_epilogue_map(CUtensorMap* out, const void* ptr, bool f32, const GemmP
     strides[0] = ldc;
     strides[1] = p.nb0 > 1 ? static_cast<uint64_t>(e.bs0) : ldc * p.M;
     strides[2] = nb1 > 1 ? static_cast<uint64_t>(e.bs1) : strides[1] * p.nb0;
-    box[1] = 32;
+    box[1] = wide ? 16 : 32;
     box[2] = box[3] = 1;
   }
-  return encode_tmap4(out, ptr, f32 ? 2 : 0, dims, strides, box, err, errlen, true);
+  return encode_tmap4(out, ptr, f32 ? 2 : 0, dims, strides, box, err, errlen, !wide);
 }
 
 // bytes the epilogue must move for `mn` output elements: every output written once, every input tensor read once
@@ -1037,8 +1263,9 @@ double epilogue_bytes(const GemmEpilogue& e, double mn) {
 
 int finish_plan(GemmPlan* plan, const GemmEpilogue& epi, int block_n, int num_sms, char* err, int errlen) {
   GemmParams& p = plan->p;
-  if (block_n < 16 || block_n > GEMM_MAX_BN_PLAIN || block_n % 16) {
-    set_err(err, errlen, "block_n must be a multiple of 16 in [16, 128]");
+  const bool wide = wide_block_n(block_n);  // gemm_plan_make keeps 192 / 256 only for plans gemm_wide_ok accepts
+  if (!wide && (block_n < 16 || block_n > GEMM_MAX_BN_PLAIN || block_n % 16)) {
+    set_err(err, errlen, "block_n must be a multiple of 16 in [16, 128], or 192 / 256");
     return -10;
   }
   if (epi.act != ACT_NONE && epi.act != ACT_QUICKGELU && epi.act != ACT_QUICKGELU_BWD && epi.act != ACT_LRELU &&
@@ -1073,9 +1300,14 @@ int finish_plan(GemmPlan* plan, const GemmEpilogue& epi, int block_n, int num_sm
     if (!rc && second) rc = encode_epilogue_map(&p.tma_d, second, f32, p, epi, err, errlen);
     if (rc) p.tma_epi = TE_NONE;  // a stride the tensor map cannot express: generic epilogue
   }
+  if (wide && (p.tma_epi == TE_NONE || p.tma_epi == TE_RES32 || p.tma_epi == TE_ERF_GELU_BWD)) {
+    set_err(err, errlen, "192- / 256-wide tiles need an fp16 tensor-map epilogue");
+    return -15;
+  }
   const int stage_bytes = A_TILE_BYTES + block_n * GEMM_BLOCK_K * 2;
-  const int epi_smem = GEMM_BAR_BYTES + GEMM_BLOCK_M * acc_ld(block_n) * 4 +
-                       GEMM_EPI_WARPS * (p.tma_epi != TE_NONE ? TE_WARP_BYTES : TB_WARP_BYTES);
+  const int epi_smem = wide ? GEMM_BAR_BYTES + WIDE_EPI_BYTES
+                            : GEMM_BAR_BYTES + GEMM_BLOCK_M * acc_ld(block_n) * 4 +
+                                  GEMM_EPI_WARPS * (p.tma_epi != TE_NONE ? TE_WARP_BYTES : TB_WARP_BYTES);
   int stages = (227 * 1024 - 1024 - epi_smem) / stage_bytes;
   if (stages > GEMM_MAX_STAGES) stages = GEMM_MAX_STAGES;
   if (stages < 2) {  // mma_tile releases a stage only after the next one has been issued
@@ -1114,11 +1346,32 @@ int finish_plan(GemmPlan* plan, const GemmEpilogue& epi, int block_n, int num_sm
           q.act = act;
           cudaFuncSetAttribute(kernel_for(q), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
         }
+    for (int bn : {192, 256})
+      for (int bm : {OP_KMAJOR, OP_MNMAJOR})
+        for (int te : {TE_F16, TE_RES16, TE_GELU, TE_GELU_BWD, TE_ERF_GELU}) {  // every wide kernel
+          GemmParams q{};
+          q.block_n = bn;
+          q.b_mode = bm;
+          q.tma_epi = te;
+          cudaFuncSetAttribute(kernel_for(q), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+        }
   });
   return 0;
 }
 
 }  // namespace
+
+bool gemm_wide_ok(const GemmOperand& A, int N, const GemmEpilogue& epi, int fmt) {
+  if (fmt != 0 || A.mode != OP_KMAJOR || A.nb0 != 1 || A.nb1 != 1 || epi.k_splits > 1) return false;
+  GemmParams q{};  // what decide_tma_epi reads of a plan; at 192 / 256 columns every 32-column block is whole
+  q.fmt = fmt;
+  q.N = N;
+  q.a_mode = A.mode;
+  q.k_splits = 1;
+  q.tiles_n = 1;
+  const int te = decide_tma_epi(q, epi, 256);
+  return te != TE_NONE && te != TE_RES32 && te != TE_ERF_GELU_BWD;
+}
 
 int gemm_plan_make(GemmPlan* plan, const GemmOperand& A, const GemmOperand& B, int M, int N, int K,
                    const GemmEpilogue& epi, int block_n, int fmt, int num_sms, char* err, int errlen) {
@@ -1128,7 +1381,7 @@ int gemm_plan_make(GemmPlan* plan, const GemmOperand& A, const GemmOperand& B, i
     set_err(err, errlen, "use conv_plan_make for conv operands");
     return -20;
   }
-  block_n = effective_block_n(block_n);
+  if (!(wide_block_n(block_n) && gemm_wide_ok(A, N, epi, fmt))) block_n = effective_block_n(block_n);
   p.M = M;
   p.N = N;
   p.fmt = fmt;
@@ -1319,7 +1572,8 @@ void splitk_reduce(const float* ws, int splits, long long pixels, int N, int ld_
 }
 
 void gemm_launch(const GemmPlan& plan, cudaStream_t stream) {
-  launch_pdl(kernel_for(plan.p), dim3(plan.grid), dim3(GEMM_THREADS), plan.smem_bytes, stream, plan.p);
+  const int threads = plan.p.block_n > GEMM_MAX_BN_PLAIN ? GEMM_WIDE_THREADS : GEMM_THREADS;
+  launch_pdl(kernel_for(plan.p), dim3(plan.grid), dim3(threads), plan.smem_bytes, stream, plan.p);
 }
 
 }  // namespace pxr

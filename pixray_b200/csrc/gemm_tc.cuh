@@ -9,10 +9,12 @@
 //   * 3x3 / 1x1 convolutions of the VQGAN decoder as implicit GEMM: the A operand is fetched by a 4-D TMA
 //     box (C, W, H, B) shifted per filter tap, out-of-image halo zero-filled by TMA.
 //
-// Structure: warps 0..7 = two MMA warpgroups (64 tile rows each, fp32 accumulators in registers) that then run the
-// epilogue, warp 8 = TMA producer.  smem ring of `stages` {A 128x64, B block_n x 64} tiles (128-byte swizzle); after the
-// main loop the fragments are staged as a row-major fp32 tile in shared memory, from which the epilogue warps read whole
-// rows and write coalesced, while the producer already streams the next tile's operands into the ring.
+// Structure (tiles up to 128 wide): warps 0..7 = two MMA warpgroups (64 tile rows each, fp32 accumulators in registers)
+// that then run the epilogue, warp 8 = TMA producer.  smem ring of `stages` {A 128x64, B block_n x 64} tiles (128-byte
+// swizzle); after the main loop the fragments are staged as a row-major fp32 tile in shared memory, from which the
+// epilogue warps read whole rows and write coalesced, while the producer already streams the next tile's operands into
+// the ring.  192- and 256-wide tiles (gemm_wide_ok) run in a second kernel: a producer warpgroup, two consumer
+// warpgroups with one m64nNk16 wgmma per k-step, and an epilogue straight from the accumulator registers.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -37,13 +39,14 @@ constexpr int GEMM_BLOCK_M = 128;
 constexpr int GEMM_BLOCK_K = 64;
 constexpr int GEMM_MAX_STAGES = 8;
 constexpr int GEMM_THREADS = 288;  // warps 0..7 MMA + epilogue, warp 8 TMA
+constexpr int GEMM_WIDE_THREADS = 384;  // 192- / 256-wide tiles: warpgroup 0 TMA, warpgroups 1..2 MMA + epilogue
 
 struct GemmParams {
   CUtensorMap tma_a;
   CUtensorMap tma_b;
   // tiling
   int M, N;            // logical output extent per batch (predication)
-  int block_n;         // multiple of 16, <= 128 (multiple of 64 when B is MN-major)
+  int block_n;         // multiple of 16, <= 128 (multiple of 64 when B is MN-major); or 192 / 256 (gemm_wide_ok)
   int stages;
   int num_k_blocks;    // taps * k_blocks_per_tap
   int k_blocks_per_tap;
@@ -120,6 +123,11 @@ struct GemmPlan {
   double flops = 0;   // 2*M*N*K*batches (algorithmic)
   double bytes = 0;   // compulsory traffic: each operand read once, each epilogue tensor read / written once
 };
+
+// Whether a plain GEMM may use 192- or 256-column tiles (the 384-thread kernel of gemm_tc.cu): fp16, A K-major and
+// unbatched, no split-K, and an epilogue the tensor-map path takes with fp16 outputs (bias, fp16 residual, QuickGELU
+// forward / backward, exact GELU forward).  gemm_plan_make runs any other request wider than 128 columns as 128.
+bool gemm_wide_ok(const GemmOperand& A, int N, const GemmEpilogue& epi, int fmt);
 
 // Plain (possibly batched) GEMM.  K is the reduction length; M, N output extents per batch.
 // Returns 0 on success; on failure writes a message to err (if non-null).
