@@ -381,6 +381,11 @@ int pxr_test_raster_samples(uint64_t seed, int iter, int H, int W, float* out);
 int pxr_test_attention(const void* qkv, void* o, float* lse, const void* d_o, void* gqkv, int B, int T, int H, int W,
                        float scale, int repeat, char* err, int errlen);
 
+/* streaming fused attention (attn_long.cu), same arguments: any T >= 1, 64-wide heads (W = 64 H).  The backward's
+ * [B*H*T] fp32 workspace is allocated and freed inside the call */
+int pxr_test_attention_long(const void* qkv, void* o, float* lse, const void* d_o, void* gqkv, int B, int T, int H,
+                            int W, float scale, int repeat, char* err, int errlen);
+
 /* GroupNorm(32, C, eps 1e-6)(+ swish) of the VQGAN decoder (taming Normalize + nonlinearity), forward and -- when dy or
  * ws_dy is given -- backward, on DEVICE NHWC fp16 tensors [pixels, C].  variant 0: single-kernel grid-barrier version,
  * 1: one thread-block cluster per group; with ws / ws_dy (variant 1) the kernel is also the epilogue of a split-K

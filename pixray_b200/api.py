@@ -14,8 +14,10 @@ super_resolution, vdiff) consult it; fft, pixel and line_sketch keep their own A
 engine calls whether or not the option is given; another rule adds one set_optimizer per switch of the engine's rule.
 
 Perceptors are named in `clip_models`, as get_clip_perceptor keys on them (slip.py:173-186): the openai-CLIP ViTs
-(engine.CLIP_ARCH) and the SLIP_Base ViTs (engine.SLIP_ARCH: SLIP_VITB16, SLIP_CC3M, SLIP_CC12M, CLIP_VITB16,
-SLIP_VITL16, CLIP_VITL16), alone or two of them mixed.  The reference's `perceptors` option only picks a default
+(engine.CLIP_ARCH: ViT-B/32, ViT-B/16, ViT-L/14, ViT-L/14@336px) and the SLIP_Base ViTs (engine.SLIP_ARCH: SLIP_VITB16,
+SLIP_CC3M, SLIP_CC12M, CLIP_VITB16, SLIP_VITL16, CLIP_VITL16), alone or two of them mixed.  The cutouts are made at the
+first perceptor's input resolution (224, or 336 for ViT-L/14@336px); the engine has one cutout batch, so towers of
+different input resolutions cannot be mixed in one session.  The reference's `perceptors` option only picks a default
 `clip_models` from its quality table (pixray.py:1832-1845); naming the models in `clip_models` runs the same towers.
 What the reference fetches from the network at init time comes in through three extra settings instead:
 
@@ -347,6 +349,11 @@ def do_init(args):
                                       f"and {sorted(E.SLIP_ARCH)} (SLIP) are built")
     if len(args.clip_models) > 2:
         raise NotImplementedError("at most two perceptors per session")
+    res = {m: (E.CLIP_ARCH.get(m) or E.SLIP_ARCH[m])["image_res"] for m in args.clip_models}
+    if len(set(res.values())) > 1:
+        # pixray.py:645-649 makes one MakeCutouts per input resolution; the engine scores every tower on one cutout batch
+        raise NotImplementedError(f"perceptors {res} need cutouts at different resolutions; the engine makes one cutout "
+                                  "batch per iteration, so towers of one input resolution only")
     st.seed = _seed_everything(args)
     kind = _DRAWER_KIND[args.drawer]
     drawer_class = class_table[args.drawer]
@@ -369,7 +376,8 @@ def do_init(args):
     aspect = float(args.size[0]) / float(args.size[1])
     device = int(str(args.cuda_device).split(":")[1]) if ":" in str(args.cuda_device) else 0
     clip_cfgs = [E.CLIP_ARCH[m] if m in E.CLIP_ARCH else E.SLIP_ARCH[m] for m in args.clip_models]
-    kw = dict(drawer=kind, image_hw=engine_hw, cutn=args.num_cuts, clip=clip_cfgs, seed=st.seed, device=device)
+    kw = dict(drawer=kind, image_hw=engine_hw, cutn=args.num_cuts, cut_size=clip_cfgs[0]["image_res"], clip=clip_cfgs,
+              seed=st.seed, device=device)
     if aspect != 1.0:
         kw["cut_aspect"] = aspect
     world = int(getattr(args, "b200_world", 1) or 1)

@@ -2,7 +2,7 @@
 // openai-CLIP VisionTransformer) and of the v-diffusion U-Net for sm_90a: one kernel for the forward, one for the
 // backward, both on the tensor cores (warp-level mma.sync m16n8k16, fp16 operands, fp32 accumulators in registers).
 // Replaces, per layer, {QK^T GEMM, softmax, PV GEMM} and {dP GEMM, softmax backward, dQ / dK / dV GEMMs} of the unfused
-// path (which stays for sequences longer than 240 tokens).
+// path.  Sequences longer than 257 tokens run on the streaming kernels of attn_long.cuh; 241..257 on the unfused path.
 //
 // Flash-attention style: a CTA owns one (image, head) pair -- or, with fewer pairs than SMs, a share of the pair's
 // 16-row tiles -- and stages the pair's Q, K, V (backward: and dO) once in shared memory with cp.async; ldmatrix feeds

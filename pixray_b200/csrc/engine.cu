@@ -9,6 +9,7 @@
 #include "engine.cuh"
 #include "comm.cuh"
 #include "attn_tc.cuh"
+#include "attn_long.cuh"
 #include "transforms.h"
 #include <algorithm>
 #include <atomic>
@@ -36,7 +37,8 @@ class Engine {
   float S = 4096.f;  // grad scale
   bool gn_coop = true;        // PXR_GN_COOP=0: three-kernel GroupNorm instead of the cooperative single-kernel one
   bool stream16 = true;       // the ViT residual stream and its gradient in fp16, like the reference's CUDA path (clip.load gives a half model, slip.py:176); PXR_CLIP_STREAM=32 keeps them in fp32
-  bool fused_attn = true;     // PXR_FUSED_ATTN=0: fall back to the batched-GEMM attention (attn_tc.cu covers T <= 240)
+  bool fused_attn = true;     // PXR_FUSED_ATTN=0: fall back to the batched-GEMM attention (attn_tc.cu covers T <= 240,
+                              // attn_long.cu T > 257)
   std::map<std::string, HostWeight> weights[3];
   std::vector<void*> allocs;
   bool finalized = false;
@@ -642,13 +644,18 @@ class Engine {
   // Self-attention O = softmax(scale q k^T) v of `images` x `heads` heads of width d over T tokens, in attn_tc.cuh's
   // layout: qkv and gqkv [images T, 3 heads d] (q | k | v, head h at column h d of each third), o and d_o
   // [images T, heads d].  Appends the forward to `fwd` and, when `bwd` is given, the backward (d_o -> gqkv) to *bwd.
-  // multihead (the ViT, the U-Net): the fused kernels when attn_fused() holds, else the batched-GEMM chain with tile
-  // widths fixed for the head-batched shapes; otherwise (taming's AttnBlock) always the chain, tile widths by add_gemm.
-  // The chain's P is allocated here (and returned; nullptr on the fused path), its dP too unless the caller passes a
+  // multihead (the ViT, the U-Net): the fused kernels when attn_fused() holds (attn_tc.cu, T <= 240), the streaming
+  // ones when attn_streamed() holds (attn_long.cu, T > 257), else the batched-GEMM chain with tile widths fixed for the
+  // head-batched shapes; otherwise (taming's AttnBlock) always the chain, tile widths by add_gemm.
+  // The chain's P is allocated here (and returned; nullptr on the fused paths), its dP too unless the caller passes a
   // scratch that several calls share.
   act_t* add_attention(OpList& fwd, OpList* bwd, const act_t* qkv, act_t* o, const act_t* d_o, act_t* gqkv, int images,
                        int heads, int T, int d, float scale, bool multihead, act_t* dP = nullptr);
   bool attn_fused(int T, int d, int heads) const { return fused_attn && attn_supported(T, d, heads * d); }
+  // T = 256 / 257 (the vdiff 16^2 level, ViT-L/14) stay on the chain: the streaming kernels start past them
+  bool attn_streamed(int T, int d, int heads) const {
+    return fused_attn && T > 257 && attn_long_supported(T, d, heads * d);
+  }
   GNSaved add_gn(OpList& l, const Act& x, const NormW& n, int swish, act_t* y);
   void add_gn_bwd(OpList& l, const act_t* dy, const act_t* x, const GNSaved& s, const NormW& n, int px, int C, int swish,
                   const act_t* dres, act_t* dx);
@@ -1011,6 +1018,22 @@ act_t* Engine::add_attention(OpList& fwd, OpList* bwd, const act_t* qkv, act_t* 
     if (bwd) {  // dQ, dK, dV in one kernel (recomputes P from Q, K and the saved log-sum-exp)
       snprintf(lab, sizeof lab, "attn_bwd B=%d T=%d heads=%d", images, T, heads);
       bwd->add(1, [ap, cs] { attn_backward_launch(*ap, cs); }, ap->flops_bwd, lab, ap->bytes_bwd);
+    }
+    return nullptr;
+  }
+  if (multihead && attn_streamed(T, d, heads)) {  // K / V streamed through shared memory; S / P never leave the SM
+    float* lse = dalloc<float>((size_t)images * heads * T);
+    float* delta = bwd ? dalloc<float>((size_t)images * heads * T) : nullptr;
+    auto ap = std::make_shared<AttnLongPlan>();
+    char buf[256] = {0};
+    int rc = attn_long_plan_make(ap.get(), qkv, o, d_o, gqkv, lse, delta, images, T, heads, W, scale, buf, sizeof buf);
+    if (rc) throw EngineError(rc, std::string("attention plan: ") + buf);
+    char lab[96];
+    snprintf(lab, sizeof lab, "attn_long_fwd B=%d T=%d heads=%d", images, T, heads);
+    fwd.add(1, [ap, cs] { attn_long_forward_launch(*ap, cs); }, ap->flops_fwd, lab, ap->bytes_fwd);
+    if (bwd) {  // dQ (and D = dO . O), then dK / dV: two launches
+      snprintf(lab, sizeof lab, "attn_long_bwd B=%d T=%d heads=%d", images, T, heads);
+      bwd->add(2, [ap, cs] { attn_long_backward_launch(*ap, cs); }, ap->flops_bwd, lab, ap->bytes_bwd);
     }
     return nullptr;
   }
@@ -1736,7 +1759,7 @@ void Engine::build_clip(int i) {
   C.gh = dalloc<act_t>((size_t)M * Wd);
   C.go = dalloc<act_t>((size_t)M * Wd);
   C.gqkv = dalloc<act_t>((size_t)M * 3 * Wd);
-  const bool fuse_attn = attn_fused(T, d, Hh);  // attn_tc.cu: T <= 240
+  const bool fuse_attn = attn_fused(T, d, Hh) || attn_streamed(T, d, Hh);  // attn_tc.cu T <= 240, attn_long.cu T > 257
   C.dP = fuse_attn ? nullptr : dalloc<act_t>((size_t)B * Hh * T * ldT);
   const bool s16 = stream16;
   const size_t xbytes = (size_t)M * Wd * (s16 ? sizeof(act_t) : sizeof(float));

@@ -3,6 +3,7 @@
 #include "../../include/pixray_b200.h"
 #include "gemm_tc.cuh"
 #include "attn_tc.cuh"
+#include "attn_long.cuh"
 #include "color_jitter.cuh"
 #include "pool_bounds.cuh"
 #include "raster_samples.cuh"
@@ -150,6 +151,35 @@ extern "C" int pxr_test_attention(const void* qkv, void* o, float* lse, const vo
     return -100;
   }
   return 0;
+}
+
+// Streaming fused attention (attn_long.cu) on the same caller tensors as pxr_test_attention; the backward's D workspace
+// [B*H*T] fp32 is allocated here.
+extern "C" int pxr_test_attention_long(const void* qkv, void* o, float* lse, const void* d_o, void* gqkv, int B, int T,
+                                       int H, int W, float scale, int repeat, char* err, int errlen) {
+  float* delta = nullptr;
+  if (d_o && B > 0 && T > 0 && H > 0 && cudaMalloc(&delta, sizeof(float) * B * H * T) != cudaSuccess) {
+    if (err) snprintf(err, errlen, "cudaMalloc of the delta workspace failed");
+    return -100;
+  }
+  AttnLongPlan plan;
+  int rc = attn_long_plan_make(&plan, static_cast<const __half*>(qkv), static_cast<__half*>(o),
+                               static_cast<const __half*>(d_o), static_cast<__half*>(gqkv), lse, delta, B, T, H, W, scale,
+                               err, errlen);
+  if (!rc) {
+    for (int i = 0; i < (repeat > 0 ? repeat : 1); ++i) {
+      attn_long_forward_launch(plan, nullptr);
+      if (d_o) attn_long_backward_launch(plan, nullptr);
+    }
+    cudaError_t ce = cudaGetLastError();
+    if (ce == cudaSuccess && delta) ce = cudaDeviceSynchronize();  // the workspace is freed below
+    if (ce != cudaSuccess) {
+      if (err) snprintf(err, errlen, "launch failed: %s", cudaGetErrorString(ce));
+      rc = -100;
+    }
+  }
+  cudaFree(delta);
+  return rc;
 }
 
 // The engine's row softmax (softmax_forward / softmax_backward, unfused attention) on caller DEVICE fp16 [rows, ld]:

@@ -28,6 +28,8 @@ CLIP_ARCH = {
     "ViT-B/32": dict(width=768, layers=12, heads=12, patch=32, image_res=224, out_dim=512),
     "ViT-B/16": dict(width=768, layers=12, heads=12, patch=16, image_res=224, out_dim=512),
     "ViT-L/14": dict(width=1024, layers=24, heads=16, patch=14, image_res=224, out_dim=768),
+    # 24^2 + 1 = 577 tokens: its attention runs on the streaming kernels (attn_long.cu)
+    "ViT-L/14@336px": dict(width=1024, layers=24, heads=16, patch=14, image_res=336, out_dim=768),
 }
 # Image towers (pxr_set_clip_tower): openai-CLIP's VisionTransformer, or the timm VisionTransformer of SLIP_Base
 TOWER_OPENAI_CLIP, TOWER_TIMM_VIT = 0, 1
