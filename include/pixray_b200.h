@@ -183,6 +183,14 @@ int pxr_set_color_jitter(pxr_handle h, float p, float saturation, float hue);
 int pxr_make_cutouts(pxr_handle h, const float* img, const pxr_cut_params* p, int iter,
                      float* out_batch /* [cutn_local,3,cs,cs] */);
 int pxr_encode_image(pxr_handle h, int clip_idx, const float* batch, float* out_embeds /* [cutn_local, D] */);
+
+/* Text tower of perceptor clip_idx (CLIP.encode_text, SLIP/models.py:136-150): built at pxr_finalize when the weights
+ * loaded for the perceptor include token_embedding.weight, positional_embedding, transformer.resblocks.*, ln_final.* and
+ * text_projection.  pxr_text_tower returns 1 and its shape when it exists, 0 when not (the outputs are then 0), < 0 on
+ * error.  pxr_encode_text: tokens_host [n, ctx] int32 host ids (ctx == the tower's context, every id inside the
+ * vocabulary) -> out device fp32 [n, D], the un-normalised embeddings of encode_text(...).float(); any n. */
+int pxr_text_tower(pxr_handle h, int clip_idx, int* width, int* layers, int* ctx, int* out_dim);
+int pxr_encode_text(pxr_handle h, int clip_idx, const int32_t* tokens_host, int n, int ctx, float* out);
 int pxr_prompt_loss(pxr_handle h, int clip_idx, const float* embeds, float* out_losses /* [n_prompts] */);
 int pxr_backward(pxr_handle h, float* z_grad);
 int pxr_step(pxr_handle h, float* z, float lr, int iter);
@@ -380,6 +388,11 @@ int pxr_test_raster_samples(uint64_t seed, int iter, int H, int W, float* out);
  * gqkv [B*T, 3W] fp16 device tensors, lse [B*H*T] fp32; heads are 64 wide (W = 64 H), T <= 240 */
 int pxr_test_attention(const void* qkv, void* o, float* lse, const void* d_o, void* gqkv, int B, int T, int H, int W,
                        float scale, int repeat, char* err, int errlen);
+
+/* causal attention forward (the text towers): o [B*T, W] from qkv [B*T, 3W] fp16 device tensors, row t attending to
+ * keys <= t; 64-wide heads (W = 64 H), T <= 240.  The fused kernel, or with PXR_FUSED_ATTN=0 in the environment the
+ * batched-GEMM chain with the causal row softmax, as the engine would choose */
+int pxr_test_attention_causal(const void* qkv, void* o, int B, int T, int H, int W, float scale, char* err, int errlen);
 
 /* streaming fused attention (attn_long.cu), same arguments: any T >= 1, 64-wide heads (W = 64 H).  The backward's
  * [B*H*T] fp32 workspace is allocated and freed inside the call */

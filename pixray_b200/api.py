@@ -24,9 +24,15 @@ What the reference fetches from the network at init time comes in through three 
     b200_weights        {"vqgan": state_dict | path, "ViT-B/16": state_dict | path, "SLIP_VITB16": ...} with the
                         reference's own keys (taming `state_dict`, openai-CLIP `visual.*`, the SLIP checkpoint's
                         {'state_dict', 'args'} with its `module.` prefix); None = seeded synthetic weights (benchmarks)
-    b200_text_encoder   callable(clip_model_name, text) -> [1, D] tensor (e.g. the reference's perceptor.encode_text);
-                        the text towers are init-time and stay in PyTorch
-    b200_allow_synthetic  accept seeded pseudo-embeddings for text prompts when no encoder is given (default False)
+    b200_text_encoder   callable(clip_model_name, text) -> [1, D] tensor (e.g. the reference's perceptor.encode_text)
+    b200_bpe_vocab      path of CLIP's bpe_simple_vocab_16e6.txt.gz for the engine's text towers; None looks in the
+                        installed `clip` package, then $PIXRAY_ROOT/SLIP/
+    b200_allow_synthetic  accept seeded pseudo-embeddings for text prompts when there is no text tower (default False)
+
+Text prompts, spot prompts and the vdiff drawer's clip_embed are encoded by, in this order: b200_text_encoder when
+given; else the engine's own text tower of the perceptor, which exists when its b200_weights state_dict carries the
+text keys (token_embedding.weight, positional_embedding, transformer.resblocks.*, ln_final.*, text_projection -- the
+whole openai-CLIP / SLIP checkpoint has them); else seeded pseudo-embeddings when b200_allow_synthetic; else ValueError.
 
 One session per process, like the reference's module globals (pixray.py:1022-1063)."""
 import argparse
@@ -110,6 +116,7 @@ _OPTIONS = [
     (("--output",), "output", str, "output.png"), (("--outdir",), "outdir", str, "outputs/%DATE%_%SEQ%"),
 ]
 _ENGINE_OPTIONS = [(("--b200_weights",), "b200_weights", None, None), (("--b200_text_encoder",), "b200_text_encoder", None, None),
+                   (("--b200_bpe_vocab",), "b200_bpe_vocab", str, None),
                    (("--b200_allow_synthetic",), "b200_allow_synthetic", str2bool, False),
                    # checkdrop / learning-rate drops / auto-stop decided on the device, no per-iteration host sync
                    # (pxr_set_schedule); False keeps the reference's host-side control flow (one loss readback per iteration)
@@ -320,9 +327,13 @@ def _vector_table(name):
     raise FileNotFoundError(f"vector prompt file not found (tried {cands}); set PIXRAY_ROOT or vector_prompts='none'")
 
 
-def _text_embed(args, clip_model, txt, out_dim):
+def _text_embed(args, clip_model, txt, out_dim, tower=None):
+    """[1, D] embedding of one prompt text: b200_text_encoder, else `tower` (the perceptor's encode_text when the engine
+    built its text tower), else seeded pseudo-embeddings when allowed."""
     if args.b200_text_encoder is not None:
         return torch.as_tensor(args.b200_text_encoder(clip_model, txt), dtype=torch.float32).reshape(1, out_dim).cpu()
+    if tower is not None:
+        return torch.as_tensor(tower(txt), dtype=torch.float32).reshape(1, out_dim).cpu()
     if not args.b200_allow_synthetic:
         raise ValueError("text prompts need a text tower: pass b200_text_encoder=callable(clip_model, text) -> [1, D] "
                          "(e.g. the reference's perceptor.encode_text), or b200_allow_synthetic=True for seeded "
@@ -474,7 +485,9 @@ def do_init(args):
         st.overlay_rgba = ov
     st.side = (sideX, sideY)
     st.drawer = drawer
-    st.perceptors = [P.Perceptor(st.session, i) for i in range(len(args.clip_models))]
+    st.perceptors = [P.Perceptor(st.session, i, "slip" if m in E.SLIP_ARCH else "clip", getattr(args, "b200_bpe_vocab", None))
+                     for i, m in enumerate(args.clip_models)]
+    towers = [p.encode_text if p.has_text_tower() else None for p in st.perceptors]
     st.make_cutouts = P.MakeCutouts(clip_cfgs[0]["image_res"], args.num_cuts, st.session, cut_pow=args.cut_pow, seed=st.seed,
                                     aspect=aspect)
 
@@ -484,7 +497,12 @@ def do_init(args):
     for prompt in args.prompts:
         for i, m in enumerate(args.clip_models):
             txt, weight, stop = P.parse_prompt(prompt)
-            embed = _text_embed(args, m, txt, clip_cfgs[i]["out_dim"])
+            if txt[:1] == "=" and args.b200_text_encoder is None and towers[i] is not None:
+                # pixray.py:864-870 calls perceptor.encode_text(tokens, stops), which neither perceptor accepts
+                raise ValueError(f"prompt {txt!r}: a text starting with '=' takes the reference's encode_text(tokens, "
+                                 "stops) branch, which fails there (CLIP_Base.encode_text takes one argument); the "
+                                 "engine's text tower does not encode it either")
+            embed = _text_embed(args, m, txt, clip_cfgs[i]["out_dim"], towers[i])
             if kind == E.DRAWER_VDIFF and m == drawer.clip_model:
                 clip_embeds.append(embed)
                 clip_weights.append(weight)
@@ -514,12 +532,17 @@ def do_init(args):
     spot_on, spot_off = split_pipes(args.spot_prompts) or [], split_pipes(args.spot_prompts_off) or []
     if spot_on or spot_off:
         eng.set_spot_mask(_spot_mask(args, clip_cfgs[0]["image_res"], aspect))
+        parsed = {which: [P.parse_prompt(p) for p in plist] for which, plist in ((1, spot_on), (0, spot_off))}
+        embeds = {(which, i): [] for which in (1, 0) for i in range(len(args.clip_models))}
+        for which in (1, 0):  # encoded in the reference's order: prompt, then perceptor
+            for (txt, _, _) in parsed[which]:
+                for i, m in enumerate(args.clip_models):
+                    embeds[which, i].append(_text_embed(args, m, txt, clip_cfgs[i]["out_dim"], towers[i]))
         for i, m in enumerate(args.clip_models):
-            for which, plist in ((1, spot_on), (0, spot_off)):
-                parsed = [P.parse_prompt(p) for p in plist]
-                embeds = [_text_embed(args, m, txt, clip_cfgs[i]["out_dim"]) for (txt, _, _) in parsed]
-                eng.set_spot_prompts(i, which, torch.cat(embeds).numpy() if embeds else [], [w for (_, w, _) in parsed],
-                                     [s_ for (_, _, s_) in parsed])
+            for which in (1, 0):
+                e = embeds[which, i]
+                eng.set_spot_prompts(i, which, torch.cat(e).numpy() if e else [], [w for (_, w, _) in parsed[which]],
+                                     [s_ for (_, _, s_) in parsed[which]])
     if args.image_prompts:
         imgs = [_load_image(p, sideX, sideY) for p in args.image_prompts]
         w = None if args.image_prompt_weight is None else [args.image_prompt_weight] * len(imgs)

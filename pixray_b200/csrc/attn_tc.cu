@@ -40,6 +40,10 @@ __device__ __forceinline__ void tile_range(int NT, int& lo, int& hi) {
 // ------------------------------------------------------------------------------------------------------------ forward
 // CTA = (split, head, image): K and V of the pair and the CTA's query tiles are staged once.  Warp w owns the 16-row
 // query tiles lo + w, lo + w + 8, ...: online softmax over 64-key blocks, whose 16-key chunks past T are skipped.
+// CAUSAL: row q attends to keys <= q only.  A query tile's key blocks end after its last row's key (later 16-key chunks do
+// no MMA work), and the keys past each row in the diagonal chunk are masked to -inf before the row max, so they add exact
+// zeros: row q's output depends on tokens <= q alone.
+template <bool CAUSAL>
 __global__ void __launch_bounds__(AT_THREADS, 2) attn_fwd_kernel(const __grid_constant__ AttnParams p) {
   pdl_prologue();
   extern __shared__ uint4 smem_at[];
@@ -61,11 +65,13 @@ __global__ void __launch_bounds__(AT_THREADS, 2) attn_fwd_kernel(const __grid_co
     for (int kc = 0; kc < 4; ++kc) ldsm4(qa[kc], frag_a(Qs, (qt - lo) * 16, 2 * kc, lane));
     float o[8][4] = {};
     float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
-    for (int kb = 0; kb * 64 < T; ++kb) {
+    const int q0 = qt * 16 + g, q1 = q0 + 8;
+    const int kend = CAUSAL ? min(T, qt * 16 + 16) : T;  // keys [0, kend) reach some row of the tile
+    for (int kb = 0; kb * 64 < kend; ++kb) {
       float s[8][4] = {};
 #pragma unroll
       for (int j2 = 0; j2 < 4; ++j2) {  // 16 keys
-        if (kb * 64 + j2 * 16 >= T) break;
+        if (kb * 64 + j2 * 16 >= kend) break;
 #pragma unroll
         for (int kc = 0; kc < 4; ++kc) {
           uint32_t kf[4];
@@ -80,7 +86,8 @@ __global__ void __launch_bounds__(AT_THREADS, 2) attn_fwd_kernel(const __grid_co
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
           const int key = kb * 64 + j * 8 + 2 * t + (e & 1);
-          s[j][e] = key < T ? s[j][e] * c : -INFINITY;
+          const bool live = key < T && (!CAUSAL || key <= (e < 2 ? q0 : q1));
+          s[j][e] = live ? s[j][e] * c : -INFINITY;
           if (e < 2) x0 = fmaxf(x0, s[j][e]);
           else x1 = fmaxf(x1, s[j][e]);
         }
@@ -89,7 +96,8 @@ __global__ void __launch_bounds__(AT_THREADS, 2) attn_fwd_kernel(const __grid_co
         x0 = fmaxf(x0, __shfl_xor_sync(0xffffffffu, x0, off));
         x1 = fmaxf(x1, __shfl_xor_sync(0xffffffffu, x1, off));
       }
-      const float n0 = fmaxf(m0, x0), n1 = fmaxf(m1, x1);  // every key block holds a key < T: finite
+      // every key block holds a key < T (causal: key kb * 64 <= qt * 16 <= the row): finite
+      const float n0 = fmaxf(m0, x0), n1 = fmaxf(m1, x1);
       const float a0 = exp2f(m0 - n0), a1 = exp2f(m1 - n1);
       m0 = n0;
       m1 = n1;
@@ -110,7 +118,7 @@ __global__ void __launch_bounds__(AT_THREADS, 2) attn_fwd_kernel(const __grid_co
       }
 #pragma unroll
       for (int j2 = 0; j2 < 4; ++j2) {  // 16 keys: O += P V, V read transposed by ldmatrix.trans
-        if (kb * 64 + j2 * 16 >= T) break;
+        if (kb * 64 + j2 * 16 >= kend) break;
         uint32_t pa[4];
         acc_to_a(pa, s[2 * j2], s[2 * j2 + 1]);
 #pragma unroll
@@ -127,7 +135,6 @@ __global__ void __launch_bounds__(AT_THREADS, 2) attn_fwd_kernel(const __grid_co
       l0 += __shfl_xor_sync(0xffffffffu, l0, off);
       l1 += __shfl_xor_sync(0xffffffffu, l1, off);
     }
-    const int q0 = qt * 16 + g, q1 = q0 + 8;
     const float i0 = 1.f / l0, i1 = 1.f / l1;
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
@@ -313,7 +320,7 @@ int bwd_smem(int T) { return 4 * round16(T) * ROW_BYTES + 2 * round16(T) * 4; }
 bool attn_supported(int T, int head_dim, int W) { return head_dim == 64 && T >= 1 && T <= 240 && W % 64 == 0; }
 
 int attn_plan_make(AttnPlan* plan, const __half* qkv, __half* o, const __half* d_o, __half* gqkv, float* lse, int B,
-                   int T, int H, int W, float scale, int num_sms, char* err, int errlen) {
+                   int T, int H, int W, float scale, int num_sms, char* err, int errlen, bool causal) {
   *plan = AttnPlan{};
   if (!attn_supported(T, W / H, W) || W != 64 * H) {
     if (err && errlen > 0) snprintf(err, errlen, "fused attention needs 64-wide heads and T <= 240");
@@ -330,6 +337,7 @@ int attn_plan_make(AttnPlan* plan, const __half* qkv, __half* o, const __half* d
   p.B = B;
   p.W = W;
   p.scale = scale;
+  p.causal = causal ? 1 : 0;
   // One CTA per (image, head) pair stages the pair once.  With fewer pairs than SMs, the pair's 16-row tiles are split
   // over up to num_sms / pairs CTAs (each stages the pair again) so that every SM gets work.
   const long pairs = (long)B * H;
@@ -346,7 +354,8 @@ int attn_plan_make(AttnPlan* plan, const __half* qkv, __half* o, const __half* d
   plan->bytes_bwd = 3 * mw + mw + mw + 3 * mw + 4.0 * B * H * T;
   static std::once_flag once;
   std::call_once(once, [] {
-    cudaFuncSetAttribute(attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, fwd_smem(240, 1));
+    cudaFuncSetAttribute(attn_fwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, fwd_smem(240, 1));
+    cudaFuncSetAttribute(attn_fwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, fwd_smem(240, 1));
     cudaFuncSetAttribute(attn_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bwd_smem(240));
   });
   return 0;
@@ -354,7 +363,8 @@ int attn_plan_make(AttnPlan* plan, const __half* qkv, __half* o, const __half* d
 
 void attn_forward_launch(const AttnPlan& plan, cudaStream_t st) {
   const AttnParams& p = plan.p;
-  launch_pdl(attn_fwd_kernel, dim3(plan.splits, p.H, p.B), dim3(AT_THREADS), plan.smem_fwd, st, p);
+  if (p.causal) launch_pdl(attn_fwd_kernel<true>, dim3(plan.splits, p.H, p.B), dim3(AT_THREADS), plan.smem_fwd, st, p);
+  else launch_pdl(attn_fwd_kernel<false>, dim3(plan.splits, p.H, p.B), dim3(AT_THREADS), plan.smem_fwd, st, p);
 }
 
 void attn_backward_launch(const AttnPlan& plan, cudaStream_t st) {

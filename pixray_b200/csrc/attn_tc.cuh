@@ -27,6 +27,7 @@ struct AttnParams {
   __half* gqkv;           // backward out [B*T, 3W]: dq | dk | dv
   int T, H, B, W;
   float scale;            // S = scale * q k^T
+  int causal;             // forward only: row q attends to keys <= q (the text towers' mask); 0 in every ViT / U-Net block
 };
 
 struct AttnPlan {
@@ -39,9 +40,10 @@ struct AttnPlan {
 
 // true when the fused kernels cover this shape (head width 64, T <= 240, 16-byte aligned rows)
 bool attn_supported(int T, int head_dim, int W);
-// qkv: [B*T, 3W]; o: [B*T, W]; d_o: [B*T, W]; gqkv: [B*T, 3W]; lse: [B*H*T]
+// qkv: [B*T, 3W]; o: [B*T, W]; d_o: [B*T, W]; gqkv: [B*T, 3W]; lse: [B*H*T].  causal: the forward masks keys after each
+// row (the backward kernel has no mask: a causal plan is forward only)
 int attn_plan_make(AttnPlan* plan, const __half* qkv, __half* o, const __half* d_o, __half* gqkv, float* lse, int B,
-                   int T, int H, int W, float scale, int num_sms, char* err, int errlen);
+                   int T, int H, int W, float scale, int num_sms, char* err, int errlen, bool causal = false);
 void attn_forward_launch(const AttnPlan& plan, cudaStream_t st);
 void attn_backward_launch(const AttnPlan& plan, cudaStream_t st);
 

@@ -192,6 +192,29 @@ class Engine {
     OpList fwd, bwd;
   };
   Clip clip[2];
+  // ---- text towers (engine_text.inc): encode_text of a perceptor whose weights carry token_embedding.weight.  Built at
+  // finalize (host weights are dropped there), forward only, TEXT_CHUNK sequences per run of the op list.
+  struct Text {
+    int W = 0, L = 0, T = 0, D = 0, heads = 0, vocab = 0;
+    act_t *tok = nullptr, *proj16 = nullptr;  // token_embedding [vocab, W], text_projection [W, D]
+    float* pos = nullptr;                     // positional_embedding [T, W]
+    NormW ln_final;
+    struct Layer {
+      act_t *wqkv, *wo, *wfc, *wproj;
+      float *bqkv, *bo, *bfc, *bproj;
+      NormW ln1, ln2;
+    };
+    std::vector<Layer> layers;
+    int *ids = nullptr, *eot = nullptr;  // [TEXT_CHUNK * T] token ids, [TEXT_CHUNK] row of each sequence's EOT
+    void *x0 = nullptr, *x1 = nullptr, *xe = nullptr;  // residual stream ping-pong, gathered EOT rows
+    act_t *h16 = nullptr, *qkv = nullptr, *o = nullptr, *u = nullptr, *gact = nullptr, *he = nullptr;
+    float *stats = nullptr, *e = nullptr;  // e: [TEXT_CHUNK, D] embeddings
+    OpList fwd;
+  };
+  static constexpr int TEXT_CHUNK = 32;
+  std::unique_ptr<Text> text[2];
+  void build_text(int i);
+  void encode_text(int i, const int32_t* tokens, int n, int ctx, float* out);
   float* losses_dev = nullptr;   // [total prompts]
   float* losses_scratch = nullptr;  // loss vector of the passes b > 0 of an iteration (batches > 1)
   float* losses_host = nullptr;  // pinned
@@ -648,9 +671,10 @@ class Engine {
   // ones when attn_streamed() holds (attn_long.cu, T > 257), else the batched-GEMM chain with tile widths fixed for the
   // head-batched shapes; otherwise (taming's AttnBlock) always the chain, tile widths by add_gemm.
   // The chain's P is allocated here (and returned; nullptr on the fused paths), its dP too unless the caller passes a
-  // scratch that several calls share.
+  // scratch that several calls share.  causal (the text towers): row t attends to tokens <= t; forward only, multihead,
+  // on the fused kernel or the chain with a causal row softmax (T <= 240 either way).
   act_t* add_attention(OpList& fwd, OpList* bwd, const act_t* qkv, act_t* o, const act_t* d_o, act_t* gqkv, int images,
-                       int heads, int T, int d, float scale, bool multihead, act_t* dP = nullptr);
+                       int heads, int T, int d, float scale, bool multihead, act_t* dP = nullptr, bool causal = false);
   bool attn_fused(int T, int d, int heads) const { return fused_attn && attn_supported(T, d, heads * d); }
   // T = 256 / 257 (the vdiff 16^2 level, ViT-L/14) stay on the chain: the streaming kernels start past them
   bool attn_streamed(int T, int d, int heads) const {
@@ -1003,17 +1027,19 @@ void Engine::attnblock_bwd(const AttnBlock& a) {
 }
 
 act_t* Engine::add_attention(OpList& fwd, OpList* bwd, const act_t* qkv, act_t* o, const act_t* d_o, act_t* gqkv,
-                             int images, int heads, int T, int d, float scale, bool multihead, act_t* dP) {
+                             int images, int heads, int T, int d, float scale, bool multihead, act_t* dP, bool causal) {
   const int W = heads * d, ldT = round_up(T, 8);
   cudaStream_t cs = st;
+  if (causal && (bwd || !multihead || !attn_supported(T, d, W)))
+    throw EngineError(-54, "causal attention is forward only, with 64-wide heads and T <= 240");
   if (multihead && attn_fused(T, d, heads)) {  // S, softmax and PV in one kernel; S / P never leave the SM
     float* lse = dalloc<float>((size_t)images * heads * T);
     auto ap = std::make_shared<AttnPlan>();
     char buf[256] = {0};
-    int rc = attn_plan_make(ap.get(), qkv, o, d_o, gqkv, lse, images, T, heads, W, scale, num_sms, buf, sizeof buf);
+    int rc = attn_plan_make(ap.get(), qkv, o, d_o, gqkv, lse, images, T, heads, W, scale, num_sms, buf, sizeof buf, causal);
     if (rc) throw EngineError(rc, std::string("attention plan: ") + buf);
     char lab[96];
-    snprintf(lab, sizeof lab, "attn_fwd B=%d T=%d heads=%d", images, T, heads);
+    snprintf(lab, sizeof lab, "attn_fwd%s B=%d T=%d heads=%d", causal ? "_causal" : "", images, T, heads);
     fwd.add(1, [ap, cs] { attn_forward_launch(*ap, cs); }, ap->flops_fwd, lab, ap->bytes_fwd);
     if (bwd) {  // dQ, dK, dV in one kernel (recomputes P from Q, K and the saved log-sum-exp)
       snprintf(lab, sizeof lab, "attn_bwd B=%d T=%d heads=%d", images, T, heads);
@@ -1054,7 +1080,8 @@ act_t* Engine::add_attention(OpList& fwd, OpList* bwd, const act_t* qkv, act_t* 
     add_gemm(fwd, opK(qkv, 3 * W, T, d, heads, qs0, images, qs1), opK(qkv + W, 3 * W, T, d, heads, qs0, images, qs1), T,
              T, d, e, bn_s);
   }
-  fwd.add(1, [=] { softmax_forward(P, rows, T, ldT, cs); }, 0.0, "softmax_forward");
+  if (causal) fwd.add(1, [=] { softmax_forward_causal(P, rows, T, ldT, cs); }, 0.0, "softmax_forward_causal");
+  else fwd.add(1, [=] { softmax_forward(P, rows, T, ldT, cs); }, 0.0, "softmax_forward");
   {  // O = P v
     GemmEpilogue e;
     e.out_f16 = o;
@@ -2528,6 +2555,7 @@ void Engine::finalize() {
   build_cutouts();
   if (cfg.n_clip < 1 || cfg.n_clip > 2) throw EngineError(-53, "n_clip must be 1 or 2");
   for (int i = 0; i < cfg.n_clip; ++i) build_clip(i);
+  for (int i = 0; i < cfg.n_clip; ++i) build_text(i);
   losses_dev = dalloc<float>(64);
   losses_scratch = dalloc<float>(64);
   aux_part = dalloc<double>(std::max(4 * AUX_MAX_BLOCKS, n_local) + 8);
@@ -2607,6 +2635,7 @@ void Engine::finalize() {
 
 #include "engine_vdiff.inc"
 #include "engine_superres.inc"
+#include "engine_text.inc"
 
 }  // namespace pxr
 
@@ -2683,6 +2712,33 @@ int pxr_set_clip_tower(pxr_handle h, int clip_idx, int kind) {
     if (kind != PXR_TOWER_OPENAI_CLIP && kind != PXR_TOWER_TIMM_VIT)
       throw EngineError(-10, "unknown tower kind (0 openai-CLIP, 1 timm ViT)");
     e->clip[clip_idx].tower = kind;
+  });
+}
+
+int pxr_text_tower(pxr_handle h, int clip_idx, int* width, int* layers, int* ctx, int* out_dim) {
+  int has = 0;
+  const int rc = [&]() -> int {
+    PXR_TRY(h, {
+      Engine* e = h->e;
+      if (!e->finalized) throw EngineError(-13, "call pxr_finalize first");
+      if (clip_idx < 0 || clip_idx >= e->cfg.n_clip) throw EngineError(-14, "bad clip index");
+      const Engine::Text* t = e->text[clip_idx].get();
+      has = t ? 1 : 0;
+      if (width) *width = t ? t->W : 0;
+      if (layers) *layers = t ? t->L : 0;
+      if (ctx) *ctx = t ? t->T : 0;
+      if (out_dim) *out_dim = t ? t->D : 0;
+    });
+  }();
+  return rc ? rc : has;
+}
+
+int pxr_encode_text(pxr_handle h, int clip_idx, const int32_t* tokens_host, int n, int ctx, float* out) {
+  PXR_TRY(h, {
+    Engine* e = h->e;
+    if (!e->finalized) throw EngineError(-13, "call pxr_finalize first");
+    if (clip_idx < 0 || clip_idx >= e->cfg.n_clip) throw EngineError(-14, "bad clip index");
+    e->encode_text(clip_idx, tokens_host, n, ctx, out);
   });
 }
 

@@ -297,6 +297,15 @@ void add_pos_embed(const float* t, const float* pos, int T, int rows, int W, act
 // in-place row softmax over the first `cols` of each row of length ld (pad columns zeroed); rows total; any ld % 8 == 0
 void softmax_forward(act_t* s, int rows, int cols, int ld, cudaStream_t st);
 void softmax_backward(const act_t* p, act_t* dp_to_ds, int rows, int cols, int ld, cudaStream_t st);
+// causal attention rows (blocks of `cols` rows, one per (head, sequence)): row r keeps columns [0, r % cols], the rest
+// become exact zeros.  ld <= 1024; -1 without launching anything otherwise
+int softmax_forward_causal(act_t* s, int rows, int cols, int ld, cudaStream_t st);
+// Text towers (kernels_text.cu).  x[r] = tok_emb[ids[r]] + pos[r % T] into the residual stream: y16 (fp16) when non-null,
+// else y32.  tok_emb [vocab, W] fp16, pos [T, W] fp32, ids [rows] already checked against the vocabulary; W % 4 == 0
+void text_embed(const int* ids, const act_t* tok_emb, const float* pos, int T, int rows, int W, act_t* y16, float* y32,
+                cudaStream_t st);
+// y[b] = x[src[b]] for b < n: rows of W elements (elem_bytes 2 or 4, W * elem_bytes % 16 == 0) gathered into a compact buffer
+void gather_rows(const void* x, const int* src, int n, int W, int elem_bytes, void* y, cudaStream_t st);
 // Prompt.forward for all prompts of one perceptor + its gradient w.r.t. the un-normalised embeds.
 //   e [B, D]; prompts [n, D] (unit rows), weights/stops [n]; de [B, D].  slots / inv_rows (nullable): row j adds into
 //   losses[slots[j]] with 1 / (rows of its Prompt) -- multi-row embeds (image prompts).  losses += partial, caller zeroes;

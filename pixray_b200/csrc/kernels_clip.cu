@@ -280,13 +280,16 @@ __global__ void __launch_bounds__(256) layernorm_bwd16_kernel(const act_t* __res
   }
 }
 
-// one warp per row; lane owns NV 16-byte vectors (8 halfs) of the row: ld % 8 == 0, ld <= 256 * NV
-template <int NV>
+// one warp per row; lane owns NV 16-byte vectors (8 halfs) of the row: ld % 8 == 0, ld <= 256 * NV.
+// CAUSAL: the rows come in blocks of `cols` (one attention head of one sequence) and row r keeps only its first
+// r % cols + 1 columns; the others are left out of the max and the sum and written as exact zeros.
+template <int NV, bool CAUSAL = false>
 __global__ void __launch_bounds__(256) softmax_fwd_kernel(act_t* __restrict__ s, long long rows, int cols, int ld) {
   pdl_prologue();
   const long long row = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (row >= rows) return;
+  if (CAUSAL) cols = (int)(row % cols) + 1;
   act_t* r = s + row * ld;
   const int nvec = ld / 8;
   float v[NV][8];
@@ -883,6 +886,15 @@ void softmax_forward(act_t* s, int rows, int cols, int ld, cudaStream_t st) {
   else if (nv == 2) launch_pdl(softmax_fwd_kernel<2>, dim3(grid), dim3(256), 0, st, s, rows, cols, ld);
   else if (nv <= 4) launch_pdl(softmax_fwd_kernel<4>, dim3(grid), dim3(256), 0, st, s, rows, cols, ld);
   else launch_pdl(softmax_fwd_long_kernel, dim3(grid), dim3(256), 0, st, s, rows, cols, ld);
+}
+int softmax_forward_causal(act_t* s, int rows, int cols, int ld, cudaStream_t st) {
+  const int nv = (ld / 8 + 31) / 32;
+  const int grid = (rows + 7) / 8;
+  if (nv <= 1) launch_pdl(softmax_fwd_kernel<1, true>, dim3(grid), dim3(256), 0, st, s, rows, cols, ld);
+  else if (nv == 2) launch_pdl(softmax_fwd_kernel<2, true>, dim3(grid), dim3(256), 0, st, s, rows, cols, ld);
+  else if (nv <= 4) launch_pdl(softmax_fwd_kernel<4, true>, dim3(grid), dim3(256), 0, st, s, rows, cols, ld);
+  else return -1;
+  return 0;
 }
 void softmax_backward(const act_t* p, act_t* dp_to_ds, int rows, int cols, int ld, cudaStream_t st) {
   const int nv = (ld / 8 + 31) / 32;

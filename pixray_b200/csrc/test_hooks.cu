@@ -153,6 +153,75 @@ extern "C" int pxr_test_attention(const void* qkv, void* o, float* lse, const vo
   return 0;
 }
 
+// Causal attention forward on caller tensors, on the path the engine's add_attention takes: the fused kernel, or with
+// PXR_FUSED_ATTN=0 the batched-GEMM chain S = scale q k^T -> causal row softmax -> O = P v (P allocated here).
+extern "C" int pxr_test_attention_causal(const void* qkv, void* o, int B, int T, int H, int W, float scale, char* err,
+                                         int errlen) {
+  if (!qkv || !o || B < 1 || H < 1 || !attn_supported(T, W / H, W) || W != 64 * H) {
+    if (err && errlen > 0) snprintf(err, errlen, "causal attention needs 64-wide heads and 1 <= T <= 240");
+    return -1;
+  }
+  const char* fa = getenv("PXR_FUSED_ATTN");
+  const __half* q = static_cast<const __half*>(qkv);
+  if (!(fa && atoi(fa) == 0)) {
+    float* lse = nullptr;
+    if (cudaMalloc(&lse, sizeof(float) * B * H * T) != cudaSuccess) return -100;
+    AttnPlan plan;
+    int rc = attn_plan_make(&plan, q, static_cast<__half*>(o), nullptr, nullptr, lse, B, T, H, W, scale, num_sms(), err,
+                            errlen, true);
+    if (!rc) {
+      attn_forward_launch(plan, nullptr);
+      rc = cudaDeviceSynchronize() == cudaSuccess ? 0 : -100;
+    }
+    cudaFree(lse);
+    return rc;
+  }
+  const int ldT = (T + 7) / 8 * 8, rows = B * H * T;
+  // (head, sequence) batch strides of qkv, o and P, as add_attention lays them out
+  const long long qs0 = 64, qs1 = (long long)T * 3 * W, os0 = 64, os1 = (long long)T * W;
+  const long long ps0 = (long long)T * ldT, ps1 = (long long)H * T * ldT;
+  auto op = [&](const void* p, int mode, long long ld, long long mn, long long k, long long bs0, long long bs1) {
+    GemmOperand g;
+    g.ptr = p;
+    g.mode = mode;
+    g.ld = ld;
+    g.mn_extent = mn;
+    g.k_extent = k;
+    g.nb0 = H;
+    g.nb1 = B;
+    g.bs0 = bs0;
+    g.bs1 = bs1;
+    return g;
+  };
+  __half* P = nullptr;
+  if (cudaMalloc(&P, sizeof(__half) * rows * ldT) != cudaSuccess) return -100;
+  GemmPlan s_plan, o_plan;
+  GemmEpilogue es, eo;
+  es.alpha = scale;
+  es.out_f16 = P;
+  es.ldc = ldT;
+  es.bs0 = ps0;
+  es.bs1 = ps1;
+  eo.out_f16 = static_cast<__half*>(o);
+  eo.ldc = W;
+  eo.bs0 = os0;
+  eo.bs1 = os1;
+  const int bn_s = T <= 32 ? (T + 15) / 16 * 16 : T <= 128 ? (T + 63) / 64 * 64 : 128;
+  int rc = gemm_plan_make(&s_plan, op(q, OP_KMAJOR, 3 * W, T, 64, qs0, qs1), op(q + W, OP_KMAJOR, 3 * W, T, 64, qs0, qs1),
+                          T, T, 64, es, bn_s, 0, num_sms(), err, errlen);
+  if (!rc)
+    rc = gemm_plan_make(&o_plan, op(P, OP_KMAJOR, ldT, T, ldT, ps0, ps1), op(q + 2 * W, OP_MNMAJOR, 3 * W, 64, T, qs0, qs1),
+                        T, 64, T, eo, 64, 0, num_sms(), err, errlen);
+  if (!rc) {
+    gemm_launch(s_plan, nullptr);
+    rc = softmax_forward_causal(P, rows, T, ldT, nullptr);
+    if (!rc) gemm_launch(o_plan, nullptr);
+    if (!rc && cudaDeviceSynchronize() != cudaSuccess) rc = -100;
+  }
+  cudaFree(P);
+  return rc;
+}
+
 // Streaming fused attention (attn_long.cu) on the same caller tensors as pxr_test_attention; the backward's D workspace
 // [B*H*T] fp32 is allocated here.
 extern "C" int pxr_test_attention_long(const void* qkv, void* o, float* lse, const void* d_o, void* gqkv, int B, int T,

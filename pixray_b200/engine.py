@@ -449,6 +449,30 @@ class B200Engine:
         self.sync()
         return out
 
+    def text_tower(self, clip_idx=0):
+        """dict(width, layers, ctx, out_dim) of perceptor clip_idx's text tower, or None when its weights had no text keys
+        (pxr_text_tower)."""
+        v = [C.c_int() for _ in range(4)]
+        rc = self.lib.pxr_text_tower(self.h, int(clip_idx), *(C.byref(x) for x in v))
+        if rc < 0:
+            self._check(rc, "pxr_text_tower")
+        return dict(zip(("width", "layers", "ctx", "out_dim"), (x.value for x in v))) if rc == 1 else None
+
+    def encode_text(self, clip_idx, tokens):
+        """encode_text(tokens).float() of perceptor clip_idx: token ids [n, ctx] (pixray_b200.tokenizer) -> un-normalised
+        embeddings [n, D] on the device (pxr_encode_text)."""
+        t = np.ascontiguousarray(np.asarray(tokens.cpu() if torch.is_tensor(tokens) else tokens, dtype=np.int64))
+        t = t.reshape(-1, t.shape[-1])
+        if t.size and (t.min() < 0 or t.max() > np.iinfo(np.int32).max):
+            raise EngineError(f"token ids must lie in [0, 2^31): got [{t.min()}, {t.max()}]")
+        t = t.astype(np.int32)
+        out = self._new(t.shape[0], self.clip_dims[clip_idx])
+        torch.cuda.current_stream().synchronize()
+        rc = self.lib.pxr_encode_text(self.h, int(clip_idx), t.ctypes.data_as(C.c_void_p), int(t.shape[0]),
+                                      int(t.shape[1]), self._p(out))
+        self._check(rc, "pxr_encode_text")
+        return out
+
     def prompt_loss(self, clip_idx=0, embeds=None):
         if embeds is not None:
             embeds = embeds.to(self.device, torch.float32).contiguous()

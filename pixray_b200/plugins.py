@@ -16,6 +16,7 @@ from torch.nn import functional as F
 
 from . import cutouts as cut_sampler
 from . import engine as E
+from . import tokenizer
 
 
 class DrawingInterface:
@@ -682,11 +683,14 @@ class MakeCutouts:
 class Perceptor:
     """CLIP_Base surface (slip.py:44-74): input_resolution, output_dim, encode_image -> unit-norm [N, D]."""
 
-    def __init__(self, session: Session, clip_idx=0):
+    def __init__(self, session: Session, clip_idx=0, family="clip", bpe_vocab=None):
+        """family: "clip" (openai-CLIP, clip.tokenize) or "slip" (SLIP's SimpleTokenizer), the tokenizer's over-length
+        rule; bpe_vocab: path of bpe_simple_vocab_16e6.txt.gz (None: tokenizer.find_vocab looks for it)."""
         self.session, self.clip_idx = session, clip_idx
         self.device = session.engine.device
         c = session.engine.cfg.clip[clip_idx]
         self.input_resolution, self.output_dim = c.image_res, c.out_dim
+        self.family, self.bpe_vocab = family, bpe_vocab
 
     def encode_image(self, imgs, input_range=None, apply_preprocess=True):
         if input_range is not None or not apply_preprocess:
@@ -695,8 +699,19 @@ class Perceptor:
         self.session.last_embeds[self.clip_idx] = e
         return e
 
+    def has_text_tower(self):
+        tower = getattr(self.session.engine, "text_tower", None)
+        return tower is not None and tower(self.clip_idx) is not None
+
     def encode_text(self, text):
-        raise NotImplementedError("text towers are init-time (SURVEY.md row 10); pass prompt embeddings")
+        """CLIP_Base / SLIP_Base.encode_text (slip.py:68-70, 159-163): str or list of str -> [n, D] float embeddings
+        (not normalised), tokenised by this perceptor's family and encoded by the engine's text tower."""
+        if not self.has_text_tower():
+            raise NotImplementedError("this perceptor has no text tower: load the whole CLIP / SLIP state_dict "
+                                      "(token_embedding.weight, positional_embedding, transformer.resblocks.*, ln_final.*, "
+                                      "text_projection next to visual.*) before finalize, or pass prompt embeddings")
+        tok = tokenizer.get(tokenizer.find_vocab(self.bpe_vocab))
+        return self.session.engine.encode_text(self.clip_idx, tok(text, self.family))
 
 
 class Prompt:

@@ -43,6 +43,32 @@ def clip_state_dict(arch, seed=0):
     return sd
 
 
+def clip_text_state_dict(width, layers, out_dim, seed=0, vocab=49408, context=77):
+    """The text-tower tensors of a CLIP / SLIP checkpoint (token_embedding, positional_embedding, transformer.resblocks.*,
+    ln_final, text_projection; init pattern of SLIP/models.py:106-120), to merge with a visual state_dict."""
+    g = torch.Generator().manual_seed(seed)
+    W, L = width, layers
+    sd = {"token_embedding.weight": _randn(g, vocab, W, std=0.02), "positional_embedding": _randn(g, context, W, std=0.01)}
+    proj_std, attn_std, fc_std = (W ** -0.5) * ((2 * L) ** -0.5), W ** -0.5, (2 * W) ** -0.5
+    for i in range(L):
+        p = f"transformer.resblocks.{i}."
+        sd[p + "attn.in_proj_weight"] = _randn(g, 3 * W, W, std=attn_std)
+        sd[p + "attn.in_proj_bias"] = _randn(g, 3 * W, std=0.02)
+        sd[p + "attn.out_proj.weight"] = _randn(g, W, W, std=proj_std)
+        sd[p + "attn.out_proj.bias"] = _randn(g, W, std=0.02)
+        sd[p + "mlp.c_fc.weight"] = _randn(g, 4 * W, W, std=fc_std)
+        sd[p + "mlp.c_fc.bias"] = _randn(g, 4 * W, std=0.02)
+        sd[p + "mlp.c_proj.weight"] = _randn(g, W, 4 * W, std=proj_std)
+        sd[p + "mlp.c_proj.bias"] = _randn(g, W, std=0.02)
+        for nm in ("ln_1", "ln_2"):
+            sd[p + nm + ".weight"] = 1 + 0.1 * _randn(g, W)
+            sd[p + nm + ".bias"] = 0.05 * _randn(g, W)
+    sd["ln_final.weight"] = 1 + 0.1 * _randn(g, W)
+    sd["ln_final.bias"] = 0.05 * _randn(g, W)
+    sd["text_projection"] = _randn(g, W, out_dim, std=W ** -0.5)
+    return sd
+
+
 def slip_state_dict(arch, seed=0):
     """The image-tower tensors of a SLIP_Base checkpoint (after `module.` is stripped, slip.py:126-128): timm's
     VisionTransformer under 'visual.*' and 'image_projection' (SLIP/models.py:130-134), at the scales of clip_state_dict."""
