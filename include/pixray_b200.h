@@ -35,8 +35,11 @@ enum { PXR_DRAWER_VQGAN = 0, PXR_DRAWER_PIXEL = 1, PXR_DRAWER_FFT = 2, PXR_DRAWE
 enum { PXR_PAD_REFLECTION = 0, PXR_PAD_BORDER = 1, PXR_PAD_ZEROS = 2 };
 enum { PXR_DTYPE_F16 = 0, PXR_DTYPE_BF16 = 1 };
 /* module ids for pxr_load_weight */
-enum { PXR_MOD_VQGAN = 0, PXR_MOD_CLIP0 = 1, PXR_MOD_CLIP1 = 2 };
+enum { PXR_MOD_VQGAN = 0, PXR_MOD_CLIP0 = 1, PXR_MOD_CLIP1 = 2, PXR_MOD_CLIP2 = 3 };
 
+/* ViT towers: the fields as named.  CLIP ResNet towers (PXR_TOWER_CLIP_RESNET): width = the stem width w (64 for RN50),
+ * layers = the number of bottleneck blocks over all four stages (16 for RN50), heads = the attention pool's heads
+ * (64-wide), patch unused (0). */
 typedef struct {
   int width;     /* transformer width (768 for ViT-B) */
   int layers;    /* 12 */
@@ -59,8 +62,8 @@ typedef struct {
   int grid_rows, grid_cols;
   /* MakeCutouts(cut_size, cutn) pixray.py:400-443; cutn is the GLOBAL count, this rank owns a slice */
   int cutn, cut_size;
-  int n_clip;
-  pxr_clip_cfg clip[2];
+  int n_clip;            /* 1 to 3 perceptors */
+  pxr_clip_cfg clip[3];
   float noise_fac;       /* pixray.py:439 (0.1) */
   uint64_t seed;
   int op_dtype;          /* PXR_DTYPE_*: tensor-core operand type (accumulation is always fp32) */
@@ -117,8 +120,14 @@ int pxr_finalize(pxr_handle h);
  *   TIMM_VIT     timm VisionTransformer of SLIP_Base (slip.py:84-157, SLIP/models.py:130-134): ImageNet mean / std,
  *                patch_embed.proj with bias, cls_token + pos_embed without a LayerNorm before the blocks, exact GELU,
  *                LayerNorm eps 1e-6, final norm, image_projection; keys visual.* and image_projection after the
- *                checkpoint's `module.` prefix is stripped */
-enum { PXR_TOWER_OPENAI_CLIP = 0, PXR_TOWER_TIMM_VIT = 1 };
+ *                checkpoint's `module.` prefix is stripped
+ *   CLIP_RESNET  openai-CLIP ModifiedResNet (clip.load of RN50 / RN101 / RN50x4 / RN50x16 / RN50x64): CLIP mean / std,
+ *                a three-conv stem (conv1 stride 2) with AvgPool2d(2), four stages of bottlenecks (AvgPool2d before the
+ *                stride-2 convs), eval-mode BatchNorm (eps 1e-5, folded into the convs at pxr_finalize), ReLU, and the
+ *                attention pool (mean token + positional_embedding, q / k / v / c_proj, token 0 as the only query).
+ *                The block counts per stage are read from the visual.layerN.i.* keys; their sum must equal
+ *                pxr_clip_cfg.layers, and the pool's positional_embedding must have (image_res / 32)^2 + 1 rows. */
+enum { PXR_TOWER_OPENAI_CLIP = 0, PXR_TOWER_TIMM_VIT = 1, PXR_TOWER_CLIP_RESNET = 2 };
 int pxr_set_clip_tower(pxr_handle h, int clip_idx, int kind);
 
 /* Prompt(embed, weight, stop) list of one perceptor (pixray.py:859-915).  embeds host [n, D]. */

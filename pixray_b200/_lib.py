@@ -24,7 +24,7 @@ class Config(C.Structure):
         ("ch_mult", C.c_int * 8),
         ("grid_rows", C.c_int), ("grid_cols", C.c_int),
         ("cutn", C.c_int), ("cut_size", C.c_int),
-        ("n_clip", C.c_int), ("clip", ClipCfg * 2),
+        ("n_clip", C.c_int), ("clip", ClipCfg * 3),
         ("noise_fac", C.c_float), ("seed", C.c_uint64),
         ("op_dtype", C.c_int), ("grad_scale", C.c_float),
         ("beta1", C.c_float), ("beta2", C.c_float), ("adam_eps", C.c_float),

@@ -355,12 +355,13 @@ def do_init(args):
     for m in args.clip_models:
         if m in E.SLIP_UNSUPPORTED:
             raise NotImplementedError(f"perceptor '{m}': {E.SLIP_UNSUPPORTED[m]}")
-        if m not in E.CLIP_ARCH and m not in E.SLIP_ARCH:
-            raise NotImplementedError(f"perceptor '{m}': only the ViT image towers {sorted(E.CLIP_ARCH)} (openai-CLIP) "
-                                      f"and {sorted(E.SLIP_ARCH)} (SLIP) are built")
-    if len(args.clip_models) > 2:
-        raise NotImplementedError("at most two perceptors per session")
-    res = {m: (E.CLIP_ARCH.get(m) or E.SLIP_ARCH[m])["image_res"] for m in args.clip_models}
+        if m not in E.CLIP_ARCH and m not in E.SLIP_ARCH and m not in E.RESNET_ARCH:
+            raise NotImplementedError(f"perceptor '{m}': only the image towers {sorted(E.CLIP_ARCH)}, "
+                                      f"{sorted(E.RESNET_ARCH)} (openai-CLIP) and {sorted(E.SLIP_ARCH)} (SLIP) are built")
+    if len(args.clip_models) > 3:
+        raise NotImplementedError("at most three perceptors per session")
+    arch = {m: E.CLIP_ARCH.get(m) or E.RESNET_ARCH.get(m) or E.SLIP_ARCH[m] for m in args.clip_models}
+    res = {m: arch[m]["image_res"] for m in args.clip_models}
     if len(set(res.values())) > 1:
         # pixray.py:645-649 makes one MakeCutouts per input resolution; the engine scores every tower on one cutout batch
         raise NotImplementedError(f"perceptors {res} need cutouts at different resolutions; the engine makes one cutout "
@@ -386,7 +387,7 @@ def do_init(args):
     # != 1 stretches the pooled image before the warps and changes the wide augmentation stack (pixray.py:420-432, 468-472)
     aspect = float(args.size[0]) / float(args.size[1])
     device = int(str(args.cuda_device).split(":")[1]) if ":" in str(args.cuda_device) else 0
-    clip_cfgs = [E.CLIP_ARCH[m] if m in E.CLIP_ARCH else E.SLIP_ARCH[m] for m in args.clip_models]
+    clip_cfgs = [arch[m] for m in args.clip_models]
     kw = dict(drawer=kind, image_hw=engine_hw, cutn=args.num_cuts, cut_size=clip_cfgs[0]["image_res"], clip=clip_cfgs,
               seed=st.seed, device=device)
     if aspect != 1.0:
@@ -411,6 +412,8 @@ def do_init(args):
                 raise ValueError(f"{dest}: the line_sketch drawer has no latent to anchor to (get_z_copy is None)")
         kw["strokes"] = (args.strokes, args.stroke_length, P.LineDrawer.max_width(args, sideY), bool(args.allow_paper_color))
     eng = _engine_factory(**kw)
+    if any(m in E.RESNET_ARCH for m in args.clip_models) and E.TOWER_CLIP_RESNET not in getattr(eng, "TOWERS", ()):
+        raise NotImplementedError("this engine build has no ResNet image towers")
     weights = args.b200_weights or {}
     if kind in (E.DRAWER_VQGAN, E.DRAWER_VDIFF, E.DRAWER_SUPERRES):
         key = {E.DRAWER_VQGAN: "vqgan", E.DRAWER_VDIFF: "vdiff", E.DRAWER_SUPERRES: "super_resolution"}[kind]
@@ -430,6 +433,10 @@ def do_init(args):
     for i, m in enumerate(args.clip_models):
         if m in weights:
             sd = _load_state_dict(weights[m])
+            if m in E.RESNET_ARCH:
+                E.check_resnet_state_dict(m, sd)
+        elif m in E.RESNET_ARCH:
+            sd = S.clip_resnet_state_dict(E.RESNET_ARCH[m], 1 + i)
         elif m in E.SLIP_ARCH:
             sd = S.slip_state_dict(E.SLIP_ARCH[m], 1 + i)
         else:

@@ -3,7 +3,7 @@
 // and the per-iteration cutout parameters.  One handle = one rank = one CUDA stream.
 //
 // Hot path order per iteration (pixray.py:1243-1406, 1436-1512):
-//   drawer.synth -> pool -> cutouts -> [per perceptor: patchify -> ViT -> head -> Prompt loss]
+//   drawer.synth -> pool -> cutouts -> [per perceptor: patchify -> ViT -> head (or stem -> ResNet -> attnpool) -> Prompt loss]
 //   -> backward of all of the above by hand (dgrad only: every network is frozen, vqgan.py:125, slip.py:176)
 //   -> [allreduce z.grad] -> Adam -> clip_z
 #include "engine.cuh"
@@ -39,7 +39,7 @@ class Engine {
   bool stream16 = true;       // the ViT residual stream and its gradient in fp16, like the reference's CUDA path (clip.load gives a half model, slip.py:176); PXR_CLIP_STREAM=32 keeps them in fp32
   bool fused_attn = true;     // PXR_FUSED_ATTN=0: fall back to the batched-GEMM attention (attn_tc.cu covers T <= 240,
                               // attn_long.cu T > 257)
-  std::map<std::string, HostWeight> weights[3];
+  std::map<std::string, HostWeight> weights[4];
   std::vector<void*> allocs;
   bool finalized = false;
   std::map<std::string, std::pair<void*, size_t>> dbg;  // named internal buffers (tests / debugging)
@@ -191,7 +191,7 @@ class Engine {
     } spot[2];
     OpList fwd, bwd;
   };
-  Clip clip[2];
+  Clip clip[3];
   // ---- text towers (engine_text.inc): encode_text of a perceptor whose weights carry token_embedding.weight.  Built at
   // finalize (host weights are dropped there), forward only, TEXT_CHUNK sequences per run of the op list.
   struct Text {
@@ -212,9 +212,27 @@ class Engine {
     OpList fwd;
   };
   static constexpr int TEXT_CHUNK = 32;
-  std::unique_ptr<Text> text[2];
+  std::unique_ptr<Text> text[3];
   void build_text(int i);
   void encode_text(int i, const int32_t* tokens, int n, int ctx, float* out);
+  // ---- CLIP ResNet image towers (engine_resnet.inc): the perceptor's Clip keeps its prompts, embeddings and op lists;
+  // this holds the tower's own weights and the stem's im2col rows the input stage reads and writes
+  struct RnConv {  // a conv with its BatchNorm folded, channel counts padded to multiples of 64
+    act_t *w = nullptr, *wd = nullptr;
+    float* b = nullptr;
+    int cin = 0, cout = 0, ks = 1;
+  };
+  struct Resnet {
+    act_t *cols = nullptr, *g_cols = nullptr;  // [B (cs/2)^2, 64]
+    act_t *wq = nullptr, *wkv = nullptr, *wc = nullptr;
+    float *bq = nullptr, *bkv = nullptr, *bc = nullptr, *pos = nullptr;
+  };
+  std::unique_ptr<Resnet> rn[3];
+  RnConv rn_conv(int mod, const std::string& conv, const std::string& bn, int cin, int cout, int ks, bool flat);
+  void build_resnet(int i);
+  // the tower's input stage: the cutouts (batch, range) -> its first GEMM operand, and back into g_batch
+  void clip_input(int i);
+  void clip_input_backward(int i, bool accumulate, FxPass fx);
   float* losses_dev = nullptr;   // [total prompts]
   float* losses_scratch = nullptr;  // loss vector of the passes b > 0 of an iteration (batches > 1)
   float* losses_host = nullptr;  // pinned
@@ -505,16 +523,16 @@ class Engine {
   }
   // in_ld: pixel stride of `in` (0: cin); the conv reads its first cin channels
   void add_conv(OpList& l, const act_t* in, int H, int Wd, int cin, const act_t* wt, int cout_pad, int n_out, int ks,
-                const GemmEpilogue& e, long long in_ld = 0) {
+                const GemmEpilogue& e, long long in_ld = 0, int batch = 1) {
     if (in_ld <= 0) in_ld = cin;
-    const long long m_tiles = (long long)(H * Wd + 127) / 128;
+    const long long m_tiles = (long long)(H * Wd + 127) / 128 * batch;
     int bn = pick_bn(cout_pad < 64 ? cout_pad : n_out, false, m_tiles);
     if (bn > cout_pad) bn = cout_pad;
     cudaStream_t s = st;
     char kind[32];
     snprintf(kind, sizeof kind, "conv%dx%d", ks, ks);
     const int nkb = ks * ks * cin / 64;
-    const int splits = splitk_count(e, (long long)H * Wd, n_out, nkb, m_tiles * ((n_out + bn - 1) / bn));
+    const int splits = batch > 1 ? 1 : splitk_count(e, (long long)H * Wd, n_out, nkb, m_tiles * ((n_out + bn - 1) / bn));
     auto plan = std::make_shared<GemmPlan>();
     char buf[256] = {0};
     if (splits > 1) {
@@ -549,7 +567,7 @@ class Engine {
       q.sk.out = out;
       return;
     }
-    int rc = conv_plan_make(plan.get(), in, in_ld, 1, H, Wd, cin, wt, cout_pad, n_out, ks, e, bn, fmt, num_sms, buf,
+    int rc = conv_plan_make(plan.get(), in, in_ld, batch, H, Wd, cin, wt, cout_pad, n_out, ks, e, bn, fmt, num_sms, buf,
                             sizeof buf);
     if (rc) throw EngineError(rc, std::string("conv plan: ") + buf);
     l.add(1, [plan, s] { gemm_launch(*plan, s); }, plan->flops, gemm_label(kind, *plan, OP_KMAJOR, OP_KMAJOR, e), plan->bytes);
@@ -1724,6 +1742,7 @@ void Engine::forward_cutouts() {
 // ===================================================================================================== CLIP ViT
 void Engine::build_clip(int i) {
   Clip& C = clip[i];
+  if (C.tower == PXR_TOWER_CLIP_RESNET) return build_resnet(i);
   C.c = cfg.clip[i];
   const int mod = PXR_MOD_CLIP0 + i;
   const int Wd = C.c.width, L = C.c.layers, Hh = C.c.heads, P = C.c.patch, D = C.c.out_dim;
@@ -1995,11 +2014,26 @@ void Engine::build_clip(int i) {
   }
 }
 
-void Engine::forward_clip(int i) {
+void Engine::clip_input(int i) {
   Clip& C = clip[i];
-  patchify_forward(batch, range, n_local, cfg.cut_size, C.c.patch, C.Kp, C.patches, C.norm, st);
+  if (C.tower == PXR_TOWER_CLIP_RESNET) rn_stem_forward(batch, range, n_local, cfg.cut_size, rn[i]->cols, C.norm, st);
+  else patchify_forward(batch, range, n_local, cfg.cut_size, C.c.patch, C.Kp, C.patches, C.norm, st);
   launches += 1;
-  run(C.fwd);
+}
+
+void Engine::clip_input_backward(int i, bool accumulate, FxPass fx) {
+  Clip& C = clip[i];
+  if (C.tower == PXR_TOWER_CLIP_RESNET)
+    rn_stem_backward(rn[i]->g_cols, batch, range, n_local, cfg.cut_size, accumulate, g_batch, sums_fx, fx, C.norm, st);
+  else
+    patchify_backward(C.g_patches, batch, range, n_local, cfg.cut_size, C.c.patch, C.Kp, accumulate, g_batch, sums_fx, fx,
+                      C.norm, st);
+  launches += 1;
+}
+
+void Engine::forward_clip(int i) {
+  clip_input(i);
+  run(clip[i].fwd);
   check_launch("clip forward");
 }
 
@@ -2098,14 +2132,14 @@ void Engine::encode_image_prompts() {
     for (int i = 0; i < cfg.n_clip; ++i) {
       Clip& C = clip[i];
       const int D = C.c.out_dim;
-      patchify_forward(batch, range, n_local, cfg.cut_size, C.c.patch, C.Kp, C.patches, C.norm, st);
+      clip_input(i);
       run(C.fwd);
       float* rows = C.prompts + (size_t)(C.n_text + k * cfg.cutn) * D;
       if (comm) PXR_CUDA(cudaMemsetAsync(rows, 0, sizeof(float) * cfg.cutn * D, st));
       // zero prompt rows: the kernel only normalises (slip.py:66) into `rows`; de is overwritten by the main pass
       prompt_loss(C.e, C.B, D, C.prompts, C.pweights, C.pstops, C.pslot, C.pinv, 0, cfg.cutn, S,
                   rows + (size_t)first_global * D, losses_dev + C.loss_offset, C.de, C.de16, nullptr, nullptr, st);
-      launches += 2;
+      launches += 1;
       if (comm)  // every rank needs all cutn rows; each rank filled its own, the others are zero: the sum is exact
         nccl_check(Comm::api().all_reduce(rows, rows, (size_t)cfg.cutn * D, Comm::kFloat32, Comm::kSum, comm, st),
                    "allreduce(image prompt rows)");
@@ -2216,10 +2250,8 @@ void Engine::backward_to_image(const CutoutArgs& a, int mask_which, bool accumul
     Clip& C = clip[i];
     if (mask_which >= 0 && C.spot[mask_which].n == 0) continue;
     run(C.bwd);
-    patchify_backward(C.g_patches, batch, range, n_local, cfg.cut_size, C.c.patch, C.Kp, !first, g_batch, sums_fx, fx_sums,
-                      C.norm, st);
+    clip_input_backward(i, !first, fx_sums);
     first = false;
-    launches += 1;
   }
   if (main_pass && !aux.empty()) aux_on_cutouts();
   range_sums_finish(sums_fx, fx_sums, sums, st);  // fixed point -> fp32 (and the accumulator is clean for the next pass)
@@ -2553,7 +2585,7 @@ void Engine::finalize() {
     drop_status_dev = static_cast<DropStatus*>(dp);
   }
   build_cutouts();
-  if (cfg.n_clip < 1 || cfg.n_clip > 2) throw EngineError(-53, "n_clip must be 1 or 2");
+  if (cfg.n_clip < 1 || cfg.n_clip > 3) throw EngineError(-53, "n_clip must be 1, 2 or 3");
   for (int i = 0; i < cfg.n_clip; ++i) build_clip(i);
   for (int i = 0; i < cfg.n_clip; ++i) build_text(i);
   losses_dev = dalloc<float>(64);
@@ -2601,6 +2633,12 @@ void Engine::finalize() {
     for (int i = 0; i < cfg.n_clip; ++i) {
       Clip& C = clip[i];
       std::string p = "clip" + std::to_string(i) + ".";
+      if (C.tower == PXR_TOWER_CLIP_RESNET) {  // the tower's own taps (clipN.rn.*) are registered by build_resnet
+        reg(p + "e", C.e, (size_t)C.B * C.c.out_dim * 4);
+        reg(p + "de", C.de, (size_t)C.B * C.c.out_dim * 4);
+        reg(p + "de16", C.de16, (size_t)C.B * C.c.out_dim * 2);
+        continue;
+      }
       const size_t mw = (size_t)C.M * C.c.width;
       reg(p + "patches", C.patches, (size_t)C.B * C.np * C.Kp * 2);
       reg(p + "g_patches", C.g_patches, (size_t)C.B * C.np * C.Kp * 2);
@@ -2636,6 +2674,7 @@ void Engine::finalize() {
 #include "engine_vdiff.inc"
 #include "engine_superres.inc"
 #include "engine_text.inc"
+#include "engine_resnet.inc"
 
 }  // namespace pxr
 
@@ -2692,7 +2731,7 @@ void pxr_destroy(pxr_handle h) {
 
 int pxr_load_weight(pxr_handle h, int module_id, const char* name, const float* data, const int64_t* dims, int ndim) {
   PXR_TRY(h, {
-    if (module_id < 0 || module_id > 2) throw EngineError(-11, "bad module id");
+    if (module_id < 0 || module_id > 3) throw EngineError(-11, "bad module id");
     if (h->e->finalized) throw EngineError(-12, "weights cannot change after pxr_finalize");
     pxr::HostWeight w;
     w.dims.assign(dims, dims + ndim);
@@ -2709,8 +2748,8 @@ int pxr_set_clip_tower(pxr_handle h, int clip_idx, int kind) {
     Engine* e = h->e;
     if (e->finalized) throw EngineError(-12, "pxr_set_clip_tower: the tower cannot change after pxr_finalize");
     if (clip_idx < 0 || clip_idx >= e->cfg.n_clip) throw EngineError(-14, "bad clip index");
-    if (kind != PXR_TOWER_OPENAI_CLIP && kind != PXR_TOWER_TIMM_VIT)
-      throw EngineError(-10, "unknown tower kind (0 openai-CLIP, 1 timm ViT)");
+    if (kind != PXR_TOWER_OPENAI_CLIP && kind != PXR_TOWER_TIMM_VIT && kind != PXR_TOWER_CLIP_RESNET)
+      throw EngineError(-10, "unknown tower kind (0 openai-CLIP, 1 timm ViT, 2 CLIP ResNet)");
     e->clip[clip_idx].tower = kind;
   });
 }

@@ -202,7 +202,8 @@ struct BlockMap {
 __device__ __forceinline__ int prefetch_kind(const GemmParams& p) {
   return p.res_f32 ? 1
                    : (p.res_f16 ? 2
-                                : ((p.act == ACT_QUICKGELU_BWD || p.act == ACT_GELU_BWD || p.act == ACT_LRELU_BWD) ? 3 : 0));
+                                : ((p.act == ACT_QUICKGELU_BWD || p.act == ACT_GELU_BWD || p.act == ACT_LRELU_BWD ||
+                                    p.act == ACT_RELU_BWD) ? 3 : 0));
 }
 
 // Issue the global loads of the block's input tensor BEFORE the accumulator block is read, so their DRAM latency
@@ -294,6 +295,12 @@ __device__ __forceinline__ void epilogue_block(const GemmParams& p, const float*
       else ld_f16<E>(p.aux_in + o, vec, nv, u);
 #pragma unroll
       for (int j = 0; j < E; ++j) neg |= (col + j >= p.act_col0 && !(u[j] > 0.f)) ? 1u << j : 0u;
+    } else if (p.act == ACT_RELU_BWD) {
+      float u[E];
+      if (vec && kind == 3) unpack_pf<E>(pf[it], 3, u);
+      else ld_f16<E>(p.aux_in + o, vec, nv, u);
+#pragma unroll
+      for (int j = 0; j < E; ++j) neg |= !(u[j] > 0.f) ? 1u << j : 0u;
     } else if (p.act == ACT_QUICKGELU) {
       if (p.aux_out) st_f16<E>(p.aux_out + o, vec, nv, x);
 #pragma unroll
@@ -332,7 +339,11 @@ __device__ __forceinline__ void epilogue_block(const GemmParams& p, const float*
     if (neg) {
 #pragma unroll
       for (int j = 0; j < E; ++j)
-        if (neg & (1u << j)) x[j] *= 0.2f;
+        if (neg & (1u << j)) x[j] = p.act == ACT_RELU_BWD ? 0.f : x[j] * 0.2f;
+    }
+    if (p.act == ACT_RELU) {
+#pragma unroll
+      for (int j = 0; j < E; ++j) x[j] = fmaxf(x[j], 0.f);
     }
     if (p.out_f32) st_f32<E>(p.out_f32 + o, vec, nv, x);
     if (p.out_f16) st_f16<E>(p.out_f16 + o, vec, nv, x);
@@ -1062,7 +1073,8 @@ void (*plain_kernel(const GemmParams& p))(GemmParams) {
     default: break;
   }
   const bool erf = p.act == ACT_GELU || p.act == ACT_GELU_BWD;
-  if (p.res_f32 || p.res_f16 || p.act == ACT_QUICKGELU_BWD || p.act == ACT_GELU_BWD || p.act == ACT_LRELU_BWD)
+  if (p.res_f32 || p.res_f16 || p.act == ACT_QUICKGELU_BWD || p.act == ACT_GELU_BWD || p.act == ACT_LRELU_BWD ||
+      p.act == ACT_RELU_BWD)
     return erf ? gemm_tc_in_kernel<NF, true> : gemm_tc_in_kernel<NF>;
   return erf ? gemm_tc_kernel<NF, true> : gemm_tc_kernel<NF>;
 }
@@ -1269,13 +1281,14 @@ int finish_plan(GemmPlan* plan, const GemmEpilogue& epi, int block_n, int num_sm
     return -10;
   }
   if (epi.act != ACT_NONE && epi.act != ACT_QUICKGELU && epi.act != ACT_QUICKGELU_BWD && epi.act != ACT_LRELU &&
-      epi.act != ACT_LRELU_BWD && epi.act != ACT_GELU && epi.act != ACT_GELU_BWD) {
+      epi.act != ACT_LRELU_BWD && epi.act != ACT_GELU && epi.act != ACT_GELU_BWD && epi.act != ACT_RELU &&
+      epi.act != ACT_RELU_BWD) {
     set_err(err, errlen, "unknown epilogue activation (act must be 0 none, 1 QuickGELU, 2 QuickGELU backward, 4 LeakyReLU, "
-                         "5 LeakyReLU backward, 6 GELU or 7 GELU backward)");
+                         "5 LeakyReLU backward, 6 GELU, 7 GELU backward, 8 ReLU or 9 ReLU backward)");
     return -12;
   }
-  if (epi.act == ACT_LRELU_BWD && !epi.aux_in) {
-    set_err(err, errlen, "the LeakyReLU backward needs the saved post-activation (aux_in)");
+  if ((epi.act == ACT_LRELU_BWD || epi.act == ACT_RELU_BWD) && !epi.aux_in) {
+    set_err(err, errlen, "the (Leaky)ReLU backward needs the saved post-activation (aux_in)");
     return -14;
   }
   if (epi.act == ACT_GELU_BWD && !epi.aux_in) {

@@ -31,8 +31,12 @@ enum OperandMode : int { OP_KMAJOR = 0, OP_MNMAJOR = 1, OP_CONV = 2 };
 // ACT_GELU / ACT_GELU_BWD: exact (erf) GELU of timm's ViT MLP (nn.GELU()), the counterparts of the QuickGELU pair:
 // forward stores the pre-activation u to aux_out as fp16 and returns gelu of exactly that fp16 value; backward multiplies
 // the sum by Phi(u) + u phi(u) of the saved fp16 u.  Both are evaluated in fp32 (erfcf / expf).
+// ACT_RELU / ACT_RELU_BWD: the CLIP ResNet blocks.  Forward: max(0, accumulator + bias + residual), the ReLU after the
+// residual add (relu(main + identity) of a bottleneck).  Backward: the same sum where the saved post-activation aux_in is
+// > 0, else 0.  Both run on the generic epilogue.
 enum EpiAct : int {
-  ACT_NONE = 0, ACT_QUICKGELU = 1, ACT_QUICKGELU_BWD = 2, ACT_LRELU = 4, ACT_LRELU_BWD = 5, ACT_GELU = 6, ACT_GELU_BWD = 7
+  ACT_NONE = 0, ACT_QUICKGELU = 1, ACT_QUICKGELU_BWD = 2, ACT_LRELU = 4, ACT_LRELU_BWD = 5, ACT_GELU = 6, ACT_GELU_BWD = 7,
+  ACT_RELU = 8, ACT_RELU_BWD = 9
 };
 
 constexpr int GEMM_BLOCK_M = 128;

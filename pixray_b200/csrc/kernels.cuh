@@ -496,6 +496,31 @@ void vd_zgrad(const float* g_pred, const act_t* g_in, int ld, float alpha, float
 void vd_renoise(float* x, const float* pred, const float* v, const float* noise, float alpha_i, float sigma_i,
                 float alpha_next, float adjusted_sigma, float ddim_sigma, long long n, cudaStream_t st);
 
+// ------------------------------------------------------------------ CLIP ResNet image towers (kernels_resnet.cu; openai-CLIP
+// ModifiedResNet).  Activations NHWC fp16 with C a multiple of 8; B images of HW pixels each.
+// Stem input (kernels_cutouts.cu): cols [n (cs/2)^2, 64] = the stride-2, pad-1 3x3 im2col of the normalised cutouts
+// (column (c * 3 + ky) * 3 + kx, columns >= 27 zero), and its adjoint gathered into g_batch (=|+=) with the range sums
+// accumulated as patchify_backward does.
+void rn_stem_forward(const float* batch, const float* range, int n, int cs, act_t* cols, const ChannelNorm& nrm,
+                     cudaStream_t st);
+void rn_stem_backward(const act_t* g_cols, const float* batch, const float* range, int n, int cs, int accumulate,
+                      float* g_batch, long long* sums_fx, FxPass fx, const ChannelNorm& nrm, cudaStream_t st);
+// gx = avgpool2x_backward(gy) * (y > 0): the adjoint of AvgPool2d(2) after a ReLU whose output is y.  rows = images * H.
+void rn_pool_bwd_relu(const act_t* gy, const act_t* y, int rows, int W, int C, act_t* gx, cudaStream_t st);
+// attnpool tokens: tok[b, 0] = mean_p x[b, p] + pos[0], tok[b, 1 + p] = x[b, p] + pos[1 + p]; tok fp16 [B, HW + 1, C]
+void rn_pool_tokens(const act_t* x, int B, int HW, int C, const float* pos, act_t* tok, cudaStream_t st);
+// single-query attention of the pool: q fp32 [B, C] (token 0's projection), kv fp16 [B T, 2C] (k | v), 64-wide heads,
+// T <= RN_POOL_MAX_T.  o fp16 [B, C]; p fp32 [B, C / 64, T] the softmax, kept for the backward.
+constexpr int RN_POOL_MAX_T = 256;
+void rn_attnpool_forward(const float* q, const act_t* kv, int B, int T, int C, float scale, act_t* o, float* p,
+                         cudaStream_t st);
+// its backward from g_o fp16 [B, C]: g_q fp16 [B, C], g_kv fp16 [B T, 2C]
+void rn_attnpool_backward(const float* q, const act_t* kv, const float* p, const act_t* g_o, int B, int T, int C,
+                          float scale, act_t* g_q, act_t* g_kv, cudaStream_t st);
+// adjoint of rn_pool_tokens times the block ReLU: gx[b, p] = (g_tok[b, 1 + p] + (g_tok[b, 0] + g_tok0[b]) / HW) * (y[b, p] > 0)
+void rn_pool_tokens_backward(const act_t* g_tok, const act_t* g_tok0, const act_t* y, int B, int HW, int C, act_t* gx,
+                             cudaStream_t st);
+
 void fill_f32(float* p, float v, long long n, cudaStream_t st);
 void cast_f32_to_f16(const float* x, act_t* y, long long n, float scale, cudaStream_t st);
 

@@ -604,6 +604,32 @@ __global__ void __launch_bounds__(256) patchify_bwd_kernel(const act_t* __restri
   }
 }
 
+// The block's share of the two range sums of the preprocess backward (sum g, sum g (x - min) / R): a fixed-order warp and
+// block reduction, then one fixed-point add each.  256-thread blocks.
+__device__ __forceinline__ void range_sums_block_add(float s1, float s2, long long* sums, unsigned int* poison,
+                                                     unsigned int pass) {
+  __shared__ float r1[8], r2[8];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    s1 += __shfl_xor_sync(0xffffffffu, s1, o);
+    s2 += __shfl_xor_sync(0xffffffffu, s2, o);
+  }
+  if ((threadIdx.x & 31) == 0) {
+    r1[threadIdx.x >> 5] = s1;
+    r2[threadIdx.x >> 5] = s2;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float a = 0.f, b2 = 0.f;
+    for (int i = 0; i < 8; ++i) {
+      a += r1[i];
+      b2 += r2[i];
+    }
+    fx_add(&sums[0], a, FX_SUM, FX_SUM_MAX, poison, pass);
+    fx_add(&sums[1], b2, FX_SUM, FX_SUM_MAX, poison, pass);
+  }
+}
+
 // Any patch size (e.g. ViT-L/14: P = 14): one thread per patch element, coalesced over k.
 __global__ void __launch_bounds__(256) patchify_fwd_generic_kernel(const float* __restrict__ batch,
                                                                    const float* __restrict__ range, int n, int cs,
@@ -651,26 +677,77 @@ __global__ void __launch_bounds__(256) patchify_bwd_generic_kernel(const act_t* 
     s2 += g * (batch[t] - mn) / R;
     g_batch[t] = accumulate ? g_batch[t] + g : g;
   }
-  __shared__ float r1[8], r2[8];
+  range_sums_block_add(s1, s2, sums, poison, pass);
+}
+
+// CLIP ResNet stem input: the stride-2, pad-1 3x3 im2col of the normalised cutouts, one thread per 8 of the 64 columns of
+// an output pixel's row.  Column k < 27 = (c * 3 + ky) * 3 + kx (conv1.weight's [cout, 3, 3, 3] order); taps outside the
+// image and columns 27..63 are 0 (the conv pads the normalised image with zeros).
+__global__ void __launch_bounds__(256) rn_stem_fwd_kernel(const float* __restrict__ batch, const float* __restrict__ range,
+                                                          int n, int cs, act_t* __restrict__ cols, ChannelNorm nrm) {
+  pdl_prologue();
+  const int ho = cs / 2;
+  const long long total = (long long)n * ho * ho * 8;
+  const float mn = range[0], R = range[1];
+  for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < total; t += (long long)gridDim.x * blockDim.x) {
+    const int kv = (int)(t & 7);
+    const long long row = t >> 3;
+    const int ox = (int)(row % ho), oy = (int)((row / ho) % ho), b = (int)(row / ((long long)ho * ho));
+    float v[8];
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    s1 += __shfl_xor_sync(0xffffffffu, s1, o);
-    s2 += __shfl_xor_sync(0xffffffffu, s2, o);
-  }
-  if ((threadIdx.x & 31) == 0) {
-    r1[threadIdx.x >> 5] = s1;
-    r2[threadIdx.x >> 5] = s2;
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    float a = 0.f, b2 = 0.f;
     for (int i = 0; i < 8; ++i) {
-      a += r1[i];
-      b2 += r2[i];
+      const int k = kv * 8 + i;
+      v[i] = 0.f;
+      if (k < 27) {
+        const int c = k / 9, ky = (k / 3) % 3, kx = k % 3;
+        const int y = 2 * oy - 1 + ky, x = 2 * ox - 1 + kx;
+        if (y >= 0 && y < cs && x >= 0 && x < cs) {
+          const float a = batch[(((size_t)b * 3 + c) * cs + y) * cs + x];
+          v[i] = (((a - mn) / R) - by_channel(nrm.mean, c)) / by_channel(nrm.std, c);
+        }
+      }
     }
-    fx_add(&sums[0], a, FX_SUM, FX_SUM_MAX, poison, pass);
-    fx_add(&sums[1], b2, FX_SUM, FX_SUM_MAX, poison, pass);
+    uint4 u;
+    __half2* h = reinterpret_cast<__half2*>(&u);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) h[i] = __floats2half2_rn(v[2 * i], v[2 * i + 1]);
+    *reinterpret_cast<uint4*>(cols + (size_t)row * 64 + kv * 8) = u;
   }
+}
+
+// its adjoint as a gather: one thread per batch element sums the (at most 4) column entries that read it, in a fixed tap
+// order, so repeated runs give the same bits; the range sums as patchify_bwd_generic_kernel
+__global__ void __launch_bounds__(256) rn_stem_bwd_kernel(const act_t* __restrict__ g_cols, const float* __restrict__ batch,
+                                                          const float* __restrict__ range, int n, int cs, int accumulate,
+                                                          float* __restrict__ g_batch, long long* __restrict__ sums,
+                                                          unsigned int* poison, unsigned int pass, ChannelNorm nrm) {
+  pdl_prologue();
+  const int ho = cs / 2;
+  const long long total = (long long)n * 3 * cs * cs;
+  const float mn = range[0], R = range[1];
+  float s1 = 0.f, s2 = 0.f;
+  for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < total; t += (long long)gridDim.x * blockDim.x) {
+    const int x = (int)(t % cs), y = (int)((t / cs) % cs), c = (int)((t / ((long long)cs * cs)) % 3);
+    const int b = (int)(t / ((long long)3 * cs * cs));
+    float g = 0.f;
+#pragma unroll
+    for (int ky = 0; ky < 3; ++ky) {
+      const int yy = y + 1 - ky;  // = 2 oy
+      if (yy < 0 || (yy & 1) || (yy >> 1) >= ho) continue;
+#pragma unroll
+      for (int kx = 0; kx < 3; ++kx) {
+        const int xx = x + 1 - kx;
+        if (xx < 0 || (xx & 1) || (xx >> 1) >= ho) continue;
+        const long long row = ((long long)b * ho + (yy >> 1)) * ho + (xx >> 1);
+        g += __half2float(g_cols[(size_t)row * 64 + (c * 3 + ky) * 3 + kx]);
+      }
+    }
+    g /= by_channel(nrm.std, c) * R;
+    s1 += g;
+    s2 += g * (batch[t] - mn) / R;
+    g_batch[t] = accumulate ? g_batch[t] + g : g;
+  }
+  range_sums_block_add(s1, s2, sums, poison, pass);
 }
 
 __global__ void __launch_bounds__(CUT_THREADS) cutout_bwd_kernel(CutoutArgs a, const float* __restrict__ g_batch,
@@ -822,6 +899,17 @@ void patchify_backward(const act_t* g_patches, const float* batch, const float* 
   const long long total = (long long)n * (cs / P) * (cs / P) * (3 * P * P / 8);
   launch_pdl(patchify_bwd_kernel, dim3(patch_grid(total)), dim3(256), 0, st, g_patches, batch, range, n, cs, P, ld, accumulate, g_batch,
                                                          sums, fx.poison, fx.pass, nrm);
+}
+void rn_stem_forward(const float* batch, const float* range, int n, int cs, act_t* cols, const ChannelNorm& nrm,
+                     cudaStream_t st) {
+  const long long total = (long long)n * (cs / 2) * (cs / 2) * 8;
+  launch_pdl(rn_stem_fwd_kernel, dim3(patch_grid(total)), dim3(256), 0, st, batch, range, n, cs, cols, nrm);
+}
+void rn_stem_backward(const act_t* g_cols, const float* batch, const float* range, int n, int cs, int accumulate,
+                      float* g_batch, long long* sums, FxPass fx, const ChannelNorm& nrm, cudaStream_t st) {
+  const long long total = (long long)n * 3 * cs * cs;
+  launch_pdl(rn_stem_bwd_kernel, dim3(patch_grid(total)), dim3(256), 0, st, g_cols, batch, range, n, cs, accumulate, g_batch,
+             sums, fx.poison, fx.pass, nrm);
 }
 void cutout_backward(const CutoutArgs& a, const float* g_batch, const float* range, const int* irange,
                      const float* sums, long long* acc, FxPass fx, float* g_pooled, cudaStream_t st) {

@@ -15,7 +15,7 @@ LOSS_SYMMETRY, LOSS_SATURATION, LOSS_PALETTE, LOSS_SMOOTHNESS, LOSS_EDGE, LOSS_G
 ANCHOR_SPHERICAL, ANCHOR_MSE, ANCHOR_COS, ANCHOR_PIX = 0, 1, 2, 3
 FILTER_TILER, FILTER_WALLPAPER, FILTER_LOOKUP = range(3)
 PAD_REFLECTION, PAD_BORDER = 0, 1
-MOD_VQGAN, MOD_CLIP0, MOD_CLIP1 = 0, 1, 2
+MOD_VQGAN, MOD_CLIP0, MOD_CLIP1, MOD_CLIP2 = 0, 1, 2, 3
 # optimiser update rules (pxr_set_optimizer), by the reference's args.optimiser names (pixray.py:536-551)
 OPT_ADAM, OPT_ADAMW, OPT_ADAGRAD, OPT_ADAMAX, OPT_DIFFGRAD = range(5)
 OPTIMISERS = {"Adam": OPT_ADAM, "AdamW": OPT_ADAMW, "Adagrad": OPT_ADAGRAD, "Adamax": OPT_ADAMAX, "DiffGrad": OPT_DIFFGRAD}
@@ -31,8 +31,41 @@ CLIP_ARCH = {
     # 24^2 + 1 = 577 tokens: its attention runs on the streaming kernels (attn_long.cu)
     "ViT-L/14@336px": dict(width=1024, layers=24, heads=16, patch=14, image_res=336, out_dim=768),
 }
-# Image towers (pxr_set_clip_tower): openai-CLIP's VisionTransformer, or the timm VisionTransformer of SLIP_Base
-TOWER_OPENAI_CLIP, TOWER_TIMM_VIT = 0, 1
+# Image towers (pxr_set_clip_tower): openai-CLIP's VisionTransformer, the timm VisionTransformer of SLIP_Base, or
+# openai-CLIP's ModifiedResNet
+TOWER_OPENAI_CLIP, TOWER_TIMM_VIT, TOWER_CLIP_RESNET = 0, 1, 2
+# openai-CLIP ModifiedResNet towers.  In the ClipCfg, width = the stem width w, layers = the bottleneck blocks of all four
+# stages, heads = the attention pool's (32 w / 64).  `blocks` (per stage) is what a checkpoint's visual.layerN.i. keys are
+# checked against (resnet_arch_of); like `tower` it is not a ClipCfg field.
+RESNET_ARCH = {
+    name: dict(width=w, layers=sum(b), heads=w // 2, patch=0, image_res=res, out_dim=d, tower=TOWER_CLIP_RESNET, blocks=b)
+    for name, w, b, res, d in (("RN50", 64, (3, 4, 6, 3), 224, 1024), ("RN101", 64, (3, 4, 23, 3), 224, 512),
+                               ("RN50x4", 80, (4, 6, 10, 6), 288, 640), ("RN50x16", 96, (6, 8, 18, 8), 384, 768),
+                               ("RN50x64", 128, (3, 15, 36, 10), 448, 1024))
+}
+_NOT_CLIPCFG = ("tower", "blocks")
+
+
+def resnet_arch_of(state_dict):
+    """The ModifiedResNet shape a CLIP state_dict describes, as openai-CLIP's build_model derives it: the block count of
+    each stage from the visual.layerN.i. keys, the stem width from layer1.0.conv1, the input side from the attention
+    pool's positional_embedding (32 * sqrt(rows - 1)), out_dim from c_proj."""
+    blocks = tuple(len({k.split(".")[2] for k in state_dict if k.startswith(f"visual.layer{s}.")}) for s in (1, 2, 3, 4))
+    w = int(state_dict["visual.layer1.0.conv1.weight"].shape[0])
+    side = round((state_dict["visual.attnpool.positional_embedding"].shape[0] - 1) ** 0.5)
+    return dict(width=w, layers=sum(blocks), heads=w // 2, patch=0, image_res=32 * side,
+                out_dim=int(state_dict["visual.attnpool.c_proj.weight"].shape[0]), tower=TOWER_CLIP_RESNET, blocks=blocks)
+
+
+def check_resnet_state_dict(name, state_dict):
+    """Refuse a checkpoint whose ModifiedResNet shape is not the one RESNET_ARCH gives `name`."""
+    got, want = resnet_arch_of(state_dict), RESNET_ARCH[name]
+    if got != want:
+        raise EngineError(f"perceptor '{name}': the weights describe a ResNet with {got['blocks']} blocks per stage, stem "
+                          f"width {got['width']}, input {got['image_res']} and out_dim {got['out_dim']}; {name} has "
+                          f"{want['blocks']}, {want['width']}, {want['image_res']} and {want['out_dim']}")
+
+
 # SLIP_Base models (slip.py:84-157, SLIP/models.py:288-331) whose image tower the engine builds: timm ViTs with 64-wide
 # heads.  SLIP_CC3M / SLIP_CC12M are the B/16 architecture on other data (slip.py:134-135).  `tower` is not a ClipCfg
 # field: B200Engine hands it to pxr_set_clip_tower.
@@ -60,6 +93,9 @@ def stroke_z_layout(n_paths, n_segments):
 
 
 class B200Engine:
+    # the image-tower kinds this library builds (pxr_set_clip_tower)
+    TOWERS = (TOWER_OPENAI_CLIP, TOWER_TIMM_VIT, TOWER_CLIP_RESNET)
+
     def __init__(self, *, drawer=DRAWER_VQGAN, image_hw=(256, 256), vqgan=None, grid=None, cutn=64, cut_size=224,
                  clip=(), noise_fac=0.1, seed=0, device=0, rank=0, world=1, grad_scale=0.0, lr_betas=(0.9, 0.999),
                  adam_eps=1e-8, fft_decay=0.0, fft_colors=0.0, fft_contrast=0.0, cut_aspect=1.0, polygons=None,
@@ -115,7 +151,7 @@ class B200Engine:
         cfg.n_clip = len(clip)
         for i, c in enumerate(clip):
             for k, val in c.items():
-                if k != "tower":
+                if k not in _NOT_CLIPCFG:
                     setattr(cfg.clip[i], k, val)
         cfg.noise_fac, cfg.seed = noise_fac, seed
         cfg.op_dtype, cfg.grad_scale = 0, grad_scale

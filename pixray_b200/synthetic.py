@@ -190,6 +190,72 @@ def z0_vqgan(codebook, hw, seed=0):
     return (z + 0.05 * torch.randn(z.shape, generator=g)).contiguous()
 
 
+def _resnet_shapes(arch):
+    """(name, cin, cout, ks, output pixels) of every conv of a ModifiedResNet, stem first, in forward order."""
+    w, res = arch["width"], arch["image_res"]
+    h = res // 2
+    out = [("conv1", 3, w // 2, 3, h * h), ("conv2", w // 2, w // 2, 3, h * h), ("conv3", w // 2, w, 3, h * h)]
+    h //= 2
+    cin = w
+    for s, n in enumerate(arch["blocks"]):
+        planes = w << s
+        for i in range(n):
+            stride = 2 if (s > 0 and i == 0) else 1
+            p, ho = f"layer{s + 1}.{i}.", h // stride
+            out += [(p + "conv1", cin, planes, 1, h * h), (p + "conv2", planes, planes, 3, h * h),
+                    (p + "conv3", planes, 4 * planes, 1, ho * ho)]
+            if stride > 1 or cin != 4 * planes:
+                out.append((p + "downsample.0", cin, 4 * planes, 1, ho * ho))
+            cin, h = 4 * planes, ho
+    return out
+
+
+def clip_resnet_state_dict(arch, seed=0, text=None, last_gamma=0.2):
+    """openai-CLIP ModifiedResNet 'visual.*' tensors under the checkpoint's own keys, BatchNorm included (weight, bias,
+    running_mean, running_var, num_batches_tracked) with non-trivial running statistics.  Convs are He-scaled and each
+    block's bn3 has gamma ~ last_gamma, so the residual stream stays O(1) in fp16 through RN50x64's 36-block stage.
+    text = (width, layers) merges a text tower (clip_text_state_dict) with out_dim = arch['out_dim']."""
+    g = torch.Generator().manual_seed(seed)
+    w, D = arch["width"], arch["out_dim"]
+    C = 32 * w
+    side = arch["image_res"] // 32
+    sd = {}
+
+    def bn(prefix, c, gamma=1.0):
+        sd[prefix + ".weight"] = gamma * (1 + 0.1 * _randn(g, c))
+        sd[prefix + ".bias"] = 0.05 * _randn(g, c)
+        sd[prefix + ".running_mean"] = 0.1 * _randn(g, c)
+        sd[prefix + ".running_var"] = 0.5 + torch.rand(c, generator=g)
+        sd[prefix + ".num_batches_tracked"] = torch.tensor(1000, dtype=torch.int64)
+
+    for name, cin, cout, ks, _ in _resnet_shapes(arch):
+        sd[f"visual.{name}.weight"] = _randn(g, cout, cin, ks, ks, std=(2.0 / (cin * ks * ks)) ** 0.5)
+        if name.startswith("conv"):
+            bn("visual.bn" + name[-1], cout)
+        elif name.endswith("downsample.0"):
+            bn(f"visual.{name[:-1]}1", cout)
+        else:
+            bn(f"visual.{name[:-6]}.bn{name[-1]}", cout, last_gamma if name.endswith("conv3") else 1.0)
+    p = "visual.attnpool."
+    sd[p + "positional_embedding"] = _randn(g, side * side + 1, C, std=C ** -0.5)
+    for nm in ("q_proj", "k_proj", "v_proj"):
+        sd[p + nm + ".weight"] = _randn(g, C, C, std=C ** -0.5)
+        sd[p + nm + ".bias"] = _randn(g, C, std=0.02)
+    sd[p + "c_proj.weight"] = _randn(g, D, C, std=C ** -0.5)
+    sd[p + "c_proj.bias"] = _randn(g, D, std=0.02)
+    if text is not None:
+        sd.update(clip_text_state_dict(text[0], text[1], D, seed + 1))
+    return sd
+
+
+def resnet_fwd_flops(arch):
+    """Algorithmic forward FLOPs of one image through a ModifiedResNet: every conv at its real (unpadded) channel counts,
+    and the attention pool's projections and single-query attention."""
+    fl = sum(2.0 * px * cin * cout * ks * ks for _, cin, cout, ks, px in _resnet_shapes(arch))
+    C, T = 32 * arch["width"], (arch["image_res"] // 32) ** 2 + 1
+    return fl + 2.0 * T * C * 2 * C + 2.0 * C * C + 4.0 * T * C + 2.0 * C * arch["out_dim"]
+
+
 def vit_fwd_flops(arch):
     """Algorithmic forward FLOPs of one image through the ViT (SURVEY.md 8d formula)."""
     W, L, P = arch["width"], arch["layers"], arch["patch"]
