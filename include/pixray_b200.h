@@ -35,7 +35,7 @@ enum { PXR_DRAWER_VQGAN = 0, PXR_DRAWER_PIXEL = 1, PXR_DRAWER_FFT = 2, PXR_DRAWE
 enum { PXR_PAD_REFLECTION = 0, PXR_PAD_BORDER = 1, PXR_PAD_ZEROS = 2 };
 enum { PXR_DTYPE_F16 = 0, PXR_DTYPE_BF16 = 1 };
 /* module ids for pxr_load_weight */
-enum { PXR_MOD_VQGAN = 0, PXR_MOD_CLIP0 = 1, PXR_MOD_CLIP1 = 2, PXR_MOD_CLIP2 = 3 };
+enum { PXR_MOD_VQGAN = 0, PXR_MOD_CLIP0 = 1, PXR_MOD_CLIP1 = 2, PXR_MOD_CLIP2 = 3, PXR_MOD_CLIP3 = 4 };
 
 /* ViT towers: the fields as named.  CLIP ResNet towers (PXR_TOWER_CLIP_RESNET): width = the stem width w (64 for RN50),
  * layers = the number of bottleneck blocks over all four stages (16 for RN50), heads = the attention pool's heads
@@ -45,7 +45,7 @@ typedef struct {
   int layers;    /* 12 */
   int heads;     /* 12 */
   int patch;     /* 16 or 32 */
-  int image_res; /* 224 == MakeCutouts cut_size (pixray.py:643-649) */
+  int image_res; /* the cut_size of the perceptor's MakeCutouts (pixray.py:643-649); the first perceptor's == cut_size */
   int out_dim;   /* 512 */
 } pxr_clip_cfg;
 
@@ -62,8 +62,10 @@ typedef struct {
   int grid_rows, grid_cols;
   /* MakeCutouts(cut_size, cutn) pixray.py:400-443; cutn is the GLOBAL count, this rank owns a slice */
   int cutn, cut_size;
-  int n_clip;            /* 1 to 3 perceptors */
-  pxr_clip_cfg clip[3];
+  /* 1 to 4 perceptors.  One cutout set per distinct image_res, in order of first appearance (pixray.py:642-649): set 0 is
+   * cut_size (the first perceptor's), and each perceptor scores only its own set's batch. */
+  int n_clip;
+  pxr_clip_cfg clip[4];
   float noise_fac;       /* pixray.py:439 (0.1) */
   uint64_t seed;
   int op_dtype;          /* PXR_DTYPE_*: tensor-core operand type (accumulation is always fp32) */
@@ -152,7 +154,8 @@ int pxr_set_image_prompts_sized(pxr_handle h, const float* const* imgs, const in
  * (make_cutouts(out, spot=1) zeroes mask >= 0.5), which = 0: with everything but the spot zeroed.  Every pxr_iterate then
  * runs one more cutout + encode + backward pass per kind (cached transforms of the iteration, no ColorJitter, fresh noise);
  * their losses come FIRST in the perceptor's part of the loss vector (spot, spot off, prompts, image prompts).
- * mask: host bytes [3, cut_size, cut_size], != 0 where the resized RGB mask image is >= 0.5. */
+ * mask: host bytes [3, cut_size, cut_size], != 0 where the resized RGB mask image is >= 0.5.  Both fail (-69) in a session
+ * with more than one cutout set (the reference cuts those with the last set's MakeCutouts, pixray.py:1270-1276). */
 int pxr_set_spot_prompts(pxr_handle h, int clip_idx, int which, const float* embeds, int n, int D, const float* weights,
                          const float* stops);
 int pxr_set_spot_mask(pxr_handle h, const unsigned char* mask);
@@ -191,6 +194,15 @@ int pxr_vqgan_encode(pxr_handle h, const float* img, float* z_out);
 int pxr_set_color_jitter(pxr_handle h, float p, float saturation, float hue);
 int pxr_make_cutouts(pxr_handle h, const float* img, const pxr_cut_params* p, int iter,
                      float* out_batch /* [cutn_local,3,cs,cs] */);
+/* Cutout sets (after pxr_finalize): returns their number and writes each one's cut size to cut_sizes[0..3] (0 past the
+ * last).  pxr_make_cutouts_set cuts set `set` (its own augmentations and noise, Philox streams of its own; the fill grey
+ * and padding mode are shared) into out_batch [cutn_local, 3, cs, cs] of that set's cs; pxr_make_cutouts is set 0.
+ * pxr_encode_image reads the batch of the perceptor's own set: a caller batch must have that set's size, and without
+ * one the set must have been cut since the last pxr_backward.  pxr_backward takes back every set cut since the last
+ * backward (set 0 when none was), adding their image gradients. */
+int pxr_cutout_sets(pxr_handle h, int* cut_sizes /* [4] */);
+int pxr_make_cutouts_set(pxr_handle h, int set, const float* img, const pxr_cut_params* p, int iter,
+                         float* out_batch /* [cutn_local,3,cs,cs] */);
 int pxr_encode_image(pxr_handle h, int clip_idx, const float* batch, float* out_embeds /* [cutn_local, D] */);
 
 /* Text tower of perceptor clip_idx (CLIP.encode_text, SLIP/models.py:136-150): built at pxr_finalize when the weights
@@ -205,8 +217,13 @@ int pxr_backward(pxr_handle h, float* z_grad);
 int pxr_step(pxr_handle h, float* z, float lr, int iter);
 int pxr_iterate(pxr_handle h, float* z, float lr, int iter, const pxr_cut_params* p,
                 float* out_losses_host /* pinned or pageable; may be NULL */);
+/* pxr_iterate with one pxr_cut_params per cutout set, in set order (p NULL: the engine draws every set's).  A session
+ * with more than one set takes explicit parameters only here: pxr_iterate with p != NULL fails (-69). */
+int pxr_iterate_sets(pxr_handle h, float* z, float lr, int iter, const pxr_cut_params* p /* [n_sets] or NULL */,
+                     float* out_losses_host);
 /* Auxiliary losses: Losses/*.py behind LossInterface.get_loss, summed into the iteration's loss list by ascend_txt
- * (pixray.py:1384-1393, custom_loss spec "name:weight").  Each becomes one more entry of the loss vector (after the
+ * (pixray.py:1384-1393, custom_loss spec "name:weight").  Each becomes one more entry of the loss vector (a cutout-space
+ * one, marked (cutouts) below, one entry per cutout set in set order, pixray.py:1392-1398) (after the
  * prompts, in the order added) and one more term of the gradient.  params (host floats), by kind:
  *   SYMMETRY   {symmetry_weight}                                            Losses/SymmetryLoss.py:14-17   (image)
  *   SATURATION {saturation_weight}                                          Losses/SaturationLoss.py:15-30 (cutouts)

@@ -24,7 +24,7 @@ class Config(C.Structure):
         ("ch_mult", C.c_int * 8),
         ("grid_rows", C.c_int), ("grid_cols", C.c_int),
         ("cutn", C.c_int), ("cut_size", C.c_int),
-        ("n_clip", C.c_int), ("clip", ClipCfg * 3),
+        ("n_clip", C.c_int), ("clip", ClipCfg * 4),
         ("noise_fac", C.c_float), ("seed", C.c_uint64),
         ("op_dtype", C.c_int), ("grad_scale", C.c_float),
         ("beta1", C.c_float), ("beta2", C.c_float), ("adam_eps", C.c_float),
@@ -75,6 +75,7 @@ EXPORTS = [
     "pxr_set_polygons", "pxr_set_synth_iteration", "pxr_test_raster_samples", "pxr_set_strokes", "pxr_set_optimizer",
     "pxr_test_splitk_reduce", "pxr_test_groupnorm_unet", "pxr_test_resample", "pxr_test_gemv",
     "pxr_test_prompt_loss", "pxr_text_tower", "pxr_encode_text", "pxr_test_attention_causal",
+    "pxr_cutout_sets", "pxr_make_cutouts_set", "pxr_iterate_sets",
 ]
 
 _lib = None

@@ -15,9 +15,12 @@ engine calls whether or not the option is given; another rule adds one set_optim
 
 Perceptors are named in `clip_models`, as get_clip_perceptor keys on them (slip.py:173-186): the openai-CLIP ViTs
 (engine.CLIP_ARCH: ViT-B/32, ViT-B/16, ViT-L/14, ViT-L/14@336px) and the SLIP_Base ViTs (engine.SLIP_ARCH: SLIP_VITB16,
-SLIP_CC3M, SLIP_CC12M, CLIP_VITB16, SLIP_VITL16, CLIP_VITL16), alone or two of them mixed.  The cutouts are made at the
-first perceptor's input resolution (224, or 336 for ViT-L/14@336px); the engine has one cutout batch, so towers of
-different input resolutions cannot be mixed in one session.  The reference's `perceptors` option only picks a default
+SLIP_CC3M, SLIP_CC12M, CLIP_VITB16, SLIP_VITL16, CLIP_VITL16) and the openai-CLIP ResNets (engine.RESNET_ARCH), up to four
+per session, mixed as the reference mixes them.  Like the reference's cutoutsTable (pixray.py:642-649) there is one
+cutout batch per distinct input resolution (224, 288 for RN50x4, 336 for ViT-L/14@336px, ...), each cut from the same image,
+and every tower scores its own resolution's batch; so quality "best" and "supreme" run.  Spot prompts are refused when
+the resolutions differ (the reference cuts those with its last MakeCutouts, pixray.py:1270-1276).  The reference's
+`perceptors` option only picks a default
 `clip_models` from its quality table (pixray.py:1832-1845); naming the models in `clip_models` runs the same towers.
 What the reference fetches from the network at init time comes in through three extra settings instead:
 
@@ -358,14 +361,24 @@ def do_init(args):
         if m not in E.CLIP_ARCH and m not in E.SLIP_ARCH and m not in E.RESNET_ARCH:
             raise NotImplementedError(f"perceptor '{m}': only the image towers {sorted(E.CLIP_ARCH)}, "
                                       f"{sorted(E.RESNET_ARCH)} (openai-CLIP) and {sorted(E.SLIP_ARCH)} (SLIP) are built")
-    if len(args.clip_models) > 3:
-        raise NotImplementedError("at most three perceptors per session")
+    # what the engine class builds: an engine that does not declare them has one cutout batch and three perceptors
+    max_perceptors = getattr(_engine_factory, "MAX_PERCEPTORS", 3)
+    mixed = getattr(_engine_factory, "MIXED_RESOLUTIONS", False)
+    if len(args.clip_models) > max_perceptors:
+        raise NotImplementedError("at most three perceptors per session" if max_perceptors == 3
+                                  else f"at most {max_perceptors} perceptors per session")
     arch = {m: E.CLIP_ARCH.get(m) or E.RESNET_ARCH.get(m) or E.SLIP_ARCH[m] for m in args.clip_models}
     res = {m: arch[m]["image_res"] for m in args.clip_models}
     if len(set(res.values())) > 1:
-        # pixray.py:645-649 makes one MakeCutouts per input resolution; the engine scores every tower on one cutout batch
-        raise NotImplementedError(f"perceptors {res} need cutouts at different resolutions; the engine makes one cutout "
-                                  "batch per iteration, so towers of one input resolution only")
+        if not mixed:
+            # pixray.py:645-649 makes one MakeCutouts per input resolution; this engine scores every tower on one batch
+            raise NotImplementedError(f"perceptors {res} need cutouts at different resolutions; the engine makes one "
+                                      "cutout batch per iteration, so towers of one input resolution only")
+        if split_pipes(args.spot_prompts) or split_pipes(args.spot_prompts_off):
+            raise ValueError(f"spot prompts with perceptors of different input resolutions {res} are not built: the "
+                             "reference cuts every resolution's spot batch with the last MakeCutouts (pixray.py:1270-1276 "
+                             "reuses the loop variable make_cutouts) and rescales it to each perceptor with torchvision's "
+                             "Resize (slip.py:53-57), whose antialiasing depends on the torchvision version")
     st.seed = _seed_everything(args)
     kind = _DRAWER_KIND[args.drawer]
     drawer_class = class_table[args.drawer]
@@ -495,8 +508,13 @@ def do_init(args):
     st.perceptors = [P.Perceptor(st.session, i, "slip" if m in E.SLIP_ARCH else "clip", getattr(args, "b200_bpe_vocab", None))
                      for i, m in enumerate(args.clip_models)]
     towers = [p.encode_text if p.has_text_tower() else None for p in st.perceptors]
-    st.make_cutouts = P.MakeCutouts(clip_cfgs[0]["image_res"], args.num_cuts, st.session, cut_pow=args.cut_pow, seed=st.seed,
-                                    aspect=aspect)
+    # cutoutsTable (pixray.py:642-649): one MakeCutouts per input resolution, in order of first appearance; the engine's
+    # cutout set k is the table's k-th entry
+    st.cutouts_table = {}
+    for k, cs in enumerate(E.cutout_sets(clip_cfgs[0]["image_res"], [c["image_res"] for c in clip_cfgs])[0]):
+        st.cutouts_table[cs] = P.MakeCutouts(cs, args.num_cuts, st.session, cut_pow=args.cut_pow, seed=st.seed + k,
+                                             aspect=aspect, cut_set=k)
+    st.make_cutouts = st.cutouts_table[clip_cfgs[0]["image_res"]]
 
     # ---- prompts, in the order ascend_txt scores them (pixray.py:859-958): text, vector, noise; then image prompts
     tables = [[] for _ in args.clip_models]

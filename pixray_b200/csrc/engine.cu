@@ -39,7 +39,7 @@ class Engine {
   bool stream16 = true;       // the ViT residual stream and its gradient in fp16, like the reference's CUDA path (clip.load gives a half model, slip.py:176); PXR_CLIP_STREAM=32 keeps them in fp32
   bool fused_attn = true;     // PXR_FUSED_ATTN=0: fall back to the batched-GEMM attention (attn_tc.cu covers T <= 240,
                               // attn_long.cu T > 257)
-  std::map<std::string, HostWeight> weights[4];
+  std::map<std::string, HostWeight> weights[5];
   std::vector<void*> allocs;
   bool finalized = false;
   std::map<std::string, std::pair<void*, size_t>> dbg;  // named internal buffers (tests / debugging)
@@ -116,14 +116,41 @@ class Engine {
   int cur_cut_h() const { return filtered_valid ? cut_h : cfg.image_h; }
   int cur_cut_w() const { return filtered_valid ? cut_w : cfg.image_w; }
 
-  // ---- cutouts
-  float *pooled = nullptr, *g_pooled = nullptr, *batch = nullptr, *g_batch = nullptr;
+  // ---- cutouts: one cutout set per distinct perceptor input resolution, in order of first appearance (the reference's
+  // cutoutsTable, pixray.py:642-649).  Set 0 has the first perceptor's resolution, cfg.cut_size.  Every set is cut from the
+  // same image with its own augmentations and noise; its perceptors see only its batch.
+  static constexpr int RING = 8;
+  struct CutSet {
+    int cs = 0;
+    float *pooled = nullptr, *g_pooled = nullptr, *batch = nullptr, *g_batch = nullptr;
+    int src_h = 0, src_w = 0;
+    float *cut_src = nullptr, *g_cut_src = nullptr;  // [3, src_h, src_w]; == pooled / g_pooled when square
+    int* pool_argmax = nullptr;
+    float *part_min = nullptr, *part_max = nullptr, *range = nullptr, *sums = nullptr;
+    int *part_imin = nullptr, *part_imax = nullptr, *irange = nullptr;
+    int n_parts = 0;
+    float* minv_host[RING] = {nullptr};   // pinned
+    float* facs_host[RING] = {nullptr};
+    cudaEvent_t ring_ev[RING] = {nullptr};
+    int ring_pos = 0;
+    float *minv_dev = nullptr, *facs_dev = nullptr;
+    CutoutArgs cut_args;
+    float* img_prompts = nullptr;  // [n_img, 3, src_h, src_w]: the pooled (and stretched) image prompt targets
+    // cutout-space auxiliary losses' scratch
+    float* aux_A = nullptr;       // smoothness per-pixel factor
+    float* aux_halo = nullptr;    // smoothness rows of the neighbouring ranks
+    float* aux_xbuf = nullptr;    // smoothness halo exchange buffer
+    float* aux_blur = nullptr;    // smoothness_gaussian_kernel: blurred batch, its gradient, the one-axis scratch
+    float* aux_g_blur = nullptr;  //   (allocated when the first blurred smoothness loss is added, [n_local, 3, cs, cs] each)
+    float* aux_blur_tmp = nullptr;
+    int* aux_best = nullptr;      // palette argmin per pixel (bookkeeping, also a debug buffer)
+    bool cut = false;             // cut since the last backward (the per-op path's pxr_backward takes these back)
+  };
+  std::vector<CutSet> sets;
+  int set_of[4] = {0, 0, 0, 0};  // cutout set of each perceptor
+  int n_sets() const { return (int)sets.size(); }
   // non-square canvas (cfg.cut_aspect != 1): the warps sample from a stretch of the pooled image (pixray.py:468-472)
   double aspect = 1.0;
-  int src_h = 0, src_w = 0;
-  float *cut_src = nullptr, *g_cut_src = nullptr;  // [3, src_h, src_w]; == pooled / g_pooled when square
-  int* pool_argmax = nullptr;
-  float *part_min = nullptr, *part_max = nullptr, *range = nullptr, *sums = nullptr;
   long long *sums_fx = nullptr, *grad_fx = nullptr;  // 64-bit fixed-point accumulators (order-independent sums, kernels_cutouts.cu)
   unsigned int* fx_poison = nullptr;                   // [2]: pass id of the last non-finite contribution to {gradient images, range sums}
   unsigned int fx_pass = 0;
@@ -133,16 +160,7 @@ class Engine {
     f.pass = ++fx_pass;
     return f;
   }
-  int *part_imin = nullptr, *part_imax = nullptr, *irange = nullptr;
-  int n_parts = 0;
-  static constexpr int RING = 8;
-  float* minv_host[RING] = {nullptr};   // pinned
-  float* facs_host[RING] = {nullptr};
-  cudaEvent_t ring_ev[RING] = {nullptr};
-  int ring_pos = 0;
-  float *minv_dev = nullptr, *facs_dev = nullptr;
   float cj_p = 0.8f, cj_sat = 0.1f, cj_hue = 0.1f;  // K.ColorJitter(hue=0.1, saturation=0.1, p=0.8), pixray.py:416, 436
-  CutoutArgs cut_args;
 
   // ---- perceptors
   struct Clip {
@@ -191,7 +209,7 @@ class Engine {
     } spot[2];
     OpList fwd, bwd;
   };
-  Clip clip[3];
+  Clip clip[4];
   // ---- text towers (engine_text.inc): encode_text of a perceptor whose weights carry token_embedding.weight.  Built at
   // finalize (host weights are dropped there), forward only, TEXT_CHUNK sequences per run of the op list.
   struct Text {
@@ -212,7 +230,7 @@ class Engine {
     OpList fwd;
   };
   static constexpr int TEXT_CHUNK = 32;
-  std::unique_ptr<Text> text[3];
+  std::unique_ptr<Text> text[4];
   void build_text(int i);
   void encode_text(int i, const int32_t* tokens, int n, int ctx, float* out);
   // ---- CLIP ResNet image towers (engine_resnet.inc): the perceptor's Clip keeps its prompts, embeddings and op lists;
@@ -227,7 +245,7 @@ class Engine {
     act_t *wq = nullptr, *wkv = nullptr, *wc = nullptr;
     float *bq = nullptr, *bkv = nullptr, *bc = nullptr, *pos = nullptr;
   };
-  std::unique_ptr<Resnet> rn[3];
+  std::unique_ptr<Resnet> rn[4];
   RnConv rn_conv(int mod, const std::string& conv, const std::string& bn, int cin, int cout, int ks, bool flat);
   void build_resnet(int i);
   // the tower's input stage: the cutouts (batch, range) -> its first GEMM operand, and back into g_batch
@@ -238,13 +256,13 @@ class Engine {
   float* losses_host = nullptr;  // pinned
   int total_prompts = 0;
   // image prompts (pixray.py:1308-1336): target images, cut + encoded every iteration with the cached transforms
-  float* img_prompts = nullptr;  // [n_img, 3, cs, cs]: the POOLED targets ((avg + max) / 2 of each image at its own size,
-                                 // pixray.py:463): constants, pooled once when they are set, not every iteration
+  // the targets are each set's img_prompts, POOLED ((avg + max) / 2 of each image at its own size, pixray.py:463):
+  // constants, pooled once when they are set, not every iteration
   int n_img = 0;
   std::vector<float> img_w;
   void rebuild_prompt_rows();
-  void encode_image_prompts();
-  // spot passes: the mask (device [3, cs, cs], != 0 where the mask image is >= 0.5) and the masked pooled image
+  void encode_image_prompts(int s);
+  // spot passes (one cutout set only): the mask (device [3, cs, cs], != 0 where the mask image is >= 0.5) and the masked pooled image
   unsigned char* spot_mask = nullptr;
   float* pooled_masked = nullptr;
   bool any_spot(int which) const {
@@ -252,9 +270,15 @@ class Engine {
       if (clip[i].spot[which].n > 0) return true;
     return false;
   }
+  static const char* spot_multiset_error() {
+    return "spot prompts with perceptors of different input resolutions are not built: the reference cuts every "
+           "resolution's spot batch with the last MakeCutouts (pixray.py:1270-1276 reuses the loop variable make_cutouts) "
+           "and rescales it to each perceptor with torchvision's Resize (slip.py:53-57), whose antialiasing depends on "
+           "the torchvision version";
+  }
   bool spot_accumulated = false;  // a spot pass of this iteration already wrote d loss / d image: the main pass adds to it
   bool spot_pass(int which, bool accumulate_img);
-  void backward_to_image(const CutoutArgs& a, int mask_which, bool accumulate_img, bool main_pass);
+  void backward_to_image(int s, const CutoutArgs& a, int mask_which, bool accumulate_img, bool main_pass);
   void backward_drawer();
 
   // ---- auxiliary losses (Losses/*.py; pixray.py:1384-1393): extra loss-vector entries after the prompts
@@ -268,13 +292,6 @@ class Engine {
   std::vector<AuxLoss> aux;
   double* aux_part = nullptr;   // reduction scratch
   double* aux_sums = nullptr;   // saturation moments (4)
-  float* aux_A = nullptr;       // smoothness per-pixel factor
-  float* aux_halo = nullptr;    // smoothness rows of the neighbouring ranks
-  float* aux_xbuf = nullptr;    // smoothness halo exchange buffer
-  float* aux_blur = nullptr;    // smoothness_gaussian_kernel: blurred batch, its gradient, the one-axis scratch
-  float* aux_g_blur = nullptr;  //   (allocated when the first blurred smoothness loss is added, [n_local, 3, cs, cs] each)
-  float* aux_blur_tmp = nullptr;
-  int* aux_best = nullptr;      // palette argmin per pixel (bookkeeping, also a debug buffer)
   // ---- anchors to a stored copy (pixray.py:1344-1375): loss-vector entries between the prompts and the auxiliary losses
   struct Anchor {
     int kind;      // PXR_ANCHOR_*
@@ -286,9 +303,20 @@ class Engine {
   void anchors_on_image();  // init_weight_pix: into the (filtered) image gradient, before the drawer backward
   void anchors_on_z();      // z-space terms: into z.grad, after the drawer backward
   int aux_base() const { return total_prompts + (int)anchors.size(); }
-  int num_losses() const { return aux_base() + (int)aux.size(); }  // total_prompts includes the filter slots in front
+  // a cutout-space loss (saturation, palette, smoothness) has one entry per cutout set, in set order (the list its
+  // get_loss returns, spliced into the loss vector by pixray.py:1392-1398); every other loss has one
+  static bool aux_per_set(int kind) {
+    return kind == PXR_LOSS_SATURATION || kind == PXR_LOSS_PALETTE || kind == PXR_LOSS_SMOOTHNESS;
+  }
+  int aux_width(int kind) const { return aux_per_set(kind) ? n_sets() : 1; }
+  int aux_slot(size_t k, int s = 0) const {
+    int off = aux_base();
+    for (size_t j = 0; j < k; ++j) off += aux_width(aux[j].kind);
+    return off + s;
+  }
+  int num_losses() const { return aux_slot(aux.size()); }  // total_prompts includes the filter slots in front
   void aux_after_embed();   // aesthetic: needs de of the last perceptor (after its prompt_loss)
-  void aux_on_cutouts();    // saturation / palette / smoothness: add into g_batch
+  void aux_on_cutouts(int s);  // saturation / palette / smoothness: add into the set's g_batch
   void aux_on_image();      // symmetry / edge / gaussian: add into g_img
 
   // ---- comm (multi-GPU, cutout sharding): one NCCL communicator owned by the engine (comm.cuh)
@@ -364,6 +392,17 @@ class Engine {
     PXR_CUDA(cudaEventCreate(&r.a));
     PXR_CUDA(cudaEventCreate(&r.b));
     PXR_CUDA(cudaEventRecord(r.a, st));
+  }
+  // a stage outside the op lists (the cutouts of one set) as one profile record; its launches are not counted again
+  void prof_begin_stage(ProfRec& r, const std::string& name) {
+    r.flops = r.bytes = 0.0;
+    r.launches = 0;
+    r.name = name;
+    prof_begin(r);
+  }
+  void prof_end_stage(ProfRec& r) {
+    PXR_CUDA(cudaEventRecord(r.b, st));
+    prof.push_back(r);
   }
   bool trace = false;  // PXR_TRACE=1: print every op before it runs and synchronise after it (localises a hanging kernel)
   void run(OpList& l) {
@@ -733,12 +772,12 @@ class Engine {
   SrConv sr_load_conv(const std::string& prefix, int cin, int cout, float scale);
 
   // ------------------------------------------------------------------ execution
-  void prepare_cut_params(const pxr_cut_params* p, int iter);
+  void prepare_cut_params(int s, const pxr_cut_params* p, int iter);
   void forward_drawer() {
     if (cfg.drawer == PXR_DRAWER_VDIFF) vdiff_forward();
     else run(drawer_fwd);
   }
-  void forward_cutouts();
+  void forward_cutouts(int s);
   void forward_clip(int i);
   void loss_clip(int i);
   void backward_all();
@@ -753,11 +792,12 @@ Engine::~Engine() {
   if (comm && Comm::api().destroy) Comm::api().destroy(comm);
   fft_plans_destroy(fft);
   for (void* p : allocs) cudaFree(p);
-  for (int i = 0; i < RING; ++i) {
-    if (minv_host[i]) cudaFreeHost(minv_host[i]);
-    if (facs_host[i]) cudaFreeHost(facs_host[i]);
-    if (ring_ev[i]) cudaEventDestroy(ring_ev[i]);
-  }
+  for (CutSet& K : sets)
+    for (int i = 0; i < RING; ++i) {
+      if (K.minv_host[i]) cudaFreeHost(K.minv_host[i]);
+      if (K.facs_host[i]) cudaFreeHost(K.facs_host[i]);
+      if (K.ring_ev[i]) cudaEventDestroy(K.ring_ev[i]);
+    }
   if (losses_host) cudaFreeHost(losses_host);
   if (drop_status) cudaFreeHost(const_cast<DropStatus*>(drop_status));
   if (st) cudaStreamDestroy(st);
@@ -1602,100 +1642,126 @@ void Engine::build_fft() {
 
 // ===================================================================================================== cutouts
 void Engine::build_cutouts() {
-  const int cs_ = cfg.cut_size;
-  pooled = dalloc<float>((size_t)3 * cs_ * cs_);
-  g_pooled = dalloc<float>((size_t)3 * cs_ * cs_);
-  pooled_masked = dalloc<float>((size_t)3 * cs_ * cs_);
+  if (cfg.n_clip < 1 || cfg.n_clip > 4) throw EngineError(-53, "n_clip must be 1, 2, 3 or 4");
+  sets.clear();
+  for (int i = 0; i < cfg.n_clip; ++i) {
+    const int res = i == 0 ? cfg.cut_size : cfg.clip[i].image_res;
+    int s = 0;
+    while (s < n_sets() && sets[s].cs != res) ++s;
+    if (s == n_sets()) {
+      if (res < 4 || res % 4) throw EngineError(-6, "perceptor " + std::to_string(i) + ": image_res must be a multiple of 4");
+      sets.emplace_back();
+      sets.back().cs = res;
+    }
+    set_of[i] = s;
+  }
   aspect = (cfg.cut_aspect > 0.f && cfg.cut_aspect != 1.f) ? (double)cfg.cut_aspect : 1.0;
   if (aspect > 8.0 || aspect < 0.125) throw EngineError(-66, "cut_aspect (canvas width / height) must be within [1/8, 8]");
-  source_size(cs_, aspect, src_h, src_w);
-  if (aspect != 1.0 && cfg.cut_src_h > 0 && cfg.cut_src_w > 0) {  // the caller's (double-precision) truncation wins
-    if (std::abs(cfg.cut_src_h - src_h) > 1 || std::abs(cfg.cut_src_w - src_w) > 1)
-      throw EngineError(-66, "cut_src_h / cut_src_w do not match cut_aspect");
-    src_h = cfg.cut_src_h;
-    src_w = cfg.cut_src_w;
+  size_t fx_n = 0;
+  for (int s = 0; s < n_sets(); ++s) {
+    CutSet& K = sets[s];
+    const int cs_ = K.cs;
+    K.pooled = dalloc<float>((size_t)3 * cs_ * cs_);
+    K.g_pooled = dalloc<float>((size_t)3 * cs_ * cs_);
+    source_size(cs_, aspect, K.src_h, K.src_w);
+    if (s == 0 && aspect != 1.0 && cfg.cut_src_h > 0 && cfg.cut_src_w > 0) {  // the caller's (double-precision) truncation wins
+      if (std::abs(cfg.cut_src_h - K.src_h) > 1 || std::abs(cfg.cut_src_w - K.src_w) > 1)
+        throw EngineError(-66, "cut_src_h / cut_src_w do not match cut_aspect");
+      K.src_h = cfg.cut_src_h;
+      K.src_w = cfg.cut_src_w;
+    }
+    if (aspect != 1.0) {
+      K.cut_src = dalloc<float>((size_t)3 * K.src_h * K.src_w);
+      K.g_cut_src = dalloc<float>((size_t)3 * K.src_h * K.src_w);
+    } else {
+      K.cut_src = K.pooled;
+      K.g_cut_src = K.g_pooled;
+    }
+    fx_n = std::max(fx_n, (size_t)3 * std::max(K.src_h * K.src_w, cs_ * cs_));
+    K.pool_argmax = dalloc<int>((size_t)3 * cs_ * cs_);
+    K.batch = dalloc<float>((size_t)n_local * 3 * cs_ * cs_);
+    K.g_batch = dalloc<float>((size_t)n_local * 3 * cs_ * cs_);
+    K.n_parts = cutout_num_blocks(n_local, cs_);
+    K.part_min = dalloc<float>(K.n_parts);
+    K.part_max = dalloc<float>(K.n_parts);
+    K.part_imin = dalloc<int>(K.n_parts);
+    K.part_imax = dalloc<int>(K.n_parts);
+    K.range = dalloc<float>(4);
+    K.irange = dalloc<int>(4);
+    K.sums = dalloc<float>(4);
+    K.minv_dev = dalloc<float>((size_t)n_local * 12);  // 9 homography + 3 ColorJitter floats per cutout, one H2D copy
+    K.facs_dev = dalloc<float>(n_local);
+    for (int i = 0; i < RING; ++i) {
+      PXR_CUDA(cudaMallocHost((void**)&K.minv_host[i], sizeof(float) * n_local * 12));
+      PXR_CUDA(cudaMallocHost((void**)&K.facs_host[i], sizeof(float) * n_local));
+      PXR_CUDA(cudaEventCreateWithFlags(&K.ring_ev[i], cudaEventDisableTiming));
+    }
+    CutoutArgs& ca = K.cut_args;
+    memset(&ca, 0, sizeof ca);
+    ca.pooled = K.cut_src;
+    ca.src_h = K.src_h;
+    ca.src_w = K.src_w;
+    ca.minv = K.minv_dev;
+    ca.cs = cs_;
+    ca.n_local = n_local;
+    ca.first_global = first_global;
+    ca.cutn_zoom = (int)(0.6 * cfg.cutn);  // pixray.py:407
+    ca.seed = cfg.seed;
+    ca.noise_fac = cfg.noise_fac;
+    ca.rng_stream = cut_rng_stream(s);
+    K.aux_A = dalloc<float>(((size_t)n_local * cs_ + 2) * cs_);
+    K.aux_halo = dalloc<float>((size_t)12 * cs_);
+    K.aux_xbuf = dalloc<float>((size_t)12 * cs_ * cfg.world);
+    K.aux_best = dalloc<int>((size_t)n_local * cs_ * cs_);
   }
-  if (aspect != 1.0) {
-    cut_src = dalloc<float>((size_t)3 * src_h * src_w);
-    g_cut_src = dalloc<float>((size_t)3 * src_h * src_w);
-  } else {
-    cut_src = pooled;
-    g_cut_src = g_pooled;
-  }
-  grad_fx = dalloc<long long>((size_t)3 * std::max(src_h * src_w, cs_ * cs_));  // zeroed; each use clears it again
-  pool_argmax = dalloc<int>((size_t)3 * cs_ * cs_);
-  batch = dalloc<float>((size_t)n_local * 3 * cs_ * cs_);
-  g_batch = dalloc<float>((size_t)n_local * 3 * cs_ * cs_);
-  n_parts = cutout_num_blocks(n_local, cs_);
-  part_min = dalloc<float>(n_parts);
-  part_max = dalloc<float>(n_parts);
-  part_imin = dalloc<int>(n_parts);
-  part_imax = dalloc<int>(n_parts);
-  range = dalloc<float>(4);
-  irange = dalloc<int>(4);
-  sums = dalloc<float>(4);
+  pooled_masked = dalloc<float>((size_t)3 * cfg.cut_size * cfg.cut_size);
+  grad_fx = dalloc<long long>(fx_n);  // zeroed; each use clears it again
   sums_fx = dalloc<long long>(2);  // zero-initialised; every pass leaves it zeroed again
   fx_poison = dalloc<unsigned int>(2);
   xbuf = dalloc<float>(4);
-  minv_dev = dalloc<float>((size_t)n_local * 12);  // 9 homography + 3 ColorJitter floats per cutout, one H2D copy
-  facs_dev = dalloc<float>(n_local);
-  for (int i = 0; i < RING; ++i) {
-    PXR_CUDA(cudaMallocHost((void**)&minv_host[i], sizeof(float) * n_local * 12));
-    PXR_CUDA(cudaMallocHost((void**)&facs_host[i], sizeof(float) * n_local));
-    PXR_CUDA(cudaEventCreateWithFlags(&ring_ev[i], cudaEventDisableTiming));
-  }
-  memset(&cut_args, 0, sizeof cut_args);
-  cut_args.pooled = cut_src;
-  cut_args.src_h = src_h;
-  cut_args.src_w = src_w;
-  cut_args.minv = minv_dev;
-  cut_args.cs = cs_;
-  cut_args.n_local = n_local;
-  cut_args.first_global = first_global;
-  cut_args.cutn_zoom = (int)(0.6 * cfg.cutn);  // pixray.py:407
-  cut_args.seed = cfg.seed;
-  cut_args.noise_fac = cfg.noise_fac;
 }
 
 // Host side of MakeCutouts: invert the cached "dst <- src" transforms (pixray.py:498) to the sampling maps the
 // kernel uses (kornia warp_perspective inverts the normalised homography; with align_corners=True the
 // normalisations cancel and src_pix = M^-1 dst_pix), stage them through pinned memory.
-void Engine::prepare_cut_params(const pxr_cut_params* p, int iter) {
+void Engine::prepare_cut_params(int s, const pxr_cut_params* p, int iter) {
+  CutSet& K = sets[s];
+  CutoutArgs& cut_args = K.cut_args;
   // engine-drawn parameters are keyed by (seed, rng_iter): pass b > 0 of an iteration (batches > 1) draws a fresh set,
   // like a second ascend_txt call does, while the padding mode still follows the iteration's parity (pixray.py:1250)
   const int key = rng_iter ? rng_iter : iter;
-  const int slot = ring_pos;
-  ring_pos = (ring_pos + 1) % RING;
-  PXR_CUDA(cudaEventSynchronize(ring_ev[slot]));
+  const int slot = K.ring_pos;
+  K.ring_pos = (K.ring_pos + 1) % RING;
+  PXR_CUDA(cudaEventSynchronize(K.ring_ev[slot]));
   std::vector<float> gen;
   const float* T = p ? p->transforms : nullptr;
   int zoom_padding = p ? p->zoom_padding : ((iter % 2 == 0) ? PXR_PAD_REFLECTION : PXR_PAD_BORDER);  // pixray.py:1250
   float fill = p ? p->fill : 0.f;
-  if (!T) {  // engine RNG (SURVEY.md Appendix A), keyed by (seed, iter, global cutout index)
+  if (!T) {  // engine RNG (SURVEY.md Appendix A), keyed by (seed, iter, global cutout index) and the set's streams
     gen.resize((size_t)cfg.cutn * 9);
-    sample_cutout_transforms(cfg.seed, key, cfg.cutn, cfg.cut_size, gen.data(), aspect, src_h, src_w);
+    sample_cutout_transforms(cfg.seed, key, cfg.cutn, K.cs, gen.data(), aspect, K.src_h, K.src_w, cut_args.rng_stream);
     T = gen.data();
-    if (!p) fill = sample_fill(cfg.seed, key);
+    if (!p) fill = sample_fill(cfg.seed, key);  // shared by every set (pixray.py:1255-1258)
   }
   for (int n = 0; n < n_local; ++n) {
     double m[9], inv[9];
     for (int i = 0; i < 9; ++i) m[i] = T[(size_t)(first_global + n) * 9 + i];
     if (!invert3x3(m, inv)) throw EngineError(-60, "singular cutout transform");
-    for (int i = 0; i < 9; ++i) minv_host[slot][n * 9 + i] = (float)inv[i];
+    for (int i = 0; i < 9; ++i) K.minv_host[slot][n * 9 + i] = (float)inv[i];
   }
   // ColorJitter rows: explicit, or drawn like the transforms when those are the engine's own
   const float* J = p ? p->color_jitter : nullptr;
   std::vector<float> genj;
   if (!J && !(p && p->transforms) && cj_p > 0.f) {
     genj.resize((size_t)cfg.cutn * 3);
-    sample_color_jitter(cfg.seed, key, cfg.cutn, cj_p, cj_sat, cj_hue, genj.data());
+    sample_color_jitter(cfg.seed, key, cfg.cutn, cj_p, cj_sat, cj_hue, genj.data(), cut_args.rng_stream);
     J = genj.data();
   }
-  float* jh = minv_host[slot] + (size_t)n_local * 9;
+  float* jh = K.minv_host[slot] + (size_t)n_local * 9;
   if (J)
     for (int i = 0; i < n_local * 3; ++i) jh[i] = J[(size_t)first_global * 3 + i];
-  cut_args.jitter = J ? minv_dev + (size_t)n_local * 9 : nullptr;
-  PXR_CUDA(cudaMemcpyAsync(minv_dev, minv_host[slot], sizeof(float) * n_local * (J ? 12 : 9), cudaMemcpyHostToDevice, st));
+  cut_args.jitter = J ? K.minv_dev + (size_t)n_local * 9 : nullptr;
+  PXR_CUDA(cudaMemcpyAsync(K.minv_dev, K.minv_host[slot], sizeof(float) * n_local * (J ? 12 : 9), cudaMemcpyHostToDevice, st));
   cut_args.zoom_padding = zoom_padding;
   cut_args.fill = fill;
   cut_args.iter = key;
@@ -1704,11 +1770,11 @@ void Engine::prepare_cut_params(const pxr_cut_params* p, int iter) {
   if (cfg.noise_fac <= 0.f) {
     cut_args.noise_mode = 0;
   } else if (p && p->noise && p->noise_facs) {
-    for (int n = 0; n < n_local; ++n) facs_host[slot][n] = p->noise_facs[first_global + n];
-    PXR_CUDA(cudaMemcpyAsync(facs_dev, facs_host[slot], sizeof(float) * n_local, cudaMemcpyHostToDevice, st));
+    for (int n = 0; n < n_local; ++n) K.facs_host[slot][n] = p->noise_facs[first_global + n];
+    PXR_CUDA(cudaMemcpyAsync(K.facs_dev, K.facs_host[slot], sizeof(float) * n_local, cudaMemcpyHostToDevice, st));
     cut_args.noise_mode = 1;
-    cut_args.noise = p->noise + (size_t)first_global * 3 * cfg.cut_size * cfg.cut_size;
-    cut_args.noise_facs = facs_dev;
+    cut_args.noise = p->noise + (size_t)first_global * 3 * K.cs * K.cs;
+    cut_args.noise_facs = K.facs_dev;
   } else if (p && (p->noise || p->noise_facs)) {
     throw EngineError(-61, "pxr_cut_params: noise and noise_facs must be given together");
   } else if (p && p->transforms) {
@@ -1716,26 +1782,37 @@ void Engine::prepare_cut_params(const pxr_cut_params* p, int iter) {
   } else {
     cut_args.noise_mode = 2;
   }
-  PXR_CUDA(cudaEventRecord(ring_ev[slot], st));
+  PXR_CUDA(cudaEventRecord(K.ring_ev[slot], st));
 }
 
-void Engine::forward_cutouts() {
-  if (!aux.empty())  // the cutout / embedding losses accumulate per-rank partial sums into their slots
-    PXR_CUDA(cudaMemsetAsync(losses_dev + aux_base(), 0, sizeof(float) * aux.size(), st));
-  pool_forward(cur_cut_img(), cur_cut_h(), cur_cut_w(), cfg.cut_size, pooled, pool_argmax, st);
+void Engine::forward_cutouts(int s) {
+  CutSet& K = sets[s];
+  ProfRec prof_rec;
+  if (profiling) prof_begin_stage(prof_rec, "cutouts_fwd set " + std::to_string(s));
+  // the cutout / embedding losses accumulate per-rank partial sums into their slots: set 0 clears every auxiliary slot
+  // (one set: the launch as before), another set its own cutout-space entries
+  if (s == 0 && !aux.empty()) {
+    PXR_CUDA(cudaMemsetAsync(losses_dev + aux_base(), 0, sizeof(float) * (num_losses() - aux_base()), st));
+  } else if (s > 0) {
+    for (size_t k = 0; k < aux.size(); ++k)
+      if (aux_per_set(aux[k].kind)) PXR_CUDA(cudaMemsetAsync(losses_dev + aux_slot(k, s), 0, sizeof(float), st));
+  }
+  pool_forward(cur_cut_img(), cur_cut_h(), cur_cut_w(), K.cs, K.pooled, K.pool_argmax, st);
   if (aspect != 1.0) {
-    rescale_bilinear(pooled, cfg.cut_size, cfg.cut_size, src_h, src_w, cut_src, st);
+    rescale_bilinear(K.pooled, K.cs, K.cs, K.src_h, K.src_w, K.cut_src, st);
     launches += 1;
   }
-  cutout_forward(cut_args, batch, part_min, part_max, part_imin, part_imax, st);
-  minmax_reduce(nullptr, part_min, part_max, part_imin, part_imax, n_parts, range, irange, st);
+  cutout_forward(K.cut_args, K.batch, K.part_min, K.part_max, K.part_imin, K.part_imax, st);
+  minmax_reduce(nullptr, K.part_min, K.part_max, K.part_imin, K.part_imax, K.n_parts, K.range, K.irange, st);
   launches += 3;
-  if (comm) {  // global min / max over all ranks' cutouts (slip.py:21-36 reduces over the whole batch)
-    range_pack(range, xbuf, st);
+  if (comm) {  // global min / max over all ranks' cutouts of the set (slip.py:21-36 reduces over the whole batch)
+    range_pack(K.range, xbuf, st);
     nccl_check(Comm::api().all_reduce(xbuf, xbuf, 2, Comm::kFloat32, Comm::kMin, comm, st), "allreduce(min,max)");
-    range_unpack(xbuf, range, irange, st);
+    range_unpack(xbuf, K.range, K.irange, st);
     launches += 3;
   }
+  K.cut = true;
+  if (profiling) prof_end_stage(prof_rec);
   check_launch("cutouts forward");
 }
 
@@ -1746,14 +1823,15 @@ void Engine::build_clip(int i) {
   C.c = cfg.clip[i];
   const int mod = PXR_MOD_CLIP0 + i;
   const int Wd = C.c.width, L = C.c.layers, Hh = C.c.heads, P = C.c.patch, D = C.c.out_dim;
-  if (C.c.image_res != cfg.cut_size) throw EngineError(-50, "clip image_res must equal cut_size");
+  if (i == 0 && C.c.image_res != cfg.cut_size) throw EngineError(-50, "clip image_res must equal cut_size");
+  const int res = sets[set_of[i]].cs;
   // a LayerNorm warp gives each lane whole 4-element vectors of every 128-column slice of the row
   if (Wd % 128 || Wd > 1024 || Wd != 64 * Hh)
     throw EngineError(-51, "ViT width " + std::to_string(Wd) + " with " + std::to_string(Hh) +
                                " heads: the width must be a multiple of 128 (the LayerNorm granularity), <= 1024, "
                                "with 64-wide heads");
-  if (P < 2 || cfg.cut_size % P) throw EngineError(-52, "patch size must divide cut_size");
-  const int gp = cfg.cut_size / P, np = gp * gp, T = np + 1, B = n_local, M = B * T, d = 64;
+  if (P < 2 || res % P) throw EngineError(-52, "patch size must divide the perceptor's input resolution");
+  const int gp = res / P, np = gp * gp, T = np + 1, B = n_local, M = B * T, d = 64;
   const int Kp = round_up(3 * P * P, 64), ldT = round_up(T, 8);
   C.T = T;
   C.np = np;
@@ -2016,17 +2094,19 @@ void Engine::build_clip(int i) {
 
 void Engine::clip_input(int i) {
   Clip& C = clip[i];
-  if (C.tower == PXR_TOWER_CLIP_RESNET) rn_stem_forward(batch, range, n_local, cfg.cut_size, rn[i]->cols, C.norm, st);
-  else patchify_forward(batch, range, n_local, cfg.cut_size, C.c.patch, C.Kp, C.patches, C.norm, st);
+  const CutSet& K = sets[set_of[i]];
+  if (C.tower == PXR_TOWER_CLIP_RESNET) rn_stem_forward(K.batch, K.range, n_local, K.cs, rn[i]->cols, C.norm, st);
+  else patchify_forward(K.batch, K.range, n_local, K.cs, C.c.patch, C.Kp, C.patches, C.norm, st);
   launches += 1;
 }
 
 void Engine::clip_input_backward(int i, bool accumulate, FxPass fx) {
   Clip& C = clip[i];
+  const CutSet& K = sets[set_of[i]];
   if (C.tower == PXR_TOWER_CLIP_RESNET)
-    rn_stem_backward(rn[i]->g_cols, batch, range, n_local, cfg.cut_size, accumulate, g_batch, sums_fx, fx, C.norm, st);
+    rn_stem_backward(rn[i]->g_cols, K.batch, K.range, n_local, K.cs, accumulate, K.g_batch, sums_fx, fx, C.norm, st);
   else
-    patchify_backward(C.g_patches, batch, range, n_local, cfg.cut_size, C.c.patch, C.Kp, accumulate, g_batch, sums_fx, fx,
+    patchify_backward(C.g_patches, K.batch, K.range, n_local, K.cs, C.c.patch, C.Kp, accumulate, K.g_batch, sums_fx, fx,
                       C.norm, st);
   launches += 1;
 }
@@ -2104,7 +2184,7 @@ void Engine::rebuild_prompt_rows() {
     C.loss_offset = off;
     off += C.n_prompts;
   }
-  if (off + (int)anchors.size() + (int)aux.size() > 64) throw EngineError(-16, "at most 64 losses (prompts + anchors + auxiliary) in total");
+  if (off + (int)anchors.size() + (num_losses() - aux_base()) > 64) throw EngineError(-16, "at most 64 losses (prompts + anchors + auxiliary) in total");
   total_prompts = off;
 }
 
@@ -2112,24 +2192,26 @@ void Engine::rebuild_prompt_rows() {
 // transforms (no ColorJitter on that path, pixray.py:480-486; fresh noise), perceptor.encode_image, and the [cutn, D]
 // unit embeddings become the rows of Prompt(embed, weight).  Forward only: the targets are constants.  Runs before
 // the main pass, which then overwrites every buffer used here.
-void Engine::encode_image_prompts() {
+void Engine::encode_image_prompts(int s) {
   if (n_img == 0) return;
-  const size_t ncs = (size_t)3 * src_h * src_w;
+  CutSet& K = sets[s];
+  const size_t ncs = (size_t)3 * K.src_h * K.src_w;
   for (int k = 0; k < n_img; ++k) {
-    CutoutArgs a = cut_args;
+    CutoutArgs a = K.cut_args;
     a.jitter = nullptr;
-    a.iter = cut_args.iter + (k + 1) * (1 << 24);  // engine-drawn noise: an independent Philox stream per call
-    a.pooled = img_prompts + k * ncs;
-    cutout_forward(a, batch, part_min, part_max, part_imin, part_imax, st);
-    minmax_reduce(nullptr, part_min, part_max, part_imin, part_imax, n_parts, range, irange, st);
+    a.iter = K.cut_args.iter + (k + 1) * (1 << 24);  // engine-drawn noise: an independent Philox stream per call
+    a.pooled = K.img_prompts + k * ncs;
+    cutout_forward(a, K.batch, K.part_min, K.part_max, K.part_imin, K.part_imax, st);
+    minmax_reduce(nullptr, K.part_min, K.part_max, K.part_imin, K.part_imax, K.n_parts, K.range, K.irange, st);
     launches += 2;
     if (comm) {
-      range_pack(range, xbuf, st);
+      range_pack(K.range, xbuf, st);
       nccl_check(Comm::api().all_reduce(xbuf, xbuf, 2, Comm::kFloat32, Comm::kMin, comm, st), "allreduce(min,max)");
-      range_unpack(xbuf, range, irange, st);
+      range_unpack(xbuf, K.range, K.irange, st);
       launches += 3;
     }
-    for (int i = 0; i < cfg.n_clip; ++i) {
+    for (int i = 0; i < cfg.n_clip; ++i) {  // each target is cut with its perceptor's own set (pixray.py:1308-1336)
+      if (set_of[i] != s) continue;
       Clip& C = clip[i];
       const int D = C.c.out_dim;
       clip_input(i);
@@ -2166,16 +2248,20 @@ void Engine::aux_after_embed() {
     Clip& C = clip[cfg.n_clip - 1];
     if (a.n_dev != C.c.out_dim) throw EngineError(-81, "aesthetic head width does not match the last perceptor's embedding");
     aux_aesthetic(C.e, C.B, C.c.out_dim, cfg.cutn, a.dev, a.prm[1], a.prm[0], a.weight, S, C.de, C.de16, aux_part,
-                  losses_dev + aux_base() + k, st);
+                  losses_dev + aux_slot(k), st);
     launches += 2;
   }
 }
 
-void Engine::aux_on_cutouts() {
-  const int cs_ = cfg.cut_size;
+void Engine::aux_on_cutouts(int s) {
+  CutSet& K = sets[s];
+  const int cs_ = K.cs;
+  float* const batch = K.batch;
+  float* const g_batch = K.g_batch;
   for (size_t k = 0; k < aux.size(); ++k) {
     AuxLoss& a = aux[k];
-    float* slot = losses_dev + aux_base() + k;
+    if (!aux_per_set(a.kind)) continue;
+    float* slot = losses_dev + aux_slot(k, s);
     if (a.kind == PXR_LOSS_SATURATION) {
       aux_saturation_moments(batch, n_local, cs_, aux_part, aux_sums, st);
       if (comm) nccl_check(Comm::api().all_reduce(aux_sums, aux_sums, 4, Comm::kFloat64, Comm::kSum, comm, st), "allreduce(saturation moments)");
@@ -2183,7 +2269,7 @@ void Engine::aux_on_cutouts() {
       aux_saturation_grad(batch, n_local, cs_, cfg.cutn, aux_sums, a.weight * a.prm[0], S, cfg.rank == 0, g_batch, slot, st);
       launches += 3;
     } else if (a.kind == PXR_LOSS_PALETTE) {
-      aux_palette(batch, n_local, cs_, cfg.cutn, a.dev, a.n_dev / 3, a.weight * a.prm[0], S, g_batch, aux_best, aux_part, slot, st);
+      aux_palette(batch, n_local, cs_, cfg.cutn, a.dev, a.n_dev / 3, a.weight * a.prm[0], S, g_batch, K.aux_best, aux_part, slot, st);
       launches += 2;
     } else if (a.kind == PXR_LOSS_SMOOTHNESS) {
       // {w, type, spacing[, edge_order[, n, taps]]}: a.dev holds the n 1-D taps of the blur when n > 0
@@ -2192,22 +2278,22 @@ void Engine::aux_on_cutouts() {
       int cs2 = cs_;
       if (nt) {  // the gradient runs on the blurred cutouts (SmoothnessLoss.py:92-94)
         cs2 = cs_ - nt + 1;
-        aux_smooth_blur(batch, n_local, cs_, a.dev, nt, aux_blur_tmp, aux_blur, st);
-        src = aux_blur;
+        aux_smooth_blur(batch, n_local, cs_, a.dev, nt, K.aux_blur_tmp, K.aux_blur, st);
+        src = K.aux_blur;
         launches += 2;
       }
       if (comm) {  // torch.gradient runs over the stacked rows of ALL cutouts: two halo rows from each neighbour
-        PXR_CUDA(cudaMemsetAsync(aux_xbuf, 0, sizeof(float) * 12 * cs2 * cfg.world, st));
-        aux_smooth_pack_halo(src, n_local, cs2, cfg.rank, aux_xbuf, st);
-        nccl_check(Comm::api().all_reduce(aux_xbuf, aux_xbuf, (size_t)12 * cs2 * cfg.world, Comm::kFloat32, Comm::kSum, comm, st), "allreduce(smoothness halo)");
-        aux_smooth_unpack_halo(aux_xbuf, cs2, cfg.rank, cfg.world, aux_halo, st);
+        PXR_CUDA(cudaMemsetAsync(K.aux_xbuf, 0, sizeof(float) * 12 * cs2 * cfg.world, st));
+        aux_smooth_pack_halo(src, n_local, cs2, cfg.rank, K.aux_xbuf, st);
+        nccl_check(Comm::api().all_reduce(K.aux_xbuf, K.aux_xbuf, (size_t)12 * cs2 * cfg.world, Comm::kFloat32, Comm::kSum, comm, st), "allreduce(smoothness halo)");
+        aux_smooth_unpack_halo(K.aux_xbuf, cs2, cfg.rank, cfg.world, K.aux_halo, st);
         launches += 3;
       }
-      aux_smoothness(src, n_local, cs2, first_global, cfg.cutn, aux_halo, a.prm[2], (int)a.prm[1], order,
-                     a.weight * a.prm[0], S, aux_A, nt ? aux_g_blur : g_batch, nt ? 0 : 1, aux_part, slot, st);
+      aux_smoothness(src, n_local, cs2, first_global, cfg.cutn, K.aux_halo, a.prm[2], (int)a.prm[1], order,
+                     a.weight * a.prm[0], S, K.aux_A, nt ? K.aux_g_blur : g_batch, nt ? 0 : 1, aux_part, slot, st);
       launches += 3;
       if (nt) {
-        aux_smooth_blur_adjoint(aux_g_blur, n_local, cs_, a.dev, nt, aux_blur_tmp, g_batch, st);
+        aux_smooth_blur_adjoint(K.aux_g_blur, n_local, cs_, a.dev, nt, K.aux_blur_tmp, g_batch, st);
         launches += 2;
       }
     }
@@ -2220,7 +2306,7 @@ void Engine::aux_on_image() {
   float* g_img = cur_g_cut_img();
   for (size_t k = 0; k < aux.size(); ++k) {
     AuxLoss& a = aux[k];
-    float* slot = losses_dev + aux_base() + k;
+    float* slot = losses_dev + aux_slot(k);
     if (a.kind == PXR_LOSS_SYMMETRY) {
       aux_symmetry(img, H, Wd, a.weight * a.prm[0], S, g_img, aux_part, slot, st);
       launches += 2;
@@ -2243,33 +2329,39 @@ void Engine::aux_on_image() {
 // CLIP backward of every participating perceptor -> d loss / d cutouts -> (range terms, ColorJitter, warp adjoint) ->
 // d loss / d pooled [-> un-stretch] [-> spot mask] -> d loss / d image (= or +=).  `a` = the cutout parameters of the pass
 // whose activations are live; mask_which >= 0: a spot pass (only the perceptors with spot prompts of that kind ran).
-void Engine::backward_to_image(const CutoutArgs& a, int mask_which, bool accumulate_img, bool main_pass) {
+void Engine::backward_to_image(int s, const CutoutArgs& a, int mask_which, bool accumulate_img, bool main_pass) {
+  CutSet& K = sets[s];
   bool first = true;
   const FxPass fx_sums = next_fx(1);
   for (int i = 0; i < cfg.n_clip; ++i) {
     Clip& C = clip[i];
-    if (mask_which >= 0 && C.spot[mask_which].n == 0) continue;
+    if (set_of[i] != s || (mask_which >= 0 && C.spot[mask_which].n == 0)) continue;
     run(C.bwd);
     clip_input_backward(i, !first, fx_sums);
     first = false;
   }
-  if (main_pass && !aux.empty()) aux_on_cutouts();
-  range_sums_finish(sums_fx, fx_sums, sums, st);  // fixed point -> fp32 (and the accumulator is clean for the next pass)
+  if (main_pass && !aux.empty()) aux_on_cutouts(s);
+  ProfRec prof_rec;
+  if (profiling) prof_begin_stage(prof_rec, "cutouts_bwd set " + std::to_string(s));
+  range_sums_finish(sums_fx, fx_sums, K.sums, st);  // fixed point -> fp32 (and the accumulator is clean for the next pass)
   if (comm)  // d/dmin, d/dmax terms need the sums over ALL cutouts
-    nccl_check(Comm::api().all_reduce(sums, sums, 2, Comm::kFloat32, Comm::kSum, comm, st), "allreduce(sums)");
-  cutout_backward(a, g_batch, range, irange, sums, grad_fx, next_fx(0), g_cut_src, st);
+    nccl_check(Comm::api().all_reduce(K.sums, K.sums, 2, Comm::kFloat32, Comm::kSum, comm, st), "allreduce(sums)");
+  cutout_backward(a, K.g_batch, K.range, K.irange, K.sums, grad_fx, next_fx(0), K.g_cut_src, st);
   launches += 2;
-  const int ncs = 3 * cfg.cut_size * cfg.cut_size;
+  const int ncs = 3 * K.cs * K.cs;
   if (aspect != 1.0) {
-    rescale_bilinear_backward(g_cut_src, cfg.cut_size, cfg.cut_size, src_h, src_w, grad_fx, next_fx(0), g_pooled, st);
+    rescale_bilinear_backward(K.g_cut_src, K.cs, K.cs, K.src_h, K.src_w, grad_fx, next_fx(0), K.g_pooled, st);
     launches += 2;
   }
   if (mask_which >= 0) {  // cutout[0][mask_indexes] = 0 (pixray.py:466): no gradient through the zeroed pixels
-    spot_mask_apply(g_pooled, spot_mask, mask_which == 1, ncs, g_pooled, st);
+    spot_mask_apply(K.g_pooled, spot_mask, mask_which == 1, ncs, K.g_pooled, st);
     launches += 1;
   }
-  pool_backward(g_pooled, pool_argmax, cur_cut_h(), cur_cut_w(), cfg.cut_size, cur_g_cut_img(), st, accumulate_img ? 1 : 0);
+  // the sets meet here: the first writes d loss / d image, every later one adds to it
+  pool_backward(K.g_pooled, K.pool_argmax, cur_cut_h(), cur_cut_w(), K.cs, cur_g_cut_img(), st, accumulate_img ? 1 : 0);
   launches += 2;
+  K.cut = false;
+  if (profiling) prof_end_stage(prof_rec);
 }
 
 void Engine::backward_drawer() {
@@ -2319,8 +2411,16 @@ void Engine::anchors_on_z() {
   }
 }
 
+// Every set cut since the last backward, in set order (set 0 alone when none was: a batch handed to pxr_encode_image)
 void Engine::backward_all() {
-  backward_to_image(cut_args, -1, spot_accumulated, true);
+  bool any = false;
+  for (const CutSet& K : sets) any |= K.cut;
+  bool acc = spot_accumulated;
+  for (int s = 0; s < n_sets(); ++s) {
+    if (!(sets[s].cut || (s == 0 && !any))) continue;
+    backward_to_image(s, sets[s].cut_args, -1, acc, true);
+    acc = true;
+  }
   spot_accumulated = false;
   backward_drawer();
 }
@@ -2333,25 +2433,26 @@ void Engine::backward_all() {
 bool Engine::spot_pass(int which, bool accumulate_img) {
   if (!any_spot(which)) return false;
   if (!spot_mask) throw EngineError(-71, "spot prompts need a spot mask (pxr_set_spot_mask)");
-  const int ncs = 3 * cfg.cut_size * cfg.cut_size;
-  spot_mask_apply(pooled, spot_mask, which == 1, ncs, pooled_masked, st);
-  CutoutArgs a = cut_args;
+  CutSet& K = sets[0];  // spot prompts run in single-set sessions only (pxr_set_spot_prompts)
+  const int ncs = 3 * K.cs * K.cs;
+  spot_mask_apply(K.pooled, spot_mask, which == 1, ncs, pooled_masked, st);
+  CutoutArgs a = K.cut_args;
   a.jitter = nullptr;
-  a.iter = cut_args.iter + (9 + which) * (1 << 24);  // engine-drawn noise: its own Philox stream
+  a.iter = K.cut_args.iter + (9 + which) * (1 << 24);  // engine-drawn noise: its own Philox stream
   if (aspect != 1.0) {
-    rescale_bilinear(pooled_masked, cfg.cut_size, cfg.cut_size, src_h, src_w, cut_src, st);
-    a.pooled = cut_src;
+    rescale_bilinear(pooled_masked, K.cs, K.cs, K.src_h, K.src_w, K.cut_src, st);
+    a.pooled = K.cut_src;
     launches += 1;
   } else {
     a.pooled = pooled_masked;
   }
-  cutout_forward(a, batch, part_min, part_max, part_imin, part_imax, st);
-  minmax_reduce(nullptr, part_min, part_max, part_imin, part_imax, n_parts, range, irange, st);
+  cutout_forward(a, K.batch, K.part_min, K.part_max, K.part_imin, K.part_imax, st);
+  minmax_reduce(nullptr, K.part_min, K.part_max, K.part_imin, K.part_imax, K.n_parts, K.range, K.irange, st);
   launches += 3;
   if (comm) {
-    range_pack(range, xbuf, st);
+    range_pack(K.range, xbuf, st);
     nccl_check(Comm::api().all_reduce(xbuf, xbuf, 2, Comm::kFloat32, Comm::kMin, comm, st), "allreduce(min,max)");
-    range_unpack(xbuf, range, irange, st);
+    range_unpack(xbuf, K.range, K.irange, st);
     launches += 3;
   }
   for (int i = 0; i < cfg.n_clip; ++i) {
@@ -2363,7 +2464,7 @@ bool Engine::spot_pass(int which, bool accumulate_img) {
                 losses_dev + sp.loss_offset, C.de, C.de16, C.ploss_part, C.ploss_count, st);
     launches += 1;
   }
-  backward_to_image(a, which, accumulate_img, false);
+  backward_to_image(0, a, which, accumulate_img, false);
   return true;
 }
 
@@ -2585,35 +2686,39 @@ void Engine::finalize() {
     drop_status_dev = static_cast<DropStatus*>(dp);
   }
   build_cutouts();
-  if (cfg.n_clip < 1 || cfg.n_clip > 3) throw EngineError(-53, "n_clip must be 1, 2 or 3");
   for (int i = 0; i < cfg.n_clip; ++i) build_clip(i);
   for (int i = 0; i < cfg.n_clip; ++i) build_text(i);
   losses_dev = dalloc<float>(64);
   losses_scratch = dalloc<float>(64);
   aux_part = dalloc<double>(std::max(4 * AUX_MAX_BLOCKS, n_local) + 8);
   aux_sums = dalloc<double>(4);
-  aux_A = dalloc<float>(((size_t)n_local * cfg.cut_size + 2) * cfg.cut_size);
-  aux_halo = dalloc<float>((size_t)12 * cfg.cut_size);
-  aux_xbuf = dalloc<float>((size_t)12 * cfg.cut_size * cfg.world);
-  aux_best = dalloc<int>((size_t)n_local * cfg.cut_size * cfg.cut_size);
   PXR_CUDA(cudaMallocHost((void**)&losses_host, 64 * sizeof(float)));
   PXR_CUDA(cudaStreamSynchronize(st));
   {
-    const size_t npx = (size_t)3 * cfg.image_h * cfg.image_w, ncs = (size_t)3 * cfg.cut_size * cfg.cut_size;
+    const size_t npx = (size_t)3 * cfg.image_h * cfg.image_w;
     reg("img", img, npx * 4);
     reg("img_pre", img_pre, npx * 4);
     reg("g_img", g_img, npx * 4);
     reg("filtered", img, npx * 4);  // the filter chain's output and its gradient; rebuild_filters moves them
     reg("g_filtered", g_img, npx * 4);
-    reg("pooled", pooled, ncs * 4);
-    reg("cut_src", cut_src, (size_t)3 * src_h * src_w * 4);
-    reg("pool_argmax", pool_argmax, ncs * 4);
-    reg("g_pooled", g_pooled, ncs * 4);
-    reg("batch", batch, ncs * n_local * 4);
-    reg("g_batch", g_batch, ncs * n_local * 4);
-    reg("range", range, 16);
-    reg("irange", irange, 16);
-    reg("sums", sums, 16);
+    // set 0's buffers under their plain names, every set's as setN.<name>
+    for (int s = 0; s < n_sets(); ++s) {
+      const CutSet& K = sets[s];
+      const size_t kcs = (size_t)3 * K.cs * K.cs;
+      for (const std::string& p : s == 0 ? std::vector<std::string>{"", "set0."} : std::vector<std::string>{"set" + std::to_string(s) + "."}) {
+        reg(p + "pooled", K.pooled, kcs * 4);
+        reg(p + "cut_src", K.cut_src, (size_t)3 * K.src_h * K.src_w * 4);
+        reg(p + "pool_argmax", K.pool_argmax, kcs * 4);
+        reg(p + "g_pooled", K.g_pooled, kcs * 4);
+        reg(p + "batch", K.batch, kcs * n_local * 4);
+        reg(p + "g_batch", K.g_batch, kcs * n_local * 4);
+        reg(p + "range", K.range, 16);
+        reg(p + "irange", K.irange, 16);
+        reg(p + "sums", K.sums, 16);
+        reg(p + "palette_best", K.aux_best, kcs / 3 * n_local * 4);
+        reg(p + "minv", K.minv_dev, (size_t)n_local * 36);
+      }
+    }
     reg("z_grad", z_grad, z_numel * 4);
     reg("z_grad_acc", z_grad_acc, z_numel * 4);
     reg("best_z", best_z, z_numel * 4);
@@ -2628,8 +2733,6 @@ void Engine::finalize() {
       reg("vd_pred", vd_pred, npx * 4);
       reg("vd_v", vd_v, npx * 4);
     }
-    reg("palette_best", aux_best, ncs / 3 * n_local * 4);
-    reg("minv", minv_dev, (size_t)n_local * 36);
     for (int i = 0; i < cfg.n_clip; ++i) {
       Clip& C = clip[i];
       std::string p = "clip" + std::to_string(i) + ".";
@@ -2731,7 +2834,7 @@ void pxr_destroy(pxr_handle h) {
 
 int pxr_load_weight(pxr_handle h, int module_id, const char* name, const float* data, const int64_t* dims, int ndim) {
   PXR_TRY(h, {
-    if (module_id < 0 || module_id > 3) throw EngineError(-11, "bad module id");
+    if (module_id < 0 || module_id > PXR_MOD_CLIP3) throw EngineError(-11, "bad module id");
     if (h->e->finalized) throw EngineError(-12, "weights cannot change after pxr_finalize");
     pxr::HostWeight w;
     w.dims.assign(dims, dims + ndim);
@@ -2813,14 +2916,15 @@ int pxr_set_image_prompts_sized(pxr_handle h, const float* const* imgs, const in
     Engine* e = h->e;
     if (!e->finalized) throw EngineError(-13, "call pxr_finalize first");
     if (n < 0 || (n > 0 && (!imgs || !hs || !ws))) throw EngineError(-17, "pxr_set_image_prompts: bad arguments");
-    const size_t ncs = (size_t)3 * e->src_h * e->src_w;
     e->n_img = n;
     e->img_w.assign(n, 1.f);
     if (weights)
       for (int k = 0; k < n; ++k) e->img_w[k] = weights[k];
-    e->dfree(e->img_prompts);
-    if (n > 0) {
-      e->img_prompts = e->dalloc<float>(ncs * n);
+    for (Engine::CutSet& K : e->sets) e->dfree(K.img_prompts);
+    for (Engine::CutSet& K : e->sets) {
+      if (n == 0) break;
+      const size_t ncs = (size_t)3 * K.src_h * K.src_w;
+      K.img_prompts = e->dalloc<float>(ncs * n);
       for (int k = 0; k < n; ++k) {
         if (hs[k] < 1 || ws[k] < 1 || !imgs[k]) throw EngineError(-17, "pxr_set_image_prompts: empty image");
         float* tmp = nullptr;
@@ -2829,10 +2933,10 @@ int pxr_set_image_prompts_sized(pxr_handle h, const float* const* imgs, const in
         cudaError_t ce = cudaMemcpyAsync(tmp, imgs[k], bytes, cudaMemcpyDefault, e->st);
         if (ce == cudaSuccess) {
           if (e->aspect != 1.0) {  // pooled like the canvas, then stretched like the canvas (pixray.py:463-472)
-            pxr::pool_forward(tmp, hs[k], ws[k], e->cfg.cut_size, e->pooled, e->pool_argmax, e->st);
-            pxr::rescale_bilinear(e->pooled, e->cfg.cut_size, e->cfg.cut_size, e->src_h, e->src_w, e->img_prompts + k * ncs, e->st);
+            pxr::pool_forward(tmp, hs[k], ws[k], K.cs, K.pooled, K.pool_argmax, e->st);
+            pxr::rescale_bilinear(K.pooled, K.cs, K.cs, K.src_h, K.src_w, K.img_prompts + k * ncs, e->st);
           } else {
-            pxr::pool_forward(tmp, hs[k], ws[k], e->cfg.cut_size, e->img_prompts + k * ncs, e->pool_argmax, e->st);
+            pxr::pool_forward(tmp, hs[k], ws[k], K.cs, K.img_prompts + k * ncs, K.pool_argmax, e->st);
           }
           ce = cudaStreamSynchronize(e->st);
         }
@@ -2854,6 +2958,7 @@ int pxr_set_spot_prompts(pxr_handle h, int clip_idx, int which, const float* emb
     if (!e->finalized) throw EngineError(-13, "call pxr_finalize first");
     if (clip_idx < 0 || clip_idx >= e->cfg.n_clip) throw EngineError(-14, "bad clip index");
     if (which != 0 && which != 1) throw EngineError(-72, "pxr_set_spot_prompts: which = 1 (spot) or 0 (spot off)");
+    if (e->n_sets() > 1 && n > 0) throw EngineError(-69, e->spot_multiset_error());
     auto& C = e->clip[clip_idx];
     if (n > 0 && D != C.c.out_dim) throw EngineError(-15, "prompt embedding width does not match the perceptor");
     auto& sp = C.spot[which];
@@ -2878,6 +2983,7 @@ int pxr_set_spot_mask(pxr_handle h, const unsigned char* mask) {
     Engine* e = h->e;
     if (!e->finalized) throw EngineError(-13, "call pxr_finalize first");
     if (!mask) throw EngineError(-10, "pxr_set_spot_mask: null mask");
+    if (e->n_sets() > 1) throw EngineError(-69, e->spot_multiset_error());
     const size_t n = (size_t)3 * e->cfg.cut_size * e->cfg.cut_size;
     if (!e->spot_mask) e->spot_mask = e->dalloc<unsigned char>(n);
     PXR_CUDA(cudaMemcpyAsync(e->spot_mask, mask, n, cudaMemcpyHostToDevice, e->st));
@@ -2982,20 +3088,35 @@ int pxr_set_color_jitter(pxr_handle h, float p, float saturation, float hue) {
 }
 
 int pxr_make_cutouts(pxr_handle h, const float* img, const pxr_cut_params* p, int iter, float* out_batch) {
+  return pxr_make_cutouts_set(h, 0, img, p, iter, out_batch);
+}
+
+int pxr_cutout_sets(pxr_handle h, int* cut_sizes) {
   PXR_TRY(h, {
     Engine* e = h->e;
+    if (!e->finalized) throw EngineError(-13, "call pxr_finalize first");
+    if (!cut_sizes) throw EngineError(-10, "pxr_cutout_sets: null cut_sizes");
+    for (int s = 0; s < 4; ++s) cut_sizes[s] = s < e->n_sets() ? e->sets[s].cs : 0;
+    return e->n_sets();
+  });
+}
+
+int pxr_make_cutouts_set(pxr_handle h, int set, const float* img, const pxr_cut_params* p, int iter, float* out_batch) {
+  PXR_TRY(h, {
+    Engine* e = h->e;
+    if (set < 0 || set >= e->n_sets()) throw EngineError(-83, "bad cutout set index");
     if (img) {
       PXR_CUDA(cudaMemcpyAsync(e->img, img, sizeof(float) * 3 * e->cfg.image_h * e->cfg.image_w,
                                cudaMemcpyDeviceToDevice, e->st));
       e->filtered_valid = false;
     }
-    e->prepare_cut_params(p, iter);
-    e->encode_image_prompts();
-    e->forward_cutouts();
+    const Engine::CutSet& K = e->sets[set];
+    e->prepare_cut_params(set, p, iter);
+    e->encode_image_prompts(set);
+    e->forward_cutouts(set);
     if (out_batch)
-      PXR_CUDA(cudaMemcpyAsync(out_batch, e->batch,
-                               sizeof(float) * e->n_local * 3 * e->cfg.cut_size * e->cfg.cut_size,
-                               cudaMemcpyDeviceToDevice, e->st));
+      PXR_CUDA(cudaMemcpyAsync(out_batch, K.batch, sizeof(float) * e->n_local * 3 * K.cs * K.cs, cudaMemcpyDeviceToDevice,
+                               e->st));
   });
 }
 
@@ -3003,15 +3124,21 @@ int pxr_encode_image(pxr_handle h, int clip_idx, const float* batch, float* out_
   PXR_TRY(h, {
     Engine* e = h->e;
     if (clip_idx < 0 || clip_idx >= e->cfg.n_clip) throw EngineError(-14, "bad clip index");
+    Engine::CutSet& K = e->sets[e->set_of[clip_idx]];
     if (batch) {
-      // a caller-provided batch: recompute its global range exactly like CLIP_Base.preprocess does
-      PXR_CUDA(cudaMemcpyAsync(e->batch, batch, sizeof(float) * e->n_local * 3 * e->cfg.cut_size * e->cfg.cut_size,
-                               cudaMemcpyDeviceToDevice, e->st));
-      const int np_ = e->n_parts < 1024 ? e->n_parts : 1024;
-      pxr::minmax_partials(e->batch, (long long)e->n_local * 3 * e->cfg.cut_size * e->cfg.cut_size, np_, e->part_min,
-                           e->part_max, e->part_imin, e->part_imax, e->st);
-      pxr::minmax_reduce(nullptr, e->part_min, e->part_max, e->part_imin, e->part_imax, np_, e->range, e->irange, e->st);
+      // a caller-provided batch at the perceptor's resolution: recompute its global range exactly like
+      // CLIP_Base.preprocess does
+      const long long n = (long long)e->n_local * 3 * K.cs * K.cs;
+      PXR_CUDA(cudaMemcpyAsync(K.batch, batch, sizeof(float) * n, cudaMemcpyDeviceToDevice, e->st));
+      const int np_ = K.n_parts < 1024 ? K.n_parts : 1024;
+      pxr::minmax_partials(K.batch, n, np_, K.part_min, K.part_max, K.part_imin, K.part_imax, e->st);
+      pxr::minmax_reduce(nullptr, K.part_min, K.part_max, K.part_imin, K.part_imax, np_, K.range, K.irange, e->st);
       e->launches += 2;
+      K.cut = true;
+    } else if (e->n_sets() > 1 && !K.cut) {
+      throw EngineError(-83, "perceptor " + std::to_string(clip_idx) + " reads cutout set " +
+                                 std::to_string(e->set_of[clip_idx]) + " (" + std::to_string(K.cs) +
+                                 " px), which has not been cut since the last backward: pxr_make_cutouts_set first");
     }
     e->forward_clip(clip_idx);
     auto& C = e->clip[clip_idx];
@@ -3077,6 +3204,15 @@ int pxr_step(pxr_handle h, float* z, float lr, int iter) {
 }
 
 int pxr_iterate(pxr_handle h, float* z, float lr, int iter, const pxr_cut_params* p, float* out_losses_host) {
+  if (h && p && h->e->n_sets() > 1) {
+    h->e->err = "pxr_iterate: this session has " + std::to_string(h->e->n_sets()) +
+                " cutout sets; pass their cutout parameters to pxr_iterate_sets (one pxr_cut_params per set)";
+    return -69;
+  }
+  return pxr_iterate_sets(h, z, lr, iter, p, out_losses_host);
+}
+
+int pxr_iterate_sets(pxr_handle h, float* z, float lr, int iter, const pxr_cut_params* p, float* out_losses_host) {
   PXR_TRY(h, {
     Engine* e = h->e;
     if (z) PXR_CUDA(cudaMemcpyAsync(e->z_buf, z, e->z_numel * sizeof(float), cudaMemcpyDeviceToDevice, e->st));
@@ -3087,29 +3223,33 @@ int pxr_iterate(pxr_handle h, float* z, float lr, int iter, const pxr_cut_params
       // every pass is one ascend_txt + backward (pixray.py:1464-1482): fresh augmentations, gradients accumulate in z.grad;
       // checkdrop and the reported loss vector use the FIRST pass (`if i == 0`, pixray.py:1466)
       e->rng_iter = b == 0 ? 0 : iter + b * (1 << 20);
-      e->prepare_cut_params(p, iter);
+      for (int s = 0; s < e->n_sets(); ++s) e->prepare_cut_params(s, p ? p + s : nullptr, iter);
       if (b == 0) PXR_CUDA(cudaMemsetAsync(e->losses_dev, 0, 64 * sizeof(float), e->st));
       else PXR_CUDA(cudaMemsetAsync(e->losses_scratch, 0, 64 * sizeof(float), e->st));
       float* keep = e->losses_dev;
       if (b > 0) e->losses_dev = e->losses_scratch;  // later passes must not disturb the first pass's loss vector
       try {
-        e->encode_image_prompts();
+        for (int s = 0; s < e->n_sets(); ++s) e->encode_image_prompts(s);
         if (b == 0) {
           e->forward_drawer();  // same z: the image of the later passes is the same image
           if (!e->filters.empty()) e->filters_forward(iter);
         }
         if (e->any_spot(1) || e->any_spot(0)) {  // spot / spot-off prompts: their own masked cutout batches (pixray.py:1262-1293)
-          pxr::pool_forward(e->cur_cut_img(), e->cur_cut_h(), e->cur_cut_w(), e->cfg.cut_size, e->pooled, e->pool_argmax, e->st);
+          Engine::CutSet& K = e->sets[0];
+          pxr::pool_forward(e->cur_cut_img(), e->cur_cut_h(), e->cur_cut_w(), K.cs, K.pooled, K.pool_argmax, e->st);
           e->launches += 1;
           bool acc = false;
           acc |= e->spot_pass(1, acc);
           acc |= e->spot_pass(0, acc);
           e->spot_accumulated = acc;
         }
-        e->forward_cutouts();
-        for (int i = 0; i < e->cfg.n_clip; ++i) {
-          e->forward_clip(i);
-          e->loss_clip(i);
+        for (int s = 0; s < e->n_sets(); ++s) {  // each set is cut from the same image (pixray.py:1266-1268)
+          e->forward_cutouts(s);
+          for (int i = 0; i < e->cfg.n_clip; ++i) {
+            if (e->set_of[i] != s) continue;
+            e->forward_clip(i);
+            e->loss_clip(i);
+          }
         }
         e->backward_all();
       } catch (...) {
@@ -3211,7 +3351,7 @@ int pxr_profile_iteration2(pxr_handle h, float* z, float lr, int iter, double* o
   PXR_TRY(h, {
     Engine* e = h->e;
     if (z) PXR_CUDA(cudaMemcpyAsync(e->z_buf, z, e->z_numel * sizeof(float), cudaMemcpyDeviceToDevice, e->st));
-    e->prepare_cut_params(nullptr, iter);
+    for (int s = 0; s < e->n_sets(); ++s) e->prepare_cut_params(s, nullptr, iter);
     PXR_CUDA(cudaMemsetAsync(e->losses_dev, 0, 64 * sizeof(float), e->st));
     e->prof.clear();
     e->profiling = true;
@@ -3221,10 +3361,13 @@ int pxr_profile_iteration2(pxr_handle h, float* z, float lr, int iter, double* o
     PXR_CUDA(cudaEventCreate(&t1));
     PXR_CUDA(cudaEventRecord(t0, e->st));
     e->forward_drawer();
-    e->forward_cutouts();
-    for (int i = 0; i < e->cfg.n_clip; ++i) {
-      e->forward_clip(i);
-      e->loss_clip(i);
+    for (int s = 0; s < e->n_sets(); ++s) {
+      e->forward_cutouts(s);
+      for (int i = 0; i < e->cfg.n_clip; ++i) {
+        if (e->set_of[i] != s) continue;
+        e->forward_clip(i);
+        e->loss_clip(i);
+      }
     }
     e->backward_all();
     e->step(lr);
@@ -3320,7 +3463,8 @@ int pxr_add_aux_loss(pxr_handle h, int kind, float weight, const float* params, 
   PXR_TRY(h, {
     Engine* e = h->e;
     if (!e->finalized) throw EngineError(-13, "call pxr_finalize first");
-    if (e->num_losses() >= 64) throw EngineError(-16, "at most 64 losses (prompts + auxiliary) in total");
+    if (e->num_losses() + e->aux_width(kind) > 64)
+      throw EngineError(-16, "at most 64 losses (prompts + auxiliary, a cutout-space loss once per cutout set) in total");
     auto need = [&](int n, const char* what) {
       if (n_params < n || !params) throw EngineError(-80, std::string("pxr_add_aux_loss: ") + what);
     };
@@ -3349,7 +3493,9 @@ int pxr_add_aux_loss(pxr_handle h, int kind, float weight, const float* params, 
         const int n = (int)nf;
         if (n_params != (n_params > 4 ? 5 + n * n : n_params))
           throw EngineError(-80, "pxr_add_aux_loss: smoothness blur needs n * n taps after n");
-        const int cs2 = e->cfg.cut_size - (n ? n - 1 : 0);
+        int min_cs = e->cfg.cut_size;
+        for (const Engine::CutSet& K : e->sets) min_cs = std::min(min_cs, K.cs);
+        const int cs2 = min_cs - (n ? n - 1 : 0);
         if (cs2 < order + 1)
           throw EngineError(-80, "pxr_add_aux_loss: smoothness blur leaves " + std::to_string(cs2) + " pixels per cutout side; "
                                  "torch.gradient with edge_order " + std::to_string(order) + " needs at least " +
@@ -3373,11 +3519,12 @@ int pxr_add_aux_loss(pxr_handle h, int kind, float weight, const float* params, 
               throw EngineError(-80, "pxr_add_aux_loss: smoothness blur taps must be separable (an outer product u u^T)");
           a.dev = e->upload(std::vector<float>(u.begin(), u.end()));
           a.n_dev = n;
-          if (!e->aux_blur) {
-            const size_t sz = (size_t)e->n_local * 3 * e->cfg.cut_size * e->cfg.cut_size;
-            e->aux_blur = e->dalloc<float>(sz);
-            e->aux_g_blur = e->dalloc<float>(sz);
-            e->aux_blur_tmp = e->dalloc<float>(sz);
+          for (Engine::CutSet& K : e->sets) {
+            if (K.aux_blur) continue;
+            const size_t sz = (size_t)e->n_local * 3 * K.cs * K.cs;
+            K.aux_blur = e->dalloc<float>(sz);
+            K.aux_g_blur = e->dalloc<float>(sz);
+            K.aux_blur_tmp = e->dalloc<float>(sz);
           }
         }
         break;

@@ -227,6 +227,7 @@ struct CutoutArgs {
   float fill;
   uint64_t seed;
   int iter;
+  uint32_t rng_stream;     // Philox stream offset of the cutout set (transforms.h cut_rng_stream; 0 for set 0)
 };
 int cutout_num_blocks(int n_local, int cs);
 // batch [n_local,3,cs,cs] fp32; block partial min/max (+ element index) for the global range normalise (slip.py:21-36)

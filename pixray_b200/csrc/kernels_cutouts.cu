@@ -263,11 +263,11 @@ __global__ void __launch_bounds__(CUT_THREADS) cutout_fwd_kernel(CutoutArgs a, f
     } else if (a.noise_mode == 2) {
       // engine RNG: Philox keyed by (seed, iter), counted by the GLOBAL element index -> shard invariant.
       // facs ~ U(0, noise_fac) per cutout (pixray.py:509), noise ~ N(0,1) per element (pixray.py:510)
-      fac = philox_uniform(a.seed, (uint32_t)a.iter, 1u, (uint64_t)n_global) * a.noise_fac;
+      fac = philox_uniform(a.seed, (uint32_t)a.iter, 1u + a.rng_stream, (uint64_t)n_global) * a.noise_fac;
 #pragma unroll
       for (int c = 0; c < 3; ++c) {
         uint64_t e = (((uint64_t)n_global * 3 + c) * cs + v) * cs + u0;
-        philox_normal4(a.seed, (uint32_t)a.iter, 0u, e >> 2, nz[c]);
+        philox_normal4(a.seed, (uint32_t)a.iter, a.rng_stream, e >> 2, nz[c]);
       }
     }
     int cj_code = 0;

@@ -64,12 +64,18 @@ inline bool perspective_from_points(const double src[4][2], const double dst[4][
   return true;
 }
 
+// Philox stream words of the draws of cutout set s: 0 noise, 1 noise factors, 2 homographies, 4 / 5 ColorJitter, each
+// plus cut_rng_stream(s).  Set 0 adds nothing; the other sets get words of their own, above the shared fill (3) and the
+// filters' shifts (6).  The image-prompt and spot passes move the iteration word instead (engine.cu), so no two collide.
+inline uint32_t cut_rng_stream(int set) { return 16u * (uint32_t)set; }
+
 struct CutRng {
   uint64_t seed;
   uint32_t iter;
   uint64_t base;
+  uint32_t stream = 0;  // cut_rng_stream of the set
   uint32_t k = 0;
-  double uni() { return (double)philox_uniform(seed, iter, 2u, base + (k++)); }        // (0, 1]
+  double uni() { return (double)philox_uniform(seed, iter, 2u + stream, base + (k++)); }        // (0, 1]
   double uni(double lo, double hi) { return lo + (hi - lo) * uni(); }
 };
 
@@ -179,7 +185,7 @@ inline void sample_affine_hw(CutRng& r, int h, int w, double lo, double hi, doub
 
 // out: [cutn, 9] row-major dst<-src homographies; zoom group first (global index < int(0.6 * cutn), pixray.py:407)
 inline void sample_cutout_transforms(uint64_t seed, int iter, int cutn, int cut_size, float* out, double aspect = 1.0,
-                                     int src_h = 0, int src_w = 0) {
+                                     int src_h = 0, int src_w = 0, uint32_t stream = 0) {
   const int cutn_zoom = (int)(0.6 * cutn);
   int sh, sw;
   source_size(cut_size, aspect, sh, sw);
@@ -188,7 +194,7 @@ inline void sample_cutout_transforms(uint64_t seed, int iter, int cutn, int cut_
     sw = src_w;
   }
   for (int n = 0; n < cutn; ++n) {
-    CutRng r{seed, (uint32_t)iter, (uint64_t)n * 64};
+    CutRng r{seed, (uint32_t)iter, (uint64_t)n * 64, stream};
     double A[9], B[9], H[9];
     if (aspect != 1.0) {
       if (n < cutn_zoom) {
@@ -227,21 +233,23 @@ inline void sample_cutout_transforms(uint64_t seed, int iter, int cutn, int cut_
 // per cutout Bernoulli(p), saturation_factor ~ U(1 - s, 1 + s), hue_factor ~ U(-h, h); one randperm(4) application
 // order per group (each stack is its own module, called once per iteration).  out: [cutn, 3] rows
 // {code, saturation_factor, hue_factor} in the encoding of color_jitter.cuh.
-inline void sample_color_jitter(uint64_t seed, int iter, int cutn, float p, float sat, float hue, float* out) {
+inline void sample_color_jitter(uint64_t seed, int iter, int cutn, float p, float sat, float hue, float* out,
+                                uint32_t stream = 0) {
   const int cutn_zoom = (int)(0.6 * cutn);
   int code[2];
   for (int g = 0; g < 2; ++g) {
     int order[4] = {0, 1, 2, 3};
     for (int k = 3; k > 0; --k) {  // Fisher-Yates
-      int j = (int)(philox_uniform(seed, (uint32_t)iter, 5u, (uint64_t)g * 4 + k) * 0.999999f * (k + 1));
+      int j = (int)(philox_uniform(seed, (uint32_t)iter, 5u + stream, (uint64_t)g * 4 + k) * 0.999999f * (k + 1));
       std::swap(order[k], order[j]);
     }
     code[g] = 256 + order[0] + 4 * order[1] + 16 * order[2] + 64 * order[3];
   }
   for (int n = 0; n < cutn; ++n) {
     const uint64_t base = (uint64_t)n * 4;
-    const bool apply = philox_uniform(seed, (uint32_t)iter, 4u, base) <= p;
-    const float u1 = philox_uniform(seed, (uint32_t)iter, 4u, base + 1), u2 = philox_uniform(seed, (uint32_t)iter, 4u, base + 2);
+    const bool apply = philox_uniform(seed, (uint32_t)iter, 4u + stream, base) <= p;
+    const float u1 = philox_uniform(seed, (uint32_t)iter, 4u + stream, base + 1),
+                u2 = philox_uniform(seed, (uint32_t)iter, 4u + stream, base + 2);
     out[n * 3] = apply ? (float)code[n < cutn_zoom ? 0 : 1] : 0.f;
     out[n * 3 + 1] = 1.f - sat + 2.f * sat * u1;
     out[n * 3 + 2] = -hue + 2.f * hue * u2;

@@ -15,7 +15,7 @@ LOSS_SYMMETRY, LOSS_SATURATION, LOSS_PALETTE, LOSS_SMOOTHNESS, LOSS_EDGE, LOSS_G
 ANCHOR_SPHERICAL, ANCHOR_MSE, ANCHOR_COS, ANCHOR_PIX = 0, 1, 2, 3
 FILTER_TILER, FILTER_WALLPAPER, FILTER_LOOKUP = range(3)
 PAD_REFLECTION, PAD_BORDER = 0, 1
-MOD_VQGAN, MOD_CLIP0, MOD_CLIP1, MOD_CLIP2 = 0, 1, 2, 3
+MOD_VQGAN, MOD_CLIP0, MOD_CLIP1, MOD_CLIP2, MOD_CLIP3 = 0, 1, 2, 3, 4
 # optimiser update rules (pxr_set_optimizer), by the reference's args.optimiser names (pixray.py:536-551)
 OPT_ADAM, OPT_ADAMW, OPT_ADAGRAD, OPT_ADAMAX, OPT_DIFFGRAD = range(5)
 OPTIMISERS = {"Adam": OPT_ADAM, "AdamW": OPT_ADAMW, "Adagrad": OPT_ADAGRAD, "Adamax": OPT_ADAMAX, "DiffGrad": OPT_DIFFGRAD}
@@ -87,6 +87,24 @@ class EngineError(RuntimeError):
     pass
 
 
+def aux_loss_width(kind, n_sets):
+    """Loss-vector entries of one auxiliary loss: a cutout-space loss (saturation, palette, smoothness) has one per
+    cutout set, in set order (its get_loss returns a list, spliced in by pixray.py:1392-1398); the others one."""
+    return n_sets if kind in (LOSS_SATURATION, LOSS_PALETTE, LOSS_SMOOTHNESS) else 1
+
+
+def cutout_sets(cut_size, image_res):
+    """(cut sizes, set of each perceptor): set 0 at cut_size (the first perceptor's resolution), then every other
+    resolution in order of first appearance, as the reference fills cutoutsTable (pixray.py:642-649)."""
+    sizes, set_of = [int(cut_size)], []
+    for i, r in enumerate(image_res):
+        r = int(cut_size) if i == 0 else int(r)
+        if r not in sizes:
+            sizes.append(r)
+        set_of.append(sizes.index(r))
+    return sizes, set_of
+
+
 def stroke_z_layout(n_paths, n_segments):
     """Sizes of the line drawer's z ranges: (points, widths, paper RGBA)."""
     return n_paths * (3 * n_segments + 1) * 2, n_paths, 4
@@ -95,6 +113,9 @@ def stroke_z_layout(n_paths, n_segments):
 class B200Engine:
     # the image-tower kinds this library builds (pxr_set_clip_tower)
     TOWERS = (TOWER_OPENAI_CLIP, TOWER_TIMM_VIT, TOWER_CLIP_RESNET)
+    # perceptors per session, and whether they may have different input resolutions (one cutout set each)
+    MAX_PERCEPTORS = 4
+    MIXED_RESOLUTIONS = True
 
     def __init__(self, *, drawer=DRAWER_VQGAN, image_hw=(256, 256), vqgan=None, grid=None, cutn=64, cut_size=224,
                  clip=(), noise_fac=0.1, seed=0, device=0, rank=0, world=1, grad_scale=0.0, lr_betas=(0.9, 0.999),
@@ -168,6 +189,9 @@ class B200Engine:
         self.n_local = cutn // world
         self.image_hw = tuple(image_hw)
         self.clip_dims = [c["out_dim"] for c in clip]
+        # the cutout sets (the reference's cutoutsTable, pixray.py:642-649): set 0 at cut_size, then every other input
+        # resolution in order of first appearance; set_of[i] is perceptor i's set
+        self.cut_sets, self.set_of = cutout_sets(cut_size, [c["image_res"] for c in clip])
         self.n_prompts = [0 for _ in clip]  # loss slots per perceptor: text prompts + image prompts
         self._n_text = [0 for _ in clip]
         self._n_spot = [[0, 0] for _ in clip]  # [spot off, spot] prompts per perceptor (scored in the fused path only)
@@ -305,7 +329,7 @@ class B200Engine:
         a = np.ascontiguousarray(np.asarray(params, dtype=np.float32).reshape(-1))
         rc = self.lib.pxr_add_aux_loss(self.h, int(kind), C.c_float(float(weight)), a.ctypes.data_as(C.c_void_p), int(a.size))
         self._check(rc, "pxr_add_aux_loss")
-        return self.num_losses() - 1
+        return self.num_losses() - aux_loss_width(kind, len(self.cut_sets))
 
     def add_filter(self, kind, weight, params):
         """One more filter between synth and the cutouts (pxr_add_filter; filters/*.py).  Its loss takes the next entry at the
@@ -417,9 +441,13 @@ class B200Engine:
         self._check(self.lib.pxr_set_color_jitter(self.h, C.c_float(p), C.c_float(saturation), C.c_float(hue)),
                     "pxr_set_color_jitter")
 
-    def _cut_params(self, transforms, zoom_padding, fill, noise_facs, noise, color_jitter=None):
+    def _cut_params(self, transforms, zoom_padding, fill, noise_facs, noise, color_jitter=None, cs=None, keep=None):
+        """pxr_cut_params for a set of cut size cs; the arrays it points to are kept alive in `keep` (default: until
+        the next call)."""
         p = _lib.CutParams()
-        keep = []
+        if keep is None:
+            keep = []
+            self._keep = keep
         if color_jitter is not None:
             cj = np.ascontiguousarray(np.asarray(color_jitter, dtype=np.float32).reshape(self.cutn, 3))
             keep.append(cj)
@@ -435,9 +463,10 @@ class B200Engine:
             p.noise_facs = f.ctypes.data_as(C.c_void_p)
         if noise is not None:
             nz = noise.to(self.device, torch.float32).contiguous()
+            if cs is not None and nz.numel() != self.cutn * 3 * cs * cs:
+                raise EngineError(f"noise must be [cutn, 3, {cs}, {cs}] for a cutout set of size {cs}")
             keep.append(nz)
             p.noise = C.c_void_p(nz.data_ptr())
-        self._keep = keep
         return p
 
     # ------------------------------------------------------------------ per-op entry points (parity tests)
@@ -463,22 +492,38 @@ class B200Engine:
         return out
 
     def make_cutouts(self, img=None, *, transforms=None, zoom_padding=PAD_REFLECTION, fill=0.0, noise_facs=None,
-                     noise=None, it=0, use_engine_rng=False, color_jitter=None):
+                     noise=None, it=0, use_engine_rng=False, color_jitter=None, cut_set=0):
+        """The cutouts of cutout set `cut_set` (pxr_make_cutouts_set): [cutn_local, 3, cs, cs] at that set's size."""
         if img is not None:
             img = img.to(self.device, torch.float32).contiguous()
-        out = self._new(self.n_local, 3, self.cut_size, self.cut_size)
+        cs = self.cut_sets[cut_set]
+        out = self._new(self.n_local, 3, cs, cs)
         p = None if use_engine_rng else self._cut_params(transforms, zoom_padding, fill, noise_facs, noise,
-                                                                color_jitter)
+                                                                color_jitter, cs)
         torch.cuda.current_stream().synchronize()
-        rc = self.lib.pxr_make_cutouts(self.h, self._p(img), None if p is None else C.byref(p), it, self._p(out))
-        self._check(rc, "pxr_make_cutouts")
+        rc = self.lib.pxr_make_cutouts_set(self.h, int(cut_set), self._p(img), None if p is None else C.byref(p), it,
+                                           self._p(out))
+        self._check(rc, "pxr_make_cutouts_set")
         self.sync()
         return out
 
+    def cutout_sets(self):
+        """The engine's cutout sets as it built them (pxr_cutout_sets): their cut sizes, in set order."""
+        sizes = (C.c_int * 4)()
+        rc = self.lib.pxr_cutout_sets(self.h, sizes)
+        if rc < 0:
+            self._check(rc, "pxr_cutout_sets")
+        return list(sizes[:rc])
+
     def encode_image(self, clip_idx=0, batch=None):
-        """Unit-norm embeddings of the engine's current cutouts, or of `batch` [cutn_local,3,cs,cs] when given."""
+        """Unit-norm embeddings of the current cutouts of the perceptor's set, or of `batch` [cutn_local,3,cs,cs] at
+        that set's size when given."""
         out = self._new(self.n_local, self.clip_dims[clip_idx])
         if batch is not None:
+            cs = self.cut_sets[self.set_of[clip_idx]]
+            if tuple(batch.shape) != (self.n_local, 3, cs, cs):
+                raise EngineError(f"encode_image: perceptor {clip_idx} reads {cs} x {cs} cutouts, got a batch of shape "
+                                  f"{tuple(batch.shape)} (expected {(self.n_local, 3, cs, cs)})")
             batch = batch.to(self.device, torch.float32).contiguous()
             torch.cuda.current_stream().synchronize()
         self._check(self.lib.pxr_encode_image(self.h, clip_idx, self._p(batch), self._p(out)), "pxr_encode_image")
@@ -581,21 +626,29 @@ class B200Engine:
     # ------------------------------------------------------------------ the fast path (what bench.py times)
     def iterate(self, z, lr, it, *, params=None, losses_out=None):
         """One train() iteration entirely inside the library.  params: dict(transforms, zoom_padding, fill,
-        noise_facs, noise, color_jitter) or None for the engine's own Philox draws.  losses_out: float32 numpy array (host) to
-        receive the per-prompt losses (forces a stream sync), or None."""
+        noise_facs, noise, color_jitter), a list of such dicts (one per cutout set, pxr_iterate_sets), or None for the
+        engine's own Philox draws.  losses_out: float32 numpy array (host) to receive the per-prompt losses (forces a
+        stream sync), or None."""
         p = None
+        per_set = isinstance(params, (list, tuple))
+        if per_set and len(params) != len(self.cut_sets):
+            raise EngineError(f"iterate: {len(params)} cutout parameter sets for {len(self.cut_sets)} cutout sets")
         if params is not None:
-            p = self._cut_params(params.get("transforms"), params.get("zoom_padding", it % 2),
-                                 params.get("fill", 0.0), params.get("noise_facs"), params.get("noise"),
-                                 params.get("color_jitter"))
+            keep = []
+            self._keep = keep
+            plist = [self._cut_params(q.get("transforms"), q.get("zoom_padding", it % 2), q.get("fill", 0.0),
+                                      q.get("noise_facs"), q.get("noise"), q.get("color_jitter"), cs, keep)
+                     for q, cs in zip(params if per_set else [params], self.cut_sets)]
+            p = (_lib.CutParams * len(plist))(*plist)
         # z / noise may have been produced on torch's stream (e.g. an H2D copy still in flight): order the engine's
         # non-blocking stream after it without a host sync
         if self._ext is None:
             self._ext = torch.cuda.ExternalStream(self.stream_ptr())
         self._ext.wait_stream(torch.cuda.current_stream())
         lp = None if losses_out is None else losses_out.ctypes.data_as(C.c_void_p)
-        rc = self.lib.pxr_iterate(self.h, self._p_inplace(z, "z"), C.c_float(lr), it, None if p is None else C.byref(p), lp)
-        self._check(rc, "pxr_iterate")
+        fn, name = (self.lib.pxr_iterate_sets, "pxr_iterate_sets") if per_set else (self.lib.pxr_iterate, "pxr_iterate")
+        rc = fn(self.h, self._p_inplace(z, "z"), C.c_float(lr), it, p, lp)
+        self._check(rc, name)
 
     def debug_read(self, name, shape, dtype=torch.float32):
         out = torch.empty(*shape, device=self.device, dtype=dtype)

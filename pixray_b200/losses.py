@@ -59,12 +59,18 @@ class LossInterface:
         """lossClasses.append({"loss": lossInstance, "weight": weight}) (pixray.py:979-981) for the engine."""
         self._session = session
         self._index = session.engine.add_aux_loss(self.kind, weight, self.engine_params(args, session))
+        self._width = E.aux_loss_width(self.kind, len(getattr(session.engine, "cut_sets", (0,))))
         return self
 
     def get_loss(self, cur_cutouts, out, args, globals=None, lossGlobals=None):
+        """The engine's value of this loss for the last iteration.  A cutout-space loss in a session with several cutout
+        sets returns one entry per set, in set order, as the reference's loop over cur_cutouts does."""
         if self._session is None:
             raise RuntimeError(f"{type(self).__name__}.attach(session, args, weight) must be called first")
-        return torch.as_tensor(self._session.engine.read_losses()[self._index])
+        v = self._session.engine.read_losses()
+        if self._width > 1:
+            return [torch.as_tensor(v[self._index + s]) for s in range(self._width)]
+        return torch.as_tensor(v[self._index])
 
 
 class SymmetryLoss(LossInterface):

@@ -644,8 +644,9 @@ class MakeCutouts:
     """pixray.py:399-511.  `transforms` is the per-iteration cache of composed 3x3s (pixray.py:498); when it is None
     a fresh set is sampled (the distributions of the reference's augmentation stacks, pixray_b200/cutouts.py)."""
 
-    def __init__(self, cut_size, cutn, session: Session, cut_pow=1.0, seed=0, aspect=1.0):
+    def __init__(self, cut_size, cutn, session: Session, cut_pow=1.0, seed=0, aspect=1.0, cut_set=0):
         self.cut_size, self.cutn, self.cut_pow = cut_size, cutn, cut_pow
+        self.cut_set = cut_set  # the engine's cutout set of this resolution (set 0: the first perceptor's)
         self.aspect = aspect  # global_aspect_width (pixray.py:402, 1931)
         self.cutn_zoom = int(0.6 * cutn)
         self.noise_fac = 0.1
@@ -675,9 +676,10 @@ class MakeCutouts:
         if self.noise_fac:
             facs = (self._rng.random(self.cutn) * self.noise_fac).astype(np.float32)        # pixray.py:509
             noise = torch.randn(self.cutn, 3, self.cut_size, self.cut_size, device=s.engine.device)  # pixray.py:510
+        kw = dict(cut_set=self.cut_set) if self.cut_set else {}
         return s.engine.make_cutouts(input, transforms=self.transforms.numpy(), zoom_padding=pad,
                                      fill=s.global_fill_color, noise_facs=facs, noise=noise, it=s.cur_iteration,
-                                     color_jitter=jitter)
+                                     color_jitter=jitter, **kw)
 
 
 class Perceptor:
@@ -802,16 +804,27 @@ class Optimizer:
 
 def train_iteration(session: Session, drawer, make_cutouts, perceptors, prompt_table, opt):
     """The body of train()/ascend_txt for the default settings (pixray.py:1243-1406, 1436-1512), expressed with the
-    plugin objects exactly like the reference does.  Returns the list of scalar losses."""
+    plugin objects exactly like the reference does.  make_cutouts: one MakeCutouts, or the cutoutsTable {cut_size:
+    MakeCutouts} of perceptors with different input resolutions (pixray.py:1266-1268: every entry cuts the same image,
+    each perceptor encodes its own resolution's cutouts).  Returns the list of scalar losses."""
+    table = make_cutouts if isinstance(make_cutouts, dict) else None
+    have = table.keys() if table else [getattr(make_cutouts, "cut_size", None)]
+    for p in perceptors:
+        res = getattr(p, "input_resolution", None)
+        if None not in have and res is not None and res not in have:
+            raise ValueError(f"a perceptor with input resolution {res} needs a MakeCutouts of that size "
+                             f"(have {sorted(have)}): pass the cutoutsTable {{cut_size: MakeCutouts}} (pixray.py:642-649)")
     opt.zero_grad()
     out = drawer.synth(session.cur_iteration)
-    cutouts = make_cutouts(out)
+    cur_cutouts = {cs: mc(out) for cs, mc in table.items()} if table else None
+    cutouts = None if table else make_cutouts(out)
     result = []
     for i, perceptor in enumerate(perceptors):
-        iii = perceptor.encode_image(cutouts).float()
+        iii = perceptor.encode_image(cur_cutouts[perceptor.input_resolution] if table else cutouts).float()
         for prompt in prompt_table[i]:
             result.append(prompt(iii))
-    make_cutouts.transforms = None  # clear the per-iteration cache (pixray.py:1339-1342)
+    for mc in (table.values() if table else [make_cutouts]):
+        mc.transforms = None  # clear the per-iteration cache (pixray.py:1339-1342)
     session.backward(drawer)
     opt.step()
     drawer.clip_z()
