@@ -163,6 +163,39 @@ class Engine {
   float cj_p = 0.8f, cj_sat = 0.1f, cj_hue = 0.1f;  // K.ColorJitter(hue=0.1, saturation=0.1, p=0.8), pixray.py:416, 436
 
   // ---- perceptors
+  // the weights of one pre-norm transformer block (openai-CLIP ResidualAttentionBlock, timm Block), image or text tower
+  struct BlockW {
+    act_t *wqkv, *wo, *wfc, *wproj;
+    float *bqkv, *bo, *bfc, *bproj;
+    NormW ln1, ln2;
+  };
+  BlockW load_block(int mod, const std::string& prefix, int Wd, bool timm);
+  // What add_block reads and writes.  The residual stream runs x_in -> x_mid (after the attention) -> x_out (after the
+  // MLP); ln_1, qkv and the attention cover all images * T rows at pitch W, the row-wise tail from out_proj on covers
+  // `rows` rows `ld` apart (the class rows only, pitch T W, in the ViT's last layer).  h16 / gact / u hold the tail's
+  // rows compactly.  The g* buffers are read only when add_block builds a backward (gx == nullptr on an fp16 stream).
+  struct BlockIO {
+    const void* x_in;
+    void *x_mid, *x_out;
+    float *stats1, *stats2;
+    act_t *h16, *qkv, *o, *u, *gact;
+    int images, heads, T, rows;
+    long long ld;
+    int act;  // ACT_QUICKGELU or ACT_GELU
+    float eps;
+    bool causal;
+    act_t *go = nullptr, *gqkv = nullptr, *dP = nullptr, *g4 = nullptr, *gh = nullptr, *gx16 = nullptr;
+    float* gx = nullptr;
+  };
+  act_t* add_block(OpList& fwd, OpList* bwd, const BlockW& w, const BlockIO& b);
+  void add_head(OpList& l, const void* x, long long ld, int rows, const NormW& n, float eps, act_t* h16, float* stats,
+                const act_t* proj16, int Wd, int D, float* out);
+  // The residual stream's element type (fp16 with stream16, else fp32) is decided here: a LayerNorm of its rows (pitch
+  // ld), its backward (gx, gx16 rows ld apart too), and a GEMM epilogue out = res + A B^T into the stream.
+  Op stream_ln_fwd(const void* x, long long ld, const NormW& n, int rows, int Wd, float eps, act_t* y16, float* stats) const;
+  Op stream_ln_bwd(const act_t* dy, const void* x, long long ld, const float* stats, const NormW& n, int rows, int Wd,
+                   int accumulate, float* gx, act_t* gx16) const;
+  void stream_residual(GemmEpilogue& e, const void* res, void* out) const;
   struct Clip {
     pxr_clip_cfg c;
     int tower = PXR_TOWER_OPENAI_CLIP;  // pxr_set_clip_tower
@@ -170,12 +203,10 @@ class Engine {
     int T, np, Kp, ldT, M, B;
     // weights
     act_t* conv1 = nullptr;
-    float *cls = nullptr, *pos = nullptr, *proj = nullptr, *conv1_b = nullptr;
+    float *cls = nullptr, *pos = nullptr, *conv1_b = nullptr;
     NormW ln_pre, ln_post;
     struct Layer {
-      act_t *wqkv, *wo, *wfc, *wproj;
-      float *bqkv, *bo, *bfc, *bproj;
-      NormW ln1, ln2;
+      BlockW w;
       // saved activations
       void *x_in, *x_mid;  // residual stream before / between the two sub-blocks: fp32, or fp16 with stream16
       float *stats1, *stats2;
@@ -217,12 +248,7 @@ class Engine {
     act_t *tok = nullptr, *proj16 = nullptr;  // token_embedding [vocab, W], text_projection [W, D]
     float* pos = nullptr;                     // positional_embedding [T, W]
     NormW ln_final;
-    struct Layer {
-      act_t *wqkv, *wo, *wfc, *wproj;
-      float *bqkv, *bo, *bfc, *bproj;
-      NormW ln1, ln2;
-    };
-    std::vector<Layer> layers;
+    std::vector<BlockW> layers;
     int *ids = nullptr, *eot = nullptr;  // [TEXT_CHUNK * T] token ids, [TEXT_CHUNK] row of each sequence's EOT
     void *x0 = nullptr, *x1 = nullptr, *xe = nullptr;  // residual stream ping-pong, gathered EOT rows
     act_t *h16 = nullptr, *qkv = nullptr, *o = nullptr, *u = nullptr, *gact = nullptr, *he = nullptr;
@@ -668,7 +694,9 @@ class Engine {
   FftPlans* fft = nullptr;
   void build_cutouts();
   void build_clip(int i);
-  ConvW load_conv(const std::string& prefix, int cin, int cout, int ks, int cin_real = 0);
+  ConvW load_conv(const std::string& prefix, int cin, int cout, int ks, int cin_real = 0, bool has_bias = true);
+  act_t* pack_conv(const std::vector<float>& w, int cout, int cin, int taps, size_t n, size_t s_tap, size_t s_co,
+                   size_t s_ci, bool flip, int ci0 = 0, int ci1 = INT_MAX);
   // VQGAN encoder (taming Encoder + quant_conv + nearest code): VqganDrawer.init_from_tensor / reapply_from_tensor /
   // get_z_from_tensor (vqgan.py:174-185).  Forward only; built at finalize when the checkpoint carries encoder.* tensors.
   OpList enc_fwd;
@@ -845,11 +873,23 @@ NormW Engine::load_norm(int mod, const std::string& prefix, int c) {
   return n;
 }
 
+// The one conv weight packer: scatters a PyTorch weight w [cout][cin][taps] into a zeroed fp16 operand of n elements,
+// (co, ci, t) to t' s_tap + co s_co + (ci - ci0) s_ci, where t' = t, or taps - 1 - t with flip (a dgrad: dx[p] = sum_t
+// dy[p + off(t)] W[.., flipped t]).  Only the input channels [ci0, ci1) are packed.
+act_t* Engine::pack_conv(const std::vector<float>& w, int cout, int cin, int taps, size_t n, size_t s_tap, size_t s_co,
+                         size_t s_ci, bool flip, int ci0, int ci1) {
+  std::vector<float> f(n, 0.f);
+  for (int co = 0; co < cout; ++co)
+    for (int ci = ci0; ci < std::min(ci1, cin); ++ci)
+      for (int t = 0; t < taps; ++t)
+        f[(flip ? taps - 1 - t : t) * s_tap + co * s_co + (ci - ci0) * s_ci] = w[((size_t)co * cin + ci) * taps + t];
+  return upload_f16(f);
+}
+
 // cin_real < cin: the stored tensor has cin_real input channels and the activation is zero-padded to cin (conv_in: 3 -> 64)
-ConvW Engine::load_conv(const std::string& prefix, int cin, int cout, int ks, int cin_real) {
+ConvW Engine::load_conv(const std::string& prefix, int cin, int cout, int ks, int cin_real, bool has_bias) {
   if (cin_real <= 0) cin_real = cin;
   const HostWeight& w = W(PXR_MOD_VQGAN, prefix + ".weight", {cout, cin_real, ks, ks});
-  const HostWeight& b = W(PXR_MOD_VQGAN, prefix + ".bias", {cout});
   ConvW c;
   c.cin = cin;
   c.cout = cout;
@@ -859,21 +899,10 @@ ConvW Engine::load_conv(const std::string& prefix, int cin, int cout, int ks, in
   c.cin_rows = round_up(cin, 16);
   const int taps = ks * ks;
   if (cin % 64) throw EngineError(-42, "conv '" + prefix + "': input channels must be a multiple of 64");
-  std::vector<float> f((size_t)taps * c.cout_pad * cin, 0.f), d((size_t)taps * c.cin_rows * c.cout_k, 0.f);
-  for (int co = 0; co < cout; ++co)
-    for (int ci = 0; ci < cin_real; ++ci)
-      for (int ty = 0; ty < ks; ++ty)
-        for (int tx = 0; tx < ks; ++tx) {
-          float v = w.data[(((size_t)co * cin_real + ci) * ks + ty) * ks + tx];
-          int t = ty * ks + tx;
-          f[((size_t)t * c.cout_pad + co) * cin + ci] = v;
-          // dgrad: dx[p] = sum_t dy[p + off(t)] * W[.., flipped t]
-          int tf = (ks - 1 - ty) * ks + (ks - 1 - tx);
-          d[((size_t)tf * c.cin_rows + ci) * c.cout_k + co] = v;
-        }
-  c.w = upload_f16(f);
-  c.wd = upload_f16(d);
-  c.bias = upload(b.data);
+  c.w = pack_conv(w.data, cout, cin_real, taps, (size_t)taps * c.cout_pad * cin, (size_t)c.cout_pad * cin, cin, 1, false);
+  c.wd = pack_conv(w.data, cout, cin_real, taps, (size_t)taps * c.cin_rows * c.cout_k, (size_t)c.cin_rows * c.cout_k, 1,
+                   c.cout_k, true);
+  if (has_bias) c.bias = upload(W(PXR_MOD_VQGAN, prefix + ".bias", {cout}).data);
   return c;
 }
 
@@ -1817,6 +1846,154 @@ void Engine::forward_cutouts(int s) {
 }
 
 // ===================================================================================================== CLIP ViT
+// The same tensors under two naming schemes: openai-CLIP's (the CLIP image tower under visual.transformer.resblocks.N,
+// every text tower under transformer.resblocks.N) and timm's (SLIP's image tower): in_proj = attn.qkv (q | k | v, heads
+// contiguous), out_proj = attn.proj, c_fc / c_proj = mlp.fc1 / mlp.fc2, ln_1 / ln_2 = norm1 / norm2.
+Engine::BlockW Engine::load_block(int mod, const std::string& p, int Wd, bool timm) {
+  static const char* const keys[2][10] = {
+      {".attn.in_proj_weight", ".attn.in_proj_bias", ".attn.out_proj.weight", ".attn.out_proj.bias", ".mlp.c_fc.weight",
+       ".mlp.c_fc.bias", ".mlp.c_proj.weight", ".mlp.c_proj.bias", ".ln_1", ".ln_2"},
+      {".attn.qkv.weight", ".attn.qkv.bias", ".attn.proj.weight", ".attn.proj.bias", ".mlp.fc1.weight", ".mlp.fc1.bias",
+       ".mlp.fc2.weight", ".mlp.fc2.bias", ".norm1", ".norm2"}};
+  const char* const* k = keys[timm];
+  BlockW b;
+  b.wqkv = upload_f16(W(mod, p + k[0], {3 * Wd, Wd}).data);
+  b.bqkv = upload(W(mod, p + k[1], {3 * Wd}).data);
+  b.wo = upload_f16(W(mod, p + k[2], {Wd, Wd}).data);
+  b.bo = upload(W(mod, p + k[3], {Wd}).data);
+  b.wfc = upload_f16(W(mod, p + k[4], {4 * Wd, Wd}).data);
+  b.bfc = upload(W(mod, p + k[5], {4 * Wd}).data);
+  b.wproj = upload_f16(W(mod, p + k[6], {Wd, 4 * Wd}).data);
+  b.bproj = upload(W(mod, p + k[7], {Wd}).data);
+  b.ln1 = load_norm(mod, p + k[8], Wd);
+  b.ln2 = load_norm(mod, p + k[9], Wd);
+  return b;
+}
+
+Op Engine::stream_ln_fwd(const void* x, long long ld, const NormW& n, int rows, int Wd, float eps, act_t* y16,
+                         float* stats) const {
+  cudaStream_t cs = st;
+  if (stream16) {
+    const act_t* x16 = static_cast<const act_t*>(x);
+    return [=] { layernorm_forward(x16, ld, nullptr, 1, n.gamma, n.beta, rows, Wd, eps, y16, nullptr, stats, cs); };
+  }
+  const float* x32 = static_cast<const float*>(x);
+  return [=] { layernorm_forward(x32, ld, nullptr, 1, n.gamma, n.beta, rows, Wd, eps, y16, nullptr, stats, cs); };
+}
+
+Op Engine::stream_ln_bwd(const act_t* dy, const void* x, long long ld, const float* stats, const NormW& n, int rows,
+                         int Wd, int accumulate, float* gx, act_t* gx16) const {
+  cudaStream_t cs = st;
+  if (stream16) {
+    const act_t* x16 = static_cast<const act_t*>(x);
+    return [=] { layernorm_backward(dy, x16, ld, nullptr, 1, stats, n.gamma, rows, Wd, accumulate, gx, gx16, cs); };
+  }
+  const float* x32 = static_cast<const float*>(x);
+  return [=] { layernorm_backward(dy, x32, ld, nullptr, 1, stats, n.gamma, rows, Wd, accumulate, gx, gx16, cs); };
+}
+
+void Engine::stream_residual(GemmEpilogue& e, const void* res, void* out) const {
+  if (stream16) {
+    e.res_f16 = static_cast<const act_t*>(res);
+    e.out_f16 = static_cast<act_t*>(out);
+  } else {
+    e.res_f32 = static_cast<const float*>(res);
+    e.out_f32 = static_cast<float*>(out);
+  }
+}
+
+// One pre-norm block, 64-wide heads:  x_mid = x_in + attn(ln_1(x_in)) Wo^T + bo,
+// x_out = x_mid + act(ln_2(x_mid) Wfc^T + bfc) Wproj^T + bproj.  Appends the forward to `fwd` and, when `bwd` is given,
+// the backward (gx16 / gx of x_out -> of x_in, accumulated in place) to *bwd in execution order; returns the attention
+// chain's P (nullptr on the fused paths).
+act_t* Engine::add_block(OpList& fwd, OpList* bwd, const BlockW& w, const BlockIO& b) {
+  const int Wd = 64 * b.heads, M = b.images * b.T, Mr = b.rows;
+  const long long xld = b.ld;
+  fwd.add(1, stream_ln_fwd(b.x_in, Wd, w.ln1, M, Wd, b.eps, b.h16, b.stats1), 0.0, "layernorm_forward");
+  {
+    GemmEpilogue e;
+    e.bias = w.bqkv;
+    e.out_f16 = b.qkv;
+    e.ldc = 3 * Wd;
+    add_gemm(fwd, opK(b.h16, Wd, M, Wd), opK(w.wqkv, Wd, 3 * Wd, Wd), M, 3 * Wd, Wd, e);
+  }
+  OpList attn_bwd;
+  act_t* P = add_attention(fwd, bwd ? &attn_bwd : nullptr, b.qkv, b.o, b.go, b.gqkv, b.images, b.heads, b.T, 64,
+                           1.f / std::sqrt(64.f), true, b.dP, b.causal);
+  {  // x_mid = x_in + O Wo^T + bo
+    GemmEpilogue e;
+    e.bias = w.bo;
+    stream_residual(e, b.x_in, b.x_mid);
+    e.ldc = xld;
+    add_gemm(fwd, opK(b.o, xld, Mr, Wd), opK(w.wo, Wd, Wd, Wd), Mr, Wd, Wd, e);
+  }
+  fwd.add(1, stream_ln_fwd(b.x_mid, xld, w.ln2, Mr, Wd, b.eps, b.h16, b.stats2), 0.0, "layernorm_forward");
+  {  // gact = act(h Wfc^T + bfc), keep the pre-activation u
+    GemmEpilogue e;
+    e.bias = w.bfc;
+    e.act = b.act;
+    e.aux_out = b.u;
+    e.out_f16 = b.gact;
+    e.ldc = 4 * Wd;
+    add_gemm(fwd, opK(b.h16, Wd, Mr, Wd), opK(w.wfc, Wd, 4 * Wd, Wd), Mr, 4 * Wd, Wd, e);
+  }
+  {  // x_out = x_mid + gact Wproj^T + bproj
+    GemmEpilogue e;
+    e.bias = w.bproj;
+    stream_residual(e, b.x_mid, b.x_out);
+    e.ldc = xld;
+    add_gemm(fwd, opK(b.gact, 4 * Wd, Mr, 4 * Wd), opK(w.wproj, 4 * Wd, Wd, 4 * Wd), Mr, Wd, 4 * Wd, e);
+  }
+  if (!bwd) return P;
+  {  // g4 = (gx Wproj) * act'(u)
+    GemmEpilogue e;
+    e.act = b.act == ACT_GELU ? ACT_GELU_BWD : ACT_QUICKGELU_BWD;
+    e.aux_in = b.u;
+    e.out_f16 = b.g4;
+    e.ldc = 4 * Wd;
+    add_gemm(*bwd, opK(b.gx16, xld, Mr, Wd), opMN(w.wproj, 4 * Wd, 4 * Wd, Wd), Mr, 4 * Wd, Wd, e);
+  }
+  {  // gh = g4 Wfc
+    GemmEpilogue e;
+    e.out_f16 = b.gh;
+    e.ldc = Wd;
+    add_gemm(*bwd, opK(b.g4, 4 * Wd, Mr, 4 * Wd), opMN(w.wfc, Wd, Wd, 4 * Wd), Mr, Wd, 4 * Wd, e);
+  }
+  bwd->add(1, stream_ln_bwd(b.gh, b.x_mid, xld, b.stats2, w.ln2, Mr, Wd, 1, b.gx, b.gx16), 0.0, "layernorm_backward");
+  if (Mr < M) {  // the attention backward reads dO = go for every token: zero outside the tail's rows
+    const size_t go_bytes = (size_t)M * Wd * sizeof(act_t);
+    act_t* go = b.go;
+    cudaStream_t cs = st;
+    bwd->add(1, [=] { cudaMemsetAsync(go, 0, go_bytes, cs); }, 0.0, "memset go");
+  }
+  {  // go = gx Wo
+    GemmEpilogue e;
+    e.out_f16 = b.go;
+    e.ldc = xld;
+    add_gemm(*bwd, opK(b.gx16, xld, Mr, Wd), opMN(w.wo, Wd, Wd, Wd), Mr, Wd, Wd, e);
+  }
+  bwd->append(attn_bwd);
+  {  // gh = gqkv Wqkv
+    GemmEpilogue e;
+    e.out_f16 = b.gh;
+    e.ldc = Wd;
+    add_gemm(*bwd, opK(b.gqkv, 3 * Wd, M, 3 * Wd), opMN(w.wqkv, Wd, Wd, 3 * Wd), M, Wd, 3 * Wd, e);
+  }
+  bwd->add(1, stream_ln_bwd(b.gh, b.x_in, Wd, b.stats1, w.ln1, M, Wd, 1, b.gx, b.gx16), 0.0, "layernorm_backward");
+  return P;
+}
+
+// A tower's head: LayerNorm of one row per sequence (`rows` rows ld apart in the stream x), then e = ln @ proj against
+// the fp16 projection [W, D] read MN-major, fp32 embeddings [rows, D]
+void Engine::add_head(OpList& l, const void* x, long long ld, int rows, const NormW& n, float eps, act_t* h16,
+                      float* stats, const act_t* proj16, int Wd, int D, float* out) {
+  l.add(1, stream_ln_fwd(x, ld, n, rows, Wd, eps, h16, stats), 0.0, "layernorm_forward");
+  GemmEpilogue e;
+  e.out_f32 = out;
+  e.ldc = D;
+  add_gemm(l, opK(h16, Wd, rows, Wd), opMN(proj16, D, D, Wd), rows, D, Wd, e);
+}
+
 void Engine::build_clip(int i) {
   Clip& C = clip[i];
   if (C.tower == PXR_TOWER_CLIP_RESNET) return build_resnet(i);
@@ -1860,7 +2037,6 @@ void Engine::build_clip(int i) {
   if (timm) C.conv1_b = upload(W(mod, "visual.patch_embed.proj.bias", {Wd}).data);
   C.cls = upload(w_cls.data);
   C.pos = upload(w_pos.data);
-  C.proj = upload(W(mod, k_proj, {Wd, D}).data);
   C.proj16 = upload_f16(W(mod, k_proj, {Wd, D}).data);
   if (!timm) C.ln_pre = load_norm(mod, "visual.ln_pre", Wd);
   C.ln_post = load_norm(mod, timm ? "visual.norm" : "visual.ln_post", Wd);
@@ -1901,30 +2077,8 @@ void Engine::build_clip(int i) {
   C.gcls = dalloc<act_t>((size_t)B * Wd);
   void* x_cur = xalloc();
   void* x0 = x_cur;
-  // LayerNorm on either stream type
-  auto ln_fwd = [s16, cs, eps](const void* x, long long stride, const float* pos, int T_, const NormW& nw, int rows,
-                               int W_, act_t* y16, float* y32, float* stats) {
-    if (s16) layernorm_forward(static_cast<const act_t*>(x), stride, pos, T_, nw.gamma, nw.beta, rows, W_, eps, y16, y32, stats, cs);
-    else layernorm_forward(static_cast<const float*>(x), stride, pos, T_, nw.gamma, nw.beta, rows, W_, eps, y16, y32, stats, cs);
-  };
-  auto ln_bwd = [s16, cs](const act_t* dy, const void* x, long long stride, const float* stats, const NormW& nw, int rows,
-                          int W_, int accumulate, float* gx, act_t* gx16) {
-    if (s16) layernorm_backward(dy, static_cast<const act_t*>(x), stride, nullptr, 1, stats, nw.gamma, rows, W_, accumulate, gx, gx16, cs);
-    else layernorm_backward(dy, static_cast<const float*>(x), stride, nullptr, 1, stats, nw.gamma, rows, W_, accumulate, gx, gx16, cs);
-  };
-  // residual epilogue x_out = x_res + A B^T + bias on either stream type
-  auto residual_epilogue = [s16](GemmEpilogue& e, const void* res, void* out) {
-    if (s16) {
-      e.res_f16 = static_cast<const act_t*>(res);
-      e.out_f16 = static_cast<act_t*>(out);
-    } else {
-      e.res_f32 = static_cast<const float*>(res);
-      e.out_f32 = static_cast<float*>(out);
-    }
-  };
   C.layers.resize(L);
-  const float scale = 1.f / std::sqrt((float)d);
-  std::vector<OpList> attn_bwd(L);  // per layer, built with the forward, spliced into the backward
+  std::vector<OpList> block_bwd(L);  // per layer, built with the forward, spliced into the backward in reverse
 
   // ---- forward: patch embed (conv1 as GEMM over im2col'd patches, written straight into the token rows 1..np)
   {
@@ -1947,83 +2101,46 @@ void Engine::build_clip(int i) {
         layernorm_forward(c->t, Wd, c->pos, T, c->ln_pre.gamma, c->ln_pre.beta, M, Wd, eps, xo16, xo32, c->stats_pre, cs);
       }, 0.0, "layernorm_forward");
   }
+  BlockIO b;  // what every layer shares; the loop sets the rest
+  b.h16 = C.h16;
+  b.gact = C.gact;
+  b.images = B;
+  b.heads = Hh;
+  b.T = T;
+  b.act = timm ? ACT_GELU : ACT_QUICKGELU;
+  b.eps = eps;
+  b.causal = false;
+  b.go = C.go;
+  b.gqkv = C.gqkv;
+  b.dP = C.dP;
+  b.g4 = C.g4;
+  b.gh = C.gh;
+  b.gx16 = C.gx16;
+  b.gx = C.gx;
   for (int l = 0; l < L; ++l) {
     Clip::Layer& Ly = C.layers[l];
-    // the same tensors under each tower's names: in_proj = attn.qkv (q | k | v, heads contiguous), out_proj = attn.proj,
-    // c_fc / c_proj = mlp.fc1 / mlp.fc2, ln_1 / ln_2 = norm1 / norm2
-    std::string p = (timm ? "visual.blocks." : "visual.transformer.resblocks.") + std::to_string(l);
-    Ly.wqkv = upload_f16(W(mod, p + (timm ? ".attn.qkv.weight" : ".attn.in_proj_weight"), {3 * Wd, Wd}).data);
-    Ly.bqkv = upload(W(mod, p + (timm ? ".attn.qkv.bias" : ".attn.in_proj_bias"), {3 * Wd}).data);
-    Ly.wo = upload_f16(W(mod, p + (timm ? ".attn.proj.weight" : ".attn.out_proj.weight"), {Wd, Wd}).data);
-    Ly.bo = upload(W(mod, p + (timm ? ".attn.proj.bias" : ".attn.out_proj.bias"), {Wd}).data);
-    Ly.wfc = upload_f16(W(mod, p + (timm ? ".mlp.fc1.weight" : ".mlp.c_fc.weight"), {4 * Wd, Wd}).data);
-    Ly.bfc = upload(W(mod, p + (timm ? ".mlp.fc1.bias" : ".mlp.c_fc.bias"), {4 * Wd}).data);
-    Ly.wproj = upload_f16(W(mod, p + (timm ? ".mlp.fc2.weight" : ".mlp.c_proj.weight"), {Wd, 4 * Wd}).data);
-    Ly.bproj = upload(W(mod, p + (timm ? ".mlp.fc2.bias" : ".mlp.c_proj.bias"), {Wd}).data);
-    Ly.ln1 = load_norm(mod, p + (timm ? ".norm1" : ".ln_1"), Wd);
-    Ly.ln2 = load_norm(mod, p + (timm ? ".norm2" : ".ln_2"), Wd);
-    Ly.x_in = x_cur;
-    Ly.x_mid = xalloc();
-    void* x_next = xalloc();
-    Ly.stats1 = dalloc<float>((size_t)M * 2);
-    Ly.stats2 = dalloc<float>((size_t)M * 2);
-    Ly.qkv = dalloc<act_t>((size_t)M * 3 * Wd);
-    Ly.u = dalloc<act_t>((size_t)M * 4 * Wd);
+    Ly.w = load_block(mod, (timm ? "visual.blocks." : "visual.transformer.resblocks.") + std::to_string(l), Wd, timm);
+    b.x_in = Ly.x_in = x_cur;
+    b.x_mid = Ly.x_mid = xalloc();
+    b.x_out = x_cur = xalloc();
+    b.stats1 = Ly.stats1 = dalloc<float>((size_t)M * 2);
+    b.stats2 = Ly.stats2 = dalloc<float>((size_t)M * 2);
+    b.qkv = Ly.qkv = dalloc<act_t>((size_t)M * 3 * Wd);
+    b.u = Ly.u = dalloc<act_t>((size_t)M * 4 * Wd);
     if (fuse_attn) Ly.o = dalloc<act_t>((size_t)M * Wd);
-    Clip::Layer ly = Ly;
-    Clip* c = &C;
-    C.fwd.add(1, [=] { ln_fwd(ly.x_in, Wd, nullptr, T, ly.ln1, M, Wd, c->h16, nullptr, ly.stats1); }, 0.0, "layernorm_forward");
-    {
-      GemmEpilogue e;
-      e.bias = ly.bqkv;
-      e.out_f16 = ly.qkv;
-      e.ldc = 3 * Wd;
-      add_gemm(C.fwd, opK(C.h16, Wd, M, Wd), opK(ly.wqkv, Wd, 3 * Wd, Wd), M, 3 * Wd, Wd, e);
-    }
-    Ly.P = add_attention(C.fwd, &attn_bwd[l], ly.qkv, fuse_attn ? ly.o : C.o16, C.go, C.gqkv, B, Hh, T, d, scale, true,
-                         C.dP);
+    b.o = fuse_attn ? Ly.o : C.o16;
     // Last layer: only the class token's row of every image reaches ln_post / proj (slip.py:62-66 ->
     // VisionTransformer.forward takes x[:, 0, :]), and everything after the attention is row-wise -- out_proj, ln_2, the MLP
     // and their backward run on those B rows (row pitch T * W inside the [M, W] buffers) instead of on all M = B T rows.
     // Exact: the other rows' outputs are never read and their gradients are zero.  PXR_CLIP_LAST_CLS=0 computes all rows.
     const bool cls_only = clip_last_cls && l == L - 1;
-    const int Mr = cls_only ? B : M;                                     // rows of the row-wise tail of this layer
-    const long long xld = cls_only ? (long long)T * Wd : (long long)Wd;   // their pitch inside the token-major buffers
-    {  // x_mid = x_in + O Wo^T + bo
-      GemmEpilogue e;
-      e.bias = ly.bo;
-      residual_epilogue(e, ly.x_in, ly.x_mid);
-      e.ldc = xld;
-      add_gemm(C.fwd, opK(fuse_attn ? ly.o : C.o16, xld, Mr, Wd), opK(ly.wo, Wd, Wd, Wd), Mr, Wd, Wd, e);
-    }
-    C.fwd.add(1, [=] { ln_fwd(ly.x_mid, xld, nullptr, T, ly.ln2, Mr, Wd, c->h16, nullptr, ly.stats2); }, 0.0, "layernorm_forward");
-    {  // gact = quickgelu / gelu(h Wfc^T + bfc), keep pre-activation u   (h16 / gact / u hold the Mr rows compactly)
-      GemmEpilogue e;
-      e.bias = ly.bfc;
-      e.act = timm ? ACT_GELU : ACT_QUICKGELU;
-      e.aux_out = ly.u;
-      e.out_f16 = C.gact;
-      e.ldc = 4 * Wd;
-      add_gemm(C.fwd, opK(C.h16, Wd, Mr, Wd), opK(ly.wfc, Wd, 4 * Wd, Wd), Mr, 4 * Wd, Wd, e);
-    }
-    {  // x_next = x_mid + gact Wproj^T + bproj
-      GemmEpilogue e;
-      e.bias = ly.bproj;
-      residual_epilogue(e, ly.x_mid, x_next);
-      e.ldc = xld;
-      add_gemm(C.fwd, opK(C.gact, 4 * Wd, Mr, 4 * Wd), opK(ly.wproj, 4 * Wd, Wd, 4 * Wd), Mr, Wd, 4 * Wd, e);
-    }
-    x_cur = x_next;
+    b.rows = cls_only ? B : M;
+    b.ld = cls_only ? (long long)T * Wd : (long long)Wd;
+    Ly.P = add_block(C.fwd, &block_bwd[l], Ly.w, b);
   }
   C.x_out = x_cur;
-  {  // head: ln_post on the class-token rows (row stride T*W), then e = ln @ proj as a GEMM (proj [W, D] is MN-major)
-    Clip* c = &C;
-    C.fwd.add(1, [=] { ln_fwd(c->x_out, (long long)T * Wd, nullptr, T, c->ln_post, B, Wd, c->hcls, nullptr, c->stats_post); }, 0.0, "layernorm_forward");
-    GemmEpilogue e;
-    e.out_f32 = C.e;
-    e.ldc = D;
-    add_gemm(C.fwd, opK(C.hcls, Wd, B, Wd), opMN(C.proj16, D, D, Wd), B, D, Wd, e);
-  }
+  // head: ln_post on the class-token rows (row stride T*W), then e = ln @ proj
+  add_head(C.fwd, C.x_out, (long long)T * Wd, B, C.ln_post, eps, C.hcls, C.stats_post, C.proj16, Wd, D, C.e);
 
   // ---- backward (execution order).  Weight operands of the dgrad GEMMs are MN-major views of the forward weights.
   {  // head backward: gcls = de proj^T (proj [W, D] read K-major: n = W rows, k = D), then LN backward on class rows
@@ -2033,52 +2150,14 @@ void Engine::build_clip(int i) {
     e.ldc = Wd;
     add_gemm(C.bwd, opK(C.de16, D, B, D), opK(C.proj16, D, Wd, D), B, Wd, D, e);
     const size_t nbytes32 = (size_t)M * Wd * sizeof(float), nbytes16 = (size_t)M * Wd * sizeof(act_t);
+    const Op ln_bwd = stream_ln_bwd(C.gcls, C.x_out, (long long)T * Wd, C.stats_post, C.ln_post, B, Wd, 0, C.gx, C.gx16);
     C.bwd.add(1, [=] {
       if (c->gx) cudaMemsetAsync(c->gx, 0, nbytes32, cs);
       cudaMemsetAsync(c->gx16, 0, nbytes16, cs);
-      ln_bwd(c->gcls, c->x_out, (long long)T * Wd, c->stats_post, c->ln_post, B, Wd, 0, c->gx, c->gx16);
+      ln_bwd();
     });
   }
-  for (int l = L - 1; l >= 0; --l) {
-    Clip::Layer ly = C.layers[l];
-    Clip* c = &C;
-    const bool cls_only = clip_last_cls && l == L - 1;  // see the forward: the row-wise tail of the last layer, class rows only
-    const int Mr = cls_only ? B : M;
-    const long long xld = cls_only ? (long long)T * Wd : (long long)Wd;
-    {  // g4 = (gx Wproj) * quickgelu'(u) / gelu'(u)
-      GemmEpilogue e;
-      e.act = timm ? ACT_GELU_BWD : ACT_QUICKGELU_BWD;
-      e.aux_in = ly.u;
-      e.out_f16 = C.g4;
-      e.ldc = 4 * Wd;
-      add_gemm(C.bwd, opK(C.gx16, xld, Mr, Wd), opMN(ly.wproj, 4 * Wd, 4 * Wd, Wd), Mr, 4 * Wd, Wd, e);
-    }
-    {  // gh = g4 Wfc
-      GemmEpilogue e;
-      e.out_f16 = C.gh;
-      e.ldc = Wd;
-      add_gemm(C.bwd, opK(C.g4, 4 * Wd, Mr, 4 * Wd), opMN(ly.wfc, Wd, Wd, 4 * Wd), Mr, Wd, 4 * Wd, e);
-    }
-    C.bwd.add(1, [=] { ln_bwd(c->gh, ly.x_mid, xld, ly.stats2, ly.ln2, Mr, Wd, 1, c->gx, c->gx16); }, 0.0, "layernorm_backward");
-    if (cls_only) {  // the attention backward reads dO = go for every token: zero outside the class rows
-      const size_t go_bytes = (size_t)M * Wd * sizeof(act_t);
-      C.bwd.add(1, [=] { cudaMemsetAsync(c->go, 0, go_bytes, cs); }, 0.0, "memset go");
-    }
-    {  // go = gx Wo
-      GemmEpilogue e;
-      e.out_f16 = C.go;
-      e.ldc = xld;
-      add_gemm(C.bwd, opK(C.gx16, xld, Mr, Wd), opMN(ly.wo, Wd, Wd, Wd), Mr, Wd, Wd, e);
-    }
-    C.bwd.append(attn_bwd[l]);
-    {  // gh = gqkv Wqkv
-      GemmEpilogue e;
-      e.out_f16 = C.gh;
-      e.ldc = Wd;
-      add_gemm(C.bwd, opK(C.gqkv, 3 * Wd, M, 3 * Wd), opMN(ly.wqkv, Wd, Wd, 3 * Wd), M, Wd, 3 * Wd, e);
-    }
-    C.bwd.add(1, [=] { ln_bwd(c->gh, ly.x_in, Wd, ly.stats1, ly.ln1, M, Wd, 1, c->gx, c->gx16); }, 0.0, "layernorm_backward");
-  }
+  for (int l = L - 1; l >= 0; --l) C.bwd.append(block_bwd[l]);
   {  // ln_pre backward (x = t + pos), then patch-embed dgrad on token rows 1..np of every image.  timm: x0 = t + pos_embed,
      // so the stream gradient in gx16 already is d/dt
     Clip* c = &C;

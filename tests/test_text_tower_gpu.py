@@ -124,15 +124,17 @@ def tower(request):
     return sd, D, ids, want
 
 
+@pytest.mark.parametrize("stream", [16, 32])
 @pytest.mark.parametrize("fused", [True, False])
-def test_full_depth_tower_against_float64(monkeypatch, tower, fused):
+def test_full_depth_tower_against_float64(monkeypatch, tower, fused, stream):
     sd, D, ids, want = tower
     monkeypatch.setenv("PXR_FUSED_ATTN", "1" if fused else "0")
+    monkeypatch.setenv("PXR_CLIP_STREAM", str(stream))
     eng = _engine(sd, D)
     assert eng.text_tower(0) == dict(width=sd["token_embedding.weight"].shape[1], layers=12, ctx=77, out_dim=D)
     w = sd["token_embedding.weight"].shape[1]
     for n in (1, 3, 80):
-        _compare(eng.encode_text(0, ids[:n]), want[:n], f"W={w} fused={fused} n={n}")
+        _compare(eng.encode_text(0, ids[:n]), want[:n], f"W={w} fused={fused} stream={stream} n={n}")
     # chunking: 80 sequences in one call are the rows of the calls on each 32-sequence chunk, and of single calls
     all80 = eng.encode_text(0, ids)
     parts = torch.cat([eng.encode_text(0, ids[c:c + 32]) for c in range(0, 80, 32)])
