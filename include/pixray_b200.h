@@ -380,6 +380,9 @@ typedef struct {
   /* act 5: out = (alpha acc + bias + residual) * (aux_in > 0 ? 1 : 0.2) in the columns >= act_col0, aux_in = the saved
    * post-activation (same layout as the output); the columns below act_col0 are stored unmasked */
   int act_col0;
+  /* pxr_test_conv only: 1 runs the plan on the 288-thread kernel (tiles at most 128 wide) even when the 384-thread one
+   * would take it, so that a test can compare the two on the same inputs.  0: the kernel the engine would use. */
+  int narrow_kernel;
   /* > 1: split-K.  The plan runs ceil(nkb / ceil(nkb / k_splits)) splits of ceil(nkb / k_splits) 64-deep k-blocks each and
    * writes split s's fp32 partial sums to slab s of out_f32 (slab pitch M * ldc for a GEMM, H * W * ldc for a conv);
    * needs one unbatched image, out_f32 only, no bias, residual or activation.  0 or 1: one split. */

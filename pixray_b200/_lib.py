@@ -60,7 +60,7 @@ class TestGemmDesc(C.Structure):
         ("out_f32", C.c_void_p), ("out_f16", C.c_void_p),
         ("ldc", C.c_longlong), ("c_bs0", C.c_longlong), ("c_bs1", C.c_longlong),
         ("stream", C.c_void_p), ("repeat", C.c_int), ("cta_group", C.c_int), ("tma_epi", C.c_int),
-        ("act_col0", C.c_int), ("k_splits", C.c_int),
+        ("act_col0", C.c_int), ("narrow_kernel", C.c_int), ("k_splits", C.c_int),
     ]
 
 

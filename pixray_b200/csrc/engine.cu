@@ -483,8 +483,8 @@ class Engine {
   }
   // Tile width by a wave-quantisation cost model: a persistent grid of num_sms CTAs runs ceil(tiles / num_sms) waves
   // of tiles whose cost grows with bn (plus a fixed per-tile overhead); e.g. M = 12608, N = 768 is 297 tiles of 256
-  // (3 waves for 2.007 waves of work) but 396 tiles of 192 (3 cheaper waves).  wide: the GEMM may use 192- and 256-wide
-  // tiles (gemm_wide_ok); every other GEMM and convolution has tiles of at most 128 columns.
+  // (3 waves for 2.007 waves of work) but 396 tiles of 192 (3 cheaper waves).  wide: the GEMM or convolution may use
+  // 192- and 256-wide tiles (gemm_wide_ok); every other one has tiles of at most 128 columns.
   int pick_bn(int N, bool b_mn, long long m_tiles, bool wide = false) const {
     const int step = b_mn ? 64 : 16;
     {  // PXR_GEMM_BN="3072:256,768:192": tile width by output width, for A/B measurements of the cost model's choices
@@ -598,6 +598,11 @@ class Engine {
     snprintf(kind, sizeof kind, "conv%dx%d", ks, ks);
     const int nkb = ks * ks * cin / 64;
     const int splits = batch > 1 ? 1 : splitk_count(e, (long long)H * Wd, n_out, nkb, m_tiles * ((n_out + bn - 1) / bn));
+    if (splits == 1 && cout_pad >= 64) {  // a conv the 384-thread kernel takes may also use 192- / 256-wide tiles
+      GemmOperand A;
+      A.mode = OP_CONV;
+      if (gemm_wide_ok(A, n_out, e, fmt)) bn = std::min(pick_bn(n_out, false, m_tiles, true), cout_pad);
+    }
     auto plan = std::make_shared<GemmPlan>();
     char buf[256] = {0};
     if (splits > 1) {

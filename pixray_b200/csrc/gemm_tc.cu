@@ -832,9 +832,11 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tce_kernel(const __grid_
   gemm_body<false, MODE, NF>(p);
 }
 
-// -------------------------------------------------------------------------------- wide kernel: 128 x 192 / 128 x 256
-// For fp16 GEMMs with a K-major, unbatched A, no split-K and a tensor-map epilogue other than TE_RES32 (the ViT linear
-// layers and their dgrads), a requested block_n of 192 or 256 runs here instead of in gemm_body.
+// ----------------------------------------------------------------- wide kernel: 128 x 192 / 128 x 256, conv 128 x 128
+// For fp16 GEMMs with no split-K and a tensor-map epilogue with fp16 outputs (gemm_wide_ok), a requested block_n of 192
+// or 256 runs here instead of in gemm_body: the ViT linear layers and their dgrads (A K-major and unbatched), and the
+// implicit-GEMM convolutions with bias and / or fp16 residual (the VQGAN decoder, the vdiff U-Net), which also run here
+// at 128 columns.
 //   * 384 threads.  Warpgroup 0 is the producer: one lane walks producer_tiles, the warpgroup drops to 40 registers.
 //     Warpgroups 1 and 2 own tile rows [0, 64) and [64, 128) and rise to 232 registers: 40 * 128 + 232 * 256 = 64,512
 //     = 168 * 384, what one CTA holds at __launch_bounds__(384, 1).  A 64 x 256 fp32 accumulator is 128 of them.
@@ -847,9 +849,13 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tce_kernel(const __grid_
 //     pre-activation) arrives by TMA in the same box up to two chunks ahead and is read into the fragment layout with
 //     ldmatrix.  No staged fp32 tile and no barrier between the consumer warpgroups; the producer refills the ring for
 //     the next tile while they run it.
+//   * Convolutions: the producer walks producer_tiles<OP_CONV> (one tap-shifted (C, W, H, image) box per k-block, halo
+//     zero-filled), so every output sums in the k order of gemm_body.  A warp's 16 tile rows are 16 / tile_w image rows
+//     of tile_w pixels: its boxes are {64, tile_w, 16 / tile_w, 1} at (col, w0, h0 + r / tile_w, image), and TMA clips
+//     ragged W and H.
 // Shared memory (227 KiB = 232,448 bytes): 1 KiB alignment slack, the stage ring, GEMM_BAR_BYTES of barriers and two
 // 2 KiB boxes per consumer warp (32 KiB); the ring gets the remaining 197,632 bytes: 4 stages of 48 KiB at BN = 256,
-// 4 of 40 KiB at BN = 192.
+// 4 of 40 KiB at BN = 192, 6 of 32 KiB at BN = 128.
 constexpr int WB_BYTES = 2048;  // one box: 16 rows x 64 fp16 columns
 constexpr int WB_BOXES = 2;     // per consumer warp
 constexpr int WIDE_CONSUMER_WARPS = 8;
@@ -881,7 +887,8 @@ __device__ __forceinline__ void mma_tile_wide(float (&acc)[BN / 2], int wg, int 
       const uint64_t bd = b_desc0 + stage * (stage_bytes >> 4) + k * b_kstep;
       const uint32_t scale_d = (kb | k) ? 1u : 0u;
       if constexpr (BN == 256) wgmma_m64n256<0, TB>(acc, ad, bd, scale_d);
-      else wgmma_m64n192<0, TB>(acc, ad, bd, scale_d);
+      else if constexpr (BN == 192) wgmma_m64n192<0, TB>(acc, ad, bd, scale_d);
+      else wgmma_m64n128<0, TB>(acc, ad, bd, scale_d);
     }
     wgmma_commit();
     if (kb == 0) first();
@@ -897,20 +904,30 @@ __device__ __forceinline__ void mma_tile_wide(float (&acc)[BN / 2], int wg, int 
   if (prev >= 0 && elected) mbar_arrive(&empty_bar[prev]);
 }
 
-// TMA load of the input tensor's 64-column chunk at `col` into one box of this warp (lane 0)
-__device__ __forceinline__ void wide_in_load(const GemmParams& p, uint64_t* bar, uint8_t* box, int col, int row0,
-                                             const TileCoord& t) {
-  mbar_arrive_expect_tx(bar, WB_BYTES);
-  tma_load_4d(&p.tma_d, bar, box, col, row0, t.b0, t.b1);
+// Tensor-map coordinates (after the column) of one consumer warp's 16 tile rows [r, r + 16): (row, b0, b1) or, for a
+// convolution, (w, h, image).
+struct WideRows {
+  int c1, c2, c3;
+};
+template <int AM>
+__device__ __forceinline__ WideRows wide_rows(const GemmParams& p, const TileCoord& t, int r) {
+  if (AM == OP_CONV) return {t.w0, t.h0 + r / p.tile_w, t.z};
+  return {t.m0 + r, t.b0, t.b1};
 }
 
-// One tile's epilogue for one consumer warp: rows [row0, row0 + 16) of the output, the 64-column chunks with at least one
+// TMA load of the input tensor's 64-column chunk at `col` into one box of this warp (lane 0)
+__device__ __forceinline__ void wide_in_load(const GemmParams& p, uint64_t* bar, uint8_t* box, int col, const WideRows& w) {
+  mbar_arrive_expect_tx(bar, WB_BYTES);
+  tma_load_4d(&p.tma_d, bar, box, col, w.c1, w.c2, w.c3);
+}
+
+// One tile's epilogue for one consumer warp: its 16 rows of the output (at `rows`), the 64-column chunks with at least one
 // column inside N.  `cnt` counts the chunks this warp has processed: chunk j of the tile goes to box (cnt + j) % 2 (the
 // forward activations use both boxes for every chunk).  in_ph: the parity of each box's input barrier.
 template <int MODE, int BN>
 __device__ __forceinline__ void wide_epilogue_tile(const GemmParams& p, const TileCoord& t, const float (&acc)[BN / 2],
-                                                   uint8_t* wbuf, uint64_t* in_bar, int row0, int lane, uint32_t& cnt,
-                                                   uint32_t& in_ph) {
+                                                   uint8_t* wbuf, uint64_t* in_bar, const WideRows& rows, int lane,
+                                                   uint32_t& cnt, uint32_t& in_ph) {
   constexpr bool ACT_FWD = (MODE == TE_GELU || MODE == TE_ERF_GELU);
   constexpr bool IN = (MODE == TE_RES16 || MODE == TE_GELU_BWD || MODE == TE_ERF_GELU_BWD);
   const int nch = (min(p.N - t.n0, BN) + 63) / 64;
@@ -971,15 +988,15 @@ __device__ __forceinline__ void wide_epilogue_tile(const GemmParams& p, const Ti
       __syncwarp();
       if (lane == 0) {
         if (ACT_FWD) {
-          tma_store_4d(&p.tma_d, wbuf, col, row0, t.b0, t.b1);
-          tma_store_4d(&p.tma_c, wbuf + WB_BYTES, col, row0, t.b0, t.b1);
+          tma_store_4d(&p.tma_d, wbuf, col, rows.c1, rows.c2, rows.c3);
+          tma_store_4d(&p.tma_c, wbuf + WB_BYTES, col, rows.c1, rows.c2, rows.c3);
         } else {
-          tma_store_4d(&p.tma_c, wbuf + b * WB_BYTES, col, row0, t.b0, t.b1);
+          tma_store_4d(&p.tma_c, wbuf + b * WB_BYTES, col, rows.c1, rows.c2, rows.c3);
         }
         bulk_commit_group();
         if (IN && j + 2 < nch) {
           bulk_wait_group_read<0>();  // the store just issued has read the box
-          wide_in_load(p, &in_bar[b], wbuf + b * WB_BYTES, col + 128, row0, t);
+          wide_in_load(p, &in_bar[b], wbuf + b * WB_BYTES, col + 128, rows);
         }
       }
     }
@@ -987,7 +1004,7 @@ __device__ __forceinline__ void wide_epilogue_tile(const GemmParams& p, const Ti
   cnt += nch;
 }
 
-template <int MODE, int BN, int TB>
+template <int MODE, int BN, int TB, int AM>
 __global__ void __launch_bounds__(GEMM_WIDE_THREADS, 1) gemm_wide_kernel(const __grid_constant__ GemmParams p) {
   pdl_launch_dependents();
   extern __shared__ uint8_t smem_raw[];
@@ -1018,7 +1035,7 @@ __global__ void __launch_bounds__(GEMM_WIDE_THREADS, 1) gemm_wide_kernel(const _
 
   if (threadIdx.x < 128) {
     setmaxnreg_dec<40>();
-    if (threadIdx.x == 0) producer_tiles<OP_KMAJOR, TB ? OP_MNMAJOR : OP_KMAJOR>(p, smem, full_bar, empty_bar, stage_bytes);
+    if (threadIdx.x == 0) producer_tiles<AM, TB ? OP_MNMAJOR : OP_KMAJOR>(p, smem, full_bar, empty_bar, stage_bytes);
     return;
   }
   setmaxnreg_inc<232>();
@@ -1033,16 +1050,16 @@ __global__ void __launch_bounds__(GEMM_WIDE_THREADS, 1) gemm_wide_kernel(const _
   float acc[BN / 2];
   for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
     const TileCoord t = decode_tile(p, tile);
-    const int row0 = t.m0 + 64 * wg + 16 * (cw & 3);
+    const WideRows rows = wide_rows<AM>(p, t, 64 * wg + 16 * (cw & 3));
     mma_tile_wide<BN, TB>(acc, wg, p.num_k_blocks, p.stages, smem0, full0, empty_bar, stage, phase, [&] {
       if (IN && lane == 0) {  // the first two input chunks, while the rest of the tile's k-blocks run
         const int nch = (min(p.N - t.n0, BN) + 63) / 64;
         bulk_wait_group_read<0>();  // the previous tile's stores have read the boxes
         for (int j = 0; j < WB_BOXES && j < nch; ++j)
-          wide_in_load(p, &in_bar[(cnt + j) & 1], wbuf + ((cnt + j) & 1) * WB_BYTES, t.n0 + 64 * j, row0, t);
+          wide_in_load(p, &in_bar[(cnt + j) & 1], wbuf + ((cnt + j) & 1) * WB_BYTES, t.n0 + 64 * j, rows);
       }
     });
-    wide_epilogue_tile<MODE, BN>(p, t, acc, wbuf, in_bar, row0, lane, cnt, in_ph);
+    wide_epilogue_tile<MODE, BN>(p, t, acc, wbuf, in_bar, rows, lane, cnt, in_ph);
   }
   if (lane == 0) bulk_wait_group<0>();
 }
@@ -1050,11 +1067,19 @@ __global__ void __launch_bounds__(GEMM_WIDE_THREADS, 1) gemm_wide_kernel(const _
 template <int BN, int TB>
 void (*wide_kernel(const GemmParams& p))(GemmParams) {
   switch (p.tma_epi) {
-    case TE_F16: return gemm_wide_kernel<TE_F16, BN, TB>;
-    case TE_RES16: return gemm_wide_kernel<TE_RES16, BN, TB>;
-    case TE_GELU: return gemm_wide_kernel<TE_GELU, BN, TB>;
-    case TE_GELU_BWD: return gemm_wide_kernel<TE_GELU_BWD, BN, TB>;
-    case TE_ERF_GELU: return gemm_wide_kernel<TE_ERF_GELU, BN, TB>;
+    case TE_F16: return gemm_wide_kernel<TE_F16, BN, TB, OP_KMAJOR>;
+    case TE_RES16: return gemm_wide_kernel<TE_RES16, BN, TB, OP_KMAJOR>;
+    case TE_GELU: return gemm_wide_kernel<TE_GELU, BN, TB, OP_KMAJOR>;
+    case TE_GELU_BWD: return gemm_wide_kernel<TE_GELU_BWD, BN, TB, OP_KMAJOR>;
+    case TE_ERF_GELU: return gemm_wide_kernel<TE_ERF_GELU, BN, TB, OP_KMAJOR>;
+    default: return nullptr;
+  }
+}
+template <int BN>
+void (*wide_conv_kernel(const GemmParams& p))(GemmParams) {
+  switch (p.tma_epi) {
+    case TE_F16: return gemm_wide_kernel<TE_F16, BN, 0, OP_CONV>;
+    case TE_RES16: return gemm_wide_kernel<TE_RES16, BN, 0, OP_CONV>;
     default: return nullptr;
   }
 }
@@ -1079,6 +1104,11 @@ void (*plain_kernel(const GemmParams& p))(GemmParams) {
   return erf ? gemm_tc_kernel<NF, true> : gemm_tc_kernel<NF>;
 }
 void (*kernel_for(const GemmParams& p))(GemmParams) {
+  if (p.wide && p.a_mode == OP_CONV) {
+    if (p.block_n == 256) return wide_conv_kernel<256>(p);
+    if (p.block_n == 192) return wide_conv_kernel<192>(p);
+    return wide_conv_kernel<128>(p);
+  }
   if (p.block_n == 256) return p.b_mode == OP_MNMAJOR ? wide_kernel<256, 1>(p) : wide_kernel<256, 0>(p);
   if (p.block_n == 192) return p.b_mode == OP_MNMAJOR ? wide_kernel<192, 1>(p) : wide_kernel<192, 0>(p);
   if (p.fmt == 0 && p.block_n == 128) return plain_kernel<2>(p);
@@ -1188,11 +1218,18 @@ namespace {
 // Widest tile of gemm_body: the staged fp32 accumulator tile (128 x block_n) shares the 227 KiB of shared memory with the
 // stage ring and the epilogue buffers; at 128 columns two stages still fit beside the tensor-map epilogue's boxes, three
 // beside the generic epilogue's.  192 and 256 run in gemm_wide_kernel when the plan allows it (gemm_wide_ok); any other
-// wider request runs as 128.
+// wider request runs as 128.  A convolution gemm_wide_ok accepts runs its 128-column tiles in gemm_wide_kernel too, with
+// six stages instead of two.
 constexpr int GEMM_MAX_BN_PLAIN = 128;
 
 int effective_block_n(int block_n) { return block_n > GEMM_MAX_BN_PLAIN ? GEMM_MAX_BN_PLAIN : block_n; }
 bool wide_block_n(int block_n) { return block_n == 192 || block_n == 256; }
+// The tensor-map epilogues gemm_wide_kernel is instantiated with: fp16 outputs, and for convolutions only the two that
+// their forward and dgrad plans reach (bias and / or fp16 residual).
+bool wide_epi_ok(int te, int a_mode) {
+  if (a_mode == OP_CONV) return te == TE_F16 || te == TE_RES16;
+  return te != TE_NONE && te != TE_RES32 && te != TE_ERF_GELU_BWD;
+}
 
 // Tensor-map epilogue (see tma_epilogue_tile) when the epilogue is one of its shapes and every tensor can be described
 // by a tensor map; anything else keeps the generic epilogue.  PXR_GEMM_TMA_EPI=0 disables it globally.
@@ -1231,7 +1268,7 @@ int decide_tma_epi(const GemmParams& p, const GemmEpilogue& e, int block_n) {
 // 128-byte swizzle (wide_epilogue_tile).
 int encode_epilogue_map(CUtensorMap* out, const void* ptr, bool f32, const GemmParams& p, const GemmEpilogue& e,
                         char* err, int errlen) {
-  const bool wide = p.block_n > GEMM_MAX_BN_PLAIN;
+  const bool wide = p.wide;
   uint64_t dims[4], strides[3];
   uint32_t box[4];
   const uint64_t ldc = static_cast<uint64_t>(e.ldc);
@@ -1245,7 +1282,7 @@ int encode_epilogue_map(CUtensorMap* out, const void* ptr, bool f32, const GemmP
     strides[1] = ldc * p.conv_W;
     strides[2] = ldc * p.conv_W * p.conv_H;
     box[1] = p.tile_w;
-    box[2] = 32 / p.tile_w;
+    box[2] = (wide ? 16 : 32) / p.tile_w;
     box[3] = 1;
   } else {
     const int nb1 = p.total_tiles / (p.tiles_m * p.tiles_n * p.nb0);
@@ -1275,7 +1312,7 @@ double epilogue_bytes(const GemmEpilogue& e, double mn) {
 
 int finish_plan(GemmPlan* plan, const GemmEpilogue& epi, int block_n, int num_sms, char* err, int errlen) {
   GemmParams& p = plan->p;
-  const bool wide = wide_block_n(block_n);  // gemm_plan_make keeps 192 / 256 only for plans gemm_wide_ok accepts
+  const bool wide = p.wide;  // set by the plan makers, only for plans gemm_wide_ok accepts
   if (!wide && (block_n < 16 || block_n > GEMM_MAX_BN_PLAIN || block_n % 16)) {
     set_err(err, errlen, "block_n must be a multiple of 16 in [16, 128], or 192 / 256");
     return -10;
@@ -1313,8 +1350,8 @@ int finish_plan(GemmPlan* plan, const GemmEpilogue& epi, int block_n, int num_sm
     if (!rc && second) rc = encode_epilogue_map(&p.tma_d, second, f32, p, epi, err, errlen);
     if (rc) p.tma_epi = TE_NONE;  // a stride the tensor map cannot express: generic epilogue
   }
-  if (wide && (p.tma_epi == TE_NONE || p.tma_epi == TE_RES32 || p.tma_epi == TE_ERF_GELU_BWD)) {
-    set_err(err, errlen, "192- / 256-wide tiles need an fp16 tensor-map epilogue");
+  if (wide && !wide_epi_ok(p.tma_epi, p.a_mode)) {
+    set_err(err, errlen, "the 384-thread kernel needs an fp16 tensor-map epilogue");
     return -15;
   }
   const int stage_bytes = A_TILE_BYTES + block_n * GEMM_BLOCK_K * 2;
@@ -1361,13 +1398,23 @@ int finish_plan(GemmPlan* plan, const GemmEpilogue& epi, int block_n, int num_sm
         }
     for (int bn : {192, 256})
       for (int bm : {OP_KMAJOR, OP_MNMAJOR})
-        for (int te : {TE_F16, TE_RES16, TE_GELU, TE_GELU_BWD, TE_ERF_GELU}) {  // every wide kernel
+        for (int te : {TE_F16, TE_RES16, TE_GELU, TE_GELU_BWD, TE_ERF_GELU}) {  // every wide GEMM kernel
           GemmParams q{};
+          q.wide = 1;
           q.block_n = bn;
           q.b_mode = bm;
           q.tma_epi = te;
           cudaFuncSetAttribute(kernel_for(q), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
         }
+    for (int bn : {128, 192, 256})
+      for (int te : {TE_F16, TE_RES16}) {  // every wide conv kernel
+        GemmParams q{};
+        q.wide = 1;
+        q.a_mode = OP_CONV;
+        q.block_n = bn;
+        q.tma_epi = te;
+        cudaFuncSetAttribute(kernel_for(q), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+      }
   });
   return 0;
 }
@@ -1375,15 +1422,16 @@ int finish_plan(GemmPlan* plan, const GemmEpilogue& epi, int block_n, int num_sm
 }  // namespace
 
 bool gemm_wide_ok(const GemmOperand& A, int N, const GemmEpilogue& epi, int fmt) {
-  if (fmt != 0 || A.mode != OP_KMAJOR || A.nb0 != 1 || A.nb1 != 1 || epi.k_splits > 1) return false;
-  GemmParams q{};  // what decide_tma_epi reads of a plan; at 192 / 256 columns every 32-column block is whole
+  if (fmt != 0 || epi.k_splits > 1) return false;
+  if (A.mode != OP_CONV && (A.mode != OP_KMAJOR || A.nb0 != 1 || A.nb1 != 1)) return false;
+  GemmParams q{};  // what decide_tma_epi reads of a plan; at 128 / 192 / 256 columns every 32-column block is whole
   q.fmt = fmt;
   q.N = N;
   q.a_mode = A.mode;
   q.k_splits = 1;
   q.tiles_n = 1;
-  const int te = decide_tma_epi(q, epi, 256);
-  return te != TE_NONE && te != TE_RES32 && te != TE_ERF_GELU_BWD;
+  q.tile_w = 16;  // either conv tile width (8 or 16) divides the 32-row box
+  return wide_epi_ok(decide_tma_epi(q, epi, 256), A.mode);
 }
 
 int gemm_plan_make(GemmPlan* plan, const GemmOperand& A, const GemmOperand& B, int M, int N, int K,
@@ -1395,6 +1443,7 @@ int gemm_plan_make(GemmPlan* plan, const GemmOperand& A, const GemmOperand& B, i
     return -20;
   }
   if (!(wide_block_n(block_n) && gemm_wide_ok(A, N, epi, fmt))) block_n = effective_block_n(block_n);
+  p.wide = wide_block_n(block_n);
   p.M = M;
   p.N = N;
   p.fmt = fmt;
@@ -1441,7 +1490,7 @@ int gemm_plan_make(GemmPlan* plan, const GemmOperand& A, const GemmOperand& B, i
 
 int conv_plan_make(GemmPlan* plan, const void* in, long long in_ld, int batch, int H, int W, int c_in, const void* wt,
                    int cout_pad, int n_out, int ksize, const GemmEpilogue& epi, int block_n, int fmt, int num_sms,
-                   char* err, int errlen) {
+                   char* err, int errlen, bool allow_wide) {
   *plan = GemmPlan{};
   GemmParams& p = plan->p;
   if (c_in % 64 || (ksize != 1 && ksize != 3)) {
@@ -1455,7 +1504,12 @@ int conv_plan_make(GemmPlan* plan, const void* in, long long in_ld, int batch, i
   // M tile = tile_h x tile_w pixels (8 x 16 or 16 x 8).  Any W works: columns past the image are zero-filled by the
   // TMA loads and clipped by the stores (tensor-map epilogue) / predicated off (generic epilogue); pick the width that
   // wastes the fewest columns (pixray's presets give latents such as 9 x 9, 18 x 18, 12 x 6: pixray.py:1864-1878)
-  block_n = effective_block_n(block_n);
+  {
+    GemmOperand A;
+    A.mode = OP_CONV;
+    p.wide = allow_wide && (block_n == 128 || wide_block_n(block_n)) && gemm_wide_ok(A, n_out, epi, fmt);
+  }
+  if (!p.wide) block_n = effective_block_n(block_n);
   const int waste16 = (W + 15) / 16 * 16, waste8 = (W + 7) / 8 * 8;
   int tile_w = (waste16 <= waste8) ? 16 : 8;
   int tile_h = GEMM_BLOCK_M / tile_w;
@@ -1585,7 +1639,7 @@ void splitk_reduce(const float* ws, int splits, long long pixels, int N, int ld_
 }
 
 void gemm_launch(const GemmPlan& plan, cudaStream_t stream) {
-  const int threads = plan.p.block_n > GEMM_MAX_BN_PLAIN ? GEMM_WIDE_THREADS : GEMM_THREADS;
+  const int threads = plan.p.wide ? GEMM_WIDE_THREADS : GEMM_THREADS;
   launch_pdl(kernel_for(plan.p), dim3(plan.grid), dim3(threads), plan.smem_bytes, stream, plan.p);
 }
 

@@ -13,8 +13,9 @@
 // that then run the epilogue, warp 8 = TMA producer.  smem ring of `stages` {A 128x64, B block_n x 64} tiles (128-byte
 // swizzle); after the main loop the fragments are staged as a row-major fp32 tile in shared memory, from which the
 // epilogue warps read whole rows and write coalesced, while the producer already streams the next tile's operands into
-// the ring.  192- and 256-wide tiles (gemm_wide_ok) run in a second kernel: a producer warpgroup, two consumer
-// warpgroups with one m64nNk16 wgmma per k-step, and an epilogue straight from the accumulator registers.
+// the ring.  192- and 256-wide tiles, and convolutions with 128-wide tiles (gemm_wide_ok), run in a second kernel: a
+// producer warpgroup, two consumer warpgroups with one m64nNk16 wgmma per k-step, and an epilogue straight from the
+// accumulator registers.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -51,6 +52,7 @@ struct GemmParams {
   // tiling
   int M, N;            // logical output extent per batch (predication)
   int block_n;         // multiple of 16, <= 128 (multiple of 64 when B is MN-major); or 192 / 256 (gemm_wide_ok)
+  int wide;            // runs in gemm_wide_kernel: every 192- / 256-column plan, and convolutions at 128 (gemm_wide_ok)
   int stages;
   int num_k_blocks;    // taps * k_blocks_per_tap
   int k_blocks_per_tap;
@@ -128,9 +130,11 @@ struct GemmPlan {
   double bytes = 0;   // compulsory traffic: each operand read once, each epilogue tensor read / written once
 };
 
-// Whether a plain GEMM may use 192- or 256-column tiles (the 384-thread kernel of gemm_tc.cu): fp16, A K-major and
-// unbatched, no split-K, and an epilogue the tensor-map path takes with fp16 outputs (bias, fp16 residual, QuickGELU
-// forward / backward, exact GELU forward).  gemm_plan_make runs any other request wider than 128 columns as 128.
+// Whether a GEMM may use the 384-thread kernel of gemm_tc.cu: fp16, no split-K, and an epilogue the tensor-map path
+// takes with fp16 outputs.  A plain GEMM (A K-major and unbatched) qualifies with bias, fp16 residual, QuickGELU
+// forward / backward or exact GELU forward, at 192 or 256 columns; gemm_plan_make runs any other request wider than 128
+// columns as 128.  A convolution (A.mode == OP_CONV, any batch) qualifies with bias and / or fp16 residual only, at 128,
+// 192 or 256 columns.
 bool gemm_wide_ok(const GemmOperand& A, int N, const GemmEpilogue& epi, int fmt);
 
 // Plain (possibly batched) GEMM.  K is the reduction length; M, N output extents per batch.
@@ -141,9 +145,11 @@ int gemm_plan_make(GemmPlan* plan, const GemmOperand& A, const GemmOperand& B, i
 // Implicit-GEMM convolution (ksize 1 or 3, stride 1, "same" zero padding) over NHWC activations:
 //   out[b, h, w, n] = sum_{tap, c} in[b, h+dy(tap), w+dx(tap), c] * Wt[tap * cout_pad + n, c]
 // `in` has c_in (multiple of 64) channels at pixel stride in_ld; `wt` is [taps * cout_pad, c_in] K-major.
+// A block_n of 128, 192 or 256 runs in the 384-thread kernel when gemm_wide_ok accepts the convolution, otherwise at
+// most 128 wide in the 288-thread kernel; allow_wide = false always takes the latter (tests compare the two kernels).
 int conv_plan_make(GemmPlan* plan, const void* in, long long in_ld, int batch, int H, int W, int c_in,
                    const void* wt, int cout_pad, int n_out, int ksize, const GemmEpilogue& epi, int block_n, int fmt,
-                   int num_sms, char* err, int errlen);
+                   int num_sms, char* err, int errlen, bool allow_wide = true);
 
 void gemm_launch(const GemmPlan& plan, cudaStream_t stream);
 

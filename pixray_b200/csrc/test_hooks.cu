@@ -83,7 +83,7 @@ extern "C" int pxr_test_conv(const pxr_test_gemm_desc* d, int batch, int H, int 
   fill_epilogue(e, d);
   GemmPlan plan;
   int rc = conv_plan_make(&plan, d->a, d->lda, batch, H, W, c_in, d->b, cout_pad, d->N, ksize, e, d->block_n, d->fmt,
-                          num_sms(), err, errlen);
+                          num_sms(), err, errlen, !d->narrow_kernel);
   if (rc) return rc;
   for (int i = 0; i < (d->repeat > 0 ? d->repeat : 1); ++i) gemm_launch(plan, static_cast<cudaStream_t>(d->stream));
   cudaError_t ce = cudaGetLastError();
