@@ -399,6 +399,46 @@ int pxr_test_conv(const pxr_test_gemm_desc* d, int batch, int H, int W, int c_in
 int pxr_test_splitk_reduce(const float* ws, int splits, long long pixels, int N, int ld_ws, const float* bias, const void* res,
                            void* out, int ld_out);
 
+/* one conv weight operand the engine packed: the fp16 operand of n elements at ptr holds checkpoint weight w
+ * [cout][cin][taps] element (co, ci, t) at t' s_tap + co s_co + (ci - ci0) s_ci, t' = taps - 1 - t when flip, else t,
+ * for ci in [ci0, ci1); every other element is 0.  tag: the checkpoint prefix of the conv; src: an opaque id of the host
+ * weights it was packed from (a forward operand and its dgrad operands share tag and src). */
+typedef struct {
+  char tag[128];
+  const void* ptr;
+  const void* src;
+  long long n, s_tap, s_co, s_ci;
+  int cout, cin, taps, flip, ci0, ci1;
+} pxr_test_pack_rec;
+
+/* one convolution plan the engine built (one per add_conv), with the plan's choices.  k_splits > 1: the plan writes fp32
+ * partial sums and the split-K reduce applies bias, residual and the fp16 store; block_n .. grid are then the split
+ * plan's.  has_* / in_place / out_f32 / ldc / act describe the convolution's own epilogue (in_place: the residual is the
+ * output; out_f32: an fp32 output instead of fp16). */
+typedef struct {
+  char label[192];
+  const void* wt;
+  const float* bias;
+  int batch, H, W, c_in;
+  long long in_ld;
+  int cout_pad, n_out, ks;
+  int block_n, wide, k_splits, tma_epi, stages, grid;
+  int act, act_col0;
+  int has_bias, has_res, has_aux, in_place, out_f32;
+  long long ldc;
+} pxr_test_conv_rec;
+
+/* the conv plans built so far, in build order: fills out[0 .. min(max, n) - 1], *count = n */
+int pxr_test_conv_records(pxr_handle h, pxr_test_conv_rec* out, int max, int* count);
+/* the packed conv operands so far, in packing order, as pxr_test_conv_records.  index >= 0 also copies operand `index`
+ * (n fp16 elements) to the DEVICE buffer dst; with dst_bias, n_bias floats of `bias` too, which must be the bias of a
+ * recorded plan on that operand with n_bias <= its n_out.  Synchronous. */
+int pxr_test_packed_weights(pxr_handle h, pxr_test_pack_rec* out, int max, int* count, int index, void* dst,
+                            const float* bias, float* dst_bias, int n_bias);
+/* builds the plan pxr_test_conv would run, without launching it: out = {wide, block_n, stages, tma_epi, grid, k_splits} */
+int pxr_test_conv_plan_info(const pxr_test_gemm_desc* d, int batch, int H, int W, int c_in, int cout_pad, int ksize,
+                            int out[6]);
+
 /* host-side evaluation of the ColorJitter pixel body and its vector-Jacobian product (no GPU needed) */
 int pxr_test_color_jitter_host(const float* rgb, int n, int code, float saturation, float hue, const float* g_out,
                                float* out, float* g_in);

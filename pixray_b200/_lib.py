@@ -64,6 +64,22 @@ class TestGemmDesc(C.Structure):
     ]
 
 
+class TestPackRec(C.Structure):
+    _fields_ = [("tag", C.c_char * 128), ("ptr", C.c_void_p), ("src", C.c_void_p),
+                ("n", C.c_longlong), ("s_tap", C.c_longlong), ("s_co", C.c_longlong), ("s_ci", C.c_longlong),
+                ("cout", C.c_int), ("cin", C.c_int), ("taps", C.c_int), ("flip", C.c_int), ("ci0", C.c_int), ("ci1", C.c_int)]
+
+
+class TestConvRec(C.Structure):
+    _fields_ = [("label", C.c_char * 192), ("wt", C.c_void_p), ("bias", C.c_void_p),
+                ("batch", C.c_int), ("H", C.c_int), ("W", C.c_int), ("c_in", C.c_int), ("in_ld", C.c_longlong),
+                ("cout_pad", C.c_int), ("n_out", C.c_int), ("ks", C.c_int),
+                ("block_n", C.c_int), ("wide", C.c_int), ("k_splits", C.c_int), ("tma_epi", C.c_int), ("stages", C.c_int),
+                ("grid", C.c_int), ("act", C.c_int), ("act_col0", C.c_int),
+                ("has_bias", C.c_int), ("has_res", C.c_int), ("has_aux", C.c_int), ("in_place", C.c_int), ("out_f32", C.c_int),
+                ("ldc", C.c_longlong)]
+
+
 # every symbol include/pixray_b200.h declares (tests check the library exports all of them)
 EXPORTS = [
     "pxr_last_error", "pxr_version", "pxr_create", "pxr_destroy", "pxr_load_weight", "pxr_finalize", "pxr_set_clip_tower",
@@ -76,6 +92,7 @@ EXPORTS = [
     "pxr_test_splitk_reduce", "pxr_test_groupnorm_unet", "pxr_test_resample", "pxr_test_gemv",
     "pxr_test_prompt_loss", "pxr_text_tower", "pxr_encode_text", "pxr_test_attention_causal",
     "pxr_cutout_sets", "pxr_make_cutouts_set", "pxr_iterate_sets",
+    "pxr_test_conv_records", "pxr_test_packed_weights", "pxr_test_conv_plan_info",
 ]
 
 _lib = None

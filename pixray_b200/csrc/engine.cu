@@ -44,6 +44,9 @@ class Engine {
   bool finalized = false;
   std::map<std::string, std::pair<void*, size_t>> dbg;  // named internal buffers (tests / debugging)
   void reg(const std::string& n, void* p, size_t bytes) { dbg[n] = {p, bytes}; }
+  // what pack_conv packed and what add_conv planned, in order (pxr_test_packed_weights / pxr_test_conv_records)
+  std::vector<pxr_test_pack_rec> pack_log;
+  std::vector<pxr_test_conv_rec> conv_log;
 
   // sharding
   int n_local = 0, first_global = 0;
@@ -605,6 +608,36 @@ class Engine {
     }
     auto plan = std::make_shared<GemmPlan>();
     char buf[256] = {0};
+    auto log = [&](const std::string& label) {
+      const GemmParams& p = plan->p;
+      pxr_test_conv_rec r{};
+      snprintf(r.label, sizeof r.label, "%s", label.c_str());
+      r.wt = wt;
+      r.bias = e.bias;
+      r.batch = batch;
+      r.H = H;
+      r.W = Wd;
+      r.c_in = cin;
+      r.in_ld = in_ld;
+      r.cout_pad = cout_pad;
+      r.n_out = n_out;
+      r.ks = ks;
+      r.block_n = p.block_n;
+      r.wide = p.wide;
+      r.k_splits = p.k_splits;
+      r.tma_epi = p.tma_epi;
+      r.stages = p.stages;
+      r.grid = plan->grid;
+      r.act = e.act;
+      r.act_col0 = e.act_col0;
+      r.has_bias = e.bias != nullptr;
+      r.has_res = e.res_f16 != nullptr;
+      r.has_aux = e.aux_in != nullptr;
+      r.in_place = e.res_f16 && e.res_f16 == e.out_f16;
+      r.out_f32 = e.out_f32 != nullptr;
+      r.ldc = e.ldc;
+      conv_log.push_back(r);
+    };
     if (splits > 1) {
       GemmEpilogue pe;
       pe.out_f32 = splitk_ws;
@@ -619,6 +652,7 @@ class Engine {
       const int ld_out = (int)e.ldc;
       const long long px = (long long)H * Wd;
       std::string label = gemm_label(kind, *plan, OP_KMAJOR, OP_KMAJOR, e) + " splitK=" + std::to_string(plan->p.k_splits);
+      log(label);
       l.add(1, [=] { gemm_launch(*plan, s); }, plan->flops, label, plan->bytes);
       // the reduce is its own op so that a GroupNorm right behind it can absorb it (add_gn / add_gn_bwd)
       l.add(1, [=] { splitk_reduce(ws, plan->p.k_splits, px, n_out, n_out, bias, res, out, ld_out, s); }, 0.0,
@@ -640,7 +674,9 @@ class Engine {
     int rc = conv_plan_make(plan.get(), in, in_ld, batch, H, Wd, cin, wt, cout_pad, n_out, ks, e, bn, fmt, num_sms, buf,
                             sizeof buf);
     if (rc) throw EngineError(rc, std::string("conv plan: ") + buf);
-    l.add(1, [plan, s] { gemm_launch(*plan, s); }, plan->flops, gemm_label(kind, *plan, OP_KMAJOR, OP_KMAJOR, e), plan->bytes);
+    const std::string label = gemm_label(kind, *plan, OP_KMAJOR, OP_KMAJOR, e);
+    log(label);
+    l.add(1, [plan, s] { gemm_launch(*plan, s); }, plan->flops, label, plan->bytes);
   }
 
   // Split-K for a plain K-major GEMM with few output tiles and a long reduction (the vdiff U-Net's 4x4 ... 1x1 levels:
@@ -700,8 +736,8 @@ class Engine {
   void build_cutouts();
   void build_clip(int i);
   ConvW load_conv(const std::string& prefix, int cin, int cout, int ks, int cin_real = 0, bool has_bias = true);
-  act_t* pack_conv(const std::vector<float>& w, int cout, int cin, int taps, size_t n, size_t s_tap, size_t s_co,
-                   size_t s_ci, bool flip, int ci0 = 0, int ci1 = INT_MAX);
+  act_t* pack_conv(const std::string& tag, const std::vector<float>& w, int cout, int cin, int taps, size_t n, size_t s_tap,
+                   size_t s_co, size_t s_ci, bool flip, int ci0 = 0, int ci1 = INT_MAX);
   // VQGAN encoder (taming Encoder + quant_conv + nearest code): VqganDrawer.init_from_tensor / reapply_from_tensor /
   // get_z_from_tensor (vqgan.py:174-185).  Forward only; built at finalize when the checkpoint carries encoder.* tensors.
   OpList enc_fwd;
@@ -880,15 +916,32 @@ NormW Engine::load_norm(int mod, const std::string& prefix, int c) {
 
 // The one conv weight packer: scatters a PyTorch weight w [cout][cin][taps] into a zeroed fp16 operand of n elements,
 // (co, ci, t) to t' s_tap + co s_co + (ci - ci0) s_ci, where t' = t, or taps - 1 - t with flip (a dgrad: dx[p] = sum_t
-// dy[p + off(t)] W[.., flipped t]).  Only the input channels [ci0, ci1) are packed.
-act_t* Engine::pack_conv(const std::vector<float>& w, int cout, int cin, int taps, size_t n, size_t s_tap, size_t s_co,
-                         size_t s_ci, bool flip, int ci0, int ci1) {
+// dy[p + off(t)] W[.., flipped t]).  Only the input channels [ci0, ci1) are packed.  tag: the conv's checkpoint prefix,
+// recorded with the layout for pxr_test_packed_weights.
+act_t* Engine::pack_conv(const std::string& tag, const std::vector<float>& w, int cout, int cin, int taps, size_t n,
+                         size_t s_tap, size_t s_co, size_t s_ci, bool flip, int ci0, int ci1) {
   std::vector<float> f(n, 0.f);
   for (int co = 0; co < cout; ++co)
     for (int ci = ci0; ci < std::min(ci1, cin); ++ci)
       for (int t = 0; t < taps; ++t)
         f[(flip ? taps - 1 - t : t) * s_tap + co * s_co + (ci - ci0) * s_ci] = w[((size_t)co * cin + ci) * taps + t];
-  return upload_f16(f);
+  act_t* p = upload_f16(f);
+  pxr_test_pack_rec r{};
+  snprintf(r.tag, sizeof r.tag, "%s", tag.c_str());
+  r.ptr = p;
+  r.src = w.data();
+  r.n = (long long)n;
+  r.s_tap = (long long)s_tap;
+  r.s_co = (long long)s_co;
+  r.s_ci = (long long)s_ci;
+  r.cout = cout;
+  r.cin = cin;
+  r.taps = taps;
+  r.flip = flip;
+  r.ci0 = ci0;
+  r.ci1 = std::min(ci1, cin);
+  pack_log.push_back(r);
+  return p;
 }
 
 // cin_real < cin: the stored tensor has cin_real input channels and the activation is zero-padded to cin (conv_in: 3 -> 64)
@@ -904,9 +957,9 @@ ConvW Engine::load_conv(const std::string& prefix, int cin, int cout, int ks, in
   c.cin_rows = round_up(cin, 16);
   const int taps = ks * ks;
   if (cin % 64) throw EngineError(-42, "conv '" + prefix + "': input channels must be a multiple of 64");
-  c.w = pack_conv(w.data, cout, cin_real, taps, (size_t)taps * c.cout_pad * cin, (size_t)c.cout_pad * cin, cin, 1, false);
-  c.wd = pack_conv(w.data, cout, cin_real, taps, (size_t)taps * c.cin_rows * c.cout_k, (size_t)c.cin_rows * c.cout_k, 1,
-                   c.cout_k, true);
+  c.w = pack_conv(prefix, w.data, cout, cin_real, taps, (size_t)taps * c.cout_pad * cin, (size_t)c.cout_pad * cin, cin, 1, false);
+  c.wd = pack_conv(prefix, w.data, cout, cin_real, taps, (size_t)taps * c.cin_rows * c.cout_k, (size_t)c.cin_rows * c.cout_k,
+                   1, c.cout_k, true);
   if (has_bias) c.bias = upload(W(PXR_MOD_VQGAN, prefix + ".bias", {cout}).data);
   return c;
 }
@@ -3900,6 +3953,35 @@ int pxr_debug_read(pxr_handle h, const char* name, void* out, int64_t nbytes) {
     if (it == e->dbg.end()) throw EngineError(-19, std::string("unknown debug buffer ") + name);
     if ((size_t)nbytes > it->second.second) throw EngineError(-19, "debug read larger than the buffer");
     PXR_CUDA(cudaMemcpyAsync(out, it->second.first, nbytes, cudaMemcpyDefault, e->st));
+    PXR_CUDA(cudaStreamSynchronize(e->st));
+  });
+}
+
+int pxr_test_conv_records(pxr_handle h, pxr_test_conv_rec* out, int max, int* count) {
+  PXR_TRY(h, {
+    const auto& log = h->e->conv_log;
+    for (int i = 0; out && i < max && i < (int)log.size(); ++i) out[i] = log[i];
+    if (count) *count = (int)log.size();
+  });
+}
+
+int pxr_test_packed_weights(pxr_handle h, pxr_test_pack_rec* out, int max, int* count, int index, void* dst,
+                            const float* bias, float* dst_bias, int n_bias) {
+  PXR_TRY(h, {
+    Engine* e = h->e;
+    const auto& log = e->pack_log;
+    for (int i = 0; out && i < max && i < (int)log.size(); ++i) out[i] = log[i];
+    if (count) *count = (int)log.size();
+    if (index < 0) return 0;
+    if (index >= (int)log.size() || !dst) throw EngineError(-19, "pxr_test_packed_weights: no such operand");
+    const pxr_test_pack_rec& r = log[index];
+    PXR_CUDA(cudaMemcpyAsync(dst, r.ptr, (size_t)r.n * sizeof(pxr::act_t), cudaMemcpyDeviceToDevice, e->st));
+    if (dst_bias) {
+      bool known = false;
+      for (const pxr_test_conv_rec& c : e->conv_log) known |= c.wt == r.ptr && c.bias == bias && bias && n_bias <= c.n_out;
+      if (!known) throw EngineError(-19, "pxr_test_packed_weights: not the bias of a plan on that operand");
+      PXR_CUDA(cudaMemcpyAsync(dst_bias, bias, (size_t)n_bias * sizeof(float), cudaMemcpyDeviceToDevice, e->st));
+    }
     PXR_CUDA(cudaStreamSynchronize(e->st));
   });
 }

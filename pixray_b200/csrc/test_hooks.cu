@@ -94,6 +94,19 @@ extern "C" int pxr_test_conv(const pxr_test_gemm_desc* d, int batch, int H, int 
   return 0;
 }
 
+extern "C" int pxr_test_conv_plan_info(const pxr_test_gemm_desc* d, int batch, int H, int W, int c_in, int cout_pad,
+                                       int ksize, int out[6]) {
+  GemmEpilogue e;
+  fill_epilogue(e, d);
+  GemmPlan plan;
+  int rc = conv_plan_make(&plan, d->a, d->lda, batch, H, W, c_in, d->b, cout_pad, d->N, ksize, e, d->block_n, d->fmt,
+                          num_sms(), nullptr, 0, !d->narrow_kernel);
+  if (rc) return rc;
+  const int info[6] = {plan.p.wide, plan.p.block_n, plan.p.stages, plan.p.tma_epi, plan.grid, plan.p.k_splits};
+  for (int i = 0; i < 6; ++i) out[i] = info[i];
+  return 0;
+}
+
 static int sync_status() {
   cudaError_t ce = cudaDeviceSynchronize();
   if (ce == cudaSuccess) ce = cudaGetLastError();
