@@ -439,6 +439,46 @@ int pxr_test_packed_weights(pxr_handle h, pxr_test_pack_rec* out, int max, int* 
 int pxr_test_conv_plan_info(const pxr_test_gemm_desc* d, int batch, int H, int W, int c_in, int cout_pad, int ksize,
                             int out[6]);
 
+/* one plain GEMM plan the engine built (one per add_gemm / split add_gemm_splitk), with the plan's choices.  Operands as
+ * GemmOperand (gemm_tc.cuh): mode 0 K-major (element (r, k) at r ld + k), 1 MN-major (at k ld + r), batch (b0, b1) at
+ * b0 bs0 + b1 bs1; B's batch extents are 1 or A's.  The epilogue fields are the plan's own; in_place: the residual is the
+ * output.  k_splits > 1: the plan writes fp32 partial sums [k_splits][M][ldc] to out_f32 (the split-K workspace) and the
+ * reduce applies red_bias, red_res and the fp16 store to red_out at pitch ld_out; red_* are null otherwise.  k_blocks:
+ * the 64-deep k-blocks the plan runs over (all splits together). */
+typedef struct {
+  char label[192];
+  const void* a;
+  int a_mode, a_nb0, a_nb1;
+  long long lda, a_mn_extent, a_k_extent, a_bs0, a_bs1;
+  const void* b;
+  int b_mode, b_nb0, b_nb1;
+  long long ldb, b_mn_extent, b_k_extent, b_bs0, b_bs1;
+  int M, N, K;
+  float alpha;
+  const float* bias;
+  int bias_per_row, act, act_col0, in_place;
+  const void* aux_in;
+  void* aux_out;
+  const float* res_f32;
+  const void* res_f16;
+  float* out_f32;
+  void* out_f16;
+  long long ldc, c_bs0, c_bs1;
+  int block_n, wide, stages, tma_epi, grid, k_splits, k_blocks;
+  const float* red_bias;
+  const void* red_res;
+  void* red_out;
+  long long ld_out;
+} pxr_test_gemm_rec;
+
+/* the GEMM plans built so far, in build order, as pxr_test_conv_records */
+int pxr_test_gemm_records(pxr_handle h, pxr_test_gemm_rec* out, int max, int* count);
+/* builds the plan pxr_test_gemm would run, without launching it: out = {wide, block_n, stages, tma_epi, grid, k_splits} */
+int pxr_test_gemm_plan_info(const pxr_test_gemm_desc* d, int out[6]);
+/* the engine's live device allocations (dalloc / upload), in allocation order: ptr[i], bytes[i] for i < min(max, n),
+ * *count = n */
+int pxr_test_allocations(pxr_handle h, const void** ptr, long long* bytes, int max, int* count);
+
 /* host-side evaluation of the ColorJitter pixel body and its vector-Jacobian product (no GPU needed) */
 int pxr_test_color_jitter_host(const float* rgb, int n, int code, float saturation, float hue, const float* g_out,
                                float* out, float* g_in);

@@ -80,6 +80,25 @@ class TestConvRec(C.Structure):
                 ("ldc", C.c_longlong)]
 
 
+class TestGemmRec(C.Structure):
+    _fields_ = [("label", C.c_char * 192),
+                ("a", C.c_void_p), ("a_mode", C.c_int), ("a_nb0", C.c_int), ("a_nb1", C.c_int),
+                ("lda", C.c_longlong), ("a_mn_extent", C.c_longlong), ("a_k_extent", C.c_longlong),
+                ("a_bs0", C.c_longlong), ("a_bs1", C.c_longlong),
+                ("b", C.c_void_p), ("b_mode", C.c_int), ("b_nb0", C.c_int), ("b_nb1", C.c_int),
+                ("ldb", C.c_longlong), ("b_mn_extent", C.c_longlong), ("b_k_extent", C.c_longlong),
+                ("b_bs0", C.c_longlong), ("b_bs1", C.c_longlong),
+                ("M", C.c_int), ("N", C.c_int), ("K", C.c_int),
+                ("alpha", C.c_float), ("bias", C.c_void_p),
+                ("bias_per_row", C.c_int), ("act", C.c_int), ("act_col0", C.c_int), ("in_place", C.c_int),
+                ("aux_in", C.c_void_p), ("aux_out", C.c_void_p), ("res_f32", C.c_void_p), ("res_f16", C.c_void_p),
+                ("out_f32", C.c_void_p), ("out_f16", C.c_void_p),
+                ("ldc", C.c_longlong), ("c_bs0", C.c_longlong), ("c_bs1", C.c_longlong),
+                ("block_n", C.c_int), ("wide", C.c_int), ("stages", C.c_int), ("tma_epi", C.c_int), ("grid", C.c_int),
+                ("k_splits", C.c_int), ("k_blocks", C.c_int),
+                ("red_bias", C.c_void_p), ("red_res", C.c_void_p), ("red_out", C.c_void_p), ("ld_out", C.c_longlong)]
+
+
 # every symbol include/pixray_b200.h declares (tests check the library exports all of them)
 EXPORTS = [
     "pxr_last_error", "pxr_version", "pxr_create", "pxr_destroy", "pxr_load_weight", "pxr_finalize", "pxr_set_clip_tower",
@@ -93,6 +112,7 @@ EXPORTS = [
     "pxr_test_prompt_loss", "pxr_text_tower", "pxr_encode_text", "pxr_test_attention_causal",
     "pxr_cutout_sets", "pxr_make_cutouts_set", "pxr_iterate_sets",
     "pxr_test_conv_records", "pxr_test_packed_weights", "pxr_test_conv_plan_info",
+    "pxr_test_gemm_records", "pxr_test_gemm_plan_info", "pxr_test_allocations",
 ]
 
 _lib = None

@@ -41,12 +41,15 @@ class Engine {
                               // attn_long.cu T > 257)
   std::map<std::string, HostWeight> weights[5];
   std::vector<void*> allocs;
+  std::vector<size_t> alloc_bytes;  // bytes of allocs[i] (pxr_test_allocations)
   bool finalized = false;
   std::map<std::string, std::pair<void*, size_t>> dbg;  // named internal buffers (tests / debugging)
   void reg(const std::string& n, void* p, size_t bytes) { dbg[n] = {p, bytes}; }
   // what pack_conv packed and what add_conv planned, in order (pxr_test_packed_weights / pxr_test_conv_records)
   std::vector<pxr_test_pack_rec> pack_log;
   std::vector<pxr_test_conv_rec> conv_log;
+  // what add_gemm / add_gemm_splitk planned, in order (pxr_test_gemm_records)
+  std::vector<pxr_test_gemm_rec> gemm_log;
 
   // sharding
   int n_local = 0, first_global = 0;
@@ -368,6 +371,7 @@ class Engine {
     PXR_CUDA(cudaMalloc(&p, bytes));
     if (zero) PXR_CUDA(cudaMemsetAsync(p, 0, bytes, st));
     allocs.push_back(p);
+    alloc_bytes.push_back(bytes);
     return static_cast<T*>(p);
   }
   // release one tracked allocation early (buffers that are rebuilt when prompts change); cudaFree waits for the device
@@ -377,6 +381,7 @@ class Engine {
     auto it = std::find(allocs.begin(), allocs.end(), static_cast<void*>(p));
     if (it != allocs.end()) {
       cudaFree(*it);
+      alloc_bytes.erase(alloc_bytes.begin() + (it - allocs.begin()));
       allocs.erase(it);
     }
     p = nullptr;
@@ -534,7 +539,67 @@ class Engine {
     int rc = gemm_plan_make(plan.get(), A, B, M, N, K, e, bn, fmt, num_sms, buf, sizeof buf);
     if (rc) throw EngineError(rc, std::string("gemm plan: ") + buf);
     cudaStream_t s = st;
-    l.add(1, [plan, s] { gemm_launch(*plan, s); }, plan->flops, gemm_label("gemm", *plan, A.mode, B.mode, e), plan->bytes);
+    const std::string label = gemm_label("gemm", *plan, A.mode, B.mode, e);
+    log_gemm(label, *plan, A, B, M, N, K, e, nullptr);
+    l.add(1, [plan, s] { gemm_launch(*plan, s); }, plan->flops, label, plan->bytes);
+  }
+  // one gemm_log record: the operands and epilogue the plan was made from, its choices, and for a split-K plan (epilogue
+  // e = the fp32 partial sums) the reduce's bias, residual and output from `red`
+  void log_gemm(const std::string& label, const GemmPlan& plan, const GemmOperand& A, const GemmOperand& B, int M, int N,
+                int K, const GemmEpilogue& e, const GemmEpilogue* red) {
+    pxr_test_gemm_rec r{};
+    snprintf(r.label, sizeof r.label, "%s", label.c_str());
+    r.a = A.ptr;
+    r.a_mode = A.mode;
+    r.a_nb0 = A.nb0;
+    r.a_nb1 = A.nb1;
+    r.lda = A.ld;
+    r.a_mn_extent = A.mn_extent;
+    r.a_k_extent = A.k_extent;
+    r.a_bs0 = A.bs0;
+    r.a_bs1 = A.bs1;
+    r.b = B.ptr;
+    r.b_mode = B.mode;
+    r.b_nb0 = B.nb0;
+    r.b_nb1 = B.nb1;
+    r.ldb = B.ld;
+    r.b_mn_extent = B.mn_extent;
+    r.b_k_extent = B.k_extent;
+    r.b_bs0 = B.bs0;
+    r.b_bs1 = B.bs1;
+    r.M = M;
+    r.N = N;
+    r.K = K;
+    r.alpha = e.alpha;
+    r.bias = e.bias;
+    r.bias_per_row = e.bias_per_row;
+    r.act = e.act;
+    r.act_col0 = e.act_col0;
+    r.in_place = (e.res_f16 && e.res_f16 == e.out_f16) || (e.res_f32 && e.res_f32 == e.out_f32) ||
+                 (red && red->res_f16 && red->res_f16 == red->out_f16);
+    r.aux_in = e.aux_in;
+    r.aux_out = e.aux_out;
+    r.res_f32 = e.res_f32;
+    r.res_f16 = e.res_f16;
+    r.out_f32 = e.out_f32;
+    r.out_f16 = e.out_f16;
+    r.ldc = e.ldc;
+    r.c_bs0 = e.bs0;
+    r.c_bs1 = e.bs1;
+    r.block_n = plan.p.block_n;
+    r.wide = plan.p.wide;
+    r.stages = plan.p.stages;
+    r.tma_epi = plan.p.tma_epi;
+    r.grid = plan.grid;
+    r.k_splits = plan.p.k_splits;
+    r.k_blocks = plan.p.num_k_blocks;
+    if (red) {
+      r.red_bias = red->bias;
+      r.red_res = red->res_f16;
+      r.red_out = red->out_f16;
+      r.ld_out = red->ldc;
+    }
+    gemm_log.push_back(r);
   }
   static std::string gemm_label(const char* kind, const GemmPlan& p, int am, int bm, const GemmEpilogue& e) {
     char b[256];
@@ -706,6 +771,7 @@ class Engine {
     act_t* out = e.out_f16;
     const int ld_out = (int)e.ldc;
     std::string label = gemm_label("gemm", *plan, A.mode, B.mode, e) + " splitK=" + std::to_string(plan->p.k_splits);
+    log_gemm(label, *plan, A, B, M, N, K, pe, &e);
     l.add(2, [=] {
       gemm_launch(*plan, s);
       splitk_reduce(ws, plan->p.k_splits, M, N, N, bias, res, out, ld_out, s);
@@ -3962,6 +4028,25 @@ int pxr_test_conv_records(pxr_handle h, pxr_test_conv_rec* out, int max, int* co
     const auto& log = h->e->conv_log;
     for (int i = 0; out && i < max && i < (int)log.size(); ++i) out[i] = log[i];
     if (count) *count = (int)log.size();
+  });
+}
+
+int pxr_test_gemm_records(pxr_handle h, pxr_test_gemm_rec* out, int max, int* count) {
+  PXR_TRY(h, {
+    const auto& log = h->e->gemm_log;
+    for (int i = 0; out && i < max && i < (int)log.size(); ++i) out[i] = log[i];
+    if (count) *count = (int)log.size();
+  });
+}
+
+int pxr_test_allocations(pxr_handle h, const void** ptr, long long* bytes, int max, int* count) {
+  PXR_TRY(h, {
+    const Engine* e = h->e;
+    for (int i = 0; i < max && i < (int)e->allocs.size(); ++i) {
+      if (ptr) ptr[i] = e->allocs[i];
+      if (bytes) bytes[i] = (long long)e->alloc_bytes[i];
+    }
+    if (count) *count = (int)e->allocs.size();
   });
 }
 

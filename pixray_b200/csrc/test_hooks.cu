@@ -43,7 +43,8 @@ static void fill_epilogue(GemmEpilogue& e, const pxr_test_gemm_desc* d) {
   e.k_splits = d->k_splits;
 }
 
-extern "C" int pxr_test_gemm(const pxr_test_gemm_desc* d, char* err, int errlen) {
+// the plan pxr_test_gemm runs for a descriptor (B takes A's batch extents when b_batched)
+static int desc_plan(GemmPlan* plan, const pxr_test_gemm_desc* d, char* err, int errlen) {
   GemmOperand A, B;
   A.ptr = d->a;
   A.mode = d->a_mode;
@@ -65,8 +66,12 @@ extern "C" int pxr_test_gemm(const pxr_test_gemm_desc* d, char* err, int errlen)
   B.bs1 = d->b_bs1;
   GemmEpilogue e;
   fill_epilogue(e, d);
+  return gemm_plan_make(plan, A, B, d->M, d->N, d->K, e, d->block_n, d->fmt, num_sms(), err, errlen);
+}
+
+extern "C" int pxr_test_gemm(const pxr_test_gemm_desc* d, char* err, int errlen) {
   GemmPlan plan;
-  int rc = gemm_plan_make(&plan, A, B, d->M, d->N, d->K, e, d->block_n, d->fmt, num_sms(), err, errlen);
+  int rc = desc_plan(&plan, d, err, errlen);
   if (rc) return rc;
   for (int i = 0; i < (d->repeat > 0 ? d->repeat : 1); ++i) gemm_launch(plan, static_cast<cudaStream_t>(d->stream));
   cudaError_t ce = cudaGetLastError();
@@ -74,6 +79,15 @@ extern "C" int pxr_test_gemm(const pxr_test_gemm_desc* d, char* err, int errlen)
     if (err) snprintf(err, errlen, "launch failed: %s", cudaGetErrorString(ce));
     return -100;
   }
+  return 0;
+}
+
+extern "C" int pxr_test_gemm_plan_info(const pxr_test_gemm_desc* d, int out[6]) {
+  GemmPlan plan;
+  int rc = desc_plan(&plan, d, nullptr, 0);
+  if (rc) return rc;
+  const int info[6] = {plan.p.wide, plan.p.block_n, plan.p.stages, plan.p.tma_epi, plan.grid, plan.p.k_splits};
+  for (int i = 0; i < 6; ++i) out[i] = info[i];
   return 0;
 }
 
