@@ -498,6 +498,11 @@ int pxr_test_raster_samples(uint64_t seed, int iter, int H, int W, float* out);
 int pxr_test_attention(const void* qkv, void* o, float* lse, const void* d_o, void* gqkv, int B, int T, int H, int W,
                        float scale, int repeat, char* err, int errlen);
 
+/* pxr_test_attention's forward once, then its backward `repeat` times (none for 0) on the kernel bwd_kernel selects
+ * (0: as the engine chooses, 1: attn_bwd_kernel, 2: attn_bwd_wg); *used (nullable) receives the kernel taken (1 or 2) */
+int pxr_test_attention_bwd_select(const void* qkv, void* o, float* lse, const void* d_o, void* gqkv, int B, int T, int H,
+                                  int W, float scale, int bwd_kernel, int repeat, int* used, char* err, int errlen);
+
 /* causal attention forward (the text towers): o [B*T, W] from qkv [B*T, 3W] fp16 device tensors, row t attending to
  * keys <= t; 64-wide heads (W = 64 H), T <= 240.  The fused kernel, or with PXR_FUSED_ATTN=0 in the environment the
  * batched-GEMM chain with the causal row softmax, as the engine would choose */

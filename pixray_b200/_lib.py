@@ -109,7 +109,7 @@ EXPORTS = [
     "pxr_test_pool_bounds", "pxr_test_groupnorm", "pxr_test_softmax", "pxr_test_layernorm", "pxr_set_spot_prompts", "pxr_set_spot_mask", "pxr_state_size", "pxr_save_state", "pxr_load_state", "pxr_set_schedule", "pxr_poll_status", "pxr_set_batches", "pxr_set_z_grad", "pxr_vdiff_set_schedule", "pxr_vdiff_set_clip_embed", "pxr_vdiff_set_iteration", "pxr_vdiff_renoise",
     "pxr_set_polygons", "pxr_set_synth_iteration", "pxr_test_raster_samples", "pxr_set_strokes", "pxr_set_optimizer",
     "pxr_test_splitk_reduce", "pxr_test_groupnorm_unet", "pxr_test_resample", "pxr_test_gemv",
-    "pxr_test_prompt_loss", "pxr_text_tower", "pxr_encode_text", "pxr_test_attention_causal",
+    "pxr_test_prompt_loss", "pxr_text_tower", "pxr_encode_text", "pxr_test_attention_causal", "pxr_test_attention_bwd_select",
     "pxr_cutout_sets", "pxr_make_cutouts_set", "pxr_iterate_sets",
     "pxr_test_conv_records", "pxr_test_packed_weights", "pxr_test_conv_plan_info",
     "pxr_test_gemm_records", "pxr_test_gemm_plan_info", "pxr_test_allocations",

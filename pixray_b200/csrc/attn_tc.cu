@@ -6,6 +6,8 @@
 #include <algorithm>
 #include <cmath>
 #include <cstdio>
+#include <cstdlib>
+#include <cstring>
 #include <mutex>
 
 namespace pxr {
@@ -320,7 +322,7 @@ int bwd_smem(int T) { return 4 * round16(T) * ROW_BYTES + 2 * round16(T) * 4; }
 bool attn_supported(int T, int head_dim, int W) { return head_dim == 64 && T >= 1 && T <= 240 && W % 64 == 0; }
 
 int attn_plan_make(AttnPlan* plan, const __half* qkv, __half* o, const __half* d_o, __half* gqkv, float* lse, int B,
-                   int T, int H, int W, float scale, int num_sms, char* err, int errlen, bool causal) {
+                   int T, int H, int W, float scale, int num_sms, char* err, int errlen, bool causal, int bwd) {
   *plan = AttnPlan{};
   if (!attn_supported(T, W / H, W) || W != 64 * H) {
     if (err && errlen > 0) snprintf(err, errlen, "fused attention needs 64-wide heads and T <= 240");
@@ -358,6 +360,22 @@ int attn_plan_make(AttnPlan* plan, const __half* qkv, __half* o, const __half* d
     cudaFuncSetAttribute(attn_fwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, fwd_smem(240, 1));
     cudaFuncSetAttribute(attn_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bwd_smem(240));
   });
+  // The wgmma backward needs the whole pair in one CTA; with fewer pairs than SMs the split mma.sync kernel keeps every SM
+  // busy instead.
+  static const bool force_mma = [] {
+    const char* e = getenv("PXR_ATTN_BWD");
+    return e && strcmp(e, "mma") == 0;
+  }();
+  if (bwd == ATTN_BWD_AUTO)
+    bwd = !force_mma && d_o && gqkv && !causal && pairs >= sms && attn_bwd_wg_fits(T) ? ATTN_BWD_WG : ATTN_BWD_MMA;
+  if (bwd == ATTN_BWD_WG) {
+    const int rc = attn_bwd_wg_prepare(plan, err, errlen);
+    if (rc) return rc;
+  } else if (bwd != ATTN_BWD_MMA) {
+    if (err && errlen > 0) snprintf(err, errlen, "unknown attention backward kernel %d", bwd);
+    return -1;
+  }
+  plan->bwd = bwd;
   return 0;
 }
 
@@ -369,6 +387,10 @@ void attn_forward_launch(const AttnPlan& plan, cudaStream_t st) {
 
 void attn_backward_launch(const AttnPlan& plan, cudaStream_t st) {
   const AttnParams& p = plan.p;
+  if (plan.bwd == ATTN_BWD_WG) {
+    attn_bwd_wg_launch(plan, st);
+    return;
+  }
   launch_pdl(attn_bwd_kernel, dim3(plan.splits, p.H, p.B), dim3(AT_THREADS), plan.smem_bwd, st, p);
 }
 

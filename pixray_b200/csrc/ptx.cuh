@@ -142,6 +142,23 @@ __device__ __forceinline__ void wgmma_m64n16(float* d, uint64_t adesc, uint64_t 
   }
 }
 
+// fp16, A from registers: D (+)= A * B[smem desc], A the m64k16 fragment of the warpgroup (warp w rows [16 w, 16 w + 16),
+// registers as in an mma.sync m16n8k16 A fragment); TB = 1: B is MN-major in shared memory.  The A registers are read
+// asynchronously: they must not change until the wgmma group has completed.
+template <int TB>
+__device__ __forceinline__ void wgmma_m64n64_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t bdesc, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, %38;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(scale_d), "n"(TB));
+}
+// Orders the uses of an accumulator / A register after the wgmma_wait that completes it (the compiler sees the wgmma's
+// outputs as ready at issue).
+__device__ __forceinline__ void wgmma_fence_operand(float& x) { asm volatile("" : "+f"(x)::"memory"); }
+
 // fp16 only, one instruction for a 128- / 192- / 256-column fragment (64 / 96 / 128 registers, same layout as above:
 // registers [32 j, 32 j + 32) are the columns [64 j, 64 j + 64)).
 template <int TA, int TB>
@@ -189,6 +206,12 @@ __device__ __forceinline__ void setmaxnreg_inc() {
 __device__ __forceinline__ void stmatrix_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
   asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1), "r"(r2),
                "r"(r3)
+               : "memory");
+}
+// as stmatrix_x4, each 8x8 matrix stored transposed: the row address of lane 8 m + i receives column i of matrix m
+__device__ __forceinline__ void stmatrix_x4_trans(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.trans.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1),
+               "r"(r2), "r"(r3)
                : "memory");
 }
 __device__ __forceinline__ void ldmatrix_x4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {

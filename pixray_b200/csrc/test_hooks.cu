@@ -180,6 +180,32 @@ extern "C" int pxr_test_attention(const void* qkv, void* o, float* lse, const vo
   return 0;
 }
 
+// As pxr_test_attention, with the backward kernel chosen by bwd_kernel (0: as the engine chooses, 1: attn_bwd_kernel,
+// 2: attn_bwd_wg): the forward once, then the backward `repeat` times (none for repeat 0).  *used (nullable) receives the
+// backward kernel the plan took (1 or 2).
+extern "C" int pxr_test_attention_bwd_select(const void* qkv, void* o, float* lse, const void* d_o, void* gqkv, int B,
+                                             int T, int H, int W, float scale, int bwd_kernel, int repeat, int* used,
+                                             char* err, int errlen) {
+  if (!d_o || !gqkv || bwd_kernel < 0 || bwd_kernel > 2) {
+    if (err && errlen > 0) snprintf(err, errlen, "needs d_o, gqkv and a backward kernel 0, 1 or 2");
+    return -1;
+  }
+  AttnPlan plan;
+  int rc = attn_plan_make(&plan, static_cast<const __half*>(qkv), static_cast<__half*>(o),
+                          static_cast<const __half*>(d_o), static_cast<__half*>(gqkv), lse, B, T, H, W, scale,
+                          num_sms(), err, errlen, false, bwd_kernel);
+  if (rc) return rc;
+  if (used) *used = plan.bwd;
+  attn_forward_launch(plan, nullptr);
+  for (int i = 0; i < repeat; ++i) attn_backward_launch(plan, nullptr);
+  cudaError_t ce = cudaGetLastError();
+  if (ce != cudaSuccess) {
+    if (err) snprintf(err, errlen, "launch failed: %s", cudaGetErrorString(ce));
+    return -100;
+  }
+  return 0;
+}
+
 // Causal attention forward on caller tensors, on the path the engine's add_attention takes: the fused kernel, or with
 // PXR_FUSED_ATTN=0 the batched-GEMM chain S = scale q k^T -> causal row softmax -> O = P v (P allocated here).
 extern "C" int pxr_test_attention_causal(const void* qkv, void* o, int B, int T, int H, int W, float scale, char* err,
