@@ -475,6 +475,43 @@ typedef struct {
 int pxr_test_gemm_records(pxr_handle h, pxr_test_gemm_rec* out, int max, int* count);
 /* builds the plan pxr_test_gemm would run, without launching it: out = {wide, block_n, stages, tma_epi, grid, k_splits} */
 int pxr_test_gemm_plan_info(const pxr_test_gemm_desc* d, int out[6]);
+/* one attention the engine planned (one per add_attention call), in build order.  site: the caller (an image or text
+ * tower's block, a U-Net attention's checkpoint key, a decoder AttnBlock's prefix).  path: PXR_ATTN_FUSED (attn_tc.cu),
+ * PXR_ATTN_STREAMING (attn_long.cu) or PXR_ATTN_CHAIN (batched GEMMs around the row softmax).  backward: a backward was
+ * planned.  Tensors in attn_tc.cuh's layout: qkv / gqkv [images T, 3 W] (q | k | v, head h at column h d of each
+ * third), o / d_o [images T, W], W = heads d; d_o and gqkv may be set without a backward.  lse (fused, streaming) and
+ * delta (streaming with a backward) fp32 [images heads T], else null.  Chain: P and dP fp16 [images heads T, ldT]
+ * (dP null without a backward; dP_shared: the caller's scratch, shared with other calls), gemm[]: the indices in
+ * pxr_test_gemm_records of its S = scale q k^T, O = P v, dP = dO v^T, dq = scale dS k, dk = scale dS^T q and
+ * dv = P^T dO plans (-1: not planned).  Fused: splits (CTAs per (image, head) pair) and bwd (1 attn_bwd_kernel,
+ * 2 attn_bwd_wg); 1 and 0 on the other paths. */
+enum { PXR_ATTN_FUSED = 0, PXR_ATTN_STREAMING = 1, PXR_ATTN_CHAIN = 2 };
+typedef struct {
+  char site[96];
+  int path, multihead, causal, backward;
+  int images, heads, T, d, W;
+  float scale;
+  const void* qkv;
+  void* o;
+  const void* d_o;
+  void* gqkv;
+  float* lse;
+  float* delta;
+  void* P;
+  void* dP;
+  int ldT, dP_shared;
+  int splits, bwd;
+  int gemm[6];
+} pxr_test_attn_rec;
+
+/* the attentions planned so far, in build order, as pxr_test_conv_records */
+int pxr_test_attention_records(pxr_handle h, pxr_test_attn_rec* out, int max, int* count);
+/* rebuilds a fused or streaming record's plan from its shape, scale and causal flag on caller DEVICE tensors laid out as
+ * the record's (d_o / gqkv null: forward only; delta: the streaming backward's workspace), runs its forward and, with
+ * d_o and gqkv, its backward once, synchronously.  bwd_kernel as pxr_test_attention_bwd_select (0: the plan's own
+ * choice).  out2 = {splits, bwd} of the plan, as the record holds them. */
+int pxr_test_attention_plan(const pxr_test_attn_rec* r, const void* qkv, void* o, const void* d_o, void* gqkv, float* lse,
+                            float* delta, int bwd_kernel, int out2[2], char* err, int errlen);
 /* the engine's live device allocations (dalloc / upload), in allocation order: ptr[i], bytes[i] for i < min(max, n),
  * *count = n */
 int pxr_test_allocations(pxr_handle h, const void** ptr, long long* bytes, int max, int* count);
@@ -552,9 +589,10 @@ int pxr_test_resample(int op, const void* in, int ld_in, void* out, int ld_out, 
 int pxr_test_gemv(const void* w, int K, int R, const float* x, const float* bias, int relu, const float* res, float* y);
 
 /* the row softmax of the unfused attention on DEVICE fp16 [rows, ld] (ld % 8 == 0, cols <= ld; pad columns come back
- * 0): backward == 0 turns the scores in p_or_s into probabilities in place; backward != 0 overwrites dp (dP) with
+ * 0): op 0 turns the scores in p_or_s into probabilities in place; op 2 does the same with row r (of each block of cols
+ * rows) attending to columns <= r (the text towers' causal softmax); op 1 overwrites dp (dP) with
  * dS = P * (dP - <P, dP>), P in p_or_s.  Synchronous on the default stream. */
-int pxr_test_softmax(int backward, void* p_or_s, void* dp, int rows, int cols, int ld);
+int pxr_test_softmax(int op, void* p_or_s, void* dp, int rows, int cols, int ld);
 
 /* the Prompt loss (pixray.py:275-280) of B embeddings against n prompt rows, as the engine runs it: e [B, D] ->
  * e_unit [B, D] (nullable) = e / max(|e|, 1e-12); losses[slots[j]] += |w_j| dist_bj inv_rows[j] / cutn_global summed over

@@ -99,6 +99,19 @@ class TestGemmRec(C.Structure):
                 ("red_bias", C.c_void_p), ("red_res", C.c_void_p), ("red_out", C.c_void_p), ("ld_out", C.c_longlong)]
 
 
+class TestAttnRec(C.Structure):
+    _fields_ = [("site", C.c_char * 96),
+                ("path", C.c_int), ("multihead", C.c_int), ("causal", C.c_int), ("backward", C.c_int),
+                ("images", C.c_int), ("heads", C.c_int), ("T", C.c_int), ("d", C.c_int), ("W", C.c_int),
+                ("scale", C.c_float),
+                ("qkv", C.c_void_p), ("o", C.c_void_p), ("d_o", C.c_void_p), ("gqkv", C.c_void_p),
+                ("lse", C.c_void_p), ("delta", C.c_void_p), ("P", C.c_void_p), ("dP", C.c_void_p),
+                ("ldT", C.c_int), ("dP_shared", C.c_int), ("splits", C.c_int), ("bwd", C.c_int),
+                ("gemm", C.c_int * 6)]
+
+
+ATTN_FUSED, ATTN_STREAMING, ATTN_CHAIN = 0, 1, 2  # pxr_test_attn_rec.path
+
 # every symbol include/pixray_b200.h declares (tests check the library exports all of them)
 EXPORTS = [
     "pxr_last_error", "pxr_version", "pxr_create", "pxr_destroy", "pxr_load_weight", "pxr_finalize", "pxr_set_clip_tower",
@@ -113,6 +126,7 @@ EXPORTS = [
     "pxr_cutout_sets", "pxr_make_cutouts_set", "pxr_iterate_sets",
     "pxr_test_conv_records", "pxr_test_packed_weights", "pxr_test_conv_plan_info",
     "pxr_test_gemm_records", "pxr_test_gemm_plan_info", "pxr_test_allocations",
+    "pxr_test_attention_records", "pxr_test_attention_plan",
 ]
 
 _lib = None

@@ -7,7 +7,6 @@
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
-#include <cstring>
 #include <mutex>
 
 namespace pxr {
@@ -362,12 +361,8 @@ int attn_plan_make(AttnPlan* plan, const __half* qkv, __half* o, const __half* d
   });
   // The wgmma backward needs the whole pair in one CTA; with fewer pairs than SMs the split mma.sync kernel keeps every SM
   // busy instead.
-  static const bool force_mma = [] {
-    const char* e = getenv("PXR_ATTN_BWD");
-    return e && strcmp(e, "mma") == 0;
-  }();
   if (bwd == ATTN_BWD_AUTO)
-    bwd = !force_mma && d_o && gqkv && !causal && pairs >= sms && attn_bwd_wg_fits(T) ? ATTN_BWD_WG : ATTN_BWD_MMA;
+    bwd = d_o && gqkv && !causal && pairs >= sms && attn_bwd_wg_fits(T) ? ATTN_BWD_WG : ATTN_BWD_MMA;
   if (bwd == ATTN_BWD_WG) {
     const int rc = attn_bwd_wg_prepare(plan, err, errlen);
     if (rc) return rc;

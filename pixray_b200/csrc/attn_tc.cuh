@@ -56,7 +56,8 @@ bool attn_supported(int T, int head_dim, int W);
 // qkv: [B*T, 3W]; o: [B*T, W]; d_o: [B*T, W]; gqkv: [B*T, 3W]; lse: [B*H*T].  causal: the forward masks keys after each
 // row (the backward kernel has no mask: a causal plan is forward only).  bwd: ATTN_BWD_AUTO takes attn_bwd_wg for a
 // non-causal backward with at least one (image, head) pair per SM and T <= 208 (attn_bwd_wg_fits), attn_bwd_kernel
-// otherwise, or always with PXR_ATTN_BWD=mma; ATTN_BWD_MMA / ATTN_BWD_WG force one (the latter fails where it cannot run).
+// otherwise; ATTN_BWD_MMA / ATTN_BWD_WG force one (the latter fails where it cannot run; the engine forces the former
+// with PXR_ATTN_BWD=mma).
 int attn_plan_make(AttnPlan* plan, const __half* qkv, __half* o, const __half* d_o, __half* gqkv, float* lse, int B,
                    int T, int H, int W, float scale, int num_sms, char* err, int errlen, bool causal = false,
                    int bwd = ATTN_BWD_AUTO);

@@ -39,6 +39,7 @@ class Engine {
   bool stream16 = true;       // the ViT residual stream and its gradient in fp16, like the reference's CUDA path (clip.load gives a half model, slip.py:176); PXR_CLIP_STREAM=32 keeps them in fp32
   bool fused_attn = true;     // PXR_FUSED_ATTN=0: fall back to the batched-GEMM attention (attn_tc.cu covers T <= 240,
                               // attn_long.cu T > 257)
+  bool attn_bwd_mma = false;  // PXR_ATTN_BWD=mma: the fused attention backward on attn_bwd_kernel where attn_bwd_wg would run
   std::map<std::string, HostWeight> weights[5];
   std::vector<void*> allocs;
   std::vector<size_t> alloc_bytes;  // bytes of allocs[i] (pxr_test_allocations)
@@ -50,6 +51,8 @@ class Engine {
   std::vector<pxr_test_conv_rec> conv_log;
   // what add_gemm / add_gemm_splitk planned, in order (pxr_test_gemm_records)
   std::vector<pxr_test_gemm_rec> gemm_log;
+  // what add_attention planned, in order (pxr_test_attention_records)
+  std::vector<pxr_test_attn_rec> attn_log;
 
   // sharding
   int n_local = 0, first_global = 0;
@@ -190,6 +193,7 @@ class Engine {
     int act;  // ACT_QUICKGELU or ACT_GELU
     float eps;
     bool causal;
+    std::string site;  // the tower and layer, for the attention record
     act_t *go = nullptr, *gqkv = nullptr, *dP = nullptr, *g4 = nullptr, *gh = nullptr, *gx16 = nullptr;
     float* gx = nullptr;
   };
@@ -864,8 +868,9 @@ class Engine {
   // head-batched shapes; otherwise (taming's AttnBlock) always the chain, tile widths by add_gemm.
   // The chain's P is allocated here (and returned; nullptr on the fused paths), its dP too unless the caller passes a
   // scratch that several calls share.  causal (the text towers): row t attends to tokens <= t; forward only, multihead,
-  // on the fused kernel or the chain with a causal row softmax (T <= 240 either way).
-  act_t* add_attention(OpList& fwd, OpList* bwd, const act_t* qkv, act_t* o, const act_t* d_o, act_t* gqkv, int images,
+  // on the fused kernel or the chain with a causal row softmax (T <= 240 either way).  Each call appends one record to
+  // attn_log; `site` names the caller there.
+  act_t* add_attention(const std::string& site, OpList& fwd, OpList* bwd, const act_t* qkv, act_t* o, const act_t* d_o, act_t* gqkv, int images,
                        int heads, int T, int d, float scale, bool multihead, act_t* dP = nullptr, bool causal = false);
   bool attn_fused(int T, int d, int heads) const { return fused_attn && attn_supported(T, d, heads * d); }
   // T = 256 / 257 (the vdiff 16^2 level, ViT-L/14) stay on the chain: the streaming kernels start past them
@@ -957,6 +962,7 @@ void Engine::create() {
   if (fmt != PXR_DTYPE_F16) throw EngineError(-5, "only PXR_DTYPE_F16 operands are wired through the pointwise kernels");
   if (cfg.grad_scale > 0) S = cfg.grad_scale;
   if (const char* fa = getenv("PXR_FUSED_ATTN")) fused_attn = atoi(fa) != 0;
+  if (const char* ab = getenv("PXR_ATTN_BWD")) attn_bwd_mma = strcmp(ab, "mma") == 0;
   if (const char* cs16 = getenv("PXR_CLIP_STREAM")) stream16 = atoi(cs16) != 32;
   if (const char* gc = getenv("PXR_GN_COOP")) gn_coop = atoi(gc) != 0;
   if (const char* sk = getenv("PXR_CONV_SPLITK")) conv_splitk = atoi(sk) != 0;
@@ -1204,7 +1210,7 @@ Engine::AttnBlock Engine::attnblock_fwd(OpList& l, const Act& x, const std::stri
     e.ldc = 3 * c;
     add_gemm(l, opK(a.a.p, c, T, c), opK(a.wqkv, c, 3 * c, c), T, 3 * c, c, e);
   }
-  add_attention(l, grad ? &a.attn_bwd : nullptr, qkv, a.O.p, a.O.g, a.gqkv, 1, 1, T, c, 1.f / std::sqrt((float)c), false);
+  add_attention(prefix, l, grad ? &a.attn_bwd : nullptr, qkv, a.O.p, a.O.g, a.gqkv, 1, 1, T, c, 1.f / std::sqrt((float)c), false);
   {
     GemmEpilogue e;
     e.bias = a.po.bias;
@@ -1237,18 +1243,42 @@ void Engine::attnblock_bwd(const AttnBlock& a) {
   bwd_stack.push_back(std::move(b));
 }
 
-act_t* Engine::add_attention(OpList& fwd, OpList* bwd, const act_t* qkv, act_t* o, const act_t* d_o, act_t* gqkv,
-                             int images, int heads, int T, int d, float scale, bool multihead, act_t* dP, bool causal) {
+act_t* Engine::add_attention(const std::string& site, OpList& fwd, OpList* bwd, const act_t* qkv, act_t* o,
+                             const act_t* d_o, act_t* gqkv, int images, int heads, int T, int d, float scale,
+                             bool multihead, act_t* dP, bool causal) {
   const int W = heads * d, ldT = round_up(T, 8);
   cudaStream_t cs = st;
   if (causal && (bwd || !multihead || !attn_supported(T, d, W)))
     throw EngineError(-54, "causal attention is forward only, with 64-wide heads and T <= 240");
+  attn_log.emplace_back();
+  pxr_test_attn_rec& rec = attn_log.back();
+  snprintf(rec.site, sizeof rec.site, "%s", site.c_str());
+  rec.multihead = multihead;
+  rec.causal = causal;
+  rec.backward = bwd != nullptr;
+  rec.images = images;
+  rec.heads = heads;
+  rec.T = T;
+  rec.d = d;
+  rec.W = W;
+  rec.scale = scale;
+  rec.qkv = qkv;
+  rec.o = o;
+  rec.d_o = d_o;
+  rec.gqkv = gqkv;
+  rec.splits = 1;
+  for (int& g : rec.gemm) g = -1;
   if (multihead && attn_fused(T, d, heads)) {  // S, softmax and PV in one kernel; S / P never leave the SM
     float* lse = dalloc<float>((size_t)images * heads * T);
     auto ap = std::make_shared<AttnPlan>();
     char buf[256] = {0};
-    int rc = attn_plan_make(ap.get(), qkv, o, d_o, gqkv, lse, images, T, heads, W, scale, num_sms, buf, sizeof buf, causal);
+    int rc = attn_plan_make(ap.get(), qkv, o, d_o, gqkv, lse, images, T, heads, W, scale, num_sms, buf, sizeof buf, causal,
+                            attn_bwd_mma ? ATTN_BWD_MMA : ATTN_BWD_AUTO);
     if (rc) throw EngineError(rc, std::string("attention plan: ") + buf);
+    rec.path = PXR_ATTN_FUSED;
+    rec.lse = lse;
+    rec.splits = ap->splits;
+    rec.bwd = ap->bwd;
     char lab[96];
     snprintf(lab, sizeof lab, "attn_fwd%s B=%d T=%d heads=%d", causal ? "_causal" : "", images, T, heads);
     fwd.add(1, [ap, cs] { attn_forward_launch(*ap, cs); }, ap->flops_fwd, lab, ap->bytes_fwd);
@@ -1265,6 +1295,9 @@ act_t* Engine::add_attention(OpList& fwd, OpList* bwd, const act_t* qkv, act_t* 
     char buf[256] = {0};
     int rc = attn_long_plan_make(ap.get(), qkv, o, d_o, gqkv, lse, delta, images, T, heads, W, scale, buf, sizeof buf);
     if (rc) throw EngineError(rc, std::string("attention plan: ") + buf);
+    rec.path = PXR_ATTN_STREAMING;
+    rec.lse = lse;
+    rec.delta = delta;
     char lab[96];
     snprintf(lab, sizeof lab, "attn_long_fwd B=%d T=%d heads=%d", images, T, heads);
     fwd.add(1, [ap, cs] { attn_long_forward_launch(*ap, cs); }, ap->flops_fwd, lab, ap->bytes_fwd);
@@ -1281,6 +1314,11 @@ act_t* Engine::add_attention(OpList& fwd, OpList* bwd, const act_t* qkv, act_t* 
   const long long ps0 = (long long)T * ldT, ps1 = (long long)heads * T * ldT;   // ... in P / dP
   const int rows = images * heads * T;
   act_t* P = dalloc<act_t>((size_t)rows * ldT);
+  rec.path = PXR_ATTN_CHAIN;
+  rec.P = P;
+  rec.ldT = ldT;
+  int* gi = rec.gemm;  // the index the next add_gemm's record takes, for each GEMM of the chain in turn
+  *gi++ = (int)gemm_log.size();
   {  // S = scale q k^T
     GemmEpilogue e;
     e.alpha = scale;
@@ -1293,6 +1331,7 @@ act_t* Engine::add_attention(OpList& fwd, OpList* bwd, const act_t* qkv, act_t* 
   }
   if (causal) fwd.add(1, [=] { softmax_forward_causal(P, rows, T, ldT, cs); }, 0.0, "softmax_forward_causal");
   else fwd.add(1, [=] { softmax_forward(P, rows, T, ldT, cs); }, 0.0, "softmax_forward");
+  *gi++ = (int)gemm_log.size();
   {  // O = P v
     GemmEpilogue e;
     e.out_f16 = o;
@@ -1303,7 +1342,10 @@ act_t* Engine::add_attention(OpList& fwd, OpList* bwd, const act_t* qkv, act_t* 
              T, d, T, e, bn_d);
   }
   if (!bwd) return P;
+  rec.dP_shared = dP != nullptr;
   if (!dP) dP = dalloc<act_t>((size_t)rows * ldT);
+  rec.dP = dP;
+  *gi++ = (int)gemm_log.size();
   {  // dP = dO v^T
     GemmEpilogue e;
     e.out_f16 = dP;
@@ -1314,6 +1356,7 @@ act_t* Engine::add_attention(OpList& fwd, OpList* bwd, const act_t* qkv, act_t* 
              T, d, e, bn_s);
   }
   bwd->add(1, [=] { softmax_backward(P, dP, rows, T, ldT, cs); }, 0.0, "softmax_backward");  // dS, in place of dP
+  *gi++ = (int)gemm_log.size();
   {  // dq = scale dS k
     GemmEpilogue e;
     e.alpha = scale;
@@ -1324,6 +1367,7 @@ act_t* Engine::add_attention(OpList& fwd, OpList* bwd, const act_t* qkv, act_t* 
     add_gemm(*bwd, opK(dP, ldT, T, ldT, heads, ps0, images, ps1), opMN(qkv + W, 3 * W, d, T, heads, qs0, images, qs1), T,
              d, T, e, bn_d);
   }
+  *gi++ = (int)gemm_log.size();
   {  // dk = scale dS^T q
     GemmEpilogue e;
     e.alpha = scale;
@@ -1334,6 +1378,7 @@ act_t* Engine::add_attention(OpList& fwd, OpList* bwd, const act_t* qkv, act_t* 
     add_gemm(*bwd, opMN(dP, ldT, T, T, heads, ps0, images, ps1), opMN(qkv, 3 * W, d, T, heads, qs0, images, qs1), T, d,
              T, e, bn_d);
   }
+  *gi++ = (int)gemm_log.size();
   {  // dv = P^T dO
     GemmEpilogue e;
     e.out_f16 = gqkv + 2 * W;
@@ -2042,7 +2087,7 @@ act_t* Engine::add_block(OpList& fwd, OpList* bwd, const BlockW& w, const BlockI
     add_gemm(fwd, opK(b.h16, Wd, M, Wd), opK(w.wqkv, Wd, 3 * Wd, Wd), M, 3 * Wd, Wd, e);
   }
   OpList attn_bwd;
-  act_t* P = add_attention(fwd, bwd ? &attn_bwd : nullptr, b.qkv, b.o, b.go, b.gqkv, b.images, b.heads, b.T, 64,
+  act_t* P = add_attention(b.site, fwd, bwd ? &attn_bwd : nullptr, b.qkv, b.o, b.go, b.gqkv, b.images, b.heads, b.T, 64,
                            1.f / std::sqrt(64.f), true, b.dP, b.causal);
   {  // x_mid = x_in + O Wo^T + bo
     GemmEpilogue e;
@@ -2260,6 +2305,7 @@ void Engine::build_clip(int i) {
     const bool cls_only = clip_last_cls && l == L - 1;
     b.rows = cls_only ? B : M;
     b.ld = cls_only ? (long long)T * Wd : (long long)Wd;
+    b.site = "clip" + std::to_string(i) + " block " + std::to_string(l);
     Ly.P = add_block(C.fwd, &block_bwd[l], Ly.w, b);
   }
   C.x_out = x_cur;
@@ -4034,6 +4080,14 @@ int pxr_test_conv_records(pxr_handle h, pxr_test_conv_rec* out, int max, int* co
 int pxr_test_gemm_records(pxr_handle h, pxr_test_gemm_rec* out, int max, int* count) {
   PXR_TRY(h, {
     const auto& log = h->e->gemm_log;
+    for (int i = 0; out && i < max && i < (int)log.size(); ++i) out[i] = log[i];
+    if (count) *count = (int)log.size();
+  });
+}
+
+int pxr_test_attention_records(pxr_handle h, pxr_test_attn_rec* out, int max, int* count) {
+  PXR_TRY(h, {
+    const auto& log = h->e->attn_log;
     for (int i = 0; out && i < max && i < (int)log.size(); ++i) out[i] = log[i];
     if (count) *count = (int)log.size();
   });

@@ -275,6 +275,46 @@ extern "C" int pxr_test_attention_causal(const void* qkv, void* o, int B, int T,
   return rc;
 }
 
+// A fused or streaming attention record's plan, rebuilt through attn_plan_make / attn_long_plan_make on caller tensors
+// (the record's own pointers are not touched), run once.
+extern "C" int pxr_test_attention_plan(const pxr_test_attn_rec* r, const void* qkv, void* o, const void* d_o, void* gqkv,
+                                       float* lse, float* delta, int bwd_kernel, int out2[2], char* err, int errlen) {
+  if (!r || !qkv || !o || !lse || !out2 || (r->path != PXR_ATTN_FUSED && r->path != PXR_ATTN_STREAMING)) {
+    if (err && errlen > 0) snprintf(err, errlen, "needs a fused or streaming record, qkv, o, lse and out2");
+    return -1;
+  }
+  const __half* q = static_cast<const __half*>(qkv);
+  __half* oh = static_cast<__half*>(o);
+  const __half* g = static_cast<const __half*>(d_o);
+  __half* gq = static_cast<__half*>(gqkv);
+  int rc;
+  if (r->path == PXR_ATTN_FUSED) {
+    AttnPlan plan;
+    rc = attn_plan_make(&plan, q, oh, g, gq, lse, r->images, r->T, r->heads, r->W, r->scale, num_sms(), err, errlen,
+                        r->causal != 0, bwd_kernel);
+    if (rc) return rc;
+    out2[0] = plan.splits;
+    out2[1] = plan.bwd;
+    attn_forward_launch(plan, nullptr);
+    if (d_o && gqkv) attn_backward_launch(plan, nullptr);
+  } else {
+    AttnLongPlan plan;
+    rc = attn_long_plan_make(&plan, q, oh, g, gq, lse, delta, r->images, r->T, r->heads, r->W, r->scale, err, errlen);
+    if (rc) return rc;
+    out2[0] = 1;
+    out2[1] = 0;
+    attn_long_forward_launch(plan, nullptr);
+    if (d_o && gqkv) attn_long_backward_launch(plan, nullptr);
+  }
+  cudaError_t ce = cudaDeviceSynchronize();
+  if (ce == cudaSuccess) ce = cudaGetLastError();
+  if (ce != cudaSuccess) {
+    if (err) snprintf(err, errlen, "launch failed: %s", cudaGetErrorString(ce));
+    return -100;
+  }
+  return 0;
+}
+
 // Streaming fused attention (attn_long.cu) on the same caller tensors as pxr_test_attention; the backward's D workspace
 // [B*H*T] fp32 is allocated here.
 extern "C" int pxr_test_attention_long(const void* qkv, void* o, float* lse, const void* d_o, void* gqkv, int B, int T,
@@ -304,13 +344,15 @@ extern "C" int pxr_test_attention_long(const void* qkv, void* o, float* lse, con
   return rc;
 }
 
-// The engine's row softmax (softmax_forward / softmax_backward, unfused attention) on caller DEVICE fp16 [rows, ld]:
-// backward == 0: p_or_s holds the scores and is overwritten with the probabilities; backward != 0: p_or_s holds P and
-// dp holds dP, overwritten with dS = P * (dP - <P, dP>).
-extern "C" int pxr_test_softmax(int backward, void* p_or_s, void* dp, int rows, int cols, int ld) {
-  if (!p_or_s || rows < 1 || cols < 1 || ld < cols || ld % 8 || (backward && !dp)) return -1;
-  if (backward) softmax_backward(static_cast<const act_t*>(p_or_s), static_cast<act_t*>(dp), rows, cols, ld, nullptr);
-  else softmax_forward(static_cast<act_t*>(p_or_s), rows, cols, ld, nullptr);
+// The engine's row softmax (softmax_forward / softmax_forward_causal / softmax_backward, unfused attention) on caller
+// DEVICE fp16 [rows, ld]: op 0 / 2: p_or_s holds the scores and is overwritten with the probabilities (2: causal);
+// op 1: p_or_s holds P and dp holds dP, overwritten with dS = P * (dP - <P, dP>).
+extern "C" int pxr_test_softmax(int op, void* p_or_s, void* dp, int rows, int cols, int ld) {
+  if (!p_or_s || rows < 1 || cols < 1 || ld < cols || ld % 8 || op < 0 || op > 2 || (op == 1 && !dp)) return -1;
+  if (op == 1) softmax_backward(static_cast<const act_t*>(p_or_s), static_cast<act_t*>(dp), rows, cols, ld, nullptr);
+  else if (op == 2) {
+    if (softmax_forward_causal(static_cast<act_t*>(p_or_s), rows, cols, ld, nullptr)) return -1;
+  } else softmax_forward(static_cast<act_t*>(p_or_s), rows, cols, ld, nullptr);
   cudaError_t ce = cudaDeviceSynchronize();
   if (ce == cudaSuccess) ce = cudaGetLastError();
   return ce == cudaSuccess ? 0 : -100;

@@ -72,25 +72,30 @@ def _run(qkv, d_o, B, T, H, scale, repeat=1, check=True):
     return o, lse, gqkv
 
 
-def _split(t, B, T, H):
-    """[B*T, n*64*H] -> [n, B, H, T, 64]"""
-    n = t.shape[1] // (64 * H)
-    return t.reshape(B, T, n, H, 64).permute(2, 0, 3, 1, 4)
+def _split(t, B, T, H, d=64):
+    """[B*T, n*d*H] -> [n, B, H, T, d]"""
+    n = t.shape[1] // (d * H)
+    return t.reshape(B, T, n, H, d).permute(2, 0, 3, 1, 4)
 
 
-def _reference(qkv, d_o, B, T, H, scale):
-    """float64 outputs and per-element magnitudes, all [B, H, T, 64] (lse [B, H, T])."""
-    x = _split(qkv.cpu().double(), B, T, H)
+def _reference(qkv, d_o, B, T, H, scale, d=64, causal=False, device="cpu"):
+    """float64 outputs and per-element magnitudes, all [B, H, T, d] (lse [B, H, T]), on `device`.  causal: row t
+    attends to keys <= t (the forward only)."""
+    x = _split(qkv.to(device).double(), B, T, H, d)
     q, k, v = x[0], x[1], x[2]
     s = (q @ k.transpose(-1, -2)) * scale
+    keep = torch.ones(T, T, dtype=torch.bool, device=device).tril() if causal else None
+    if causal:
+        s = s.masked_fill(~keep, float("-inf"))
     lse = torch.logsumexp(s, -1)
     p = torch.exp(s - lse[..., None])
     o = p @ v
     ref = dict(o=o, lse=lse)
-    pf = p + TINY  # P as an fp16 MMA operand
-    mag = dict(o=pf @ v.abs(), lse=1 + scale * (q.abs() @ k.abs().transpose(-1, -2)).amax(-1))
+    pf = p + (TINY * keep if causal else TINY)  # P as an fp16 MMA operand (masked keys take no part)
+    sa = q.abs() @ k.abs().transpose(-1, -2)
+    mag = dict(o=pf @ v.abs(), lse=1 + scale * (sa.masked_fill(~keep, 0) if causal else sa).amax(-1))
     if d_o is not None:
-        g = _split(d_o.cpu().double(), B, T, H)[0]
+        g = _split(d_o.to(device).double(), B, T, H, d)[0]
         dp = g @ v.transpose(-1, -2)
         ds = p * (dp - (g * o).sum(-1, keepdim=True))
         ref.update(dq=scale * ds @ k, dk=scale * ds.transpose(-1, -2) @ q, dv=p.transpose(-1, -2) @ g)
@@ -128,9 +133,9 @@ def _check(label, o, lse, gqkv, ref, mag, B, T, H):
     assert not bad, "\n".join(bad)
 
 
-def _inputs(B, T, H, seed, qkv_std=1.5):
+def _inputs(B, T, H, seed, qkv_std=1.5, d=64):
     g = torch.Generator(device="cuda").manual_seed(seed)
-    W = 64 * H
+    W = d * H
     qkv = (torch.randn(B * T, 3 * W, generator=g, device="cuda") * qkv_std).half()
     d_o = torch.randn(B * T, W, generator=g, device="cuda").half()
     return qkv, d_o
@@ -166,15 +171,15 @@ def test_attention_any_scale(B, T, H, scale):
     _case(f"B={B} T={T} H={H} scale={scale}", qkv, d_o, B, T, H, scale)
 
 
-def _peaked(B, T, H, target, seed):
+def _peaked(B, T, H, target, seed, d=64, scale=0.125):
     """Every query's largest score is at key `target` (per head), about 8 above the rest: P ~ 0.94 there."""
     g = torch.Generator(device="cuda").manual_seed(seed)
-    W = 64 * H
+    W = d * H
     qkv = torch.randn(B * T, 3 * W, generator=g, device="cuda") * 0.5
-    x = qkv.view(B, T, 3, H, 64)
+    x = qkv.view(B, T, 3, H, d)
     x[:, :, 0, :, 0] = 4.0
     x[:, :, 1, :, 0] = 0.5 * torch.randn(B, T, H, generator=g, device="cuda")
-    x[:, target, 1, :, 0] = 16.0
+    x[:, target, 1, :, 0] = 2.0 / scale
     return qkv.half(), torch.randn(B * T, W, generator=g, device="cuda").half()
 
 
