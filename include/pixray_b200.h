@@ -287,6 +287,10 @@ int pxr_vdiff_set_schedule(pxr_handle h, const float* steps, const float* alphas
 int pxr_vdiff_set_clip_embed(pxr_handle h, const float* embed, int D);
 int pxr_vdiff_set_iteration(pxr_handle h, int i);
 int pxr_vdiff_renoise(pxr_handle h, float* z, int i, const float* noise);
+/* the U-Net's size (VdiffDrawer's gen_height / gen_width, vdiff.py:55-58), before pxr_finalize: sides multiples of 64,
+ * each at least the canvas's.  x (z), v, pred and the optimiser state are [1, 3, gen_h, gen_w]; the image is the canvas-size
+ * window at rows (gen_h - H) / 2.., columns (gen_w - W) / 2.. of (pred + 1) / 2 clamped.  Not called: gen = the canvas. */
+int pxr_vdiff_set_gen_size(pxr_handle h, int gen_h, int gen_w);
 
 int pxr_reset_optimizer(pxr_handle h); /* rebuild_optimisers: a fresh instance of the current rule (pixray.py:520-555, 1511) */
 
@@ -570,6 +574,13 @@ int pxr_test_groupnorm(int variant, const void* x, const float* ws, int splits, 
 int pxr_test_groupnorm_unet(const void* x, const float* gamma, const float* beta, float gamma_add, int act, const void* res,
                             float eps, int pixels, int C, void* y, float* stats, const void* dy, const void* dres, void* dx,
                             float* scratch);
+/* the same on the path `path` names: 0 the single-kernel GroupNorm (scratch as above; -1 where it does not cover the
+ * shape), 1 the three-kernel GroupNorm the U-Net takes where the single kernel does not fit (any shape with C % 32 == 0,
+ * 256 % (C / 8) == 0; scratch: 2 * 64 * partials floats (pxr_test_groupnorm_partials) then the backward's 64). */
+int pxr_test_groupnorm_unet_path(int path, const void* x, const float* gamma, const float* beta, float gamma_add, int act,
+                                 const void* res, float eps, int pixels, int C, void* y, float* stats, const void* dy,
+                                 const void* dres, void* dx, float* scratch);
+int pxr_test_groupnorm_partials(int pixels, int C); /* the three-kernel path's block partials at this shape */
 
 /* one resampling / copy kernel on DEVICE NHWC fp16 tensors, by op:
  *   0 upsample2x              in [H, W] (pixel stride ld_in) -> out [2H, 2W]             nearest

@@ -55,7 +55,7 @@ from . import losses as L
 from . import pixel_shapes as PS
 from . import plugins as P
 from . import synthetic as S
-from .util import apply_overlay, get_learning_rate_drops, parse_unit, split_pipes
+from .util import apply_overlay, get_learning_rate_drops, parse_unit, split_pipes, vdiff_gen_size, vdiff_image_size
 
 # pixray.class_table (pixray.py:74-113) restricted to the drawers of the BASELINE configs.  "pixel" contributes the reference
 # PixelDrawer's five options; its default rect grid runs as fast_pixel (the square cells diffvg renders, SURVEY.md 2,
@@ -391,6 +391,14 @@ def do_init(args):
     n_levels = len(E.VQGAN_F16_16384["ch_mult"]) if kind == E.DRAWER_VQGAN else None
     sideX, sideY = _side(args, n_levels)
     engine_hw = (sideY, sideX)
+    vdiff_gen_hw = None
+    if kind == E.DRAWER_VDIFF:
+        # VdiffDrawer runs its U-Net at the canvas rounded up to 128 per side and centre-crops the image back to the canvas
+        # (vdiff.py:55-58, 165-170); with no margin to cut the image is the whole gen-size frame
+        gw, gh, _, _ = vdiff_gen_size(sideX, sideY)
+        vdiff_gen_hw = (gh, gw)
+        iw, ih = vdiff_image_size(sideX, sideY)
+        engine_hw = (ih, iw)
     if kind == E.DRAWER_SUPERRES:
         # the start image is resized to the requested size and z is a quarter of it, rounded down; the net's x4 output,
         # which the cutouts see, is 4 * (size // 4) (super_resolution.py:75-83)
@@ -408,6 +416,8 @@ def do_init(args):
     world = int(getattr(args, "b200_world", 1) or 1)
     if world > 1:
         kw.update(rank=int(args.b200_rank), world=world)
+    if vdiff_gen_hw is not None:
+        kw["vdiff_gen_hw"] = vdiff_gen_hw
     if kind == E.DRAWER_PIXEL:  # fast_pixeldrawer.py:37-63: 40x40 / 40x50 / 80x45 default grid, pixel_scale, clamp to canvas
         kw["grid"] = P.FastPixelDrawer.grid_for((sideX, sideY), getattr(args, "pixel_size", None), getattr(args, "pixel_scale", None))
         print(f"Running fast pixeldrawer with {kw['grid'][1]}x{kw['grid'][0]} grid")

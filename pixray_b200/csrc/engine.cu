@@ -887,6 +887,7 @@ class Engine {
   VConv vd_load_conv(const std::string& prefix, int cin_real, int cin, int cout, int ks, bool has_bias, bool tiny);
   void vd_conv_fwd(OpList& l, const act_t* x, int H, int Wd, const VConv& v, GemmEpilogue e);
   void vd_conv_bwd(OpList& l, const act_t* dy, int H, int Wd, const VConv& v, GemmEpilogue e);
+  void vd_check_col(size_t elems) const;
   GNSaved vd_norm(OpList& l, const Act& x, const float* gamma, const float* beta, float gamma_add, int act,
                   const act_t* res, act_t* y);
   void vd_norm_bwd(OpList& l, const act_t* dy, const Act& x, const GNSaved& s, const float* gamma, const float* beta,
@@ -905,6 +906,11 @@ class Engine {
   float *vd_pred = nullptr, *vd_v = nullptr, *vd_gpred = nullptr, *vd_vout = nullptr, *vd_mod_out = nullptr,
         *vd_h0 = nullptr, *vd_te = nullptr, *vd_tmp[5] = {nullptr}, *vd_b[5] = {nullptr};
   act_t *vd_gv = nullptr, *vd_col = nullptr, *vd_xin = nullptr, *vd_gin = nullptr, *vd_wmod = nullptr, *vd_w[5] = {nullptr};
+  // the U-Net's size (pxr_vdiff_set_gen_size; 0: the canvas) and the canvas's window in it
+  int vd_gen_h = 0, vd_gen_w = 0;
+  VdCrop vd_crop{};
+  size_t vd_col_elems = 0, gn_part_elems = 0;
+  float* vd_gstats = nullptr;  // the three-kernel GroupNorm backward's [32][2] fold (one norm runs at a time)
 
   // ------------------------------------------------------------------ super-resolution drawer (engine_superres.inc)
   struct SrConv;
@@ -2978,9 +2984,10 @@ void Engine::finalize() {
       reg("stroke_winner", sscene.winner, npx / 3 * 4 * sizeof(int));
       reg("stroke_caps", sscene.caps, (size_t)sscene.n_caps * sizeof(float4));
     }
-    if (vd_pred) {
-      reg("vd_pred", vd_pred, npx * 4);
-      reg("vd_v", vd_v, npx * 4);
+    if (vd_pred) {  // gen-size
+      reg("vd_pred", vd_pred, z_numel * 4);
+      reg("vd_v", vd_v, z_numel * 4);
+      reg("vd_gpred", vd_gpred, z_numel * 4);
     }
     for (int i = 0; i < cfg.n_clip; ++i) {
       Clip& C = clip[i];
@@ -3290,6 +3297,25 @@ int pxr_set_strokes(pxr_handle h, int n_paths, int n_segments, float max_width, 
     e->stroke_segments = n_segments;
     e->stroke_max_width = max_width;
     e->stroke_paper = paper_trainable ? 1 : 0;
+  });
+}
+
+// The vdiff U-Net's size (VdiffDrawer's gen_width / gen_height, vdiff.py:55-58): x, v and the optimiser state are
+// [1, 3, gen_h, gen_w]; the image is the canvas-size window centred in it.  Before pxr_finalize; without it gen = canvas.
+int pxr_vdiff_set_gen_size(pxr_handle h, int gen_h, int gen_w) {
+  PXR_TRY(h, {
+    Engine* e = h->e;
+    if (e->cfg.drawer != PXR_DRAWER_VDIFF) throw EngineError(-59, "pxr_vdiff_set_gen_size: not a vdiff engine");
+    if (e->finalized) throw EngineError(-12, "pxr_vdiff_set_gen_size: the U-Net size cannot change after pxr_finalize");
+    if (gen_h < 64 || gen_w < 64 || gen_h % 64 || gen_w % 64)
+      throw EngineError(-55, "pxr_vdiff_set_gen_size: " + std::to_string(gen_h) + " x " + std::to_string(gen_w) +
+                                 "; the U-Net's sides must be multiples of 64 (six 2x down-samplings)");
+    if (gen_h < e->cfg.image_h || gen_w < e->cfg.image_w)
+      throw EngineError(-55, "pxr_vdiff_set_gen_size: " + std::to_string(gen_h) + " x " + std::to_string(gen_w) +
+                                 " is smaller than the canvas " + std::to_string(e->cfg.image_h) + " x " +
+                                 std::to_string(e->cfg.image_w));
+    e->vd_gen_h = gen_h;
+    e->vd_gen_w = gen_w;
   });
 }
 

@@ -30,15 +30,24 @@ void vq_select(const float* scores, int ld, const float* z, const float* cb, con
 // z_grad[C, hw] fp32 = dzq[hw, C] fp16 / grad_scale   (ReplaceGrad: gradient of z_q goes to z unchanged)
 void vq_backward(const act_t* dzq, float inv_scale, int C, int hw, float* z_grad, cudaStream_t st);
 
-// GroupNorm(32, C, eps) [+ swish] over NHWC fp16.  stats: [32][2] (mean, rstd); part: scratch [nblk][32][2].
+// Variants for the vdiff U-Net (cc12m_1.py:41-50, 78-97): GroupNorm(1, C) (one_group), gamma = modulation scale + 1
+// (gamma_add, gamma/beta may be null = 0), activation `swish` argument: 0 none, 1 swish, 2 ReLU, forward residual add.
+struct GnOpts {
+  int one_group = 0;
+  float gamma_add = 0.f;
+  const act_t* res = nullptr;  // forward only: y = act(norm(x)) + res
+};
+// GroupNorm(32, C, eps) [+ swish] over NHWC fp16 in three kernels (partial sums, a fixed-order fold, an elementwise pass),
+// for every shape: no shared-memory limit.  stats: [32][2] (mean, rstd); part: scratch [2 nblk][32][2] with nblk =
+// gn_num_partials.  `o` takes the U-Net's variants as the single-kernel path below does (swish 2 = ReLU).
 int gn_num_partials(int pixels, int C);
-void gn_stats(const act_t* x, int pixels, int C, float eps, float* part, float* stats, cudaStream_t st);
+void gn_stats(const act_t* x, int pixels, int C, float eps, float* part, float* stats, cudaStream_t st, GnOpts o = GnOpts());
 void gn_apply(const act_t* x, const float* stats, const float* gamma, const float* beta, int pixels, int C, int swish,
-              act_t* y, cudaStream_t st);
-// dx = GroupNorm'(x) applied to dy (through swish when set) [+ dres]; part2 scratch like gn_stats.
+              act_t* y, cudaStream_t st, GnOpts o = GnOpts());
+// dx = GroupNorm'(x) applied to dy (through the activation) [+ dres]; part scratch like gn_stats, gstats [32][2].
 void gn_backward(const act_t* dy, const act_t* x, const float* stats, const float* gamma, const float* beta,
                  int pixels, int C, int swish, const act_t* dres, float* part, float* gstats, act_t* dx,
-                 cudaStream_t st);
+                 cudaStream_t st, GnOpts o = GnOpts());
 
 // The same two operations as ONE kernel each (grid <= one block per SM, grid-wide barrier between the statistics and the apply
 // phase, the block's slab of x kept in shared memory): 1 launch and 1 HBM pass instead of 3 launches and 2 passes.
@@ -48,13 +57,6 @@ void gn_backward(const act_t* dy, const act_t* x, const float* stats, const floa
 struct GridBarrier {
   unsigned long long* counter = nullptr;  // device, zero-initialised
   unsigned long long issued = 0;
-};
-// Variants for the vdiff U-Net (cc12m_1.py:41-50, 78-97): GroupNorm(1, C) (one_group), gamma = modulation scale + 1
-// (gamma_add, gamma/beta may be null = 0), activation `swish` argument: 0 none, 1 swish, 2 ReLU, forward residual add.
-struct GnOpts {
-  int one_group = 0;
-  float gamma_add = 0.f;
-  const act_t* res = nullptr;  // forward only: y = act(norm(x)) + res
 };
 #ifdef __CUDACC__
 // The GroupNorm kernels take the variance as E[x^2] - mean^2 from fp32 partial sums, whose rounding error grows with
@@ -488,9 +490,15 @@ void copy_channels(const act_t* src, int ld_src, act_t* dst, int ld_dst, int C, 
 void im2col3x3(const act_t* x, int H, int W, int C, act_t* A, cudaStream_t st);  // A [pixels, 9 C], tap-major
 void gemv_f16(const act_t* W, int K, int R, const float* x, const float* bias, int relu, const float* res, float* y,
               cudaStream_t st);
-void vd_finish(const float* vout, int ld, const float* x, float alpha, float sigma, int pixels, float* v_planar,
+// The U-Net runs at the gen size (gh, gw); the canvas (h, w) is its window at rows my.., columns mx.. (VdiffDrawer.synth's
+// centre crop, vdiff.py:165-170).  v / pred / g_pred / g_v are gen-size, pre / img / g_img canvas-size; g_pred and g_v are
+// zero outside the window.
+struct VdCrop {
+  int gh, gw, h, w, my, mx;
+};
+void vd_finish(const float* vout, int ld, const float* x, float alpha, float sigma, VdCrop c, float* v_planar,
                float* pred, float* pre, float* img, cudaStream_t st);
-void vd_finish_backward(const float* g_img, const float* pre, float sigma, int pixels, int ld, float* g_pred, act_t* g_v,
+void vd_finish_backward(const float* g_img, const float* pre, float sigma, VdCrop c, int ld, float* g_pred, act_t* g_v,
                         cudaStream_t st);
 void vd_zgrad(const float* g_pred, const act_t* g_in, int ld, float alpha, float inv_scale, int pixels, float* z_grad,
               cudaStream_t st);

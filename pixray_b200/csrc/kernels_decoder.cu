@@ -212,13 +212,14 @@ __device__ __forceinline__ void gn_block_reduce(const float (&s)[2][2], float (*
 // (d, d^2) with d = x - pivot into part[gridDim.x + block], the pivot of a group being x at pixel 0 in the group's first
 // channel (gn_pivot): gn_final_kernel takes the statistics from the second set where the first loses its precision
 // (gn_refine_variance).  MODE 1: backward sums (dxh, dxh * xh).  Block: 256 threads = (256 / (C/8)) pixel lanes x (C/8)
-// channel vectors.
+// channel vectors.  one_group (GroupNorm(1, C)): every group's pivot is x[0, 0], so gn_final_kernel can merge the groups'
+// pivoted sums; act: 0 none, 1 swish, 2 ReLU (its mask in the backward); gamma_add is added to gamma (null gamma / beta: 0).
 template <int MODE>
 __global__ void __launch_bounds__(256) gn_partial_kernel(const act_t* __restrict__ x, const act_t* __restrict__ dy,
                                                          const float* __restrict__ stats,
                                                          const float* __restrict__ gamma,
                                                          const float* __restrict__ beta, int pixels, int C, int swish,
-                                                         float* __restrict__ part) {
+                                                         float* __restrict__ part, float gamma_add, int one_group) {
   pdl_prologue();
   __shared__ float acc[GN_G][2];
   const int vecs = C / 8, cpg = C / GN_G;
@@ -232,13 +233,14 @@ __global__ void __launch_bounds__(256) gn_partial_kernel(const act_t* __restrict
   float g8[8], b8[8], mean8[8], rstd8[8], pv[2];
   if (MODE == 0) {
 #pragma unroll
-    for (int h = 0; h < 2; ++h) pv[h] = gn_pivot(x, C, (c0 + 4 * h) / cpg);
+    for (int h = 0; h < 2; ++h) pv[h] = gn_pivot(x, C, one_group ? 0 : (c0 + 4 * h) / cpg);
   }
   if (MODE == 1) {
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
-      g8[i] = gamma[c0 + i];
-      b8[i] = beta[c0 + i];
+      g8[i] = gamma ? gamma[c0 + i] : 0.f;
+      if (gamma_add != 0.f) g8[i] += gamma_add;
+      b8[i] = beta ? beta[c0 + i] : 0.f;
       int g = (c0 + i) / cpg;
       mean8[i] = stats[2 * g];
       rstd8[i] = stats[2 * g + 1];
@@ -263,10 +265,12 @@ __global__ void __launch_bounds__(256) gn_partial_kernel(const act_t* __restrict
       for (int i = 0; i < 8; ++i) {
         float xh = (xv[i] - mean8[i]) * rstd8[i];
         float d = dv[i];
-        if (swish) {
+        if (swish == 1) {
           float a = g8[i] * xh + b8[i];
           float sg = 1.f / (1.f + __expf(-a));
           d *= sg * (1.f + a * (1.f - sg));
+        } else if (swish == 2) {
+          d = (g8[i] * xh + b8[i]) > 0.f ? d : 0.f;
         }
         float dxh = d * g8[i];
         s[i >> 2][0] += dxh;
@@ -281,9 +285,10 @@ __global__ void __launch_bounds__(256) gn_partial_kernel(const act_t* __restrict
 
 // MODE 0: stats[g] = (mean, rstd), from the plain sums or, where those lose their precision, from the pivoted ones
 // (x: the tensor, for the pivots).  MODE 1: gstats[g] = (mean dxh, mean dxh*xh).  One block of 256 threads.
+// one_group: the 32 equal-sized groups' means are averaged into the whole tensor's before anything is derived from them.
 template <int MODE>
 __global__ void gn_final_kernel(const float* __restrict__ part, int nblk, double count, float eps, const act_t* x, int C,
-                                float* __restrict__ out) {
+                                float* __restrict__ out, int one_group) {
   pdl_prologue();
   const int t = threadIdx.x & 63, q = threadIdx.x >> 6;  // 256 threads: slot (group, which) x quarter of the partials
   double s = 0.0, sp = 0.0;
@@ -300,6 +305,15 @@ __global__ void gn_final_kernel(const float* __restrict__ part, int nblk, double
     shp[t] = (acc4p[0][t] + acc4p[1][t] + acc4p[2][t] + acc4p[3][t]) / count;
   }
   __syncthreads();
+  if (one_group && threadIdx.x < 4) {  // thread k merges one of sh[even], sh[odd], shp[even], shp[odd]: fixed order
+    double* v = threadIdx.x < 2 ? sh : shp;
+    const int which = threadIdx.x & 1;
+    double a = 0.0;
+    for (int g = 0; g < GN_G; ++g) a += v[2 * g + which];
+    a /= GN_G;
+    for (int g = 0; g < GN_G; ++g) v[2 * g + which] = a;
+  }
+  __syncthreads();
   if (q != 0) return;
   if (MODE == 0) {
     if ((t & 1) == 0) {
@@ -307,7 +321,7 @@ __global__ void gn_final_kernel(const float* __restrict__ part, int nblk, double
       if (var < 0) var = 0;
       if (gn_refine_variance(mean, var)) {
         const double md = shp[t];
-        mean = gn_pivot(x, C, t >> 1) + md;
+        mean = gn_pivot(x, C, one_group ? 0 : t >> 1) + md;
         var = shp[t + 1] - md * md;
         if (var < 0) var = 0;
       }
@@ -321,19 +335,24 @@ __global__ void gn_final_kernel(const float* __restrict__ part, int nblk, double
 
 __global__ void __launch_bounds__(256) gn_apply_kernel(const act_t* __restrict__ x, const float* __restrict__ stats,
                                                        const float* __restrict__ gamma, const float* __restrict__ beta,
-                                                       long long nvec, int C, int swish, act_t* __restrict__ y) {
+                                                       long long nvec, int C, int swish, act_t* __restrict__ y,
+                                                       float gamma_add, const act_t* __restrict__ res) {
   pdl_prologue();
   const int cpg = C / GN_G, vecs = C / 8;
   for (long long v = blockIdx.x * (long long)blockDim.x + threadIdx.x; v < nvec;
        v += (long long)gridDim.x * blockDim.x) {
     const int c0 = (int)(v % vecs) * 8;
-    float xv[8];
+    float xv[8], rv[8];
     load8(x + v * 8, xv);
+    if (res) load8(res + v * 8, rv);
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
       int g = (c0 + i) / cpg;
-      float a = (xv[i] - stats[2 * g]) * stats[2 * g + 1] * gamma[c0 + i] + beta[c0 + i];
-      xv[i] = swish ? a / (1.f + __expf(-a)) : a;
+      float ga = gamma ? gamma[c0 + i] : 0.f;
+      if (gamma_add != 0.f) ga += gamma_add;
+      float a = (xv[i] - stats[2 * g]) * stats[2 * g + 1] * ga + (beta ? beta[c0 + i] : 0.f);
+      a = swish == 1 ? a / (1.f + __expf(-a)) : (swish == 2 ? fmaxf(a, 0.f) : a);
+      xv[i] = res ? a + rv[i] : a;
     }
     store8(y + v * 8, xv);
   }
@@ -345,7 +364,7 @@ __global__ void __launch_bounds__(256) gn_bwd_apply_kernel(const act_t* __restri
                                                            const float* __restrict__ gamma,
                                                            const float* __restrict__ beta, long long nvec, int C,
                                                            int swish, const act_t* __restrict__ dres,
-                                                           act_t* __restrict__ dx) {
+                                                           act_t* __restrict__ dx, float gamma_add) {
   pdl_prologue();
   const int cpg = C / GN_G, vecs = C / 8;
   for (long long v = blockIdx.x * (long long)blockDim.x + threadIdx.x; v < nvec;
@@ -361,12 +380,17 @@ __global__ void __launch_bounds__(256) gn_bwd_apply_kernel(const act_t* __restri
       float rstd = stats[2 * g + 1];
       float xh = (xv[i] - stats[2 * g]) * rstd;
       float d = dv[i];
-      if (swish) {
-        float a = gamma[c0 + i] * xh + beta[c0 + i];
+      float ga = gamma ? gamma[c0 + i] : 0.f;
+      if (gamma_add != 0.f) ga += gamma_add;
+      const float be = beta ? beta[c0 + i] : 0.f;
+      if (swish == 1) {
+        float a = ga * xh + be;
         float sg = 1.f / (1.f + __expf(-a));
         d *= sg * (1.f + a * (1.f - sg));
+      } else if (swish == 2) {
+        d = (ga * xh + be) > 0.f ? d : 0.f;
       }
-      float dxh = d * gamma[c0 + i];
+      float dxh = d * ga;
       float r = rstd * (dxh - gstats[2 * g] - xh * gstats[2 * g + 1]);
       xv[i] = dres ? r + rv[i] : r;
     }
@@ -903,28 +927,32 @@ int gn_num_partials(int pixels, int C) {
   return (pixels + rpb - 1) / rpb;
 }
 
-void gn_stats(const act_t* x, int pixels, int C, float eps, float* part, float* stats, cudaStream_t st) {
+void gn_stats(const act_t* x, int pixels, int C, float eps, float* part, float* stats, cudaStream_t st, GnOpts o) {
   const int nblk = gn_num_partials(pixels, C);
-  launch_pdl(gn_partial_kernel<0>, dim3(nblk), dim3(256), 0, st, x, nullptr, nullptr, nullptr, nullptr, pixels, C, 0, part);
-  launch_pdl(gn_final_kernel<0>, dim3(1), dim3(256), 0, st, part, nblk, (double)pixels * (C / GN_G), eps, x, C, stats);
+  launch_pdl(gn_partial_kernel<0>, dim3(nblk), dim3(256), 0, st, x, nullptr, nullptr, nullptr, nullptr, pixels, C, 0, part,
+             0.f, o.one_group);
+  launch_pdl(gn_final_kernel<0>, dim3(1), dim3(256), 0, st, part, nblk, (double)pixels * (C / GN_G), eps, x, C, stats,
+             o.one_group);
 }
 
 void gn_apply(const act_t* x, const float* stats, const float* gamma, const float* beta, int pixels, int C, int swish,
-              act_t* y, cudaStream_t st) {
+              act_t* y, cudaStream_t st, GnOpts o) {
   const long long nvec = (long long)pixels * C / 8;
-  launch_pdl(gn_apply_kernel, dim3(grid_for(nvec, 256)), dim3(256), 0, st, x, stats, gamma, beta, nvec, C, swish, y);
+  launch_pdl(gn_apply_kernel, dim3(grid_for(nvec, 256)), dim3(256), 0, st, x, stats, gamma, beta, nvec, C, swish, y,
+             o.gamma_add, o.res);
 }
 
 void gn_backward(const act_t* dy, const act_t* x, const float* stats, const float* gamma, const float* beta,
                  int pixels, int C, int swish, const act_t* dres, float* part, float* gstats, act_t* dx,
-                 cudaStream_t st) {
+                 cudaStream_t st, GnOpts o) {
   const int nblk = gn_num_partials(pixels, C);
-  launch_pdl(gn_partial_kernel<1>, dim3(nblk), dim3(256), 0, st, x, dy, stats, gamma, beta, pixels, C, swish, part);
+  launch_pdl(gn_partial_kernel<1>, dim3(nblk), dim3(256), 0, st, x, dy, stats, gamma, beta, pixels, C, swish, part,
+             o.gamma_add, o.one_group);
   launch_pdl(gn_final_kernel<1>, dim3(1), dim3(256), 0, st, part, nblk, (double)pixels * (C / GN_G), 0.f,
-             (const act_t*)nullptr, C, gstats);
+             (const act_t*)nullptr, C, gstats, o.one_group);
   const long long nvec = (long long)pixels * C / 8;
   launch_pdl(gn_bwd_apply_kernel, dim3(grid_for(nvec, 256)), dim3(256), 0, st, dy, x, stats, gstats, gamma, beta, nvec, C, swish, dres,
-                                                           dx);
+                                                           dx, o.gamma_add);
 }
 
 namespace {

@@ -222,12 +222,19 @@ __global__ void vd_set_features_kernel(VdFeatures f, float* __restrict__ h0_tail
   else if (i < 144) te[i - 128] = f.v[i];
 }
 
-// pred = x alpha - v sigma; pixels = ClampWithGrad((pred + 1) / 2, 0, 1) (sampling.py:7-15, vdiff.py:159-163)
+// canvas index of gen pixel p, or -1 outside the crop window
+__device__ __forceinline__ int vd_crop_index(const VdCrop& c, int p) {
+  const int y = p / c.gw - c.my, x = p % c.gw - c.mx;
+  return (y >= 0 && y < c.h && x >= 0 && x < c.w) ? y * c.w + x : -1;
+}
+// pred = x alpha - v sigma; pixels = ClampWithGrad((pred + 1) / 2, 0, 1) (sampling.py:7-15, vdiff.py:159-163) on the
+// window (vdiff.py:165-170)
 __global__ void vd_finish_kernel(const float* __restrict__ vout, int ld, const float* __restrict__ x, float alpha,
-                                 float sigma, int pixels, float* __restrict__ v_planar, float* __restrict__ pred,
+                                 float sigma, VdCrop cr, float* __restrict__ v_planar, float* __restrict__ pred,
                                  float* __restrict__ pre, float* __restrict__ img) {
-  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  const int p = blockIdx.x * blockDim.x + threadIdx.x, pixels = cr.gh * cr.gw;
   if (p >= pixels) return;
+  const int q = vd_crop_index(cr, p), cpx = cr.h * cr.w;
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
     const size_t o = (size_t)c * pixels + p;
@@ -236,21 +243,28 @@ __global__ void vd_finish_kernel(const float* __restrict__ vout, int ld, const f
     const float u = (pr + 1.f) * 0.5f;
     v_planar[o] = v;
     pred[o] = pr;
-    pre[o] = u;
-    img[o] = fminf(fmaxf(u, 0.f), 1.f);
+    if (q >= 0) {
+      pre[(size_t)c * cpx + q] = u;
+      img[(size_t)c * cpx + q] = fminf(fmaxf(u, 0.f), 1.f);
+    }
   }
 }
-// g_pred = 0.5 g_img [g (pre - clamp pre) >= 0]; g_v = -sigma g_pred -> fp16 [pixels, ld] (scaled gradient stays scaled)
+// g_pred = 0.5 g_img [g (pre - clamp pre) >= 0] inside the window, 0 outside; g_v = -sigma g_pred -> fp16 [pixels, ld]
+// (scaled gradient stays scaled)
 __global__ void vd_finish_bwd_kernel(const float* __restrict__ g_img, const float* __restrict__ pre, float sigma,
-                                     int pixels, int ld, float* __restrict__ g_pred, act_t* __restrict__ g_v) {
-  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+                                     VdCrop cr, int ld, float* __restrict__ g_pred, act_t* __restrict__ g_v) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x, pixels = cr.gh * cr.gw;
   if (p >= pixels) return;
+  const int q = vd_crop_index(cr, p), cpx = cr.h * cr.w;
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
     const size_t o = (size_t)c * pixels + p;
-    const float g = g_img[o], u = pre[o];
-    const float cl = fminf(fmaxf(u, 0.f), 1.f);
-    const float gp = (g * (u - cl) >= 0.f) ? 0.5f * g : 0.f;
+    float gp = 0.f;
+    if (q >= 0) {
+      const float g = g_img[(size_t)c * cpx + q], u = pre[(size_t)c * cpx + q];
+      const float cl = fminf(fmaxf(u, 0.f), 1.f);
+      gp = (g * (u - cl) >= 0.f) ? 0.5f * g : 0.f;
+    }
     g_pred[o] = gp;
     g_v[(size_t)p * ld + c] = __float2half_rn(-sigma * gp);
   }
@@ -307,13 +321,15 @@ void gemv_f16(const act_t* W, int K, int R, const float* x, const float* bias, i
               cudaStream_t st) {
   gemv_f16_kernel<<<(R * 32 + 255) / 256, 256, 0, st>>>(W, K, R, x, bias, relu, res, y);
 }
-void vd_finish(const float* vout, int ld, const float* x, float alpha, float sigma, int pixels, float* v_planar,
+void vd_finish(const float* vout, int ld, const float* x, float alpha, float sigma, VdCrop c, float* v_planar,
                float* pred, float* pre, float* img, cudaStream_t st) {
-  vd_finish_kernel<<<(pixels + 255) / 256, 256, 0, st>>>(vout, ld, x, alpha, sigma, pixels, v_planar, pred, pre, img);
+  const int pixels = c.gh * c.gw;
+  vd_finish_kernel<<<(pixels + 255) / 256, 256, 0, st>>>(vout, ld, x, alpha, sigma, c, v_planar, pred, pre, img);
 }
-void vd_finish_backward(const float* g_img, const float* pre, float sigma, int pixels, int ld, float* g_pred, act_t* g_v,
+void vd_finish_backward(const float* g_img, const float* pre, float sigma, VdCrop c, int ld, float* g_pred, act_t* g_v,
                         cudaStream_t st) {
-  vd_finish_bwd_kernel<<<(pixels + 255) / 256, 256, 0, st>>>(g_img, pre, sigma, pixels, ld, g_pred, g_v);
+  const int pixels = c.gh * c.gw;
+  vd_finish_bwd_kernel<<<(pixels + 255) / 256, 256, 0, st>>>(g_img, pre, sigma, c, ld, g_pred, g_v);
 }
 void vd_zgrad(const float* g_pred, const act_t* g_in, int ld, float alpha, float inv_scale, int pixels, float* z_grad,
               cudaStream_t st) {

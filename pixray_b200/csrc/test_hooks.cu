@@ -535,6 +535,34 @@ extern "C" int pxr_test_groupnorm_unet(const void* x, const float* gamma, const 
   return sync_status();
 }
 
+// The same on either path vd_norm / vd_norm_bwd choose from: 0 the grid-barrier kernel (as above), 1 the three kernels.
+extern "C" int pxr_test_groupnorm_unet_path(int path, const void* x, const float* gamma, const float* beta, float gamma_add,
+                                            int act, const void* res, float eps, int pixels, int C, void* y, float* stats,
+                                            const void* dy, const void* dres, void* dx, float* scratch) {
+  if (path == 0) return pxr_test_groupnorm_unet(x, gamma, beta, gamma_add, act, res, eps, pixels, C, y, stats, dy, dres, dx, scratch);
+  if (path != 1 || !x || !y || !stats || !scratch || act < 0 || act > 2 || (dy && !dx) || pixels < 1 || C < 32 || C % 32 ||
+      256 % (C / 8) || (C / 32 != 4 && (C / 32) % 8))
+    return -1;
+  GnOpts o;
+  o.one_group = 1;
+  o.gamma_add = gamma_add;
+  o.res = static_cast<const act_t*>(res);
+  const act_t* xin = static_cast<const act_t*>(x);
+  gn_stats(xin, pixels, C, eps, scratch, stats, nullptr, o);
+  gn_apply(xin, stats, gamma, beta, pixels, C, act, static_cast<act_t*>(y), nullptr, o);
+  if (dy) {
+    o.res = nullptr;
+    float* gstats = scratch + 2 * 64 * gn_num_partials(pixels, C);
+    gn_backward(static_cast<const act_t*>(dy), xin, stats, gamma, beta, pixels, C, act, static_cast<const act_t*>(dres),
+                scratch, gstats, static_cast<act_t*>(dx), nullptr, o);
+  }
+  return sync_status();
+}
+
+extern "C" int pxr_test_groupnorm_partials(int pixels, int C) {
+  return pixels < 1 ? -1 : gn_num_partials(pixels, C);
+}
+
 // One resampling / copy launcher chosen by `op` (include/pixray_b200.h lists the ops and their layouts).
 extern "C" int pxr_test_resample(int op, const void* in, int ld_in, void* out, int ld_out, int H, int W, int C, int accumulate) {
   if (!in || !out || C < 8 || C % 8 || H < 1 || W < 1) return -1;

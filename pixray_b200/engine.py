@@ -120,7 +120,7 @@ class B200Engine:
     def __init__(self, *, drawer=DRAWER_VQGAN, image_hw=(256, 256), vqgan=None, grid=None, cutn=64, cut_size=224,
                  clip=(), noise_fac=0.1, seed=0, device=0, rank=0, world=1, grad_scale=0.0, lr_betas=(0.9, 0.999),
                  adam_eps=1e-8, fft_decay=0.0, fft_colors=0.0, fft_contrast=0.0, cut_aspect=1.0, polygons=None,
-                 superres=None, strokes=None):
+                 superres=None, strokes=None, vdiff_gen_hw=None):
         if not torch.cuda.is_available():
             raise EngineError("pixray_b200 needs a CUDA device (H100); there is no CPU fallback")
         self.lib = _lib.load()
@@ -138,8 +138,10 @@ class B200Engine:
             f = 2 ** (cfg.n_levels - 1)
             self.z_shape = (1, cfg.z_channels, image_hw[0] // f, image_hw[1] // f)
         elif drawer == DRAWER_VDIFF:
-            # VdiffDrawer's x (vdiff.py:118): [1, 3, gen_height, gen_width]
-            self.z_shape = (1, 3, image_hw[0], image_hw[1])
+            # VdiffDrawer's x (vdiff.py:118): [1, 3, gen_height, gen_width]; vdiff_gen_hw = (gen_h, gen_w), each side a
+            # multiple of 64 and at least the canvas's (None: the canvas); the image is the canvas-size window centred in it
+            gen_hw = tuple(image_hw) if vdiff_gen_hw is None else (int(vdiff_gen_hw[0]), int(vdiff_gen_hw[1]))
+            self.z_shape = (1, 3, gen_hw[0], gen_hw[1])
         elif drawer == DRAWER_SUPERRES:
             # SuperResolutionDrawer's z (super_resolution.py:75-76): [1, 3, H/4, W/4]; the canvas is 4x the latent
             if image_hw[0] % 4 or image_hw[1] % 4:
@@ -212,6 +214,8 @@ class B200Engine:
         if drawer == DRAWER_STROKES:
             rc = self.lib.pxr_set_strokes(self.h, n_paths, n_segments, C.c_float(float(strokes[2])), int(bool(strokes[3])))
             self._check(rc, "pxr_set_strokes")
+        if drawer == DRAWER_VDIFF and vdiff_gen_hw is not None:
+            self._check(self.lib.pxr_vdiff_set_gen_size(self.h, gen_hw[0], gen_hw[1]), "pxr_vdiff_set_gen_size")
         self._ext = None  # torch view of the engine's stream (ordering against torch-side producers of z / noise)
 
     # ------------------------------------------------------------------ plumbing

@@ -479,9 +479,23 @@ class VdiffDrawer(DrawingInterface):
         eng.vdiff_set_schedule(self.steps, self.alphas, self.sigmas)
         g = None if seed is None else torch.Generator(device=eng.device).manual_seed(seed)
         self.x = torch.randn(eng.z_shape, device=eng.device, generator=g)
-        if init_tensor is not None:  # vdiff.py:143: x = init * alpha_0 + noise * sigma_0
-            self.x = init_tensor.to(eng.device) * float(self.alphas[0]) + self.x * float(self.sigmas[0])
+        if init_tensor is not None:  # vdiff.py:131-143: x = frame * alpha_0 + noise * sigma_0
+            self.x = self.gen_frame(init_tensor) * float(self.alphas[0]) + self.x * float(self.sigmas[0])
         self.x = self.x.contiguous()
+
+    def gen_frame(self, init_tensor):
+        """The reverse centre crop (vdiff.py:131-139): a canvas-size start image placed into a zero gen-size frame at the
+        margins synth crops away; a gen-size one (no margins) is the frame itself."""
+        eng = self.session.engine
+        gh, gw = eng.z_shape[2], eng.z_shape[3]
+        h, w = eng.image_hw
+        t = init_tensor.to(eng.device, torch.float32).reshape(1, 3, h, w)
+        if (gh, gw) == (h, w):
+            return t
+        my, mx = (gh - h) // 2, (gw - w) // 2
+        frame = torch.zeros(eng.z_shape, device=eng.device, dtype=torch.float32)
+        frame[:, :, my:my + h, mx:mx + w] = t
+        return frame
 
     def set_clip_embed(self, clip_embed):
         """sample_state[3] = {"clip_embed": ...} (pixray.py:880-885)."""
@@ -492,6 +506,7 @@ class VdiffDrawer(DrawingInterface):
         return self.session.engine.vdiff_renoise(self.x, cur_it, noise)
 
     def synth(self, cur_iteration):
+        """The canvas image: the engine crops the clamped prediction to the canvas window (vdiff.py:165-170)."""
         self.session.engine.vdiff_set_iteration(cur_iteration)
         return self.session.engine.synth(self.x)
 

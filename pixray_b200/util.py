@@ -74,6 +74,26 @@ def vdiff_schedule(iterations, vdiff_skip=0.0):
             np.sin(steps * np.pi / 2).astype(np.float32))
 
 
+VDIFF_ROUNDUP = 128  # vdiff.py ROUNDUP_SIZE
+
+
+def vdiff_gen_size(width, height):
+    """VdiffDrawer's U-Net size for a canvas (vdiff.py:55-58, 165-170): gen = ceil(side / 128) * 128 per side, margins
+    int((gen - canvas) / 2).  Returns (gen_w, gen_h, margin_x, margin_y).  The image is pixels[:, :, my:my+H, mx:mx+W],
+    except when both margins are zero (each side 0 or 1 pixel short of a multiple of 128): the reference does not
+    crop then, and the image is the whole gen-size frame (vdiff_image_size)."""
+    gw = -(-int(width) // VDIFF_ROUNDUP) * VDIFF_ROUNDUP
+    gh = -(-int(height) // VDIFF_ROUNDUP) * VDIFF_ROUNDUP
+    return gw, gh, (gw - int(width)) // 2, (gh - int(height)) // 2
+
+
+def vdiff_image_size(width, height):
+    """(width, height) of the image VdiffDrawer.synth returns for a canvas: the canvas, or the gen size when no margin
+    is cut (vdiff.py:167-168)."""
+    gw, gh, mx, my = vdiff_gen_size(width, height)
+    return (int(width), int(height)) if (mx or my) else (gw, gh)
+
+
 # ------------------------------------------------------------------------------------------------ init images (host, init time)
 def _perlin_2d(rng, shape, res):
     """perlin_numpy.generate_perlin_noise_2d [UPSTREAM pvigier/perlin-numpy, un-vendored; requirements.txt]: gradient noise
