@@ -186,8 +186,15 @@ int pxr_set_strokes(pxr_handle h, int n_paths, int n_segments, float max_width, 
 int pxr_set_synth_iteration(pxr_handle h, int iter);
 /* z = model.encode(img)[0]: VqganDrawer.init_from_tensor / reapply_from_tensor / get_z_from_tensor (vqgan.py:174-185) --
  * taming Encoder + quant_conv + nearest codebook row.  img device [3,H,W] in [-1,1]; z_out device [z_channels,h,w].
- * Available when the weights loaded before pxr_finalize include the checkpoint's encoder.* and quant_conv.* tensors. */
+ * Available when the weights loaded before pxr_finalize include the checkpoint's encoder.* and quant_conv.* tensors.
+ * Refused on a GumbelVQ engine (codebook quantize.embed.weight): that one encodes with pxr_vqgan_encode_gumbel. */
 int pxr_vqgan_encode(pxr_handle h, const float* img, float* z_out);
+/* model.encode(img)[0] of a GumbelVQ (taming GumbelQuantize in eval mode, hard Gumbel-softmax): taming Encoder +
+ * quant_conv, logits = quantize.proj(h) [n_embed, h, w], then per position the first code maximising logits + noise, and
+ * z_out = that code's row of quantize.embed.weight, exactly (the reference's straight-through value differs from the row by
+ * at most one fp32 rounding).  noise: device [n_embed, h, w] fp32, the Gumbel draws -log(Exp(1)) F.gumbel_softmax adds.
+ * Needs the checkpoint's encoder.*, quant_conv.* and quantize.proj.* tensors; refused on a nearest-code engine. */
+int pxr_vqgan_encode_gumbel(pxr_handle h, const float* img, const float* noise, float* z_out);
 /* Distribution of the engine-drawn ColorJitter: Bernoulli(p) per cutout, saturation_factor ~ U(1-s, 1+s),
  * hue_factor ~ U(-hue, hue), one random order per group and iteration.  Defaults = the reference's call sites
  * (0.8, 0.1, 0.1); p = 0 turns the stage off. */

@@ -128,6 +128,7 @@ EXPORTS = [
     "pxr_test_gemm_records", "pxr_test_gemm_plan_info", "pxr_test_allocations",
     "pxr_test_attention_records", "pxr_test_attention_plan",
     "pxr_vdiff_set_gen_size", "pxr_test_groupnorm_unet_path", "pxr_test_groupnorm_partials",
+    "pxr_vqgan_encode_gumbel",
 ]
 
 _lib = None

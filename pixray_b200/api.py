@@ -315,6 +315,19 @@ def _load_state_dict(spec):
     return obj
 
 
+def _vqgan_state_dict(spec):
+    """A taming VQGAN checkpoint as one plain VQModel / GumbelVQ state_dict: the {'state_dict': ...} of a VQModel or
+    GumbelVQ without its loss.* (discriminator, LPIPS) tensors, or the first_stage_model of a Net2NetTransformer with its
+    cond_stage_model.* and transformer.* dropped (vqgan.py:122-136)."""
+    sd = _load_state_dict(spec)
+    if "state_dict" in sd:  # the checkpoint itself rather than its path
+        sd = sd["state_dict"]
+    prefix = "first_stage_model."
+    if any(k.startswith(prefix) for k in sd):
+        sd = {k[len(prefix):]: v for k, v in sd.items() if k.startswith(prefix)}
+    return {k: v for k, v in sd.items() if not k.startswith("loss.")}
+
+
 def _vector_table(name):
     """`vectors/<name>.json` next to the reference checkout (pixray.py:893-901)."""
     if "json" in name:
@@ -388,7 +401,20 @@ def do_init(args):
         else:
             PS.check_pixel_type(args.pixel_type)
             kind = E.DRAWER_POLYGON
-    n_levels = len(E.VQGAN_F16_16384["ch_mult"]) if kind == E.DRAWER_VQGAN else None
+    weights = args.b200_weights or {}
+    vq_sd, vq_cfg = None, None
+    if kind == E.DRAWER_VQGAN:
+        for dest in ("vqgan_config", "vqgan_checkpoint"):
+            if getattr(args, dest, None) is not None:
+                # vqgan.py:103, 108 read settings.config_path / settings.checkpoint_path, which the parser never sets
+                raise ValueError(f"{dest}={getattr(args, dest)!r}: the reference fails on a non-None {dest} (it reads "
+                                 "settings.config_path / settings.checkpoint_path, which do not exist); pass the "
+                                 "checkpoint as b200_weights['vqgan'] (a state_dict or a path) instead, and the "
+                                 "architecture is read from its tensors")
+        if "vqgan" in weights:
+            vq_sd = _vqgan_state_dict(weights["vqgan"])
+            vq_cfg = E.vqgan_config(vq_sd)
+    n_levels = len((vq_cfg or E.VQGAN_F16_16384)["ch_mult"]) if kind == E.DRAWER_VQGAN else None
     sideX, sideY = _side(args, n_levels)
     engine_hw = (sideY, sideX)
     vdiff_gen_hw = None
@@ -418,6 +444,8 @@ def do_init(args):
         kw.update(rank=int(args.b200_rank), world=world)
     if vdiff_gen_hw is not None:
         kw["vdiff_gen_hw"] = vdiff_gen_hw
+    if vq_cfg is not None:
+        kw["vqgan"] = vq_cfg
     if kind == E.DRAWER_PIXEL:  # fast_pixeldrawer.py:37-63: 40x40 / 40x50 / 80x45 default grid, pixel_scale, clamp to canvas
         kw["grid"] = P.FastPixelDrawer.grid_for((sideX, sideY), getattr(args, "pixel_size", None), getattr(args, "pixel_scale", None))
         print(f"Running fast pixeldrawer with {kw['grid'][1]}x{kw['grid'][0]} grid")
@@ -437,13 +465,12 @@ def do_init(args):
     eng = _engine_factory(**kw)
     if any(m in E.RESNET_ARCH for m in args.clip_models) and E.TOWER_CLIP_RESNET not in getattr(eng, "TOWERS", ()):
         raise NotImplementedError("this engine build has no ResNet image towers")
-    weights = args.b200_weights or {}
     if kind in (E.DRAWER_VQGAN, E.DRAWER_VDIFF, E.DRAWER_SUPERRES):
         key = {E.DRAWER_VQGAN: "vqgan", E.DRAWER_VDIFF: "vdiff", E.DRAWER_SUPERRES: "super_resolution"}[kind]
-        if key in weights:
+        if kind == E.DRAWER_VQGAN:  # the checkpoint was read above, for its architecture
+            vq_sd = S.vqgan_state_dict(E.VQGAN_F16_16384, 0, with_encoder=True) if vq_sd is None else vq_sd
+        elif key in weights:
             vq_sd = _load_state_dict(weights[key])
-        elif kind == E.DRAWER_VQGAN:
-            vq_sd = S.vqgan_state_dict(E.VQGAN_F16_16384, 0, with_encoder=True)
         elif not args.b200_allow_synthetic:
             ckpt = "the cc12m_1 checkpoint's" if kind == E.DRAWER_VDIFF else f"the {args.super_resolution_model} checkpoint's"
             raise ValueError(f"the {args.drawer} drawer needs b200_weights['{key}'] ({ckpt} state_dict), or "
@@ -498,7 +525,8 @@ def do_init(args):
             drawer.init_from_tensor(to_t(starting_image) * 2 - 1)
     elif kind == E.DRAWER_VQGAN:
         # init_image and init_noise both off: the legacy start (VqganDrawer.rand_init, vqgan.py:162-171): random codebook rows
-        code = torch.as_tensor(vq_sd["quantize.embedding.weight"], dtype=torch.float32)
+        code = torch.as_tensor(vq_sd["quantize.embed.weight" if vq_cfg and vq_cfg["gumbel"] else "quantize.embedding.weight"],
+                               dtype=torch.float32)
         idx = torch.randint(code.shape[0], (eng.z_shape[2] * eng.z_shape[3],))
         drawer.set_z(code[idx].T.reshape(eng.z_shape))
     elif kind == E.DRAWER_PIXEL:

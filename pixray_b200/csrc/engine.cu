@@ -814,6 +814,10 @@ class Engine {
   bool have_encoder = false;
   float* enc_img = nullptr;   // [3, H, W] input in [-1, 1]
   float* enc_z = nullptr;     // [C, hw] result
+  // a GumbelVQ checkpoint (codebook quantize.embed.weight): the encoder quantises with quantize.proj's logits plus the
+  // caller's Gumbel noise [n_embed, hw] (pxr_vqgan_encode_gumbel) instead of the nearest code
+  bool vq_gumbel = false;
+  float* enc_noise = nullptr;
   void build_vqgan_encoder();
   NormW load_norm(int mod, const std::string& prefix, int c);
   Act new_act(int H, int Wd, int C, bool grad = true) {
@@ -1423,8 +1427,14 @@ void Engine::build_vqgan() {
   gn_bar.counter = dalloc<unsigned long long>(1);
   splitk_ws_elems = (size_t)8 << 20;  // 32 MiB of fp32 partial sums: covers every conv the split-K rule selects
   splitk_ws = dalloc<float>(splitk_ws_elems, false);
-  // codebook
-  const HostWeight& cb = W(PXR_MOD_VQGAN, "quantize.embedding.weight", {ne, zc});
+  // codebook: taming VectorQuantizer's quantize.embedding or GumbelQuantize's quantize.embed.  Everything below reads it
+  // the same way for both kinds: synth's nearest code and its backward, the z bounds, the optimiser (vqgan.py:149-153,
+  // 190-195); only the encoder's quantiser differs (build_vqgan_encoder)
+  const bool has_vq = weights[PXR_MOD_VQGAN].count("quantize.embedding.weight") > 0;
+  vq_gumbel = weights[PXR_MOD_VQGAN].count("quantize.embed.weight") > 0;
+  if (has_vq && vq_gumbel)
+    throw EngineError(-41, "the VQGAN weights carry both quantize.embedding.weight and quantize.embed.weight");
+  const HostWeight& cb = W(PXR_MOD_VQGAN, vq_gumbel ? "quantize.embed.weight" : "quantize.embedding.weight", {ne, zc});
   std::vector<float> cbT((size_t)zc * ne), c2(ne), mn(zc, 1e30f), mx(zc, -1e30f);
   for (int j = 0; j < ne; ++j) {
     float s = 0.f;
@@ -1644,21 +1654,44 @@ void Engine::build_vqgan_encoder() {
   Act hq = conv(hz, qc);
   const int hw = hq.pixels();
   if ((int64_t)zc * hw != z_numel) throw EngineError(-44, "encoder output does not match the latent size");
-  // quantise: the same exact fp32 nearest-code search as synth, on the decoder's codebook copies
   float *d_cb = vq_cb, *d_cbT = vq_cbT, *d_c2 = vq_c2;
-  const int n_chunks = (ne + 1023) / 1024;
-  float* part_d = dalloc<float>((size_t)hw * n_chunks);
-  int* part_i = dalloc<int>((size_t)hw * n_chunks);
-  int* idx = dalloc<int>(hw);
-  float* z32 = dalloc<float>((size_t)zc * hw);
-  act_t* zq16 = dalloc<act_t>((size_t)hw * zc);
-  enc_z = dalloc<float>((size_t)zc * hw);
-  float* ez = enc_z;
-  enc_fwd.add(4, [=] {
-    vq_backward(hq.p, 1.f, zc, hw, z32, cs);  // NHWC fp16 -> [C, hw] fp32 (the same transpose kernel the decoder's backward ends with)
-    vq_nearest(z32, d_cbT, d_c2, d_cb, zc, hw, ne, part_d, part_i, idx, zq16, cs);
-    gather_codes(d_cb, idx, zc, hw, ez, cs);
-  }, 0.0, "encoder quantise");
+  int* idx = nullptr;
+  float *z32 = nullptr, *ez = nullptr;
+  if (vq_gumbel) {
+    // GumbelQuantize, eval mode: logits = quantize.proj(h), a 1x1 convolution to n_embed channels, in fp32 from the conv
+    // plan; then per position the arg-max of logits + noise selects the code row.  The reference's value,
+    // (y_hard - y_soft + y_soft) @ embed.weight, is that row to within one fp32 rounding; this writes the row exactly.
+    ConvW pw = load_conv("quantize.proj", zc, ne, 1);
+    const int ld = pw.cout_pad;
+    float* logits = dalloc<float>((size_t)hw * ld);
+    GemmEpilogue e;
+    e.bias = pw.bias;
+    e.out_f32 = logits;
+    e.ldc = ld;
+    add_conv(enc_fwd, hq.p, hq.H, hq.W, hq.C, pw.w, pw.cout_pad, pw.cout, 1, e);
+    float* noise = enc_noise = dalloc<float>((size_t)ne * hw);
+    idx = dalloc<int>(hw);
+    z32 = dalloc<float>((size_t)zc * hw);
+    ez = enc_z = dalloc<float>((size_t)zc * hw);
+    enc_fwd.add(2, [=] {
+      vq_backward(hq.p, 1.f, zc, hw, z32, cs);  // enc_h, as below
+      gumbel_select(logits, ld, noise, d_cb, zc, hw, ne, idx, ez, cs);
+    }, 0.0, "encoder gumbel quantise");
+  } else {
+    // quantise: the same exact fp32 nearest-code search as synth, on the decoder's codebook copies
+    const int n_chunks = (ne + 1023) / 1024;
+    float* part_d = dalloc<float>((size_t)hw * n_chunks);
+    int* part_i = dalloc<int>((size_t)hw * n_chunks);
+    idx = dalloc<int>(hw);
+    z32 = dalloc<float>((size_t)zc * hw);
+    act_t* zq16 = dalloc<act_t>((size_t)hw * zc);
+    ez = enc_z = dalloc<float>((size_t)zc * hw);
+    enc_fwd.add(4, [=] {
+      vq_backward(hq.p, 1.f, zc, hw, z32, cs);  // NHWC fp16 -> [C, hw] fp32 (the same transpose kernel the decoder's backward ends with)
+      vq_nearest(z32, d_cbT, d_c2, d_cb, zc, hw, ne, part_d, part_i, idx, zq16, cs);
+      gather_codes(d_cb, idx, zc, hw, ez, cs);
+    }, 0.0, "encoder quantise");
+  }
   reg("enc_idx", idx, sizeof(int) * hw);
   reg("enc_h", z32, sizeof(float) * zc * hw);
   have_encoder = true;
@@ -3339,16 +3372,35 @@ int pxr_synth(pxr_handle h, const float* z, float* out_img) {
 // model.encode(init_tensor)[0] (VqganDrawer.init_from_tensor / reapply_from_tensor / get_z_from_tensor, vqgan.py:174-185):
 // img device fp32 [3, H, W] in [-1, 1] -> z_out device fp32 [z_channels, h, w] = the codebook rows nearest to
 // quant_conv(encoder(img)).  Needs the checkpoint's encoder.* / quant_conv.* tensors (loaded before pxr_finalize).
+namespace {
+void vqgan_encode(Engine* e, const char* what, const float* img, const float* noise, float* z_out) {
+  if (e->cfg.drawer != PXR_DRAWER_VQGAN) throw EngineError(-67, std::string(what) + ": not a VQGAN engine");
+  if (!e->have_encoder) throw EngineError(-67, std::string(what) + ": the loaded VQGAN weights carry no encoder.* tensors");
+  if (e->vq_gumbel && !noise)
+    throw EngineError(-67, std::string(what) + ": the loaded VQGAN is a GumbelVQ (codebook quantize.embed.weight); its "
+                                               "encoder needs Gumbel noise: call pxr_vqgan_encode_gumbel");
+  if (!e->vq_gumbel && noise)
+    throw EngineError(-67, std::string(what) + ": the loaded VQGAN quantises by nearest code (codebook "
+                                               "quantize.embedding.weight), not by Gumbel noise: call pxr_vqgan_encode");
+  if (!img || !z_out) throw EngineError(-10, std::string(what) + ": null pointer");
+  PXR_CUDA(cudaMemcpyAsync(e->enc_img, img, sizeof(float) * 3 * e->cfg.image_h * e->cfg.image_w, cudaMemcpyDeviceToDevice, e->st));
+  if (noise)
+    PXR_CUDA(cudaMemcpyAsync(e->enc_noise, noise, sizeof(float) * e->cfg.n_embed * (e->z_numel / e->cfg.z_channels),
+                             cudaMemcpyDeviceToDevice, e->st));
+  e->run(e->enc_fwd);
+  e->check_launch("vqgan encode");
+  PXR_CUDA(cudaMemcpyAsync(z_out, e->enc_z, sizeof(float) * e->z_numel, cudaMemcpyDeviceToDevice, e->st));
+}
+}  // namespace
+
 int pxr_vqgan_encode(pxr_handle h, const float* img, float* z_out) {
+  PXR_TRY(h, { vqgan_encode(h->e, "pxr_vqgan_encode", img, nullptr, z_out); });
+}
+
+int pxr_vqgan_encode_gumbel(pxr_handle h, const float* img, const float* noise, float* z_out) {
   PXR_TRY(h, {
-    Engine* e = h->e;
-    if (e->cfg.drawer != PXR_DRAWER_VQGAN) throw EngineError(-67, "pxr_vqgan_encode: not a VQGAN engine");
-    if (!e->have_encoder) throw EngineError(-67, "pxr_vqgan_encode: the loaded VQGAN weights carry no encoder.* tensors");
-    if (!img || !z_out) throw EngineError(-10, "pxr_vqgan_encode: null pointer");
-    PXR_CUDA(cudaMemcpyAsync(e->enc_img, img, sizeof(float) * 3 * e->cfg.image_h * e->cfg.image_w, cudaMemcpyDeviceToDevice, e->st));
-    e->run(e->enc_fwd);
-    e->check_launch("vqgan encode");
-    PXR_CUDA(cudaMemcpyAsync(z_out, e->enc_z, sizeof(float) * e->z_numel, cudaMemcpyDeviceToDevice, e->st));
+    if (!noise) throw EngineError(-10, "pxr_vqgan_encode_gumbel: null noise pointer");
+    vqgan_encode(h->e, "pxr_vqgan_encode_gumbel", img, noise, z_out);
   });
 }
 

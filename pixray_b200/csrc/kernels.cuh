@@ -100,6 +100,11 @@ void image_to_nhwc64(const float* img, int pixels, act_t* out, cudaStream_t st);
 void subsample_odd(const act_t* full, int H, int W, int C, act_t* y, cudaStream_t st);
 // z[c, p] = codebook[idx[p], c] (fp32): the quantised latent model.encode returns
 void gather_codes(const float* cb, const int* idx, int C, int hw, float* z, cudaStream_t st);
+// GumbelQuantize's eval forward (taming GumbelVQ: F.gumbel_softmax(logits, hard=True), then the einsum with the codebook):
+// idx[p] = the first j maximising logits[p * ld + j] + noise[j * hw + p] (the temperature does not move the arg-max);
+// z[c, p] = cb[idx[p], c].  logits: quantize.proj's output [hw, ld] fp32; noise: the Gumbel draws [n_e, hw] fp32.
+void gumbel_select(const float* logits, int ld, const float* noise, const float* cb, int C, int hw, int n_e, int* idx,
+                   float* z, cudaStream_t st);
 
 // nearest, [H,W,C]->[2H,2W,C]; the input's pixel stride is ld_in (0: C), the output is dense
 void upsample2x(const act_t* x, int H, int W, int C, act_t* y, cudaStream_t st, int ld_in = 0);

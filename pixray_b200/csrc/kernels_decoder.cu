@@ -835,6 +835,47 @@ __global__ void gather_codes_kernel(const float* __restrict__ cb, const int* __r
   z[i] = cb[(size_t)idx[p] * C + k];
 }
 
+// grid hw, block 256: one latent position per block.  Each thread scans codes tid, tid + 256, ... in increasing order
+// keeping the first maximum; the block then folds the 256 candidates by (larger value, then lower index), a total order,
+// so the pick does not depend on the fold's order.  A position whose every value is NaN or -inf takes code 0, as
+// torch's argmax of an all -inf row does.
+__global__ void __launch_bounds__(256) gumbel_select_kernel(const float* __restrict__ logits, int ld,
+                                                            const float* __restrict__ noise, const float* __restrict__ cb,
+                                                            int C, int hw, int n_e, int* __restrict__ idx,
+                                                            float* __restrict__ z) {
+  pdl_prologue();
+  __shared__ float red_v[8];
+  __shared__ int red_i[8];
+  const int p = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  float best = -INFINITY;
+  int bi = n_e;
+  for (int j = tid; j < n_e; j += 256) {
+    const float v = logits[(size_t)p * ld + j] + noise[(size_t)j * hw + p];
+    if (v > best) best = v, bi = j;
+  }
+  auto fold = [&](float& v, int& i) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const float ov = __shfl_xor_sync(0xffffffffu, v, o);
+      const int oi = __shfl_xor_sync(0xffffffffu, i, o);
+      if (ov > v || (ov == v && oi < i)) v = ov, i = oi;
+    }
+  };
+  fold(best, bi);
+  if (lane == 0) red_v[warp] = best, red_i[warp] = bi;
+  __syncthreads();
+  if (warp == 0) {
+    float v = lane < 8 ? red_v[lane] : -INFINITY;
+    int i = lane < 8 ? red_i[lane] : n_e;
+    fold(v, i);
+    if (lane == 0) red_i[0] = i < n_e ? i : 0;
+  }
+  __syncthreads();
+  const int k_sel = red_i[0];
+  if (tid == 0) idx[p] = k_sel;
+  for (int c = tid; c < C; c += 256) z[(size_t)c * hw + p] = cb[(size_t)k_sel * C + c];
+}
+
 __global__ void image_finish_kernel(const float* __restrict__ conv_out, int ld, int pixels, float* __restrict__ pre,
                                     float* __restrict__ img, int shift) {
   pdl_prologue();
@@ -1062,6 +1103,10 @@ void subsample_odd(const act_t* full, int H, int W, int C, act_t* y, cudaStream_
 }
 void gather_codes(const float* cb, const int* idx, int C, int hw, float* z, cudaStream_t st) {
   launch_pdl(gather_codes_kernel, dim3((C * hw + 255) / 256), dim3(256), 0, st, cb, idx, C, hw, z);
+}
+void gumbel_select(const float* logits, int ld, const float* noise, const float* cb, int C, int hw, int n_e, int* idx,
+                   float* z, cudaStream_t st) {
+  launch_pdl(gumbel_select_kernel, dim3(hw), dim3(256), 0, st, logits, ld, noise, cb, C, hw, n_e, idx, z);
 }
 
 void image_finish(const float* conv_out, int ld, int pixels, float* pre, float* img, cudaStream_t st, int shift) {

@@ -24,6 +24,8 @@ OPTIMISERS = {"Adam": OPT_ADAM, "AdamW": OPT_ADAMW, "Adagrad": OPT_ADAGRAD, "Ada
 RRDBNET_X4PLUS = dict(num_feat=64, num_block=23, num_grow_ch=32)
 VQGAN_F16_16384 = dict(z_channels=256, n_embed=16384, ch=128, ch_mult=(1, 1, 2, 2, 4), num_res_blocks=2,
                        attn_resolution=16, resolution=256)
+# the shapes the tensor-core nearest-code search covers (kernels_vq_tc.cu, vq_tc_supported); vqgan_config refuses the rest
+VQ_TC_CHANNEL_MULTIPLE, VQ_TC_CODE_MULTIPLE, VQ_TC_MAX_CODES = 64, 8, 16384
 CLIP_ARCH = {
     "ViT-B/32": dict(width=768, layers=12, heads=12, patch=32, image_res=224, out_dim=512),
     "ViT-B/16": dict(width=768, layers=12, heads=12, patch=16, image_res=224, out_dim=512),
@@ -87,6 +89,87 @@ class EngineError(RuntimeError):
     pass
 
 
+def vqgan_config(state_dict):
+    """The architecture a taming VQGAN state_dict (VQModel or GumbelVQ keys, loss.* and any wrapper prefix removed)
+    describes, as the dict B200Engine(vqgan=...) takes plus `gumbel` (the codebook is GumbelQuantize's quantize.embed):
+    n_embed / embed_dim from the codebook, z_channels from post_quant_conv and decoder.conv_in, ch from decoder.conv_out,
+    ch_mult and num_res_blocks from the decoder.up.* keys, attn_resolution from the level that carries attn.* keys.
+    `resolution` is taming's 256: with the attention level it only places the attention blocks.  Refuses, naming the
+    tensor, weights whose shapes disagree, and architectures the engine does not build."""
+    def shape(name):
+        if name not in state_dict:
+            raise EngineError(f"VQGAN checkpoint: tensor '{name}' is missing")
+        return tuple(int(d) for d in state_dict[name].shape)
+
+    def refuse(name, why):
+        raise EngineError(f"VQGAN checkpoint: '{name}' {why}")
+
+    gumbel = "quantize.embed.weight" in state_dict
+    if gumbel == ("quantize.embedding.weight" in state_dict):
+        raise EngineError("VQGAN checkpoint: expected one codebook, 'quantize.embedding.weight' (VQModel) or "
+                          f"'quantize.embed.weight' (GumbelVQ); found {'both' if gumbel else 'neither'}")
+    cb_key = "quantize.embed.weight" if gumbel else "quantize.embedding.weight"
+    cb = shape(cb_key)
+    if len(cb) != 2:
+        refuse(cb_key, f"has shape {list(cb)}; a codebook is [n_embed, embed_dim]")
+    n_embed, embed_dim = cb
+    pq = shape("post_quant_conv.weight")
+    if len(pq) != 4 or pq[1:] != (embed_dim, 1, 1):
+        refuse("post_quant_conv.weight", f"has shape {list(pq)}; the codebook {cb_key} has embed_dim {embed_dim}, so "
+                                         f"it must be [z_channels, {embed_dim}, 1, 1]")
+    zc = pq[0]
+    if embed_dim != zc:
+        refuse(cb_key, f"has embed_dim {embed_dim} but post_quant_conv.weight has z_channels {zc}; the engine builds "
+                       "VQGANs with embed_dim == z_channels only")
+    levels = sorted({int(k.split(".")[2]) for k in state_dict if k.startswith("decoder.up.")})
+    if not levels or levels != list(range(len(levels))) or len(levels) > 8:
+        raise EngineError(f"VQGAN checkpoint: the decoder.up.* keys name levels {levels}; expected 0 .. L-1 with 1 <= L <= 8")
+    co = shape("decoder.conv_out.weight")
+    ch = co[1]
+    blocks, ch_mult = [], []
+    for lv in levels:
+        blocks.append(len({k.split(".")[4] for k in state_dict if k.startswith(f"decoder.up.{lv}.block.")}))
+        name = f"decoder.up.{lv}.block.0.conv1.weight"
+        out = shape(name)[0]
+        if out % ch:
+            refuse(name, f"has {out} output channels, not a multiple of ch = {ch} (decoder.conv_out.weight's input)")
+        ch_mult.append(out // ch)
+    if len(set(blocks)) != 1 or blocks[0] < 1:
+        raise EngineError(f"VQGAN checkpoint: the decoder.up.<level>.block.* keys give {blocks} blocks per level; "
+                          "expected the same num_res_blocks + 1 at every level")
+    if ch_mult[0] != 1:
+        refuse("decoder.up.0.block.0.conv1.weight", f"has {ch * ch_mult[0]} output channels but decoder.conv_out.weight "
+                                                   f"reads {ch}; they must agree")
+    cin = shape("decoder.conv_in.weight")
+    if cin[:2] != (ch * ch_mult[-1], zc):
+        refuse("decoder.conv_in.weight", f"has shape {list(cin)}; z_channels {zc} (post_quant_conv.weight) and the last "
+                                         f"level's {ch * ch_mult[-1]} channels make it [{ch * ch_mult[-1]}, {zc}, 3, 3]")
+    attn = [lv for lv in levels if any(k.startswith(f"decoder.up.{lv}.attn.") for k in state_dict)]
+    if len(attn) > 1:
+        raise EngineError(f"VQGAN checkpoint: decoder.up.<level>.attn.* keys at levels {attn}; the engine places attention "
+                          "at one resolution")
+    resolution = 256
+    attn_resolution = resolution >> attn[0] if attn else 0
+    if "encoder.conv_in.weight" in state_dict:
+        if shape("encoder.conv_in.weight")[0] != ch:
+            refuse("encoder.conv_in.weight", f"has {shape('encoder.conv_in.weight')[0]} output channels; the decoder's "
+                                             f"ch is {ch}")
+        enc_attn = [lv for lv in levels if any(k.startswith(f"encoder.down.{lv}.attn.") for k in state_dict)]
+        if enc_attn != attn:
+            raise EngineError(f"VQGAN checkpoint: encoder.down.<level>.attn.* keys at levels {enc_attn}, "
+                              f"decoder.up.<level>.attn.* at {attn}; they must match")
+        if gumbel and shape("quantize.proj.weight") != (n_embed, zc, 1, 1):
+            refuse("quantize.proj.weight", f"has shape {list(shape('quantize.proj.weight'))}; GumbelQuantize's projection "
+                                           f"is [{n_embed}, {zc}, 1, 1]")
+    if zc % VQ_TC_CHANNEL_MULTIPLE:
+        refuse("post_quant_conv.weight", f"gives z_channels {zc}; the engine needs a multiple of {VQ_TC_CHANNEL_MULTIPLE}")
+    if n_embed % VQ_TC_CODE_MULTIPLE or n_embed > VQ_TC_MAX_CODES:
+        refuse(cb_key, f"has {n_embed} codes; the engine's nearest-code search takes a multiple of {VQ_TC_CODE_MULTIPLE} "
+                       f"up to {VQ_TC_MAX_CODES}")
+    return dict(z_channels=zc, n_embed=n_embed, ch=ch, ch_mult=tuple(ch_mult), num_res_blocks=blocks[0] - 1,
+                attn_resolution=attn_resolution, resolution=resolution, gumbel=gumbel)
+
+
 def aux_loss_width(kind, n_sets):
     """Loss-vector entries of one auxiliary loss: a cutout-space loss (saturation, palette, smoothness) has one per
     cutout set, in set order (its get_loss returns a list, spliced in by pixray.py:1392-1398); the others one."""
@@ -137,6 +220,9 @@ class B200Engine:
                 cfg.ch_mult[i] = m
             f = 2 ** (cfg.n_levels - 1)
             self.z_shape = (1, cfg.z_channels, image_hw[0] // f, image_hw[1] // f)
+            # a GumbelVQ (vqgan_config's `gumbel`): the engine reads its codebook from quantize.embed.weight and encodes
+            # with vqgan_encode_gumbel
+            self.gumbel = bool(v.get("gumbel", False))
         elif drawer == DRAWER_VDIFF:
             # VdiffDrawer's x (vdiff.py:118): [1, 3, gen_height, gen_width]; vdiff_gen_hw = (gen_h, gen_w), each side a
             # multiple of 64 and at least the canvas's (None: the canvas); the image is the canvas-size window centred in it
@@ -492,6 +578,19 @@ class B200Engine:
         out = self._new(*self.z_shape)
         torch.cuda.current_stream().synchronize()
         self._check(self.lib.pxr_vqgan_encode(self.h, self._p(img), self._p(out)), "pxr_vqgan_encode")
+        self.sync()
+        return out
+
+    def vqgan_encode_gumbel(self, img, noise):
+        """z = model.encode(img)[0] of a GumbelVQ (GumbelQuantize in eval mode, vqgan.py:174-185): img [1, 3, H, W] in
+        [-1, 1], noise the Gumbel draws F.gumbel_softmax adds to quantize.proj's logits, [1|-, n_embed, h, w] ->
+        z [1, C, h, w] (codebook rows)."""
+        img = img.to(self.device, torch.float32).reshape(1, 3, *self.image_hw).contiguous()
+        noise = noise.to(self.device, torch.float32).reshape(self.cfg.n_embed, *self.z_shape[2:]).contiguous()
+        out = self._new(*self.z_shape)
+        torch.cuda.current_stream().synchronize()
+        self._check(self.lib.pxr_vqgan_encode_gumbel(self.h, self._p(img), self._p(noise), self._p(out)),
+                    "pxr_vqgan_encode_gumbel")
         self.sync()
         return out
 

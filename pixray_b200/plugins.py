@@ -80,6 +80,8 @@ class VqganDrawer(DrawingInterface):
     @staticmethod
     def add_settings(parser):
         parser.add_argument("--vqgan_model", type=str, help="VQGAN model", default="imagenet_f16_16384", dest="vqgan_model")
+        parser.add_argument("--vqgan_config", type=str, help="VQGAN config", default=None, dest="vqgan_config")
+        parser.add_argument("--vqgan_checkpoint", type=str, help="VQGAN checkpoint", default=None, dest="vqgan_checkpoint")
         return parser
 
     def __init__(self, settings, session: Session):
@@ -91,6 +93,8 @@ class VqganDrawer(DrawingInterface):
         self.device = device
         lo, hi = self.session.engine.z_bounds()
         self.z_min, self.z_max = lo[None, :, None, None], hi[None, :, None, None]  # vqgan.py:141-142
+        # vqgan.py:124-131 (an engine class without the flag builds nearest-code VQGANs only)
+        self.gumbel = getattr(self.session.engine, "gumbel", False)
 
     def get_opts(self, decay_divisor):
         return None  # engine builds Adam on get_z(), like pixray.py:537-539
@@ -110,7 +114,13 @@ class VqganDrawer(DrawingInterface):
             self.z.copy_(new_z)
 
     def get_z_from_tensor(self, ref_tensor):
-        return self.session.engine.vqgan_encode(ref_tensor)
+        eng = self.session.engine
+        if not self.gumbel:
+            return eng.vqgan_encode(ref_tensor)
+        # GumbelQuantize's eval forward adds F.gumbel_softmax's noise, -log(Exp(1)), to every logit: drawn here, fresh
+        # for each encode, from torch's global generator, so every rank of a sharded run draws the same
+        noise = -torch.empty(eng.cfg.n_embed, *eng.z_shape[2:], device=eng.device).exponential_().log()
+        return eng.vqgan_encode_gumbel(ref_tensor, noise)
 
     def synth(self, cur_iteration):
         return self.session.engine.synth(self.z)

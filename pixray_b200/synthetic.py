@@ -100,9 +100,11 @@ def slip_state_dict(arch, seed=0):
     return sd
 
 
-def vqgan_state_dict(v, seed=0, with_encoder=False):
+def vqgan_state_dict(v, seed=0, with_encoder=False, gumbel=False):
     """taming VQModel tensors pixray uses: quantize.embedding, post_quant_conv, decoder.* (vqgan.py:122-142) and, with
-    with_encoder, encoder.* + quant_conv (model.encode: VqganDrawer.init_from_tensor, vqgan.py:174-185)."""
+    with_encoder, encoder.* + quant_conv (model.encode: VqganDrawer.init_from_tensor, vqgan.py:174-185).  gumbel: the
+    GumbelVQ layout instead -- the codebook under quantize.embed and, with the encoder, GumbelQuantize's 1x1 projection
+    quantize.proj [n_embed, z_channels]; every other tensor is the same draw."""
     g = torch.Generator().manual_seed(seed)
     sd = {}
 
@@ -129,7 +131,7 @@ def vqgan_state_dict(v, seed=0, with_encoder=False):
 
     zc, ch, mult, nrb = v["z_channels"], v["ch"], v["ch_mult"], v["num_res_blocks"]
     L = len(mult)
-    sd["quantize.embedding.weight"] = _randn(g, v["n_embed"], zc, std=0.5)
+    sd["quantize.embed.weight" if gumbel else "quantize.embedding.weight"] = _randn(g, v["n_embed"], zc, std=0.5)
     conv("post_quant_conv", zc, zc, 1)
     block_in = ch * mult[-1]
     curr = v["resolution"] // 2 ** (L - 1)
@@ -170,6 +172,8 @@ def vqgan_state_dict(v, seed=0, with_encoder=False):
         norm("encoder.norm_out", block_in)
         conv("encoder.conv_out", block_in, zc, 3)
         conv("quant_conv", zc, zc, 1)
+        if gumbel:
+            conv("quantize.proj", zc, v["n_embed"], 1)
     return sd
 
 
